@@ -200,8 +200,7 @@ int gk_create(int device_ordinal, gk_handle** out) {
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  GK_CUDA(cudaFuncSetAttribute(wl_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF_SMEM));
-  GK_CUDA(cudaFuncSetAttribute(wl_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(wl_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
   *out = h;
@@ -514,9 +513,7 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
   GK_TRY(h->block_sums.ensure((size_t)nb * 4));
   // >= 2 V slots (load <= 0.5 at the one level where almost every vertex is a class of its own; frozen vertices stop
   // inserting after it): three rotating tables stay L2-resident for the vertex counts of the benchmark workloads.
-  size_t table_factor = 2;
-  if (const char* e = getenv("GRAKEL_B200_WL_TABLE_FACTOR")) table_factor = (size_t)std::max(2, atoi(e));
-  h->ht_cap = std::max<size_t>(next_pow2((size_t)V * table_factor), 1024);
+  h->ht_cap = std::max<size_t>(next_pow2((size_t)V * 2), 1024);
   GK_TRY(h->ht_keys.ensure(h->ht_cap * 8 * 3));  // three tables: the fused kernel rotates them over the levels
   GK_TRY(h->ht_rep.ensure(h->ht_cap * 4 * 2));
   const size_t ft_level_cap = std::max<size_t>(next_pow2((size_t)V * 2), 1024);  // one L2-sized sub-table per level
@@ -637,7 +634,6 @@ static int wl_launch_v2(gk_handle* h, const WlPlan& pl, unsigned long long seed,
       fp.coo_keys = h->ft_keys.as<unsigned long long>(); fp.coo_cnt = h->ft_cnt.as<unsigned>();
       fp.seed = seed; fp.st = fst; fp.sc = sc;
       fp.diag_frozen = h->diag_frozen.as<unsigned long long>();
-      if (const char* e = getenv("GRAKEL_B200_WL_DBG")) fp.dbg = atoi(e);
       if (prof) {
         GK_TRY(h->K_stage.ensure((size_t)G * L * 128));
         GK_CUDA(cudaMemsetAsync(h->K_stage.p, 0, (size_t)G * L * 128, h->stream));
@@ -694,7 +690,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
       GK_TRY(wl_launch_v2(h, pl, seed, fst, prof));
       h->wl_sparse_ids = L > 1;
       GK_CUDA(cudaEventRecord(h->tev[3], h->stream));  // end of the feature stage
-      if (!prof && !getenv("GRAKEL_B200_NO_PROLOGUE")) {
+      if (!prof) {
         // Gram prologue of the square (fit_transform) case, enqueued BEFORE this call's one host synchronisation:
         // self similarities + per-CTA partials (diag_finish) and the column histogram (col_hist).  gk_gram then
         // finds everything its host-side decisions need (threshold T, D_c, exactness bounds) already on the host
@@ -764,14 +760,9 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
       fp.barrier = d_barrier;
       fp.labels_all = labels_all; fp.sig_nbr = h->sig_nbr.as<int>(); fp.slot_of = h->slot_of.as<int>();
       fp.rank_pack = h->flags.as<int>();
-      // singleton shortcut (wl_fused.cuh, SKIP); GRAKEL_B200_WL_SKIP=0 selects the kernel without it
-      const char* e_skip = getenv("GRAKEL_B200_WL_SKIP");
-      const bool wl_skip = !(e_skip && atoi(e_skip) == 0);
-      if (wl_skip) {
-        GK_TRY(h->wl_single.ensure((size_t)V));
-        GK_CUDA(cudaMemsetAsync(h->wl_single.p, 0, (size_t)V, h->stream));
-        fp.single = h->wl_single.as<unsigned char>();
-      }
+      GK_TRY(h->wl_single.ensure((size_t)V));  // singleton flags (wl_fused.cuh)
+      GK_CUDA(cudaMemsetAsync(h->wl_single.p, 0, (size_t)V, h->stream));
+      fp.single = h->wl_single.as<unsigned char>();
       fp.table = h->ht_keys.as<unsigned long long>();
       fp.ht_mask = (unsigned)(h->ht_cap - 1);
       fp.coo_keys = h->ft_keys.as<unsigned long long>(); fp.coo_cnt = h->ft_cnt.as<unsigned>();
@@ -783,8 +774,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
         fp.prof = h->K_stage.as<long long>();
       }
       void* args[] = {&fp};
-      GK_CUDA(cudaLaunchCooperativeKernel(wl_skip ? (void*)wl_fused_kernel<true> : (void*)wl_fused_kernel<false>, dim3(G),
-                                          dim3(WLF_THREADS), args, WLF_SMEM, h->stream));
+      GK_CUDA(cudaLaunchCooperativeKernel((void*)wl_fused_kernel, dim3(G), dim3(WLF_THREADS), args, WLF_SMEM, h->stream));
       LAUNCH_CHECK(h);
       if (prof) {
         std::vector<long long> pr((size_t)G * L * 16);
@@ -2188,9 +2178,9 @@ int gk_tu_close(gk_tu* t) {
 static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_out, int32_t out_dtype, int64_t ld,
                          double* xdiag, gk_stats* stats, bool* done) {
   *done = false;
-  for (const char* name : {"GRAKEL_B200_NO_ASYNC", "GRAKEL_B200_PROF", "GRAKEL_B200_NO_PROLOGUE", "GRAKEL_B200_WL_V1",
-                           "GRAKEL_B200_WL_FUSED", "GRAKEL_B200_CTA2", "GRAKEL_B200_NO_TMA_STORE", "GRAKEL_B200_WIDEN",
-                           "GRAKEL_B200_NO_TRI", "GRAKEL_B200_MIRROR_TMA", "GRAKEL_B200_DEBUG"})
+  for (const char* name : {"GRAKEL_B200_NO_ASYNC", "GRAKEL_B200_PROF", "GRAKEL_B200_WL_V1", "GRAKEL_B200_WL_FUSED",
+                           "GRAKEL_B200_CTA2", "GRAKEL_B200_NO_TMA_STORE", "GRAKEL_B200_WIDEN", "GRAKEL_B200_NO_TRI",
+                           "GRAKEL_B200_MIRROR_TMA", "GRAKEL_B200_DEBUG"})
     if (getenv(name)) return GK_OK;
   if (flags & ~(GK_OUT_DEVICE | GK_DENSE_ALL)) return GK_OK;
   if (h->N <= 0 || !h->has_labels || h->V == 0 || n_iter < 0 || n_iter + 1 >= MAX_LEVELS || h->n_rows > 0) return GK_OK;

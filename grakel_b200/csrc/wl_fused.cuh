@@ -51,7 +51,7 @@ struct WlFusedParams {
   int* sig_nbr;          // [E] sorted neighbour labels of the current level
   int* slot_of;          // [V] hash slot, then representative vertex
   int* rank_pack;        // [V] valid for representatives
-  unsigned char* single; // [V] SKIP variant: the vertex's label of the previous level is held by no other vertex
+  unsigned char* single; // [V] zeroed by the host: the vertex's label of the previous level is held by no other vertex
   int* cta_count;        // [grid]
   unsigned long long* table;  // 2 x (ht_mask + 1) packed {tag, representative} words
   unsigned ht_mask;
@@ -238,13 +238,11 @@ __device__ __forceinline__ void wlf_emit(const WlFusedParams& p, int v0, int nv,
   __syncthreads();  // agg is reused by the next tile
 }
 
-// SKIP = true: vertices whose previous label is a singleton class (no other vertex of the data set carries it) are
-// not hashed, inserted or verified again -- their next label is necessarily a singleton too (the signature contains
-// the own label) -- and their feature entry is (graph, column, 1) without the in-graph count.  From level 3 on
-// that is 96 % of the vertices of BASELINE config 2.  The table word gains a "single" bit below the (then 30-bit)
-// tag: the installing CAS sets it, the first matching vertex clears it with the atomicMin that also elects the
-// smaller representative.  SKIP = false is the kernel without it.
-template <bool SKIP>
+// Vertices whose previous label is a singleton class (no other vertex of the data set carries it) are not hashed,
+// inserted or verified again -- their next label is necessarily a singleton too (the signature contains the own
+// label) -- and their feature entry is (graph, column, 1) without the in-graph count.  From level 3 on that is 96 % of
+// the vertices of BASELINE config 2.  The table word carries a "single" bit below the 30-bit tag: the installing CAS
+// sets it, the first matching vertex clears it with the atomicMin that also elects the smaller representative.
 __global__ void __launch_bounds__(WLF_THREADS, 1)
 wl_fused_kernel(WlFusedParams p) {
   extern __shared__ __align__(16) unsigned char wlf_smem[];
@@ -318,7 +316,7 @@ wl_fused_kernel(WlFusedParams p) {
         const int beg = rp_s[i];
         const int deg = rp_s[i + 1] - beg;
         if (deg > 8) continue;
-        if constexpr (SKIP) { if (p.single[v0 + i]) continue; }
+        if (p.single[v0 + i]) continue;
         int x0, x1, x2, x3, x4, x5, x6, x7;
         x0 = 0 < deg ? lab_s[col_s[beg + 0]] : 0x7fffffff;
         x1 = 1 < deg ? lab_s[col_s[beg + 1]] : 0x7fffffff;
@@ -353,7 +351,7 @@ wl_fused_kernel(WlFusedParams p) {
       for (int i0 = wid * 32; i0 < nv; i0 += WLF_THREADS) {
         const int iv = i0 + lane;
         bool big = iv < nv && (rp_s[iv + 1] - rp_s[iv]) > 8;
-        if constexpr (SKIP) { if (big && p.single[v0 + iv]) big = false; }
+        if (big && p.single[v0 + iv]) big = false;
         unsigned m = __ballot_sync(0xffffffffu, big);
         while (m) {
           const int i = i0 + __ffs(m) - 1;
@@ -423,7 +421,7 @@ wl_fused_kernel(WlFusedParams p) {
         for (int k = 0; k < WLF_VPT; ++k) {
           const int i = tid + k * WLF_THREADS;
           act[k] = i < nv;
-          if constexpr (SKIP) { if (act[k] && p.single[v0 + i]) act[k] = false; }
+          if (act[k] && p.single[v0 + i]) act[k] = false;
           key[k] = act[k] ? key_s[i] : 0ULL;
           slot[k] = (unsigned)((key[k] & 0xFFFFFFFFULL) * 0x9E3779B1ULL >> 8) & p.ht_mask;
         }
@@ -435,8 +433,8 @@ wl_fused_kernel(WlFusedParams p) {
           // for every vertex.
 #pragma unroll
           for (int k = 0; k < WLF_VPT; ++k) {
-            unsigned long long mine = (key[k] & 0xFFFFFFFF00000000ULL) | (unsigned)(v0 + tid + k * WLF_THREADS);
-            if constexpr (SKIP) mine |= 1ULL << 32;  // {30-bit tag | single = 1 | vertex}
+            // {30-bit tag | single = 1 | vertex}
+            const unsigned long long mine = (key[k] & 0xFFFFFFFF00000000ULL) | (1ULL << 32) | (unsigned)(v0 + tid + k * WLF_THREADS);
             w[k] = act[k] ? atomicCAS(&tab[slot[k]], EMPTY64, mine) : 0ULL;
           }
           any = false;
@@ -444,19 +442,12 @@ wl_fused_kernel(WlFusedParams p) {
           for (int k = 0; k < WLF_VPT; ++k) {
             if (!act[k]) continue;
             const int v = v0 + tid + k * WLF_THREADS;
-            const unsigned long long mine = (key[k] & 0xFFFFFFFF00000000ULL) | (unsigned)v;
             if (w[k] == EMPTY64) { act[k] = false; continue; }  // the CAS installed our word
-            if constexpr (SKIP) {
-              if ((w[k] >> 33) == (key[k] >> 33)) {
-                const unsigned rep = (unsigned)w[k];
-                // a second member: clear the single bit and keep the smaller representative in one atomicMin
-                if (((w[k] >> 32) & 1ULL) || rep > (unsigned)v)
-                  atomicMin(&tab[slot[k]], (key[k] & 0xFFFFFFFE00000000ULL) | (unsigned)min(rep, (unsigned)v));
-                act[k] = false;
-                continue;
-              }
-            } else if ((w[k] >> 32) == (key[k] >> 32)) {
-              if ((unsigned)w[k] > (unsigned)v) atomicMin(&tab[slot[k]], mine);
+            if ((w[k] >> 33) == (key[k] >> 33)) {
+              const unsigned rep = (unsigned)w[k];
+              // a second member: clear the single bit and keep the smaller representative in one atomicMin
+              if (((w[k] >> 32) & 1ULL) || rep > (unsigned)v)
+                atomicMin(&tab[slot[k]], (key[k] & 0xFFFFFFFE00000000ULL) | (unsigned)min(rep, (unsigned)v));
               act[k] = false;
               continue;
             }
@@ -488,22 +479,18 @@ wl_fused_kernel(WlFusedParams p) {
         const int i = tid + k * WLF_THREADS;
         r[k] = i < nv ? p.slot_of[v0 + i] : 0;
       }
-      bool sgl[WLF_VPT];  // SKIP: the vertex's label of THIS level is a singleton class
+      bool sgl[WLF_VPT];  // the vertex's label of THIS level is a singleton class
 #pragma unroll
       for (int k = 0; k < WLF_VPT; ++k) {
         const int i = tid + k * WLF_THREADS;
         sgl[k] = false;
-        if constexpr (SKIP) {
-          if (i < nv) {
-            if (p.single[v0 + i]) { r[k] = v0 + i; sgl[k] = true; }  // never inserted: its own representative
-            else {
-              const unsigned long long word = __ldcg(&tab[r[k]]);
-              r[k] = (int)(unsigned)word;
-              sgl[k] = ((word >> 32) & 1ULL) && r[k] == v0 + i;
-            }
+        if (i < nv) {
+          if (p.single[v0 + i]) { r[k] = v0 + i; sgl[k] = true; }  // never inserted: its own representative
+          else {
+            const unsigned long long word = __ldcg(&tab[r[k]]);
+            r[k] = (int)(unsigned)word;
+            sgl[k] = ((word >> 32) & 1ULL) && r[k] == v0 + i;
           }
-        } else {
-          if (i < nv) r[k] = (int)(unsigned)__ldcg(&tab[r[k]]);
         }
       }
       // verification against the representative: its CSR row and label are fetched for all (<= 4)
@@ -527,7 +514,7 @@ wl_fused_kernel(WlFusedParams p) {
         int f = 0;
         if (i < nv) {
           p.slot_of[v] = r[k];
-          if constexpr (SKIP) p.single[v] = sgl[k] ? 1 : 0;
+          p.single[v] = sgl[k] ? 1 : 0;
           f = (r[k] == v);
           if (!f) {
             bool same = (dv[k] == dr[k]) && (lo[k] == lr[k]);
@@ -595,7 +582,7 @@ wl_fused_kernel(WlFusedParams p) {
           }
         }
         __syncthreads();
-        wlf_emit(p, v0, nv, lab_s, agg, level_base, (size_t)lv * V + v0, s_warp, mx, n_new, SKIP ? p.single : nullptr);
+        wlf_emit(p, v0, nv, lab_s, agg, level_base, (size_t)lv * V + v0, s_warp, mx, n_new, p.single);
       }
       if (b == 0 && tid == 0) {
         p.sc->level_dims[lv] = total;

@@ -60,7 +60,6 @@ struct WlFused2Params {
   unsigned long long* diag_frozen;  // [N] zeroed by the host: the frozen vertices' share of st.diag (WL-OA re-adds it)
   DevScalars* sc;     // level_dims[1..] zeroed by the host, level_base[0], [1] set
   long long* prof;    // optional [grid][L][16] globaltimer stamps (GRAKEL_B200_PROF), else NULL
-  int dbg;            // GRAKEL_B200_WL_DBG: 1 = no bulk copy-out, 2 = L2 loads for the own row, 4 = print the first mismatch
 };
 
 // Feature entries of one tile from the labels in lab_s: a non-frozen vertex i emits (graph, base + label, count)
@@ -222,14 +221,8 @@ __device__ __forceinline__ void wlf2_emit(const WlFused2Params& p, int v0, int n
   __syncthreads();  // agg is reused by the next tile / overwritten by the next level's signatures
 }
 
-// CTA-local signature dedup before the global table (resident tiles): a tile of config 2 still holds about as many
-// distinct keys as vertices at level 1, and every other level pays for the shared-memory table (initialisation,
-// probing, two more block barriers).  Kept behind this switch, off; the code is compiled out.
-constexpr bool WLF2_LOCAL_DEDUP = false;
-constexpr int WLF2_LTAB = 4096;  // per-tile signature table (resident tiles): >= WLF_TILE_V slots
-static_assert(WLF2_LTAB >= WLF_TILE_V, "every vertex of a tile must find a slot");
 constexpr int WLF2_SMEM = WLF_SMEM + WLF_TILE_V /*frz_s*/ + WLF_TILE_V * 4 /*gid_s*/ + WLF_TILE_V * 4 /*gbeg_s, gend_s*/ +
-                          WLF2_LTAB * 4 /*ltab*/ + WLF2_LTAB / 8 /*lmulti*/ + WLF_TILE_V * 2 /*lslot*/;
+                          WLF_TILE_V * 4 /*slot_s | list_s*/ + WLF_TILE_V * 2 /*cf_s*/;
 static_assert(WLF2_SMEM <= 232448, "shared memory budget of one CTA");
 
 // Global -> shared staging of a tile with several loads in flight per thread.  A plain strided loop keeps ONE load
@@ -278,7 +271,7 @@ __device__ __forceinline__ void wlf2_stage_labels(const WlFused2Params& p, const
 // PAY: slot payloads (see [A3]) instead of the representative's CSR row as the verification reference.  A template
 // parameter, not a runtime switch: with both schemes live in one instance the kernel spilled 368 bytes per thread
 // at its 64-register budget.  Compiled for sm_90a, each instance alone still spills (PAY = true: 212 bytes of spill
-// stores per thread, PAY = false: 60); the register budget of this kernel on H100 is an open item (DESIGN.md §7).
+// stores per thread, PAY = false: 46); the register budget of this kernel on H100 is an open item (DESIGN.md §7).
 template <bool PAY>
 __global__ void __launch_bounds__(WLF_THREADS, 1)
 wl_fused2_kernel(WlFused2Params p) {
@@ -293,14 +286,12 @@ wl_fused2_kernel(WlFused2Params p) {
   int* gid_s = reinterpret_cast<int*>(frz_s + WLF_TILE_V);  // graph of every tile vertex
   unsigned short* gbeg_s = reinterpret_cast<unsigned short*>(gid_s + WLF_TILE_V);  // its graph's vertex range, tile-local
   unsigned short* gend_s = gbeg_s + WLF_TILE_V;
-  // resident tiles: CTA-local dedup of the signatures before the global table (see [A3])
-  unsigned* ltab = reinterpret_cast<unsigned*>(gend_s + WLF_TILE_V);   // slot -> smallest tile vertex with this key
-  unsigned* lmulti = ltab + WLF2_LTAB;                                 // bit per slot: the key has more than one vertex in the tile
-  unsigned short* lslot = reinterpret_cast<unsigned short*>(lmulti + WLF2_LTAB / 32);  // vertex -> its slot
-  // payload scheme, resident tiles: slot (| installer bit) of every tile vertex from [A] to [B] of a level; the region is
-  // the emit phase's compaction list otherwise, which runs after [B] has consumed the slots
-  unsigned* slot_s = ltab;
-  static_assert(WLF2_LTAB * 4 >= WLF_TILE_V * 4, "slot_s holds one word per tile vertex");
+  // payload scheme, resident tiles: slot (| installer bit) of every tile vertex from [A] to [B] of a level; the same
+  // region holds the emit phase's compaction list (list_s), which runs after [B] has consumed the slots
+  unsigned* slot_s = reinterpret_cast<unsigned*>(gend_s + WLF_TILE_V);
+  unsigned short* list_s = reinterpret_cast<unsigned short*>(slot_s);
+  unsigned short* cf_s = reinterpret_cast<unsigned short*>(slot_s + WLF_TILE_V);  // emit phase: in-graph count | emitter bit
+  unsigned* ct = reinterpret_cast<unsigned*>(key_s);  // emit phase: the (graph, label) table (key_s is free after [A])
   __shared__ int s_warp[32];
   __shared__ unsigned s_red[128];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -371,7 +362,7 @@ wl_fused2_kernel(WlFused2Params p) {
     }
     __syncthreads();
     WLF_STAMP(0, 1);
-    wlf2_emit(p, v0, nv, lab_s, frz_s, gid_s, gbeg_s, gend_s, lslot, reinterpret_cast<unsigned*>(key_s), reinterpret_cast<unsigned short*>(ltab), agg, 0, (size_t)v0, s_warp, mx, n_new);
+    wlf2_emit(p, v0, nv, lab_s, frz_s, gid_s, gbeg_s, gend_s, cf_s, ct, list_s, agg, 0, (size_t)v0, s_warp, mx, n_new);
     WLF_STAMP(0, 2);
   }
   if (p.L > 2) {  // table of level 2 (first touched after the barrier of level 1)
@@ -505,47 +496,13 @@ wl_fused2_kernel(WlFused2Params p) {
       {
         unsigned long long key[WLF_VPT], w[WLF_VPT];
         unsigned slot[WLF_VPT];
-        bool act[WLF_VPT], ins[WLF_VPT], lone[WLF_VPT], won[WLF_VPT];
+        bool act[WLF_VPT], ins[WLF_VPT], won[WLF_VPT];
 #pragma unroll
         for (int k = 0; k < WLF_VPT; ++k) {
           const int i = tid + k * WLF_THREADS;
           act[k] = i < nv && !frz_s[i];
           key[k] = act[k] ? key_s[i] : 0ULL;
-          lone[k] = true;
           won[k] = false;
-        }
-        if (WLF2_LOCAL_DEDUP && resident) {
-          // CTA-local dedup: slot -> smallest vertex of the tile with this key; later vertices of the key mark it "multi"
-          for (int s2 = tid; s2 < WLF2_LTAB; s2 += WLF_THREADS) ltab[s2] = 0xFFFFFFFFu;
-          for (int s2 = tid; s2 < WLF2_LTAB / 32; s2 += WLF_THREADS) lmulti[s2] = 0u;
-          __syncthreads();
-#pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            if (!act[k]) continue;
-            const unsigned i = (unsigned)(tid + k * WLF_THREADS);
-            unsigned hs = (unsigned)((key[k] >> 7) * 0x9E3779B1ULL >> 11) & (WLF2_LTAB - 1);
-            while (true) {
-              unsigned cur = ltab[hs];
-              if (cur == 0xFFFFFFFFu) {
-                cur = atomicCAS(&ltab[hs], 0xFFFFFFFFu, i);
-                if (cur == 0xFFFFFFFFu) break;  // first vertex of this key in the tile
-              }
-              if (key_s[cur] == key[k]) {
-                if (cur != i) { atomicMin(&ltab[hs], i); atomicOr(&lmulti[hs >> 5], 1u << (hs & 31)); }
-                break;
-              }
-              hs = (hs + 1) & (WLF2_LTAB - 1);
-            }
-            lslot[i] = (unsigned short)hs;
-          }
-          __syncthreads();
-#pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            if (!act[k]) continue;
-            const unsigned i = (unsigned)(tid + k * WLF_THREADS), hs = lslot[i];
-            lone[k] = !((lmulti[hs >> 5] >> (hs & 31)) & 1u);
-            if (ltab[hs] != i) act[k] = false;  // a follower: its local representative speaks for it
-          }
         }
 #pragma unroll
         for (int k = 0; k < WLF_VPT; ++k) {
@@ -558,7 +515,7 @@ wl_fused2_kernel(WlFused2Params p) {
           // slot's word back from the failed CAS
 #pragma unroll
           for (int k = 0; k < WLF_VPT; ++k) {
-            const unsigned long long mine = (key[k] & 0xFFFFFFFE00000000ULL) | (lone[k] ? (1ULL << 32) : 0ULL) |
+            const unsigned long long mine = (key[k] & 0xFFFFFFFE00000000ULL) | (1ULL << 32) |
                                             (unsigned)(v0 + tid + k * WLF_THREADS);
             w[k] = act[k] ? atomicCAS(&tab[slot[k]], EMPTY64, mine) : 0ULL;
           }
@@ -623,7 +580,7 @@ wl_fused2_kernel(WlFused2Params p) {
           for (int k = 0; k < WLF_VPT; ++k) n_ins += __syncthreads_count(ins[k] ? 1 : 0);
         }
         if (PAY && resident) {
-        } else if (2 * n_ins >= nv && !(p.dbg & 1)) {
+        } else if (2 * n_ins >= nv) {
           for (int j = tid; j < ne; j += WLF_THREADS) sig_g[e0 + j] = sig_s[j];
         } else {
 #pragma unroll
@@ -651,18 +608,12 @@ wl_fused2_kernel(WlFused2Params p) {
         stage_graphs(v0, nv);
         __syncthreads();
       }
-      int r[WLF_VPT], lrep[WLF_VPT];
-      bool act[WLF_VPT], sgl[WLF_VPT], fol[WLF_VPT];  // fol: follower of a local representative (resident tiles)
+      int r[WLF_VPT];
+      bool act[WLF_VPT], sgl[WLF_VPT];
 #pragma unroll
       for (int k = 0; k < WLF_VPT; ++k) {
         const int i = tid + k * WLF_THREADS;
         act[k] = i < nv && !frz_s[i];
-        fol[k] = false;
-        lrep[k] = i;
-        if (WLF2_LOCAL_DEDUP && act[k] && resident) {
-          lrep[k] = (int)ltab[lslot[i]];
-          if (lrep[k] != i) { fol[k] = true; act[k] = false; }
-        }
         r[k] = act[k] ? ((PAY && resident) ? (int)slot_s[i] : p.slot_of[v0 + i]) : 0;
       }
       uint4 pl0[WLF_VPT], pl1[WLF_VPT];  // payload scheme: the installer's signature (vertices that did not install)
@@ -711,13 +662,6 @@ wl_fused2_kernel(WlFused2Params p) {
         const int v = v0 + i;
         unsigned long long fz = 0ULL;  // self-similarity contribution of a vertex that freezes now
         const int gg = i < nv ? gid_s[i] : -1;  // every vertex: graphs stay contiguous lane runs
-        if (fol[k]) {  // same 64-bit key as the local representative: compare the full signatures in shared memory
-          const int l = lrep[k];
-          const int bi = rp_s[i], di = rp_s[i + 1] - bi, bl = rp_s[l], dl = rp_s[l + 1] - bl;
-          bool same = (di == dl) && (lab_s[i] == lab_s[l]);
-          for (int j = 0; same && j < di; ++j) same = sig_s[bi + j] == sig_s[bl + j];
-          if (!same) atomicOr(&p.sc->collision, 1u);
-        }
         if (PAY && chk[k]) {  // compare with the installer's signature in the slot payload
           const int pn[6] = {(int)pl0[k].z, (int)pl0[k].w, (int)pl1[k].x, (int)pl1[k].y, (int)pl1[k].z, (int)pl1[k].w};
           const int d = dv[k];
@@ -728,21 +672,12 @@ wl_fused2_kernel(WlFused2Params p) {
             for (int j = 0; j < 6; ++j)
               if (j < nd) same = same && ((resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) == pn[j]);
             if (d > 6) {
-              const int off = pn[5] - 0;  // installer's row offset in sig_nbr
+              const int off = pn[5];  // installer's row offset in sig_nbr
               for (int j = 5; same && j < d; ++j)
                 same = (resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) == __ldcg(&sig_g[off + j]);
             }
           }
-          if (!same) {
-            const unsigned before = atomicOr(&p.sc->collision, 1u << min(lv, 30));
-#ifdef WLF2_DEBUG_PRINT
-            if ((p.dbg & 4) && before == 0u)
-              printf("[wl_fused2] payload mismatch level %d cta %d tile %d v %d deg %d/%d own label %d/%d resident %d\n", lv, b, t, v, d,
-                     (int)pl0[k].y, lo[k], (int)pl0[k].x, (int)resident);
-#else
-            (void)before;
-#endif
-          }
+          if (!same) atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
         }
         if (act[k]) {
           if (PAY) {
@@ -753,7 +688,7 @@ wl_fused2_kernel(WlFused2Params p) {
               int a[8], c[8];
 #pragma unroll
               for (int j = 0; j < 8; ++j) {
-                a[j] = j < dv[k] ? (resident ? sig_s[bv[k] + j] : ((p.dbg & 2) ? __ldcg(&sig_g[bv[k] + j]) : sig_g[bv[k] + j])) : 0;
+                a[j] = j < dv[k] ? (resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) : 0;
                 c[j] = j < dv[k] ? __ldcg(&sig_g[br[k] + j]) : 0;
               }
 #pragma unroll
@@ -762,16 +697,7 @@ wl_fused2_kernel(WlFused2Params p) {
               for (int j = 0; same && j < dv[k]; ++j)
                 same = (resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) == __ldcg(&sig_g[br[k] + j]);
             }
-            if (!same) {
-              const unsigned before = atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
-#ifdef WLF2_DEBUG_PRINT
-              if ((p.dbg & 4) && before == 0u)
-                printf("[wl_fused2] mismatch level %d cta %d tile %d v %d rep %d deg %d/%d own label %d/%d resident %d first nbr %d/%d\n", lv, b, t, v,
-                       r[k], dv[k], dr[k], lo[k], lr[k], (int)resident, dv[k] ? sig_g[p.row_ptr[v]] : -1, dr[k] ? sig_g[br[k]] : -1);
-#else
-              (void)before;
-#endif
-            }
+            if (!same) atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
           } else {
             n_rep += 1u;
           }
@@ -781,7 +707,7 @@ wl_fused2_kernel(WlFused2Params p) {
             n_fz += (unsigned)(p.L - lv);
             mx = max(mx, 1u);
           }
-        } else if (i < nv && !fol[k]) {
+        } else if (i < nv) {
           n_rep += 1u;  // a frozen vertex is a class of its own at every level
         }
         // per-graph aggregation of the frozen contributions (runs of equal graph inside the warp)
@@ -800,17 +726,6 @@ wl_fused2_kernel(WlFused2Params p) {
       }
       WLF_STAMP(lv, 4);
       __syncthreads();  // every thread has read the old labels / flags of the tile it needs
-      if (WLF2_LOCAL_DEDUP && resident) {  // followers take the label of their local representative (key_s is free after [A]: new labels)
-        int* newlab = reinterpret_cast<int*>(key_s);
-#pragma unroll
-        for (int k = 0; k < WLF_VPT; ++k)
-          if (act[k]) newlab[tid + k * WLF_THREADS] = r[k];
-        __syncthreads();
-#pragma unroll
-        for (int k = 0; k < WLF_VPT; ++k)
-          if (fol[k]) { r[k] = newlab[lrep[k]]; act[k] = true; sgl[k] = false; }
-        __syncthreads();  // key_s is written again by the next level's signatures
-      }
 #pragma unroll
       for (int k = 0; k < WLF_VPT; ++k) {
         const int i = tid + k * WLF_THREADS;
@@ -822,7 +737,7 @@ wl_fused2_kernel(WlFused2Params p) {
       __syncthreads();
       for (int i = tid; i < nv; i += WLF_THREADS) lab_out[v0 + i] = lab_s[i];
       WLF_STAMP(lv, 5);
-      wlf2_emit(p, v0, nv, lab_s, frz_s, gid_s, gbeg_s, gend_s, lslot, reinterpret_cast<unsigned*>(key_s), reinterpret_cast<unsigned short*>(ltab), agg, level_base, (size_t)lv * V + v0, s_warp, mx, n_new);
+      wlf2_emit(p, v0, nv, lab_s, frz_s, gid_s, gbeg_s, gend_s, cf_s, ct, list_s, agg, level_base, (size_t)lv * V + v0, s_warp, mx, n_new);
     }
     WLF_STAMP(lv, 3);
     if (lv + 2 < p.L) {  // clear the table level lv+2 inserts into (last read in [B] of level lv-1, which every CTA has left)
