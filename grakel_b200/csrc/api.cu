@@ -1408,10 +1408,15 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
     LAUNCH_CHECK(h);
   }
   GK_TRY(h->diag_f64.ensure(N * 8));
-  rownorm_f64_kernel<<<(int)N, 256, 0, h->stream>>>(h->fattr.as<double>(), Dfeat, (int)N, h->diag_f64.as<double>());
+  DevScalars* sc = h->scalars.as<DevScalars>();
+  rownorm_f64_kernel<<<(int)N, 256, 0, h->stream>>>(h->fattr.as<double>(), Dfeat, (int)N, h->diag_f64.as<double>(),
+                                                     &sc->fattr_negative);
   LAUNCH_CHECK(h);
   GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  unsigned* h_negative = &h->h_scalars.as<DevScalars>()->fattr_negative;
+  GK_CUDA(cudaMemcpyAsync(h_negative, &sc->fattr_negative, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));  // host vectors above are sources of async copies
+  h->fattr_signed = *h_negative != 0;
   h->n_columns = Dfeat;
   h->features_ready = true; h->feat_serial++;
   h->feature_kind = 3;
@@ -1431,11 +1436,13 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
 
 static void build_tiles(std::vector<int2>& tiles, int a0, int a1, int b0, int b1, bool upper_only, int bm);
 
-// Gram of the dense fp64 SP-attr feature matrix (feature_kind == 3).  Default: the wgmma kernel with tf32
-// operands on a hi/lo split of the features (3xTF32: hi hi^T + hi lo^T + lo hi^T, fp32 accumulation in registers,
-// k range processed in chunks and summed in fp64), self similarities exact in fp64; measured against the fp64
-// CUDA-core Gram (GRAKEL_B200_SPATTR_F64=1 selects it) the relative difference is ~1e-7, the north_star's
-// tolerance for real-valued Gram entries is 1e-5.
+// Gram of the dense fp64 SP-attr feature matrix (feature_kind == 3).  Non-negative features: the wgmma kernel with
+// tf32 operands on a hi/lo split of the features (3xTF32: hi hi^T + hi lo^T + lo hi^T, fp32 accumulation in
+// registers, k range processed in chunks and summed in fp64), self similarities exact in fp64.  Its error is a small
+// multiple of 2^-22 times sum_k |phi_ik| |phi_jk| (measured on an H100: below 1e-6 of it), which for non-negative
+// features is K_ij itself: every entry within 1e-5 relative.  A feature map with a negative entry (attributes of
+// mixed sign) can have entries that cancel far below that scale, so it takes the fp64 CUDA-core Gram (1e-9).
+// GRAKEL_B200_SPATTR_F64=1 forces the fp64 Gram, =0 the tensor-core Gram.
 static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
                        int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
   if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "ShortestPathAttr Gram is fp64 only");
@@ -1453,7 +1460,7 @@ static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_b
   const int a0 = (int)((square ? 0 : n_fit) + row_begin), a1 = (int)((square ? 0 : n_fit) + row_end);
   GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
   const char* e_f64 = getenv("GRAKEL_B200_SPATTR_F64");
-  const bool use_f64 = e_f64 && atoi(e_f64) != 0;
+  const bool use_f64 = (e_f64 && *e_f64) ? atoi(e_f64) != 0 : h->fattr_signed;
   if (k_rows > 0 && !use_f64) {
     const long long D = h->fattr_dim, Dp = (D + BK_TF32 - 1) / BK_TF32 * BK_TF32, W = 3 * Dp;
     GK_TRY(h->panel.ensure((size_t)N * W * 4 * 2));
@@ -1527,7 +1534,7 @@ static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_b
     GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
   if (stats) {
-    stats->gram_path = 4;
+    stats->gram_path = use_f64 ? 5 : 4;
     stats->gemm_launches = h->launches - launches0;
     stats->ms_gemm = ev_ms(h->tev[6], h->tev[7]);
   }

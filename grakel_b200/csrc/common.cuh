@@ -104,6 +104,8 @@ struct DevScalars {
   unsigned long long sp_coo;             // wl_fused2: self-similarity units of frozen vertices (= sum of diag_frozen)
   unsigned int sp_dict_size;             // SP: number of distinct (lu,lv,d) keys
   unsigned int sp_nonint;                // SP: a non-integer / out-of-range distance was met
+  unsigned int fattr_negative;           // SP-attr: the feature map has a negative entry
+  unsigned int pad0;
 };
 
 static_assert(sizeof(DevScalars) % 8 == 0, "cleared as 64-bit words");
@@ -188,9 +190,10 @@ struct gk_handle {
   int sp_flags = 0;
   int sp_dist_esz = 0;     // gk_spattr_features: element size of the matrices it left in sp_dist (2 = u16, 8 = fp64)
 
-  // ---- SP-attr dense fp32 feature matrix
+  // ---- SP-attr dense fp64 feature matrix
   gk::DevBuf fattr;
   int64_t fattr_dim = 0;
+  bool fattr_signed = false;  // some feature is negative: entries of K may cancel (gram_spattr takes the fp64 Gram)
 
   // ---- GEMM
   gk::DevBuf tiles;  // int2 list

@@ -301,14 +301,20 @@ set_diag_f64(int a0, int a1, int b0, int b1, const double* __restrict__ diag, do
   if (r < a1 && r >= b0 && r < b1) out[(long long)(r - a0) * ld + (r - b0)] = diag[r];
 }
 
-// per-row self similarity <phi[g], phi[g]>
+// per-row self similarity <phi[g], phi[g]>; *negative |= 1 if the row has a negative entry
 __global__ void __launch_bounds__(256)
-rownorm_f64_kernel(const double* __restrict__ phi, long long D, int N, double* __restrict__ diag) {
+rownorm_f64_kernel(const double* __restrict__ phi, long long D, int N, double* __restrict__ diag, unsigned* __restrict__ negative) {
   const int g = blockIdx.x;
   if (g >= N) return;
   __shared__ double red[8];
   double s = 0.0;
-  for (long long k = threadIdx.x; k < D; k += 256) { const double x = phi[(long long)g * D + k]; s += x * x; }
+  bool neg = false;
+  for (long long k = threadIdx.x; k < D; k += 256) {
+    const double x = phi[(long long)g * D + k];
+    s += x * x;
+    neg |= x < 0.0;
+  }
+  if (__syncthreads_or(neg) && threadIdx.x == 0) atomicOr(negative, 1u);
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) s += __shfl_xor_sync(0xffffffffu, s, d);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;

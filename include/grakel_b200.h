@@ -102,7 +102,8 @@ typedef struct gk_stats {
   int64_t max_count;         /* largest single feature count */
   int64_t max_diag;          /* largest self-similarity */
   int64_t hash_retries;      /* WL: relabel passes repeated after a detected hash collision */
-  int64_t gram_path;         /* 1 = wgmma bf16 tensor-core GEMM, 2 = exact int64 CUDA-core Gram, 3 = no contracted columns */
+  int64_t gram_path;         /* 1 = wgmma bf16 tensor-core GEMM, 2 = exact int64 CUDA-core Gram, 3 = no contracted columns,
+                                ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
