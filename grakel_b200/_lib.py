@@ -20,6 +20,7 @@ GK_NORMALIZE, GK_NAN_TO_NUM, GK_GRAM_SIMT, GK_OUT_DEVICE, GK_FULL_TILES, GK_DENS
 GK_DIST, GK_DIST_GATHER = 64, 128
 GK_SP_WITH_LABELS, GK_SP_KEEP_DIST, GK_SP_DIJKSTRA_ORDER = 1, 2, 4
 GK_ERR_RANGE, GK_ERR_UNSUPPORTED = -4, -5
+GK_GH_LINEAR, GK_GH_GAUSSIAN, GK_GH_BRIDGE = 0, 1, 2
 
 
 class GkStats(C.Structure):
@@ -60,6 +61,8 @@ _SYMBOLS = {
     "gk_spattr_features": (C.c_int, [_P, C.c_int32, C.POINTER(GkStats)]),
     "gk_wl_sp_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(GkStats)]),
     "gk_wl_oa_features": (C.c_int, [_P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_gh_features": (C.c_int, [_P, C.c_int32, C.c_double, C.c_int32, C.POINTER(GkStats)]),
+    "gk_gh_node_maps": (C.c_int, [_P, C.c_int64, _P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -245,6 +248,21 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_spattr_features(self.h, GK_SP_DIJKSTRA_ORDER if dijkstra_order else 0, C.byref(st)))
         return st
+
+    def gh_features(self, node_kernel=GK_GH_LINEAR, mu=1.0):
+        """GraphHopper node maps and, for the linear node kernel, its feature map (gk_gh_features)."""
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_gh_features(self.h, int(node_kernel), float(mu), 0, C.byref(st)))
+        self.gh_delta = int(st.level_dims[0])
+        return st
+
+    def gh_node_maps(self, g, n):
+        """Graph g's n x delta x delta node maps M of the last gh_features call."""
+        out = np.empty((n, self.gh_delta, self.gh_delta), dtype=np.float64)
+        with self._lock:
+            self._check(self.lib.gk_gh_node_maps(self.h, int(g), _ptr(out)))
+        return out
 
     def gram(self, n_graphs, n_fit=None, normalize=False, nan_to_num=False, out=None, dtype=np.float64,
              row_range=None, simt=False, full_tiles=False, stats=None, want_diag=True, device_ptr=None, ld=0,

@@ -21,6 +21,7 @@
 #include "gram_tc2.cuh"
 #include "sp.cuh"
 #include "spattr.cuh"
+#include "graph_hopper.cuh"
 #include "wl.cuh"
 #include "wl_fused.cuh"
 #include "wl_fused2.cuh"
@@ -294,7 +295,8 @@ int gk_destroy(gk_handle* h) {
                         &h->tail_ent, &h->tail_cur, &h->part_max, &h->part_new, &h->diag_u64, &h->diag_f64, &h->panel,
                         &h->sp_dist, &h->sp_dict_keys, &h->sp_dict_ids, &h->sp_dkeys, &h->sp_graph_off, &h->fattr, &h->tiles,
                         &h->K, &h->K_stage, &h->wlf_buf, &h->row_map, &h->diag_rows, &h->oa_keys, &h->oa_cnt, &h->oa_colcnt, &h->wl_single,
-                        &h->diag_frozen, &h->sp_lists, &h->wl_payload, &h->gram_dyn, &h->tb_cnt, &h->tb_ent, &h->tb_ovf};
+                        &h->diag_frozen, &h->sp_lists, &h->wl_payload, &h->gram_dyn, &h->tb_cnt, &h->tb_ent, &h->tb_ovf,
+                        &h->gh_M, &h->gh_ws, &h->gh_woff, &h->gh_gdiam, &h->gh_groups, &h->gh_pairs};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1541,6 +1543,276 @@ static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_b
   return GK_OK;
 }
 
+}  // extern "C"
+
+// ---- GraphHopper (graph_hopper.cuh)
+// Launch one gh_dag_kernel pass over every graph: graphs whose working set fits `smem_cap` bytes of shared memory
+// run from shared memory, the others from a global workspace.
+template <bool MAPS>
+static int gh_dag_pass(gk_handle* h, const std::vector<int>& gdiam, double* M, long long T) {
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N;
+  const size_t smem_cap = 96 * 1024;
+  std::vector<int> small, big;
+  std::vector<long long> woff(N, 0);
+  size_t smem_max = 16, ws_total = 0;
+  for (int64_t g = 0; g < N; ++g) {
+    const long long n = ex->graph_ptr[g + 1] - ex->graph_ptr[g];
+    const size_t b = gh_ws_bytes(n, MAPS ? gdiam[g] + 1 : 0, MAPS);
+    if (b <= smem_cap) { small.push_back((int)g); smem_max = std::max(smem_max, b); }
+    else { big.push_back((int)g); woff[g] = (long long)ws_total; ws_total += b; }
+  }
+  std::vector<int> order(small);
+  order.insert(order.end(), big.begin(), big.end());
+  GK_TRY(h->sp_lists.ensure((size_t)N * 4 + 16));
+  GK_CUDA(cudaMemcpyAsync(h->sp_lists.p, order.data(), order.size() * 4, cudaMemcpyHostToDevice, h->stream));
+  GhParams p;
+  memset(&p, 0, sizeof(p));
+  p.graph_ptr = h->graph_ptr.as<int>();
+  p.row_ptr = h->row_ptr.as<int>();
+  p.col_idx = h->col_idx.as<int>();
+  p.gdiam = h->gh_gdiam.as<int>();
+  p.delta_max = h->gh_gdiam.as<int>() + N;
+  p.M = M;
+  p.delta = h->gh_delta;
+  p.T = T;
+  if (!big.empty()) {
+    GK_TRY(h->gh_ws.ensure(ws_total));
+    GK_TRY(h->gh_woff.ensure((size_t)N * 8));
+    GK_CUDA(cudaMemcpyAsync(h->gh_woff.p, woff.data(), (size_t)N * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (!small.empty()) {
+    GK_CUDA(cudaFuncSetAttribute(gh_dag_kernel<MAPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    p.glist = h->sp_lists.as<int>();
+    gh_dag_kernel<MAPS><<<(int)small.size(), GH_THREADS, smem_max, h->stream>>>(p);
+    LAUNCH_CHECK(h);
+  }
+  if (!big.empty()) {
+    p.glist = h->sp_lists.as<int>() + small.size();
+    p.ws = h->gh_ws.as<unsigned char>();
+    p.woff = h->gh_woff.as<long long>();
+    p.ws_global = 1;
+    gh_dag_kernel<MAPS><<<(int)big.size(), GH_THREADS, 0, h->stream>>>(p);
+    LAUNCH_CHECK(h);
+  }
+  // host vectors above are sources of async copies
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+extern "C" {
+
+int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_gh_features: no graphs packed");
+  if (!h->attrs.p || h->attr_dim <= 0) return fail(GK_ERR_ARG, "gk_gh_features: node attributes are required");
+  if (node_kernel != GK_GH_LINEAR && node_kernel != GK_GH_GAUSSIAN && node_kernel != GK_GH_BRIDGE)
+    return fail(GK_ERR_ARG, "gk_gh_features: unknown node kernel");
+  if (flags != 0) return fail(GK_ERR_ARG, "gk_gh_features: no flags are defined");
+  if (h->has_weights && !h->unit_weights)
+    return fail(GK_ERR_UNSUPPORTED, "GraphHopper: edge weights other than 1 (the shortest-path DAG is defined for "
+                                    "unweighted graphs only)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t N = h->N, V = h->V;
+  const int d = h->attr_dim;
+  const int64_t launches0 = h->launches;
+  h->features_ready = false; h->feat_serial++;
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  // pass 1: eccentricities -> per-graph diameter and delta = max diameter + 1
+  GK_TRY(h->gh_gdiam.ensure((size_t)(N + 1) * 4));
+  GK_CUDA(cudaMemsetAsync(h->gh_gdiam.p, 0, (size_t)(N + 1) * 4, h->stream));
+  std::vector<int> gdiam(N + 1, 0);
+  GK_TRY(gh_dag_pass<false>(h, gdiam, nullptr, 0));
+  GK_CUDA(cudaMemcpyAsync(gdiam.data(), h->gh_gdiam.p, (size_t)(N + 1) * 4, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  const int delta = std::max(gdiam[N], 1);
+  const long long T = (long long)delta * (delta + 1) / 2;
+  if ((size_t)V * T * 8 > (size_t)64 << 30) return fail(GK_ERR_UNSUPPORTED, "gk_gh_features: node maps above 64 GB");
+  h->gh_delta = delta;
+  GK_TRY(h->gh_M.ensure((size_t)std::max<int64_t>(V, 1) * T * 8));
+  GK_CUDA(cudaMemsetAsync(h->gh_M.p, 0, (size_t)V * T * 8, h->stream));
+  // pass 2: the node maps
+  GK_TRY(gh_dag_pass<true>(h, gdiam, h->gh_M.as<double>(), T));
+  GK_TRY(h->diag_f64.ensure(N * 8));
+  int64_t n_columns = T;
+  if (node_kernel == GK_GH_LINEAR) {
+    // Phi = sum_v vec(M_v) (x) x_v, then the Gram of the SP-attr route (gram_spattr)
+    const int64_t D = T * d;
+    if ((size_t)N * D * 8 > (size_t)64 << 30) return fail(GK_ERR_UNSUPPORTED, "gk_gh_features: feature matrix above 64 GB");
+    GK_TRY(h->fattr.ensure((size_t)N * D * 8));
+    gh_linear_features<<<(int)N, 256, 0, h->stream>>>(h->graph_ptr.as<int>(), h->gh_M.as<double>(), T,
+                                                      h->attrs.as<double>(), d, h->fattr.as<double>());
+    LAUNCH_CHECK(h);
+    h->fattr_dim = D;
+    n_columns = D;
+    DevScalars* sc = h->scalars.as<DevScalars>();
+    GK_TRY(init_scalars(h, 0));
+    rownorm_f64_kernel<<<(int)N, 256, 0, h->stream>>>(h->fattr.as<double>(), D, (int)N, h->diag_f64.as<double>(),
+                                                       &sc->fattr_negative);
+    LAUNCH_CHECK(h);
+    unsigned* h_negative = &h->h_scalars.as<DevScalars>()->fattr_negative;
+    GK_CUDA(cudaMemcpyAsync(h_negative, &sc->fattr_negative, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+    h->fattr_signed = *h_negative != 0;
+  } else {
+    if (node_kernel == GK_GH_GAUSSIAN)
+      gh_nodepair_diag<GH_NK_GAUSSIAN><<<(int)N, 256, 0, h->stream>>>(h->graph_ptr.as<int>(), h->gh_M.as<double>(), T,
+                                                                       h->attrs.as<double>(), d, mu, h->diag_f64.as<double>());
+    else
+      gh_nodepair_diag<GH_NK_BRIDGE><<<(int)N, 256, 0, h->stream>>>(h->graph_ptr.as<int>(), h->gh_M.as<double>(), T,
+                                                                     h->attrs.as<double>(), d, mu, h->diag_f64.as<double>());
+    LAUNCH_CHECK(h);
+    GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  h->gh_node_kernel = node_kernel;
+  h->gh_mu = mu;
+  h->n_columns = n_columns;
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = 4;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
+    stats->n_levels = 1;
+    stats->level_dims[0] = delta;
+    stats->n_columns = n_columns;
+    stats->n_dense_columns = node_kernel == GK_GH_LINEAR ? n_columns : 0;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ev_ms(h->tev[2], h->tev[3]);
+  }
+  return GK_OK;
+}
+
+int gk_gh_node_maps(gk_handle* h, int64_t g, double* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_gh_node_maps: null argument");
+  if (h->feature_kind != 4 || !h->features_ready) return fail(GK_ERR_STATE, "gk_gh_node_maps: run gk_gh_features first");
+  if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_gh_node_maps: bad graph index");
+  HandleExtra* ex = extra_of(h);
+  const int delta = h->gh_delta;
+  const long long T = (long long)delta * (delta + 1) / 2;
+  const long long v0 = ex->graph_ptr[g], n = ex->graph_ptr[g + 1] - v0;
+  std::vector<double> tri((size_t)n * T);
+  GK_CUDA(cudaSetDevice(h->dev));
+  if (n > 0) {
+    GK_CUDA(cudaMemcpyAsync(tri.data(), h->gh_M.as<double>() + v0 * T, (size_t)n * T * 8, cudaMemcpyDeviceToHost, h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  for (long long v = 0; v < n; ++v) {
+    double* o = out + v * delta * delta;
+    const double* r = tri.data() + v * T;
+    long long k = 0;
+    for (int a = 0; a < delta; ++a)
+      for (int b = 0; b < delta; ++b) o[a * delta + b] = b >= a ? r[k++] : 0.0;
+  }
+  return GK_OK;
+}
+
+// Consecutive graphs of [g0, g1) in groups of at most GH_GROUP_NODES vertices and GH_GROUP_GRAPHS graphs (a larger
+// graph is a group alone).  Appends the first graph of every group and the end.
+static void gh_groups(const std::vector<int>& gp, int g0, int g1, std::vector<int>& out) {
+  int g = g0;
+  while (g < g1) {
+    out.push_back(g);
+    int e = g + 1;
+    while (e < g1 && e - g < GH_GROUP_GRAPHS && gp[e + 1] - gp[g] <= GH_GROUP_NODES) ++e;
+    g = e;
+  }
+  out.push_back(g1);
+}
+
+// Gram of the node-pair kernels (gaussian / bridge): gh_nodepair_gram over graph-group pairs, self similarities from
+// gh_nodepair_diag.  fp64, host output, GK_NORMALIZE, n_fit / row ranges as in gram_spattr.
+static int gram_gh_nodepair(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
+                            int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
+  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "GraphHopper Gram is fp64 only");
+  if (flags & GK_OUT_DEVICE) return fail(GK_ERR_UNSUPPORTED, "GraphHopper Gram: device output not supported");
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N;
+  const bool square = n_fit == N;
+  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
+  if (row_end < 0) row_end = k_rows_total;
+  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
+  const int64_t k_rows = row_end - row_begin;
+  if (ld <= 0) ld = k_cols;
+  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
+  const int64_t launches0 = h->launches;
+  GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
+  h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
+  const int a0 = (int)((square ? 0 : n_fit) + row_begin), a1 = (int)((square ? 0 : n_fit) + row_end);
+  // groups: over all graphs (square) or over Y rows and X columns; the same groups whatever the row range, so a
+  // row block reproduces the full matrix's entries bit for bit
+  std::vector<int> rgroups, cgroups;
+  gh_groups(ex->graph_ptr, square ? 0 : (int)n_fit, (int)N, rgroups);
+  gh_groups(ex->graph_ptr, 0, (int)n_fit, cgroups);
+  const int nrg = (int)rgroups.size() - 1, ncg = (int)cgroups.size() - 1;
+  auto touches = [&](int I) { return rgroups[I] < a1 && rgroups[I + 1] > a0; };
+  std::vector<int2> pairs;
+  for (int I = 0; I < nrg; ++I)
+    for (int J = square ? I : 0; J < ncg; ++J)
+      if (touches(I) || (square && touches(J))) pairs.push_back(make_int2(I, J));
+  GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
+  if (k_rows > 0) {
+    GK_TRY(h->gh_groups.ensure((rgroups.size() + cgroups.size()) * 4));
+    GK_TRY(h->gh_pairs.ensure(std::max<size_t>(pairs.size(), 1) * sizeof(int2)));
+    GK_CUDA(cudaMemcpyAsync(h->gh_groups.p, rgroups.data(), rgroups.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    GK_CUDA(cudaMemcpyAsync(h->gh_groups.as<int>() + rgroups.size(), cgroups.data(), cgroups.size() * 4,
+                            cudaMemcpyHostToDevice, h->stream));
+    if (!pairs.empty())
+      GK_CUDA(cudaMemcpyAsync(h->gh_pairs.p, pairs.data(), pairs.size() * sizeof(int2), cudaMemcpyHostToDevice, h->stream));
+    GhGramParams p;
+    memset(&p, 0, sizeof(p));
+    p.graph_ptr = h->graph_ptr.as<int>();
+    p.M = h->gh_M.as<double>();
+    p.T = (long long)h->gh_delta * (h->gh_delta + 1) / 2;
+    p.attrs = h->attrs.as<double>();
+    p.d = h->attr_dim;
+    p.mu = h->gh_mu;
+    p.pairs = h->gh_pairs.as<int2>();
+    p.rgroups = h->gh_groups.as<int>();
+    p.cgroups = h->gh_groups.as<int>() + rgroups.size();
+    p.square = square ? 1 : 0;
+    p.a0 = a0; p.a1 = a1; p.row0 = a0;
+    p.out = h->K.as<double>();
+    p.ld = k_cols;
+    if (!pairs.empty()) {
+      if (h->gh_node_kernel == GK_GH_GAUSSIAN) {
+        GK_CUDA(cudaFuncSetAttribute(gh_nodepair_gram<GH_NK_GAUSSIAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GH_GRAM_SMEM));
+        gh_nodepair_gram<GH_NK_GAUSSIAN><<<(int)pairs.size(), 256, GH_GRAM_SMEM, h->stream>>>(p);
+      } else {
+        GK_CUDA(cudaFuncSetAttribute(gh_nodepair_gram<GH_NK_BRIDGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GH_GRAM_SMEM));
+        gh_nodepair_gram<GH_NK_BRIDGE><<<(int)pairs.size(), 256, GH_GRAM_SMEM, h->stream>>>(p);
+      }
+      LAUNCH_CHECK(h);
+    }
+    if (square) {
+      set_diag_f64<<<cdiv(k_rows, 256), 256, 0, h->stream>>>(a0, a1, 0, (int)n_fit, h->diag_f64.as<double>(), h->K.as<double>(), k_cols);
+      LAUNCH_CHECK(h);
+    }
+    if (flags & GK_NORMALIZE) {
+      normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(k_rows, k_cols, h->K.as<double>(), k_cols,
+                                                                      h->diag_f64.as<double>() + a0,
+                                                                      h->diag_f64.as<double>(), (flags & GK_NAN_TO_NUM) ? 1 : 0);
+      LAUNCH_CHECK(h);
+    }
+  }
+  GK_CUDA(cudaEventRecord(h->tev[7], h->stream));
+  if (K_out && k_rows > 0)
+    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, h->K.p, (size_t)k_cols * 8, (size_t)k_cols * 8, (size_t)k_rows,
+                              cudaMemcpyDeviceToHost, h->stream));
+  if (xdiag) GK_CUDA(cudaMemcpyAsync(xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (ydiag && !square)
+    GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));  // also keeps the host group / pair lists alive for their copies
+  if (stats) {
+    stats->gram_path = 6;
+    stats->gemm_tiles = (int64_t)pairs.size();
+    stats->gemm_launches = h->launches - launches0;
+    stats->ms_gemm = ev_ms(h->tev[6], h->tev[7]);
+  }
+  return GK_OK;
+}
+
 // ---------------------------------------------------------------------------
 }  // extern "C"
 
@@ -1659,6 +1931,14 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with ShortestPathAttr features");
     GK_CUDA(cudaSetDevice(h->dev));
     return gram_spattr(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
+  }
+  if (h->feature_kind == 4) {
+    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with GraphHopper features");
+    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with GraphHopper features");
+    GK_CUDA(cudaSetDevice(h->dev));
+    if (h->gh_node_kernel == GK_GH_LINEAR)
+      return gram_spattr(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
+    return gram_gh_nodepair(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
   }
   const bool square = n_fit == N;
   const int64_t k_rows_total = square ? N : N - n_fit;

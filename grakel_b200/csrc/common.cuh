@@ -161,7 +161,7 @@ struct gk_handle {
   int64_t pro_serial = -1;   // feat_serial for which gk_wl_features already ran the Gram prologue (square case):
                              // self similarities finished, column histogram on the host -- gk_gram then needs no
                              // host synchronisation before its launches
-  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features)
+  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
   // ---- columns / panel / diag
@@ -194,6 +194,12 @@ struct gk_handle {
   gk::DevBuf fattr;
   int64_t fattr_dim = 0;
   bool fattr_signed = false;  // some feature is negative: entries of K may cancel (gram_spattr takes the fp64 Gram)
+
+  // ---- GraphHopper (feature_kind 4): per-vertex maps M [V][delta (delta + 1) / 2] fp64
+  gk::DevBuf gh_M, gh_ws, gh_woff, gh_gdiam, gh_groups, gh_pairs;
+  int gh_delta = 0;
+  int gh_node_kernel = 0;  // GK_GH_LINEAR / GK_GH_GAUSSIAN / GK_GH_BRIDGE
+  double gh_mu = 1.0;
 
   // ---- GEMM
   gk::DevBuf tiles;  // int2 list

@@ -27,7 +27,7 @@ from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
-from .kernels import (EdgeHistogram, ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman,
+from .kernels import (EdgeHistogram, GraphHopper, ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman,
                       WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
@@ -36,7 +36,7 @@ default_n_components = 100
 _OUTSIDE = frozenset((
     "random_walk", "RW", "graphlet_sampling", "GR", "subgraph_matching", "SM", "multiscale_laplacian", "ML",
     "lovasz_theta", "LOVT", "svm_theta", "SVMT", "neighborhood_hash", "NH", "neighborhood_subgraph_pairwise_distance",
-    "NSPD", "odd_sth", "ODD", "propagation", "PR", "pyramid_match", "PM", "graph_hopper", "GH", "hadamard_code", "HC"))
+    "NSPD", "odd_sth", "ODD", "propagation", "PR", "pyramid_match", "PM", "hadamard_code", "HC"))
 
 
 def _shortest_path(params):
@@ -50,6 +50,7 @@ for _names, _framework, _build in (
         (("edge_histogram", "EH"), False, lambda p: (EdgeHistogram, p)),
         (("weisfeiler_lehman_optimal_assignment", "WL-OA"), False, lambda p: (WeisfeilerLehmanOptimalAssignment, p)),
         (("shortest_path", "SP"), False, _shortest_path),
+        (("graph_hopper", "GH"), False, lambda p: (GraphHopper, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),
         (("core_framework", "CORE"), True, lambda p: (CoreFramework, p))):
     for _n in _names:

@@ -13,8 +13,10 @@ the level-0 label dictionary), so fitted estimators pickle like the reference's
 from __future__ import annotations
 
 import copy
+import functools
 import warnings
 from collections.abc import Iterable
+from numbers import Real
 
 import numpy as np
 from sklearn.base import BaseEstimator, TransformerMixin
@@ -872,3 +874,185 @@ class ShortestPathAttr(Kernel):
 
     def _device_features(self, eng):
         return eng.spattr_features(dijkstra_order=bool(getattr(self, "_dijkstra_order", False)))
+
+
+# ------------------------------------------------------------------------------
+# GraphHopper node kernels on (M, attributes[, squared norms]) tuples (graph_hopper.py:295-365).  Module-level
+# functions, so that a fitted estimator pickles; the device computes the same values without these callbacks.
+def gh_linear_kernel(x, y):
+    """sum of <M_v, M_v'> <x_v, x_v'> over node pairs (graph_hopper.py:295-313)."""
+    M_i, NA_i = x[:2]
+    M_j, NA_j = y[:2]
+    return float(np.dot(np.dot(M_i, M_j.T).flat, np.dot(NA_i, NA_j.T).flat))
+
+
+def gh_gaussian_kernel(x, y, mu=1.0):
+    """sum of <M_v, M_v'> exp(-mu ||x_v - x_v'||^2) over node pairs (graph_hopper.py:316-339)."""
+    M_i, NA_i = x[:2]
+    M_j, NA_j = y[:2]
+    sq = np.sum((NA_i[:, None, :] - NA_j[None, :, :]) ** 2, axis=2)
+    return float(np.dot(np.dot(M_i, M_j.T).flat, np.exp(-mu * sq).flat))
+
+
+def gh_bridge_kernel(x, y):
+    """sum of <M_v, M_v'> max(0, (4 - ||x_v - x_v'||) / 4) over node pairs (graph_hopper.py:342-365)."""
+    M_i, NA_i = x[:2]
+    M_j, NA_j = y[:2]
+    dist = np.sqrt(np.sum((NA_i[:, None, :] - NA_j[None, :, :]) ** 2, axis=2))
+    return float(np.dot(np.dot(M_i, M_j.T).flat, np.maximum(0.0, (4.0 - dist) / 4.0).flat))
+
+
+class GraphHopper(Kernel):
+    """GraphHopper kernel (graph_hopper.py:19-449): K(G, G') = sum over vertex pairs of <M_v, M_v'> k(x_v, x_v'),
+    where M_v counts the shortest paths through v by the position of v on the path and the path length.
+
+    `kernel_type` is "linear", "gaussian" (mu = 1), ("gaussian", mu), "bridge" or a callable on the reference's
+    (M reshaped to n x m^2, attributes) tuples.  The node maps are built on the device for every kernel type; the
+    three named node kernels also run their Gram there, a callable is contracted pair by pair on the host.  Only
+    unit edge weights are supported (the shortest-path DAG of the reference is defined for unweighted graphs)."""
+
+    _graph_format = "all"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, kernel_type="linear"):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.kernel_type = kernel_type
+        self._initialized.update({"kernel_type": False})
+
+    def initialize(self):
+        super().initialize()
+        if not self._initialized["kernel_type"]:  # graph_hopper.py:51-85
+            kt = self.kernel_type
+            if type(kt) is str:
+                if kt == "linear":
+                    self.metric_, self.calculate_norm_, self._node_kernel = gh_linear_kernel, False, (_lib.GK_GH_LINEAR, 1.0)
+                elif kt == "gaussian":
+                    self.metric_ = functools.partial(gh_gaussian_kernel, mu=1.0)
+                    self.calculate_norm_, self._node_kernel = True, (_lib.GK_GH_GAUSSIAN, 1.0)
+                elif kt == "bridge":
+                    self.metric_, self.calculate_norm_, self._node_kernel = gh_bridge_kernel, False, (_lib.GK_GH_BRIDGE, 1.0)
+                else:
+                    raise ValueError('Unsupported kernel with name "' + str(kt) + '"')
+            elif type(kt) is tuple and len(kt) == 2 and kt[0] == "gaussian" and isinstance(kt[1], Real):
+                self.metric_ = functools.partial(gh_gaussian_kernel, mu=float(kt[1]))
+                self.calculate_norm_, self._node_kernel = True, (_lib.GK_GH_GAUSSIAN, float(kt[1]))
+            elif callable(kt):
+                self.metric_, self.calculate_norm_, self._node_kernel = kt, False, None
+            else:
+                raise TypeError('Unrecognized "kernel_type": can either be a str from the supported: "linear", '
+                                '"gaussian", "bridge" or tuple ("gaussian", mu) or a callable.')
+            self._initialized["kernel_type"] = True
+
+    # ---- input
+    def _pack(self, X):
+        """Packed block of X: adjacency semantics (entries > 0 are edges, self-loops take no part), node attributes
+        as vectors, the reference's element and attribute errors (graph_hopper.py:106-164)."""
+        if isinstance(X, Block):  # datasets.read_tu(prefer_attr_nodes=True)
+            block = X.require("sp", labels=False)
+            if block.attrs is None:
+                raise ValueError("Graph does not have any labels for vertices.")
+        else:
+            if not isinstance(X, Iterable):
+                raise TypeError("input must be an iterable\n")
+            X = list(X)
+            msg = "each element of X must be either a graph object or a list with at least a graph like object and node, "
+            from .packing import iter_elements
+            for i, (idx, _g, L) in enumerate(iter_elements(X, lambda n: n >= 2, msg)):
+                if not L:
+                    continue  # pack raises the missing-labels error
+                try:
+                    attributes = np.array(list(L.values()))
+                except TypeError:
+                    raise TypeError("All attributes of a single graph should have the same dimension.")
+                if attributes.ndim != 2 or not np.issubdtype(attributes.dtype, np.number):
+                    raise TypeError("GraphHopper needs continuous node attributes: each node label must be a numeric "
+                                    "vector, giving an array of shape (n_nodes, n_features) per graph. Got an array of "
+                                    "shape " + str(attributes.shape) + " with dtype " + str(attributes.dtype) +
+                                    " on the graph at index " + str(i) + ".")
+            block = pack(X, "sp", need_labels=True, len_ok=lambda n: n >= 2, want_weights=True,
+                         fw_zero_is_absent=True, attributes=True, type_error_msg=msg)
+        if block.weights is not None and np.any(np.asarray(block.weights) != 1.0):
+            raise NotImplementedError("GraphHopper: edge weights other than 1 are not supported (the shortest-path "
+                                      "DAG of the kernel is defined for unweighted graphs)")
+        return block
+
+    def parse_input(self, X):
+        block = self._pack(X)
+        if self._node_kernel is None:
+            return self._parse_maps(block)
+        return Fitted(block, None, {})
+
+    def _parse_maps(self, block):
+        """Callable kernel_type: one (M, attributes) tuple per graph, M from the device (gk_gh_node_maps), zero-padded
+        to max(fit delta, this input's delta) like graph_hopper.py:169-172."""
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, None, None, block.attrs)
+            self.stats_ = eng.gh_features(_lib.GK_GH_LINEAR)
+            delta = eng.gh_delta
+            if self._method_calling in (1, 2):
+                self._max_diam = delta
+            width = max(self._max_diam, delta)
+            items, gp = [], block.graph_ptr
+            for g in range(block.n_graphs):
+                n = int(gp[g + 1] - gp[g])
+                M = np.zeros((n, width, width))
+                if n:
+                    M[:, :delta, :delta] = eng.gh_node_maps(g, n)
+                items.append((M, np.array(block.attrs[gp[g]:gp[g + 1]], dtype=float)))
+        return items
+
+    def pairwise_operation(self, x, y):
+        """graph_hopper.py:268-292: both maps truncated to the smaller delta, flattened per vertex."""
+        xp, yp = x[0], y[0]
+        m = min(xp.shape[1], yp.shape[1])
+        xp, yp = xp[:, :m, :m], yp[:, :m, :m]
+        return self.metric_((xp.reshape(xp.shape[0], m * m),) + tuple(x[1:]),
+                            (yp.reshape(yp.shape[0], m * m),) + tuple(y[1:]))
+
+    # ---- estimator protocol
+    def fit(self, X, y=None):
+        super().fit(X)
+        if self._node_kernel is not None and self._method_calling == 1:
+            # delta of the fitted graphs (graph_hopper.py:169-170): one node-map pass on the device
+            with _lib.engine(getattr(self, "device_", None)) as eng:
+                b = self.X.block
+                eng.pack(b.graph_ptr, b.row_ptr, b.col_idx, None, None, b.attrs)
+                self._max_diam = int(eng.gh_features(*self._node_kernel).level_dims[0])
+        return self
+
+    def fit_transform(self, X, y=None):
+        self.initialize()
+        if self._node_kernel is None:
+            return self._pairwise_fit_transform(X)
+        self._method_calling = 2
+        self._is_transformed = False
+        self.X = self.parse_input(X)
+        K, xdiag, _ = self._run(self.X.block, None, n_fit=self.X.block.n_graphs)
+        self._max_diam = int(self.stats_.level_dims[0])
+        self._X_diag = xdiag
+        if self.normalize:
+            self._warn_unnormalizable(xdiag)
+        return K
+
+    def transform(self, X):
+        if self._node_kernel is None:
+            return self._pairwise_transform(X)
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        Y = self.parse_input(X)
+        K, xdiag, ydiag = self._run(Block.concat(self.X.block, Y.block), None, n_fit=self.X.block.n_graphs)
+        self._X_diag = xdiag
+        self._Y_diag = ydiag
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xdiag, ydiag)
+        return K
+
+    def diagonal(self):
+        if self._node_kernel is None:
+            return self._pairwise_diagonal()
+        return super().diagonal()
+
+    def _device_features(self, eng):
+        return eng.gh_features(*self._node_kernel)

@@ -103,7 +103,8 @@ typedef struct gk_stats {
   int64_t max_diag;          /* largest self-similarity */
   int64_t hash_retries;      /* WL: relabel passes repeated after a detected hash collision */
   int64_t gram_path;         /* 1 = wgmma bf16 tensor-core GEMM, 2 = exact int64 CUDA-core Gram, 3 = no contracted columns,
-                                ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram */
+                                ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram,
+                                GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -143,6 +144,23 @@ int gk_wl_sp_features(gk_handle* h, int32_t n_iter, int32_t flags, gk_stats* sta
  * -- so that gk_gram's dot products are the histogram intersections sum_c min(Hs[i,c], Hs[j,c]) of
  * :257-266 / :433-437, the self similarities the row sums of :459-461, exactly (integers). */
 int gk_wl_oa_features(gk_handle* h, int32_t n_iter, gk_stats* stats);
+
+/* GraphHopper (graph_hopper.py:19-449): per-vertex maps M_v (delta x delta, delta = largest diameter + 1 over the
+ * packed block) from the shortest-path DAG of every root, then the node kernel:
+ *   GK_GH_LINEAR    <x, x'>: explicit feature map Phi(G) = sum_v vec(M_v) (x) x_v; gk_gram takes the ShortestPathAttr
+ *                   Gram (gram_path 4 = 3xTF32 for non-negative attributes, 5 = fp64 for attributes of mixed sign)
+ *   GK_GH_GAUSSIAN  exp(-mu ||x - x'||^2)
+ *   GK_GH_BRIDGE    max(0, (4 - ||x - x'||) / 4)
+ *                   both: fused fp64 node-pair Gram (gram_path 6), exactly symmetric and deterministic
+ * Unit edge weights only (GK_ERR_UNSUPPORTED otherwise); node attributes are required; flags must be 0.
+ * stats: level_dims[0] = delta, n_columns = feature dimension (linear) or delta (delta + 1) / 2 (node-pair kernels).
+ * gk_gram: fp64 host output, GK_NORMALIZE, n_fit and row ranges; GK_DIST is GK_ERR_UNSUPPORTED. */
+#define GK_GH_LINEAR 0
+#define GK_GH_GAUSSIAN 1
+#define GK_GH_BRIDGE 2
+int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, gk_stats* stats);
+/* graph g's maps after gk_gh_features: out[n * delta * delta], M[v][a][b] at (v * delta + a) * delta + b */
+int gk_gh_node_maps(gk_handle* h, int64_t g, double* out);
 
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
