@@ -34,6 +34,7 @@ class GkStats(C.Structure):
         ("kernel_launches", C.c_int64),
         ("ms_h2d", C.c_float), ("ms_features", C.c_float), ("ms_panel", C.c_float),
         ("ms_gemm", C.c_float), ("ms_tail", C.c_float), ("ms_d2h", C.c_float), ("ms_total", C.c_float),
+        ("gemm_elem_bytes", C.c_int64),
     ]
 
     def as_dict(self):

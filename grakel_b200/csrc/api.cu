@@ -39,14 +39,29 @@ static inline size_t next_pow2(size_t x) {
 }
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// Cost model of the head/tail split of the Gram: the dense bf16 rate of the GEMM (flop/s; measured on an H100 SXM
-// at a 400 W power limit with every shared column dense: 7.8e14) and the amortised cost of one pair update of K.
+// Cost model of the head/tail split of the Gram: the dense rate of the GEMM per panel type (flop/s; measured on an
+// H100 SXM at a 400 W power limit with every shared column dense: 7.8e14 bf16; 1.51e15 u8, 2.06x the bf16 rate of
+// the same run, tools/bench_u8_gram.py) and the amortised cost of one pair update of K.
 // The update cost is not a single measured figure: below ~32 updates per 32 x 32 block of K they ride in the GEMM
 // epilogue almost for free, beyond it they overflow to global atomics into DRAM.  It is set so that the model's argmin
-// matches a sweep of the forced threshold on the same card (GRAKEL_B200_FORCE_T, config 2, ms per pass:
-// T = 8 / 16 / 32 / 64 / 128 / 256 -> 1.48 / 1.19 / 0.97 / 2.04 / 2.72 / 4.39; the model picks T = 32).
-constexpr double COST_GEMM_RATE = 7.8e14;
+// matches sweeps of the forced threshold on the same card (GRAKEL_B200_FORCE_T, config 2, ms per pass):
+//   bf16 panel: T = 8 / 16 / 32 / 64 / 128 / 256 -> 1.48 / 1.19 / 0.97 / 2.04 / 2.72 / 4.39; the model picks T = 32
+//   u8 panel:   T = 8 / 16 / 32 / 64 / 128 / 256 -> 1.15 / 0.99 / 0.92 / 2.01 / 2.75 / 4.47; the model picks T = 32
+//   (the forced passes zero the whole panel pitch; the model's own T = 32 pass runs in 0.83 ms)
+// Halving the head's cost per column does not move the argmin: the tail's cost jumps by ~0.3 ms from T = 32 to 64
+// (updates overflow the epilogue's lists), far more than the 0.09 ms of u8 MMAs the 1 279 extra head columns cost.
+constexpr double COST_GEMM_RATE_BF16 = 7.8e14;
+constexpr double COST_GEMM_RATE_U8 = 1.5e15;
 constexpr double COST_T_ATOMIC = 6.7e-11;
+
+// Element type of the integer head panel: u8 when every count is <= 255 (u8 x u8 -> s32 wgmma, twice the bf16 rate),
+// else bf16 (exact up to 256).  GRAKEL_B200_U8=0 keeps bf16 everywhere (A/B switch).
+static bool u8_panel_enabled() {
+  const char* e = getenv("GRAKEL_B200_U8");
+  return !(e && atoi(e) == 0);
+}
+static inline int panel_bk(int elem_bytes) { return elem_bytes == 1 ? BK_U8 : BK; }  // elements per 128-byte k-block
+static inline double panel_rate(int elem_bytes) { return elem_bytes == 1 ? COST_GEMM_RATE_U8 : COST_GEMM_RATE_BF16; }
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -64,14 +79,16 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-static int make_panel_map(CUtensorMap* m, void* base, long long cols, long long rows, int box_rows) {
+// integer head panel, `elem_bytes` 1 (u8) or 2 (bf16): one 128-byte swizzle row per k-block
+static int make_panel_map(CUtensorMap* m, void* base, long long cols, long long rows, int box_rows, int elem_bytes) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return fail(GK_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
+  cuuint64_t strides[1] = {(cuuint64_t)cols * elem_bytes};
+  cuuint32_t box[2] = {(cuuint32_t)panel_bk(elem_bytes), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims, strides, box, estr,
+  CUresult r = enc(m, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, dims,
+                   strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(GK_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
@@ -141,7 +158,10 @@ struct HandleExtra {
   // GEMM tile list on the device (h->tiles): rebuilt and uploaded only when its key changes
   long long tiles_key[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
   long long tiles_n = 0;
-  long long head_dc_pad = 0;  // panel width of the last pass whose threshold came from the cost model (not GK_DENSE_ALL / FORCE_T)
+  long long head_row_bytes = 0;  // panel row width (bytes) of the last pass whose threshold came from the cost model
+                                 // (not GK_DENSE_ALL / FORCE_T)
+  long long last_max_count = 0;  // largest count of the last Gram on this handle: an asynchronous pass fills a u8 panel
+                                 // unless it was 256 (a count of 256 repeats through the synchronous route once)
 };
 static std::vector<std::pair<gk_handle*, HandleExtra*>> g_extra;
 static HandleExtra* extra_of(gk_handle* h) {
@@ -199,7 +219,12 @@ int gk_create(int device_ordinal, gk_handle** out) {
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  GK_CUDA(cudaFuncSetAttribute(gram_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM2_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<float, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<float, true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(gram_tc2_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM2_SMEM));
+  GK_CUDA(cudaFuncSetAttribute(gram_tc2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
@@ -1848,8 +1873,9 @@ static int deliver_square(gk_handle* h, const float* d_k, long long d_ld, int64_
 
 template <typename OutT, bool NORM>
 static void launch_tc(gk_handle* h, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-                      const GramParams& p, int grid) {
-  gram_tc_kernel<OutT, NORM><<<grid, GEMM_THREADS, GEMM_SMEM, h->stream>>>(tmA, tmB, tmC, p);
+                      const GramParams& p, int grid, int elem_bytes) {
+  if (elem_bytes == 1) gram_tc_kernel<OutT, NORM, 2><<<grid, GEMM_THREADS, GEMM_SMEM, h->stream>>>(tmA, tmB, tmC, p);
+  else gram_tc_kernel<OutT, NORM, 0><<<grid, GEMM_THREADS, GEMM_SMEM, h->stream>>>(tmA, tmB, tmC, p);
 }
 template <typename OutT, bool NORM>
 static void launch_simt(gk_handle* h, const unsigned* panel, long long ldp, int kdim, int a0, int a1, int b0, int b1,
@@ -2018,10 +2044,14 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   // ---- choose the Gram path and the head/tail threshold (host side, from the histogram)
   int path = 1;
   if ((flags & GK_GRAM_SIMT) || max_count > 256 || max_diag >= (1LL << 24)) { path = 2; force_T = 1; }
+  // panel element bytes of the tensor-core GEMM: u8 when every count fits, bf16 for a count of 256
+  const int elem_bytes = (u8_panel_enabled() && max_count <= 255) ? 1 : 2;
+  const int bk = panel_bk(elem_bytes);
+  hx->last_max_count = max_count;
   int T = 1;
   {
-    // T = 2^k minimising  head_cols * flops_per_col / rate + tail_updates * t_atomic  (COST_GEMM_RATE, COST_T_ATOMIC)
-    const double rate = COST_GEMM_RATE;
+    // T = 2^k minimising  head_cols * flops_per_col / rate + tail_updates * t_atomic  (COST_GEMM_RATE_*, COST_T_ATOMIC)
+    const double rate = panel_rate(elem_bytes);
     const double t_atomic = COST_T_ATOMIC;
     double best = -1.0;
     for (int k = 0; k <= HIST_BUCKETS - 2; ++k) {
@@ -2067,8 +2097,8 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   LAUNCH_CHECK(h);
   if (path == 1 && Dc == 0) path = 3;
   h->Dc = Dc;
-  h->Dc_pad = (Dc + BK - 1) / BK * BK;
-  if (force_T < 0 && path == 1 && square) hx->head_dc_pad = h->Dc_pad;
+  h->Dc_pad = (Dc + bk - 1) / bk * bk;
+  if (force_T < 0 && path == 1 && square) hx->head_row_bytes = h->Dc_pad * elem_bytes;
 
   // ---- transport type.  Tensor-core results are integers < 2^24 (checked above), i.e. exact in fp32: a float64
   // HOST result is produced and moved as fp32 (half the HBM writes; a quarter of the PCIe bytes for the
@@ -2158,14 +2188,20 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     // (always at least a stub: gk_wl_gram's asynchronous pass sizes its tail by the capacity left here)
     GK_TRY(h->tail_ent.ensure((size_t)std::max<int64_t>(has_tail ? n_tail_ent : 0, 64) * sizeof(int2)));
     if (path == 1 || path == 3) {
-      const size_t panel_bytes = (size_t)N * std::max<int64_t>(h->Dc_pad, BK) * 2;
+      const size_t panel_bytes = (size_t)N * std::max<int64_t>(h->Dc_pad, bk) * elem_bytes;
       GK_TRY(h->panel.ensure(panel_bytes));
       if (Dc) GK_CUDA(cudaMemsetAsync(h->panel.p, 0, panel_bytes, h->stream));
       if (Dc || has_tail) {
-        feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
-            h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), d_row_map,
-            h->panel.as<__nv_bfloat16>(), h->Dc_pad, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(),
-            h->tail_ent.as<int2>());
+        if (elem_bytes == 1)
+          feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
+              h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), d_row_map,
+              h->panel.as<uint8_t>(), h->Dc_pad, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(),
+              h->tail_ent.as<int2>());
+        else
+          feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
+              h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), d_row_map,
+              h->panel.as<__nv_bfloat16>(), h->Dc_pad, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(),
+              h->tail_ent.as<int2>());
         LAUNCH_CHECK(h);
       }
     }
@@ -2194,8 +2230,8 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
       CUtensorMap tmA, tmB, tmC;
       PeerMaps peer_maps;
       memset(&peer_maps, 0, sizeof(peer_maps));
-      GK_TRY(make_panel_map(&tmA, h->panel.p, h->Dc_pad, N, BM));
-      GK_TRY(make_panel_map(&tmB, h->panel.p, h->Dc_pad, N, BN));
+      GK_TRY(make_panel_map(&tmA, h->panel.p, h->Dc_pad, N, BM, elem_bytes));
+      GK_TRY(make_panel_map(&tmB, h->panel.p, h->Dc_pad, N, BN, elem_bytes));
       memset(&tmC, 0, sizeof(tmC));
       p.tma_store = 0;
       if (dev_dtype == GK_F32 && !norm_in_epilogue && ((uintptr_t)d_out) % 16 == 0 && (d_ld * 4) % 16 == 0 &&
@@ -2219,7 +2255,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
       }
       p.tiles = h->tiles.as<int2>();
       p.n_tiles = (int)n_tiles;
-      p.num_k_blocks = (int)(h->Dc_pad / BK);
+      p.num_k_blocks = (int)(h->Dc_pad / bk);
       const int grid = cta2 ? 2 * (int)std::min<int64_t>(n_tiles, h->sm_count / 2) : (int)std::min<int64_t>(n_tiles, h->sm_count);
       const bool prof = !cta2 && getenv("GRAKEL_B200_PROF") != nullptr;
       if (prof) {
@@ -2229,9 +2265,10 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
       }
       GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
       if (n_tiles == 0) { /* a trailing rank without rows */ }
-      else if (cta2) gram_tc2_kernel<<<grid, GEMM_THREADS, GEMM2_SMEM, h->stream>>>(tmA, tmC, p, peer_maps);
-      else if (dev_dtype == GK_F64) { if (norm_in_epilogue) launch_tc<double, true>(h, tmA, tmB, tmC, p, grid); else launch_tc<double, false>(h, tmA, tmB, tmC, p, grid); }
-      else { if (norm_in_epilogue) launch_tc<float, true>(h, tmA, tmB, tmC, p, grid); else launch_tc<float, false>(h, tmA, tmB, tmC, p, grid); }
+      else if (cta2 && elem_bytes == 1) gram_tc2_kernel<2><<<grid, GEMM_THREADS, GEMM2_SMEM, h->stream>>>(tmA, tmC, p, peer_maps);
+      else if (cta2) gram_tc2_kernel<0><<<grid, GEMM_THREADS, GEMM2_SMEM, h->stream>>>(tmA, tmC, p, peer_maps);
+      else if (dev_dtype == GK_F64) { if (norm_in_epilogue) launch_tc<double, true>(h, tmA, tmB, tmC, p, grid, elem_bytes); else launch_tc<double, false>(h, tmA, tmB, tmC, p, grid, elem_bytes); }
+      else { if (norm_in_epilogue) launch_tc<float, true>(h, tmA, tmB, tmC, p, grid, elem_bytes); else launch_tc<float, false>(h, tmA, tmB, tmC, p, grid, elem_bytes); }
       LAUNCH_CHECK(h);
       if (prof) {
         std::vector<long long> pr((size_t)grid * 8);
@@ -2338,6 +2375,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     stats->max_count = max_count;
     stats->max_diag = max_diag;
     stats->gram_path = path;
+    stats->gemm_elem_bytes = path == 1 && k_rows > 0 ? elem_bytes : 0;
     stats->gemm_tiles = n_tiles;
     stats->gemm_launches = launches_gram;
     stats->ms_panel = ev_ms(h->tev[4], h->tev[6]);
@@ -2479,15 +2517,21 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   if (dev_out && !K_out) return GK_OK;
   if (ld > 0 && ld < N) return GK_OK;  // (the synchronous route reports the error)
   if (dev_out && (((uintptr_t)K_out) % 16 != 0 || ((ld > 0 ? ld : N) * 4) % 16 != 0)) return GK_OK;
-  // capacities left by earlier passes
-  int64_t S = (int64_t)(h->panel.cap / ((size_t)N * 2)) / BK * BK;
+  // panel type: u8 unless the switch is off or the last Gram on this handle saw a count of 256 (the device checks the
+  // counts of THIS pass against the type and sends it to the synchronous route if one does not fit)
+  const int elem_bytes = (u8_panel_enabled() && extra_of(h)->last_max_count <= 255) ? 1 : 2;
+  const int bk = panel_bk(elem_bytes);
+  // capacities left by earlier passes, reasoned in bytes (passes of either panel type share the buffer): row pitch
+  // S_bytes, a whole number of 128-byte k-blocks
+  int64_t S_bytes = (int64_t)(h->panel.cap / (size_t)N) / 128 * 128;
   {  // no wider than the last cost-model pass needed, plus a quarter (a dense-all pass may have left a much larger buffer,
      // and the whole pitch is zeroed)
-    const long long want = extra_of(h)->head_dc_pad;
+    const long long want = extra_of(h)->head_row_bytes;
     if (!(flags & GK_DENSE_ALL) && !getenv("GRAKEL_B200_FORCE_T") && want > 0)
-      S = std::min<int64_t>(S, (want + want / 4 + BK - 1) / BK * BK + BK);
+      S_bytes = std::min<int64_t>(S_bytes, (want + want / 4 + 127) / 128 * 128 + 128);
   }
-  if (S < BK || !h->tail_desc.p || !h->tail_cur.p || !h->tail_ent.p) return GK_OK;
+  const int64_t S = S_bytes / elem_bytes;  // row pitch in elements
+  if (S_bytes < 128 || !h->tail_desc.p || !h->tail_cur.p || !h->tail_ent.p) return GK_OK;
   const long long cap_tail_cols = (long long)std::min(h->tail_desc.cap / sizeof(int2), h->tail_cur.cap / 4);
   const long long cap_tail_ent = (long long)(h->tail_ent.cap / sizeof(int2));
   GK_CUDA(cudaSetDevice(h->dev));
@@ -2521,7 +2565,7 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   // owns every register file: nothing can share an SM with it)
   GK_CUDA(cudaEventRecord(h->ev_fork, h->stream));
   GK_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
-  panel_zero_rows<<<h->sm_count * 4, 256, 0, h->stream2>>>(h->panel.as<__nv_bfloat16>(), N, S, (int)(S / 8));
+  panel_zero_rows<<<h->sm_count * 4, 256, 0, h->stream2>>>(h->panel.as<unsigned char>(), N, S_bytes, (int)(S_bytes / 16));
   LAUNCH_CHECK(h);
   GK_CUDA(cudaEventRecord(h->ev_stage[0], h->stream2));
 
@@ -2559,7 +2603,7 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   CUtensorMap tmA, tmC;
   PeerMaps peer_maps;
   memset(&peer_maps, 0, sizeof(peer_maps));
-  GK_TRY(make_panel_map(&tmA, h->panel.p, S, N, BM));
+  GK_TRY(make_panel_map(&tmA, h->panel.p, S, N, BM, elem_bytes));
   GK_TRY(make_out_map(&tmC, d_out, N, N, d_ld));
   int force_T = (flags & GK_DENSE_ALL) ? 1 : -1;
   if (force_T < 0) {
@@ -2577,8 +2621,9 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
     q.diag = h->diag_u64.as<unsigned long long>(); q.diag_f64 = h->diag_f64.as<double>();
     q.n_part = (int)h->n_part; q.part_max = h->part_max.as<unsigned>(); q.part_new = h->part_new.as<unsigned>();
     q.cs = cs; q.sc = sc; q.dyn = dyn;
-    q.flops_per_col = (double)N * (double)(N + 1); q.rate = COST_GEMM_RATE; q.t_atomic = COST_T_ATOMIC;
-    q.force_T = force_T; q.stride_cap = (int)S; q.bk = BK;
+    q.flops_per_col = (double)N * (double)(N + 1); q.rate = panel_rate(elem_bytes); q.t_atomic = COST_T_ATOMIC;
+    q.force_T = force_T; q.stride_cap = (int)S; q.bk = bk;
+    q.max_panel_count = elem_bytes == 1 ? 255u : 256u;
     q.cap_tail_cols = cap_tail_cols; q.cap_tail_ent = cap_tail_ent;
     col_stats_fused<<<h->sm_count * 4, 256, 0, h->stream>>>(q);
     LAUNCH_CHECK(h);
@@ -2593,9 +2638,14 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
                                            h->tail_desc.as<int2>(), h->tail_cur.as<unsigned>(), col_counters, dyn);
   LAUNCH_CHECK(h);
   GK_CUDA(cudaStreamWaitEvent(h->stream, h->ev_stage[0], 0));  // the zeroed panel
-  feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
-      h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), nullptr,
-      h->panel.as<__nv_bfloat16>(), S, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(), h->tail_ent.as<int2>());
+  if (elem_bytes == 1)
+    feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
+        h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), nullptr,
+        h->panel.as<uint8_t>(), S, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(), h->tail_ent.as<int2>());
+  else
+    feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
+        h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), nullptr,
+        h->panel.as<__nv_bfloat16>(), S, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(), h->tail_ent.as<int2>());
   LAUNCH_CHECK(h);
   // ---- tail: bucketed by 32 x 32 block of K for the GEMM epilogue (GRAKEL_B200_TAIL_FUSED=0: the separate tail_pairs kernel)
   const char* e_tf = getenv("GRAKEL_B200_TAIL_FUSED");
@@ -2640,7 +2690,8 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   if (tail_fused) { p.tb_cnt = d_tb_cnt_all; p.tb_ent = h->tb_ent.as<unsigned>(); p.tb_nb32 = nb32; p.tb_cap = tb_cap; p.tb_sym = tb_sym; }
   const int grid = 2 * (int)std::min<int64_t>(n_tiles, h->sm_count / 2);
   GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
-  gram_tc2_kernel<<<grid, GEMM_THREADS, GEMM2_SMEM, h->stream>>>(tmA, tmC, p, peer_maps);
+  if (elem_bytes == 1) gram_tc2_kernel<2><<<grid, GEMM_THREADS, GEMM2_SMEM, h->stream>>>(tmA, tmC, p, peer_maps);
+  else gram_tc2_kernel<0><<<grid, GEMM_THREADS, GEMM2_SMEM, h->stream>>>(tmA, tmC, p, peer_maps);
   LAUNCH_CHECK(h);
   GK_CUDA(cudaEventRecord(h->tev[7], h->stream));
   if (tail_fused)
@@ -2672,7 +2723,8 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   h->features_ready = true; h->feat_serial++;
   h->feature_kind = 1;
   h->Dc = hd.Dc; h->Dc_pad = hd.Dc_pad;
-  if (force_T < 0) hx->head_dc_pad = hd.Dc_pad;
+  if (force_T < 0) hx->head_row_bytes = (long long)hd.Dc_pad * elem_bytes;
+  hx->last_max_count = (long long)hd.max_count;
   hx->pro_hist = hd.hist;
   hx->pro_max_count = (long long)hd.max_count; hx->pro_max_diag = (long long)hd.max_diag; hx->pro_n_entries = (long long)hd.n_entries;
   h->pro_serial = h->feat_serial;
@@ -2693,6 +2745,7 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
     stats->max_count = (int64_t)hd.max_count;
     stats->max_diag = (int64_t)hd.max_diag;
     stats->gram_path = 1;
+    stats->gemm_elem_bytes = elem_bytes;
     stats->gemm_tiles = n_tiles;
     stats->gemm_launches = 0;
     stats->ms_panel = ev_ms(h->tev[4], h->tev[6]);
@@ -2766,24 +2819,30 @@ int gk_sp_fit_transform(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr
 int gk_selftest_gram(gk_handle* h, int64_t n, int64_t d, const uint16_t* counts, double* out_tc, double* out_simt) {
   if (!h || !counts || n <= 0 || d <= 0) return fail(GK_ERR_ARG, "gk_selftest_gram: bad arguments");
   GK_CUDA(cudaSetDevice(h->dev));
-  const int64_t dpad = (d + BK - 1) / BK * BK;
-  std::vector<__nv_bfloat16> pb((size_t)n * dpad, __float2bfloat16(0.f));
+  // the panel type gk_gram would choose: u8 when every count is <= 255 (and the switch is on), else bf16
+  unsigned max_c = 0;
+  for (int64_t i = 0; i < n * d; ++i) max_c = std::max<unsigned>(max_c, counts[i]);
+  const int elem_bytes = (u8_panel_enabled() && max_c <= 255) ? 1 : 2;
+  const int bk = panel_bk(elem_bytes);
+  const int64_t dpad = (d + bk - 1) / bk * bk;
+  std::vector<uint8_t> pb((size_t)n * dpad * elem_bytes, 0);
   std::vector<unsigned> pu((size_t)n * d, 0u);
   std::vector<double> dg(n, 0.0);
   for (int64_t i = 0; i < n; ++i)
     for (int64_t j = 0; j < d; ++j) {
       const unsigned c = counts[i * d + j];
-      pb[i * dpad + j] = __float2bfloat16((float)c);
+      if (elem_bytes == 1) pb[i * dpad + j] = (uint8_t)c;
+      else reinterpret_cast<__nv_bfloat16*>(pb.data())[i * dpad + j] = __float2bfloat16((float)c);
       pu[i * d + j] = c;
       dg[i] += (double)c * c;
     }
   gk::DevBuf dpb, dpu, ddg, dk1, dk2, dtl;
-  GK_TRY(dpb.ensure(pb.size() * 2));
+  GK_TRY(dpb.ensure(pb.size()));
   GK_TRY(dpu.ensure(pu.size() * 4));
   GK_TRY(ddg.ensure(n * 8));
   GK_TRY(dk1.ensure((size_t)n * n * 8));
   GK_TRY(dk2.ensure((size_t)n * n * 8));
-  GK_CUDA(cudaMemcpyAsync(dpb.p, pb.data(), pb.size() * 2, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(dpb.p, pb.data(), pb.size(), cudaMemcpyHostToDevice, h->stream));
   GK_CUDA(cudaMemcpyAsync(dpu.p, pu.data(), pu.size() * 4, cudaMemcpyHostToDevice, h->stream));
   GK_CUDA(cudaMemcpyAsync(ddg.p, dg.data(), n * 8, cudaMemcpyHostToDevice, h->stream));
   GK_CUDA(cudaMemsetAsync(dk1.p, 0xFF, (size_t)n * n * 8, h->stream));  // NaN pattern: unwritten entries show up
@@ -2802,14 +2861,14 @@ int gk_selftest_gram(gk_handle* h, int64_t n, int64_t d, const uint16_t* counts,
     GK_CUDA(cudaMemcpyAsync(dtl.p, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice, h->stream));
     CUtensorMap tmA, tmB, tmC;
     memset(&tmC, 0, sizeof(tmC));
-    GK_TRY(make_panel_map(&tmA, dpb.p, dpad, n, BM));
-    GK_TRY(make_panel_map(&tmB, dpb.p, dpad, n, BN));
+    GK_TRY(make_panel_map(&tmA, dpb.p, dpad, n, BM, elem_bytes));
+    GK_TRY(make_panel_map(&tmB, dpb.p, dpad, n, BN, elem_bytes));
     p.tiles = dtl.as<int2>();
     p.n_tiles = (int)tiles.size();
-    p.num_k_blocks = (int)(dpad / BK);
+    p.num_k_blocks = (int)(dpad / bk);
     p.out = dk1.p;
     p.mirror = 1;
-    launch_tc<double, false>(h, tmA, tmB, tmC, p, (int)std::min<size_t>(tiles.size(), h->sm_count));
+    launch_tc<double, false>(h, tmA, tmB, tmC, p, (int)std::min<size_t>(tiles.size(), h->sm_count), elem_bytes);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
     if (e != cudaSuccess) rc = fail(GK_ERR_CUDA, std::string("selftest tensor-core kernel: ") + cudaGetErrorString(e));

@@ -43,9 +43,10 @@ struct ColStats {           // device-side, zeroed per gk_gram
 struct GramDyn {
   int T;             // head/tail threshold
   int Dc, Dc_pad;    // head columns, padded to the k-block
-  int num_k_blocks;  // Dc_pad / BK, or 1 when bad (the GEMM still runs, its result is discarded)
+  int num_k_blocks;  // Dc_pad / (elements per k-block), or 1 when bad (the GEMM still runs, its result is discarded)
   int n_tail_cols, n_tail_ent;
-  int bad;           // 1: counts / self similarities beyond the exact bf16 x fp32 range, 2: no head column,
+  int bad;           // 1: a count the pass's panel type cannot hold (> 255 for u8, > 256 for bf16) or a self similarity
+                     //    >= 2^24 (beyond exact fp32 output), 2: no head column,
                      // 4: panel stride too small, 8: tail buffers too small, 16: WL hash collision, 32: table overflow
   unsigned ticket;   // blocks of col_stats_fused that have finished (reset by the last one)
   unsigned long long tail_work;
@@ -164,8 +165,9 @@ struct ColFusedParams {
   const unsigned long long* diag; double* diag_f64;
   int n_part; const unsigned* part_max; const unsigned* part_new;
   ColStats* cs; DevScalars* sc; GramDyn* dyn;
-  double flops_per_col, rate, t_atomic;
-  int force_T, stride_cap, bk;
+  double flops_per_col, rate, t_atomic;  // rate: dense GEMM rate of the pass's panel type
+  int force_T, stride_cap, bk;           // stride_cap: panel row pitch; bk: elements per k-block (both of that type)
+  unsigned max_panel_count;              // largest count the panel type holds exactly (255 u8, 256 bf16)
   long long cap_tail_cols, cap_tail_ent;
 };
 __global__ void __launch_bounds__(256)
@@ -260,7 +262,7 @@ col_stats_fused(ColFusedParams q) {
     const long long Dc_pad = (Dc + q.bk - 1) / q.bk * q.bk;
     const unsigned long long max_count = sc->max_count, max_diag = sc->max_diag;
     int bad = 0;
-    if (max_count > 256ULL || max_diag >= (1ULL << 24)) bad |= 1;
+    if (max_count > (unsigned long long)q.max_panel_count || max_diag >= (1ULL << 24)) bad |= 1;
     if (Dc == 0) bad |= 2;
     if (Dc_pad > q.stride_cap) bad |= 4;
     if (n_tail_cols > q.cap_tail_cols || n_tail_ent > q.cap_tail_ent) bad |= 8;
@@ -283,14 +285,14 @@ col_stats_fused(ColFusedParams q) {
   }
 }
 
-// zero the panel: `w16` 16-byte units of every row (row pitch `ld` elements); one warp per row, grid-stride
+// zero the panel: `w16` 16-byte units of every row (row pitch `ld_bytes`); one warp per row, grid-stride
 __global__ void __launch_bounds__(256)
-panel_zero_rows(__nv_bfloat16* __restrict__ panel, long long n_rows, long long ld, int w16) {
+panel_zero_rows(unsigned char* __restrict__ panel, long long n_rows, long long ld_bytes, int w16) {
   const int lane = threadIdx.x & 31;
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const uint4 z = make_uint4(0u, 0u, 0u, 0u);
   for (long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_rows; r += n_warps) {
-    uint4* row = reinterpret_cast<uint4*>(panel + r * ld);
+    uint4* row = reinterpret_cast<uint4*>(panel + r * ld_bytes);
     for (int c = lane; c < w16; c += 32) row[c] = z;
   }
 }
@@ -357,10 +359,12 @@ col_classify(long long D, int square, int n_fit, const unsigned* __restrict__ co
   }
 }
 
-// pass 2 over the table: head entries -> zeroed bf16 panel, tail entries -> per-column lists
+// pass 2 over the table: head entries -> zeroed panel (u8 or bf16: PanelT, the host chose a type that holds every
+// count exactly), tail entries -> per-column lists
+template <typename PanelT>
 __global__ void __launch_bounds__(256)
 feat_scatter(size_t cap, const unsigned long long* __restrict__ keys, const unsigned* __restrict__ cnt,
-             const int* __restrict__ colslot, const int* __restrict__ row_map, __nv_bfloat16* __restrict__ panel,
+             const int* __restrict__ colslot, const int* __restrict__ row_map, PanelT* __restrict__ panel,
              long long ld, unsigned* __restrict__ tail_cur, const int2* __restrict__ tail_desc,
              int2* __restrict__ tail_ent) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (size_t)gridDim.x * blockDim.x) {
@@ -371,7 +375,8 @@ feat_scatter(size_t cap, const unsigned long long* __restrict__ keys, const unsi
     if (slot == -1) continue;
     const int g = row_map ? row_map[(int)(k >> 32)] : (int)(k >> 32);
     if (slot >= 0) {
-      panel[(long long)g * ld + slot] = __float2bfloat16_rn((float)cnt[i]);
+      if constexpr (sizeof(PanelT) == 1) panel[(long long)g * ld + slot] = (PanelT)cnt[i];
+      else panel[(long long)g * ld + slot] = __float2bfloat16_rn((float)cnt[i]);
     } else {
       const int t = -(slot + 2);
       const unsigned pos = atomicAdd(&tail_cur[t], 1u);
@@ -430,8 +435,8 @@ tail_pairs(long long n_tail_cols, const int2* __restrict__ tail_desc, const int2
 }
 
 // Tail fused into the GEMM epilogue (gram_tc.cuh, GramParams::tb_cnt): the ordered pairs of every tail column, bucketed by
-// 32 x 32 block of K.  Entry = row | col << 5 | value << 10 in ONE word (counts are at most 256 on this path, so a product
-// has 17 bits); a block's TB_CAP entries are one 128-byte line, the rest go to the overflow list {row, col, value} that
+// 32 x 32 block of K.  Entry = row | col << 5 | value << 10 in ONE word (counts are at most 255 on this path -- the
+// asynchronous pass fills a u8 panel, or at most 256 when it fills a bf16 one -- so a product has at most 17 bits); a block's TB_CAP entries are one 128-byte line, the rest go to the overflow list {row, col, value} that
 // tail_overflow_apply adds with global atomics after the GEMM.  Several columns may update the same element: the
 // epilogue adds entries one by one (exact integer sums in fp32).  The host clears counters AND entry lines first: a
 // fully written line is allocated in L2 without a fetch, so the 1.5 M scattered 4-byte stores below hit there instead of

@@ -1,22 +1,25 @@
-// Gram matrix K = A * B^T over the dense bf16 feature panel on Hopper's tensor cores
-// (wgmma.mma_async, fp32 accumulators in registers, operands staged by TMA with the
+// Gram matrix K = A * B^T over the dense integer feature panel on Hopper's tensor cores
+// (wgmma.mma_async, accumulators in registers, operands staged by TMA with the
 // 128-byte swizzle).  Replaces `self.X.dot(self.X.T)` / `Y[:, :D].dot(self.X.T)`
 // (vertex_histogram.py:177-179), the per-level `np.sum` (weisfeiler_lehman.py:270)
 // and `np.dot(phi_x, phi_x.T)` (shortest_path.py:404) of the reference.
 //
-// Exactness: panel entries are integer counts <= 256 (exact in bf16), products and
-// partial sums are integers < 2^24 (exact in fp32) -- the host checks both bounds
-// before choosing this path -- so the result is bit-identical to the reference's
-// float64 arithmetic.
+// Operand types (KIND): the panel holds integer counts, as u8 when every count is <= 255
+// (KIND 2: u8 x u8 -> s32, exact integer accumulation, twice the bf16 MMA rate) and as
+// bf16 when a count is 256 (KIND 0: bf16 x bf16 -> f32; products and partial sums are
+// integers < 2^24, exact in fp32).  Either way the host checks that every self similarity
+// -- and hence every entry of K -- is below 2^24 before choosing this path, so the fp32
+// result is exact and bit-identical to the reference's float64 arithmetic.  KIND 1 (tf32)
+// serves the split-precision real-valued Gram of ShortestPathAttr.
 //
 // Kernel shape (one persistent CTA per SM, 384 threads = three warpgroups):
 //   warpgroup 0     TMA producer (one elected thread); runs ahead into the next tile
 //                   while the consumers drain their accumulators
-//   warpgroups 1-2  wgmma m64n256 over 64 rows each of the 128 x 256 tile (bf16 -> f32),
+//   warpgroups 1-2  wgmma m64n256 over 64 rows each of the 128 x 256 tile,
 //                   then the epilogue of those rows (diagonal fix / normalise -> global,
 //                   plus the mirrored tile for the symmetric case)
-// smem: 4 stages x (A 128x64 + B 256x64 bf16) = 192 KiB, mbarrier ring, 32 KiB of
-// epilogue staging (two 32x32 fp32 tiles per pair of warps).
+// smem: 4 stages x (A 128 + B 256 rows of one 128-byte k-block: 64 bf16 or 128 u8) = 192 KiB,
+// mbarrier ring, 32 KiB of epilogue staging (two 32x32 fp32 tiles per pair of warps).
 #pragma once
 #include "common.cuh"
 
@@ -28,6 +31,7 @@ constexpr int A_BYTES = BM * BK * 2;
 constexpr int B_BYTES = BN * BK * 2;
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int BK_TF32 = 32;  // tf32 operands: 32 elements per 128-byte k-block
+constexpr int BK_U8 = 128;   // u8 operands: 128 elements per 128-byte k-block
 constexpr int GEMM_THREADS = 384;
 // epilogue staging for TMA stores: per pair of consumer warps (one 32-row block) two 32x32 fp32 tiles
 constexpr int EPI_BUF_BYTES = 32 * 32 * 4;
@@ -38,7 +42,7 @@ static_assert(GEMM_SMEM <= 232448, "shared memory budget of one CTA");
 struct GramParams {
   const int2* tiles;   // {first A row, first B row} in panel-row (graph) coordinates
   int n_tiles;
-  int num_k_blocks;    // Dc_pad / 64
+  int num_k_blocks;    // Dc_pad / (elements per 128-byte k-block)
   int a_row_end;       // rows >= a_row_end are not stored
   int b_row_end;
   int c_row0, c_col0;  // K[row - c_row0][col - c_col0]
@@ -151,8 +155,8 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
 // barrier of the two warps that stage one 32-row block (ids 1..4; 0 is __syncthreads)
 __device__ __forceinline__ void pair_sync(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
 
-// K-major, 128-byte-swizzled shared-memory matrix descriptor of wgmma (one 64-element bf16
-// row = 128 B; 8-row groups 1024 B apart).  Bit layout: cute::GMMA::GmmaDescriptor.
+// K-major, 128-byte-swizzled shared-memory matrix descriptor of wgmma (one 128-byte row = 64 bf16,
+// 128 u8 or 32 tf32 elements; 8-row groups 1024 B apart).  Bit layout: cute::GMMA::GmmaDescriptor.
 __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);  // start address   [0,14)
@@ -166,16 +170,28 @@ __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.alig
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// accumulator element of each operand kind: s32 for u8 x u8, fp32 otherwise
+template <int KIND> struct AccOf { using type = float; };
+template <> struct AccOf<2> { using type = int; };
+
 // keeps the compiler from moving accumulator accesses across wgmma fences and waits
 __device__ __forceinline__ void acc_fence(float (&d)[128]) {
 #pragma unroll
   for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void acc_fence(int (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
 #define GK_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
                  "+f"(d[i + 6]), "+f"(d[i + 7])
 #define GK_F128 GK_F8(0), GK_F8(8), GK_F8(16), GK_F8(24), GK_F8(32), GK_F8(40), GK_F8(48), GK_F8(56), GK_F8(64), \
                 GK_F8(72), GK_F8(80), GK_F8(88), GK_F8(96), GK_F8(104), GK_F8(112), GK_F8(120)
+#define GK_R8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), \
+                 "+r"(d[i + 6]), "+r"(d[i + 7])
+#define GK_R128 GK_R8(0), GK_R8(8), GK_R8(16), GK_R8(24), GK_R8(32), GK_R8(40), GK_R8(48), GK_R8(56), GK_R8(64), \
+                GK_R8(72), GK_R8(80), GK_R8(88), GK_R8(96), GK_R8(104), GK_R8(112), GK_R8(120)
 #define GK_D128 \
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
   "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "   \
@@ -201,11 +217,23 @@ __device__ __forceinline__ void wg_mma(float (&d)[128], uint64_t adesc, uint64_t
         : GK_F128
         : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
+// KIND 2: u8 x u8 -> s32, k = 32 (integer wgmma has no operand scale or transpose arguments)
+template <int KIND>
+__device__ __forceinline__ void wg_mma(int (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+  static_assert(KIND == 2, "s32 accumulators belong to the u8 operand kind");
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k32.s32.u8.u8 " GK_D128 ", %128, %129, p;\n\t}"
+      : GK_R128
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
 #undef GK_F8
 #undef GK_F128
+#undef GK_R8
+#undef GK_R128
 #undef GK_D128
 
-// Accumulator layout of wgmma m64nN (fp32): thread `lane` of warp `w` of the warpgroup holds, for every group i of
+// Accumulator layout of wgmma m64nN (fp32 or s32): thread `lane` of warp `w` of the warpgroup holds, for every group i of
 // 8 columns, d[4i + 2h + e] = D[16 w + lane / 4 + 8 h][8 i + 2 (lane % 4) + e]  (h, e in {0, 1}).
 
 template <typename OutT, bool NORMALIZE>
@@ -234,8 +262,9 @@ __device__ __forceinline__ uint32_t swz_addr(uint32_t buf, uint32_t r, uint32_t 
 // (`w` = warp in the warpgroup, the pair is w / 2) for fp32, un-normalised output through TMA stores: per 32 x 32
 // block, fragments -> 128B-swizzled smem tile -> ONE TMA store (the SM->L2 path is bound by write requests: 1 bulk
 // request instead of 32 row stores).  TMA clips at the matrix edge, so partial blocks need no predicates.
+template <typename AccT>
 __device__ __forceinline__ void epi_tma_store_strip(const GramParams& p, const CUtensorMap* tmC, int arow0, int tile_y,
-                                                    const float (&acc)[128], int w, int lane, uint32_t my_buf,
+                                                    const AccT (&acc)[128], int w, int lane, uint32_t my_buf,
                                                     int bar_id, const CUtensorMap* peer_maps) {
   const bool first = (w & 1) == 0;  // the first warp of the pair issues the stores and applies the direct tail list
   const bool leader = first && lane == 0;
@@ -288,7 +317,7 @@ __device__ __forceinline__ void epi_tma_store_strip(const GramParams& p, const C
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int rb = rb0 + 8 * h, cb = 8 * j + 2 * (lane & 3);
-        float v0 = acc[4 * (4 * b + j) + 2 * h], v1 = acc[4 * (4 * b + j) + 2 * h + 1];
+        float v0 = (float)acc[4 * (4 * b + j) + 2 * h], v1 = (float)acc[4 * (4 * b + j) + 2 * h + 1];
         if (diag_tile) {
           if (arow0 + rb == bcol0 + cb) v0 = dself[h];
           if (arow0 + rb == bcol0 + cb + 1) v1 = dself[h];
@@ -334,8 +363,8 @@ __device__ __forceinline__ void epi_tma_store_strip(const GramParams& p, const C
 
 // Epilogue of the 64 x 256 slab of one consumer warpgroup straight from registers (fp64 output, normalisation,
 // split-precision k-chunks that add to `out`, and fp32 output without TMA stores).
-template <typename OutT, bool NORMALIZE>
-__device__ __forceinline__ void epi_direct(const GramParams& p, int arow_base, int tile_y, const float (&acc)[128],
+template <typename OutT, bool NORMALIZE, typename AccT>
+__device__ __forceinline__ void epi_direct(const GramParams& p, int arow_base, int tile_y, const AccT (&acc)[128],
                                            bool acc_out, int lane) {
   OutT* __restrict__ out = reinterpret_cast<OutT*>(p.out);
 #pragma unroll
@@ -351,7 +380,7 @@ __device__ __forceinline__ void epi_direct(const GramParams& p, int arow_base, i
         const int bcol = tile_y + 8 * i + 2 * (lane & 3) + e;
         if (bcol >= p.b_row_end) continue;
         const double dcol = NORMALIZE ? p.diag[bcol] : 0.0;
-        OutT v = epilogue_value<OutT, NORMALIZE>(acc[4 * i + 2 * h + e], arow, bcol, drow, dcol, p);
+        OutT v = epilogue_value<OutT, NORMALIZE>((float)acc[4 * i + 2 * h + e], arow, bcol, drow, dcol, p);
         if (acc_out) v += dst_row[bcol];  // later k-chunks of a split-precision GEMM: this CTA owns the tile
         dst_row[bcol] = v;
         if (p.mirror) out[(long long)bcol * p.ld + arow] = v;
@@ -410,7 +439,7 @@ __device__ __forceinline__ void gram_body(const CUtensorMap& tmA, const CUtensor
           w_empty += clock64() - c0;
           mbar_expect_tx(full_bar(stage), STAGE_BYTES);
           const uint32_t sa = smem_base + stage * STAGE_BYTES;
-          const int kx = (p.k_block0 + kb) * (KIND == 1 ? BK_TF32 : BK);
+          const int kx = (p.k_block0 + kb) * (KIND == 1 ? BK_TF32 : KIND == 2 ? BK_U8 : BK);
           tma_load_2d(sa, &tmA, full_bar(stage), kx, tile.x + (int)rank * BM);
           if constexpr (PAIR)
             tma_load_2d_mc(sa + A_BYTES + rank * (B_BYTES / 2), &tmA, full_bar(stage), kx, tile.y + (int)rank * (BN / 2),
@@ -436,9 +465,9 @@ __device__ __forceinline__ void gram_body(const CUtensorMap& tmA, const CUtensor
         if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(empty_bar(s), peer_rank));
       }
     };
-    float acc[128];
+    typename AccOf<KIND>::type acc[128];
 #pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int i = 0; i < 128; ++i) acc[i] = 0;
     int stage = 0;
     uint32_t phase = 0;
     long long w_full = 0, t_epi = 0;
@@ -488,7 +517,7 @@ __device__ __forceinline__ void gram_body(const CUtensorMap& tmA, const CUtensor
   if constexpr (PAIR) cluster_sync_all();  // neither CTA exits while the peer may still multicast into it or arrive on it
 }
 
-template <typename OutT, bool NORMALIZE, int KIND = 0 /* 0: bf16 operands, 1: tf32 operands */>
+template <typename OutT, bool NORMALIZE, int KIND = 0 /* 0: bf16 operands, 1: tf32 operands, 2: u8 operands */>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, GramParams p) {
@@ -498,8 +527,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // ---------------------------------------------------------------------------
 // Exact CUDA-core Gram over a u32 count panel (int64 accumulation).  Used (a) as
 // the on-device cross-check of the tensor-core kernel in the tests and (b) when a
-// count exceeds 256 or a Gram value exceeds 2^24, where bf16 x bf16 -> fp32 would
-// no longer be exact.
+// count exceeds 256 or a Gram value exceeds 2^24, where neither operand type of the
+// tensor-core kernel holds the counts or fp32 no longer holds the result exactly.
 template <typename OutT, bool NORMALIZE>
 __global__ void __launch_bounds__(256)
 gram_simt_kernel(const unsigned* __restrict__ panel, long long ldp, int kdim, int a_row0, int a_row_end,

@@ -10,6 +10,8 @@
 //             peer's multicast B half complete their bytes on it
 //   empty[s]  (one per CTA)  16 arrivals: lane 0 of the eight consumer warps of EACH CTA (the peer's through mapa),
 //             because the CTA's next load of stage s writes into both CTAs' shared memory
+//
+// KIND 0: bf16 panel (f32 accumulators), KIND 2: u8 panel (s32 accumulators); the k-block is 128 bytes either way.
 #pragma once
 #include "gram_tc.cuh"
 
@@ -18,10 +20,11 @@ namespace gk {
 constexpr int BM2 = 256;  // rows of A per cluster tile (128 per CTA)
 constexpr int GEMM2_SMEM = GEMM_SMEM;
 
+template <int KIND>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
 gram_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmC, GramParams p,
                 const __grid_constant__ PeerMaps pm) {
-  gram_body<float, false, 0, true>(tmA, tmA, tmC, p, p.mirror == 2 && p.n_peers ? pm.m : nullptr);
+  gram_body<float, false, KIND, true>(tmA, tmA, tmC, p, p.mirror == 2 && p.n_peers ? pm.m : nullptr);
 }
 
 }  // namespace gk

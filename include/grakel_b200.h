@@ -102,13 +102,16 @@ typedef struct gk_stats {
   int64_t max_count;         /* largest single feature count */
   int64_t max_diag;          /* largest self-similarity */
   int64_t hash_retries;      /* WL: relabel passes repeated after a detected hash collision */
-  int64_t gram_path;         /* 1 = wgmma bf16 tensor-core GEMM, 2 = exact int64 CUDA-core Gram, 3 = no contracted columns,
+  int64_t gram_path;         /* 1 = wgmma tensor-core GEMM over the integer panel (u8 or bf16: gemm_elem_bytes), 2 = exact int64 CUDA-core Gram, 3 = no contracted columns,
                                 ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram,
                                 GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
   float ms_h2d, ms_features, ms_panel, ms_gemm, ms_tail, ms_d2h, ms_total;
+  int64_t gemm_elem_bytes;   /* element bytes of the integer head panel the tensor-core GEMM (gram_path 1) read:
+                                1 = u8 (u8 x u8 -> s32 wgmma, every count <= 255), 2 = bf16 (a count of 256, or
+                                GRAKEL_B200_U8=0), 0 = no integer tensor-core GEMM ran */
 } gk_stats;
 
 int gk_version(void);
