@@ -21,6 +21,7 @@ GK_DIST, GK_DIST_GATHER = 64, 128
 GK_SP_WITH_LABELS, GK_SP_KEEP_DIST, GK_SP_DIJKSTRA_ORDER = 1, 2, 4
 GK_ERR_RANGE, GK_ERR_UNSUPPORTED = -4, -5
 GK_GH_LINEAR, GK_GH_GAUSSIAN, GK_GH_BRIDGE = 0, 1, 2
+GK_NH_SIMPLE, GK_NH_COUNT_SENSITIVE = 0, 1
 
 
 class GkStats(C.Structure):
@@ -35,13 +36,15 @@ class GkStats(C.Structure):
         ("ms_h2d", C.c_float), ("ms_features", C.c_float), ("ms_panel", C.c_float),
         ("ms_gemm", C.c_float), ("ms_tail", C.c_float), ("ms_d2h", C.c_float), ("ms_total", C.c_float),
         ("gemm_elem_bytes", C.c_int64),
+        ("ms_hash", C.c_float), ("ms_columns", C.c_float), ("ms_combine", C.c_float),
+        ("ms_level_gram", C.c_float * 64), ("nh_order_dependent", C.c_int64),
     ]
 
     def as_dict(self):
         d = {}
         for name, _ in self._fields_:
             v = getattr(self, name)
-            d[name] = list(v)[: max(int(self.n_levels), 1)] if name == "level_dims" else v
+            d[name] = list(v)[: max(int(self.n_levels), 1)] if name in ("level_dims", "ms_level_gram") else v
         return d
 
 
@@ -64,6 +67,8 @@ _SYMBOLS = {
     "gk_wl_oa_features": (C.c_int, [_P, C.c_int32, C.POINTER(GkStats)]),
     "gk_gh_features": (C.c_int, [_P, C.c_int32, C.c_double, C.c_int32, C.POINTER(GkStats)]),
     "gk_gh_node_maps": (C.c_int, [_P, C.c_int64, _P]),
+    "gk_nh_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int64, C.c_int32, C.POINTER(GkStats)]),
+    "gk_nh_labels": (C.c_int, [_P, C.c_int32, _P, _P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -264,6 +269,25 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_gh_node_maps(self.h, int(g), _ptr(out)))
         return out
+
+    def nh_features(self, R, nh_type, bits, code_of_label, label_valid=None):
+        """NeighborhoodHash codes of R levels and one expanded count block per level (gk_nh_features).
+        `code_of_label[i]` is the initial code of packed label id i, `label_valid[i] == 0` marks it None."""
+        codes = np.ascontiguousarray(code_of_label, dtype=np.uint64)
+        valid = None if label_valid is None else np.ascontiguousarray(label_valid, dtype=np.uint8)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_nh_features(self.h, int(R), int(nh_type), int(bits), _ptr(codes), _ptr(valid),
+                                                len(codes), 0, C.byref(st)))
+        return st
+
+    def nh_labels(self, level, n_vertices):
+        """(codes u64, not-None flags bool) of every packed vertex at NeighborhoodHash level `level`."""
+        out = np.empty(n_vertices, dtype=np.uint64)
+        valid = np.empty(n_vertices, dtype=np.uint8)
+        with self._lock:
+            self._check(self.lib.gk_nh_labels(self.h, int(level), _ptr(out), _ptr(valid)))
+        return out, valid.astype(bool)
 
     def gram(self, n_graphs, n_fit=None, normalize=False, nan_to_num=False, out=None, dtype=np.float64,
              row_range=None, simt=False, full_tiles=False, stats=None, want_diag=True, device_ptr=None, ld=0,

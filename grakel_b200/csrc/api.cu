@@ -26,6 +26,7 @@
 #include "wl_fused.cuh"
 #include "wl_fused2.cuh"
 #include "wl_oa.cuh"
+#include "neighborhood_hash.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -162,6 +163,8 @@ struct HandleExtra {
                                  // (not GK_DENSE_ALL / FORCE_T)
   long long last_max_count = 0;  // largest count of the last Gram on this handle: an asynchronous pass fills a u8 panel
                                  // unless it was 256 (a count of 256 repeats through the synchronous route once)
+  // NeighborhoodHash: per level, distinct codes, columns and entries of the unary-expanded block
+  std::vector<long long> nh_dims, nh_cols, nh_entries;
 };
 static std::vector<std::pair<gk_handle*, HandleExtra*>> g_extra;
 static HandleExtra* extra_of(gk_handle* h) {
@@ -321,7 +324,8 @@ int gk_destroy(gk_handle* h) {
                         &h->sp_dist, &h->sp_dict_keys, &h->sp_dict_ids, &h->sp_dkeys, &h->sp_graph_off, &h->fattr, &h->tiles,
                         &h->K, &h->K_stage, &h->wlf_buf, &h->row_map, &h->diag_rows, &h->oa_keys, &h->oa_cnt, &h->oa_colcnt, &h->wl_single,
                         &h->diag_frozen, &h->sp_lists, &h->wl_payload, &h->gram_dyn, &h->tb_cnt, &h->tb_ent, &h->tb_ovf,
-                        &h->gh_M, &h->gh_ws, &h->gh_woff, &h->gh_gdiam, &h->gh_groups, &h->gh_pairs};
+                        &h->gh_M, &h->gh_ws, &h->gh_woff, &h->gh_gdiam, &h->gh_groups, &h->gh_pairs,
+                        &h->nh_codes, &h->nh_valid, &h->nh_blk, &h->nh_lut, &h->nh_tab, &h->nh_ws, &h->nh_cur, &h->nh_C};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1839,6 +1843,334 @@ static int gram_gh_nodepair(gk_handle* h, int64_t n_fit, int32_t flags, int64_t 
 }
 
 // ---------------------------------------------------------------------------
+// NeighborhoodHash (neighborhood_hash.cuh).  Level r's expanded block lives at nh_blk + r * nh_level_bytes:
+// keys [V] u64 | counts [V] u32 | graphs per column [V + 1] u32 | self similarities [N] u64 (at most one unary entry
+// per non-None vertex, so V entries and V columns bound every level).
+struct NhLevel {
+  unsigned long long* keys;
+  unsigned* cnt;
+  unsigned* colcnt;
+  unsigned long long* diag;
+};
+
+static size_t nh_level_bytes(int64_t V, int64_t N) {
+  const size_t V1 = (size_t)std::max<int64_t>(V, 1);
+  const size_t diag_off = (16 * V1 + 4 + 7) / 8 * 8;
+  return (diag_off + 8 * (size_t)std::max<int64_t>(N, 1) + 255) / 256 * 256;
+}
+
+static NhLevel nh_level(gk_handle* h, int r) {
+  const size_t V1 = (size_t)std::max<int64_t>(h->V, 1);
+  char* b = h->nh_blk.as<char>() + (size_t)r * h->nh_level_bytes;
+  NhLevel L;
+  L.keys = reinterpret_cast<unsigned long long*>(b);
+  L.cnt = reinterpret_cast<unsigned*>(b + 8 * V1);
+  L.colcnt = reinterpret_cast<unsigned*>(b + 12 * V1);
+  L.diag = reinterpret_cast<unsigned long long*>(b + (16 * V1 + 4 + 7) / 8 * 8);
+  return L;
+}
+
+int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const uint64_t* code_of_label,
+                   const uint8_t* label_valid, int64_t n_labels, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_nh_features: no graphs packed");
+  if (!h->has_labels) return fail(GK_ERR_ARG, "gk_nh_features: vertex labels are required");
+  if (R < 1 || R > MAX_LEVELS) return fail(GK_ERR_ARG, "gk_nh_features: R out of range [1, 64]");
+  if (nh_type != GK_NH_SIMPLE && nh_type != GK_NH_COUNT_SENSITIVE) return fail(GK_ERR_ARG, "gk_nh_features: unknown nh_type");
+  if (bits < 1 || bits > 64) return fail(GK_ERR_ARG, "gk_nh_features: bits out of range [1, 64]");
+  if (flags != 0) return fail(GK_ERR_ARG, "gk_nh_features: no flags are defined");
+  if (!code_of_label || n_labels < h->n_labels0) return fail(GK_ERR_ARG, "gk_nh_features: a code is needed for every label id");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t N = h->N, V = h->V, E = h->E;
+  const int64_t V1 = std::max<int64_t>(V, 1), L1 = std::max<int64_t>(n_labels, 1);
+  const unsigned long long mask = bits == 64 ? ~0ULL : (1ULL << bits) - 1ULL;
+  const int64_t launches0 = h->launches;
+  h->features_ready = false; h->feat_serial++;
+  HandleExtra* ex = extra_of(h);
+
+  GK_TRY(init_scalars(h, 0));  // clears ft_overflow
+  GK_TRY(h->nh_codes.ensure((size_t)(R + 1) * V1 * 8));
+  GK_TRY(h->nh_valid.ensure((size_t)(R + 1) * V1));
+  GK_TRY(h->nh_lut.ensure((size_t)L1 * 9));
+  unsigned long long* codes = h->nh_codes.as<unsigned long long>();
+  unsigned char* valid = h->nh_valid.as<unsigned char>();
+  unsigned char* d_lvalid = h->nh_lut.as<unsigned char>() + (size_t)L1 * 8;
+  if (n_labels > 0) {
+    GK_CUDA(cudaMemcpyAsync(h->nh_lut.p, code_of_label, (size_t)n_labels * 8, cudaMemcpyHostToDevice, h->stream));
+    if (label_valid) GK_CUDA(cudaMemcpyAsync(d_lvalid, label_valid, (size_t)n_labels, cudaMemcpyHostToDevice, h->stream));
+    else GK_CUDA(cudaMemsetAsync(d_lvalid, 1, (size_t)n_labels, h->stream));
+  }
+  // count-sensitive tables of the large-degree vertices: 2 slots per edge
+  // (2 E slots: row position | count | two-codes flag)
+  if (nh_type == GK_NH_COUNT_SENSITIVE && h->n_large) GK_TRY(h->nh_ws.ensure((size_t)std::max<int64_t>(E, 1) * 24));
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+
+  // ---- hash levels: gr[0] = NH(initial), gr[r] = NH(gr[r - 1])
+  if (V) {
+    nh_init<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, h->labels0.as<int>(), h->nh_lut.as<unsigned long long>(), d_lvalid,
+                                                 codes, valid);
+    LAUNCH_CHECK(h);
+  }
+  int* ws_tab = h->nh_ws.as<int>();
+  unsigned* ws_cnt = reinterpret_cast<unsigned*>(ws_tab + 2 * std::max<int64_t>(E, 1));
+  unsigned* order_dep = &h->scalars.as<DevScalars>()->nh_order_dep;
+  for (int r = 0; r < R && V; ++r) {
+    const unsigned long long* in = codes + (size_t)r * V;
+    const unsigned char* vin = valid + (size_t)r * V;
+    unsigned long long* out = codes + (size_t)(r + 1) * V;
+    unsigned char* vout = valid + (size_t)(r + 1) * V;
+    if (nh_type == GK_NH_SIMPLE)
+      nh_hash_small<NH_SIMPLE><<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, h->group_width, h->row_ptr.as<int>(),
+                                                                    h->col_idx.as<int>(), in, vin, out, vout, bits, mask, order_dep);
+    else
+      nh_hash_small<NH_COUNT><<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, h->group_width, h->row_ptr.as<int>(),
+                                                                   h->col_idx.as<int>(), in, vin, out, vout, bits, mask, order_dep);
+    LAUNCH_CHECK(h);
+    if (h->n_large) {  // vertices of degree > group_width (gk_pack_csr's large list)
+      if (nh_type == GK_NH_SIMPLE)
+        nh_hash_large<NH_SIMPLE><<<(int)h->n_large, NH_LARGE_THREADS, 0, h->stream>>>(
+            h->large_list.as<int>(), h->row_ptr.as<int>(), h->col_idx.as<int>(), in, vin, out, vout, bits, mask, nullptr, nullptr, order_dep);
+      else
+        nh_hash_large<NH_COUNT><<<(int)h->n_large, NH_LARGE_THREADS, 0, h->stream>>>(
+            h->large_list.as<int>(), h->row_ptr.as<int>(), h->col_idx.as<int>(), in, vin, out, vout, bits, mask, ws_tab, ws_cnt, order_dep);
+      LAUNCH_CHECK(h);
+    }
+  }
+  GK_CUDA(cudaEventRecord(h->tev[5], h->stream));
+
+  // ---- per-level columns, counts and unary expansion
+  const size_t cap = std::max<size_t>(next_pow2((size_t)V1 * 2), 1024);
+  h->nh_level_bytes = nh_level_bytes(V, N);
+  GK_TRY(h->nh_blk.ensure((size_t)R * h->nh_level_bytes));
+  GK_TRY(h->nh_tab.ensure(cap * 8 + (size_t)V1 * 4));  // slot -> claiming vertex | slot -> column | vertex -> slot
+  GK_TRY(h->ft_keys.ensure(cap * 8));                 // (graph, column) -> count scratch table
+  GK_TRY(h->ft_cnt.ensure(cap * 4));
+  GK_TRY(h->colmin.ensure((size_t)V1 * 4));  // largest count of every column
+  GK_TRY(h->colmax.ensure((size_t)V1 * 4));  // first expanded column of every column
+  const size_t cur_bytes = (size_t)R * (sizeof(OaCursors) + 8);
+  GK_TRY(h->nh_cur.ensure(cur_bytes));
+  GK_TRY(h->h_colstats.ensure(std::max(cur_bytes, sizeof(ColStats))));
+  OaCursors* cur = h->nh_cur.as<OaCursors>();
+  unsigned long long* dims = reinterpret_cast<unsigned long long*>(cur + R);
+  int* tab = h->nh_tab.as<int>();
+  int* colid = tab + cap;
+  int* slot_of = colid + cap;
+  GK_CUDA(cudaMemsetAsync(h->nh_cur.p, 0, cur_bytes, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->nh_blk.p, 0, (size_t)R * h->nh_level_bytes, h->stream));
+  for (int r = 0; r < R; ++r) {
+    const NhLevel lv = nh_level(h, r);
+    GK_CUDA(cudaMemsetAsync(lv.keys, 0xFF, (size_t)V1 * 8, h->stream));
+    if (!V) continue;
+    const unsigned long long* c_r = codes + (size_t)(r + 1) * V;
+    const unsigned char* v_r = valid + (size_t)(r + 1) * V;
+    GK_CUDA(cudaMemsetAsync(tab, 0xFF, cap * 4, h->stream));
+    GK_CUDA(cudaMemsetAsync(h->ft_keys.p, 0xFF, cap * 8, h->stream));
+    GK_CUDA(cudaMemsetAsync(h->ft_cnt.p, 0, cap * 4, h->stream));
+    GK_CUDA(cudaMemsetAsync(h->colmin.p, 0, (size_t)V1 * 4, h->stream));
+    nh_code_insert<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, c_r, v_r, tab, (unsigned)(cap - 1), slot_of);
+    LAUNCH_CHECK(h);
+    nh_code_number<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, v_r, tab, slot_of, colid, dims + r);
+    LAUNCH_CHECK(h);
+    nh_count<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, v_r, h->vgraph.as<int>(), slot_of, colid,
+                                                  h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
+                                                  (unsigned)(cap - 1));
+    LAUNCH_CHECK(h);
+    oa_colmax<<<h->sm_count * 8, 256, 0, h->stream>>>(cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
+                                                      h->colmin.as<unsigned>());
+    LAUNCH_CHECK(h);
+    oa_colbase<<<cdiv(V1, OA_THREADS), OA_THREADS, 0, h->stream>>>(V1, h->colmin.as<unsigned>(), h->colmax.as<unsigned>(),
+                                                                   cur + r);
+    LAUNCH_CHECK(h);
+    oa_expand<<<cdiv((long long)cap, OA_THREADS), OA_THREADS, 0, h->stream>>>(
+        cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colmax.as<unsigned>(), (size_t)V1, lv.keys,
+        lv.cnt, cur + r, lv.colcnt, lv.diag, h->scalars.as<DevScalars>());
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->h_colstats.p, h->nh_cur.p, cur_bytes, cudaMemcpyDeviceToHost, h->stream));
+  DevScalars* hs;
+  GK_TRY(read_scalars(h, &hs));  // synchronises
+  if (hs->ft_overflow) return fail(GK_ERR_STATE, "gk_nh_features: expanded feature block overflow");
+  const OaCursors* hc = h->h_colstats.as<OaCursors>();
+  const unsigned long long* hdims = reinterpret_cast<const unsigned long long*>(hc + R);
+  ex->nh_dims.assign(R, 0);
+  ex->nh_cols.assign(R, 0);
+  ex->nh_entries.assign(R, 0);
+  int64_t n_cols = 0, n_ent = 0;
+  for (int r = 0; r < R; ++r) {
+    ex->nh_dims[r] = (long long)hdims[r];
+    ex->nh_cols[r] = (long long)hc[r].n_cols;
+    ex->nh_entries[r] = (long long)hc[r].n_entries;
+    n_cols += ex->nh_cols[r];
+    n_ent += ex->nh_entries[r];
+  }
+  h->nh_R = R;
+  h->n_columns = n_cols;
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = 5;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
+    stats->n_levels = R;
+    for (int r = 0; r < R; ++r) stats->level_dims[r] = ex->nh_dims[r];
+    stats->n_columns = n_cols;
+    stats->n_entries = n_ent;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_hash = ev_ms(h->tev[2], h->tev[5]);
+    stats->ms_columns = ev_ms(h->tev[5], h->tev[3]);
+    stats->nh_order_dependent = hs->nh_order_dep ? 1 : 0;
+  }
+  return GK_OK;
+}
+
+int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_nh_labels: null argument");
+  if (h->feature_kind != 5 || !h->features_ready || level < 0 || level >= h->nh_R)
+    return fail(GK_ERR_STATE, "gk_nh_labels: no such level (run gk_nh_features first)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t V = (size_t)h->V;
+  if (V) {
+    GK_CUDA(cudaMemcpyAsync(out, h->nh_codes.as<unsigned long long>() + (size_t)(level + 1) * V, V * 8,
+                            cudaMemcpyDeviceToHost, h->stream));
+    if (valid)
+      GK_CUDA(cudaMemcpyAsync(valid, h->nh_valid.as<unsigned char>() + (size_t)(level + 1) * V, V, cudaMemcpyDeviceToHost,
+                              h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  return GK_OK;
+}
+
+// Gram of NeighborhoodHash features (gram_path 7): for every level, gk_gram's exact integer Gram of the level's
+// expanded block gives the intersection counts c_r as fp32 in nh_C; nh_combine turns the R count matrices into the
+// fp64 K.  Rows go in chunks when R count matrices of the whole request would exceed NH_C_BUDGET bytes
+// (GRAKEL_B200_NH_C_BUDGET=<bytes> lowers it, so that tests reach the chunked route; a chunk of
+// the square case then computes full rows instead of mirroring).  GK_NORMALIZE changes nothing: the reference never
+// normalises this kernel, and its self similarities are 1.
+constexpr size_t NH_C_BUDGET = (size_t)8 << 30;
+
+static int gram_nh(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
+                   int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
+  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "NeighborhoodHash Gram is fp64 only");
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N;
+  const int R = h->nh_R;
+  const bool square = n_fit == N;
+  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
+  if (row_end < 0) row_end = k_rows_total;
+  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
+  const int64_t k_rows = row_end - row_begin;
+  if (ld <= 0) ld = k_cols;
+  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
+  const bool dev_out = (flags & GK_OUT_DEVICE) != 0;
+  if (dev_out && !K_out) return fail(GK_ERR_ARG, "gk_gram: GK_OUT_DEVICE without a pointer");
+  const int64_t launches0 = h->launches;
+  double* d_out;
+  int64_t d_ld;
+  if (dev_out) {
+    d_out = reinterpret_cast<double*>(K_out);
+    d_ld = ld;
+  } else {
+    GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
+    h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
+    d_out = h->K.as<double>();
+    d_ld = k_cols;
+  }
+  const int64_t ldc = (k_cols + 7) / 8 * 8;  // 32-byte rows: TMA stores of the Gram epilogue
+  size_t c_budget = NH_C_BUDGET;
+  if (const char* e = getenv("GRAKEL_B200_NH_C_BUDGET")) c_budget = std::max<size_t>(1, strtoull(e, nullptr, 10));
+  const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(std::max<int64_t>(k_rows, 1),
+                                                                (int64_t)(c_budget / ((size_t)R * ldc * 4))));
+  GK_TRY(h->nh_C.ensure((size_t)R * chunk * ldc * 4));
+  const int32_t gflags = (flags & (GK_GRAM_SIMT | GK_DENSE_ALL | GK_FULL_TILES)) | GK_OUT_DEVICE;
+  const size_t V1 = (size_t)std::max<int64_t>(h->V, 1);
+  GK_TRY(h->part_max.ensure(4));
+  GK_TRY(h->part_new.ensure(4));
+  std::vector<float> ms_level(R, 0.f);
+  float ms_combine = 0.f;
+  gk_stats st;
+  int64_t max_T = 0, gram_launches = 0, elem_bytes = 0;
+  for (int64_t cb = row_begin; cb < row_end; cb += chunk) {
+    const int64_t ce = std::min<int64_t>(row_end, cb + chunk), rows = ce - cb;
+    for (int r = 0; r < R; ++r) {
+      // install level r as the handle's integer feature block, run the Gram, put the handle's own buffers back
+      const NhLevel lv = nh_level(h, r);
+      const unsigned part[2] = {ex->nh_entries[r] ? 1u : 0u, (unsigned)ex->nh_entries[r]};
+      GK_CUDA(cudaMemcpyAsync(h->part_max.p, &part[0], 4, cudaMemcpyHostToDevice, h->stream));
+      GK_CUDA(cudaMemcpyAsync(h->part_new.p, &part[1], 4, cudaMemcpyHostToDevice, h->stream));
+      const DevBuf s_keys = h->ft_keys, s_cnt = h->ft_cnt, s_colcnt = h->colcnt, s_diag = h->diag_u64;
+      const size_t s_ftcap = h->ft_cap;
+      const int64_t s_colcap = h->col_cap, s_ncols = h->n_columns, s_npart = h->n_part;
+      h->ft_keys.p = lv.keys; h->ft_keys.cap = V1 * 8;
+      h->ft_cnt.p = lv.cnt; h->ft_cnt.cap = V1 * 4;
+      h->colcnt.p = lv.colcnt; h->colcnt.cap = (V1 + 1) * 4;
+      h->diag_u64.p = lv.diag; h->diag_u64.cap = (size_t)N * 8;
+      h->ft_cap = V1; h->col_cap = (int64_t)V1 + 1; h->n_columns = ex->nh_cols[r]; h->n_part = 1;
+      h->feature_kind = 1;
+      memset(&st, 0, sizeof(st));
+      const int rc = gk_gram(h, n_fit, gflags, cb, ce, h->nh_C.as<float>() + (size_t)r * chunk * ldc, GK_F32, ldc, nullptr,
+                             nullptr, &st);
+      h->ft_keys = s_keys; h->ft_cnt = s_cnt; h->colcnt = s_colcnt; h->diag_u64 = s_diag;
+      h->ft_cap = s_ftcap; h->col_cap = s_colcap; h->n_columns = s_ncols; h->n_part = s_npart;
+      h->feature_kind = 5;
+      if (rc != GK_OK) return rc;
+      ms_level[r] += st.ms_total;
+      max_T = std::max<int64_t>(max_T, st.threshold);
+      gram_launches += st.gemm_launches;
+      elem_bytes = std::max<int64_t>(elem_bytes, st.gemm_elem_bytes);  // 0 when no tensor-core GEMM ran
+    }
+    if (rows > 0) {
+      NhCombineParams p;
+      p.C = h->nh_C.as<float>();
+      p.stride = chunk * ldc;
+      p.ldc = ldc;
+      p.R = R;
+      p.graph_ptr = h->graph_ptr.as<int>();
+      p.row_g0 = (int)((square ? 0 : n_fit) + cb);
+      p.rows = (int)rows;
+      p.cols = (int)k_cols;
+      p.mirror = square && cb == 0 && ce == N && !(flags & GK_FULL_TILES) ? 1 : 0;
+      p.out = d_out + (size_t)(cb - row_begin) * d_ld;
+      p.ld = d_ld;
+      const long long nbi = (rows + NH_TILE - 1) / NH_TILE, nbj = (k_cols + NH_TILE - 1) / NH_TILE;
+      const long long grid = p.mirror ? nbj * (nbj + 1) / 2 : nbi * nbj;
+      GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+      if (grid > 0) {
+        nh_combine<<<(unsigned)grid, NH_TILE * 8, 0, h->stream>>>(p);
+        LAUNCH_CHECK(h);
+      }
+      GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+      GK_CUDA(cudaEventSynchronize(h->tev[1]));
+      ms_combine += ev_ms(h->tev[0], h->tev[1]);
+    }
+  }
+  GK_CUDA(cudaEventRecord(h->ev[14], h->stream));
+  if (K_out && !dev_out && k_rows > 0)
+    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, d_out, (size_t)d_ld * 8, (size_t)k_cols * 8, (size_t)k_rows,
+                              cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaEventRecord(h->ev[15], h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  if (xdiag) for (int64_t i = 0; i < n_fit; ++i) xdiag[i] = 1.0;
+  if (ydiag && !square) for (int64_t i = 0; i < N - n_fit; ++i) ydiag[i] = 1.0;
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->n_levels = R;
+    stats->gram_path = 7;
+    stats->threshold = max_T;
+    stats->max_count = 1;
+    stats->gemm_launches = gram_launches + (h->launches - launches0);
+    stats->gemm_elem_bytes = elem_bytes;
+    float tot = ms_combine;
+    for (int r = 0; r < R; ++r) { stats->ms_level_gram[r] = ms_level[r]; tot += ms_level[r]; }
+    stats->ms_gemm = tot - ms_combine;
+    stats->ms_combine = ms_combine;
+    stats->ms_d2h = ev_ms(h->ev[14], h->ev[15]);
+    stats->ms_total = tot + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
+// ---------------------------------------------------------------------------
 }  // extern "C"
 
 // ---------------------------------------------------------------------------
@@ -1965,6 +2297,12 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     if (h->gh_node_kernel == GK_GH_LINEAR)
       return gram_spattr(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
     return gram_gh_nodepair(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
+  }
+  if (h->feature_kind == 5) {
+    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with NeighborhoodHash features");
+    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with NeighborhoodHash features");
+    GK_CUDA(cudaSetDevice(h->dev));
+    return gram_nh(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
   }
   const bool square = n_fit == N;
   const int64_t k_rows_total = square ? N : N - n_fit;

@@ -105,7 +105,7 @@ struct DevScalars {
   unsigned int sp_dict_size;             // SP: number of distinct (lu,lv,d) keys
   unsigned int sp_nonint;                // SP: a non-integer / out-of-range distance was met
   unsigned int fattr_negative;           // SP-attr: the feature map has a negative entry
-  unsigned int pad0;
+  unsigned int nh_order_dep;             // NeighborhoodHash: a count-sensitive result depended on the neighbour order
 };
 
 static_assert(sizeof(DevScalars) % 8 == 0, "cleared as 64-bit words");
@@ -161,7 +161,7 @@ struct gk_handle {
   int64_t pro_serial = -1;   // feat_serial for which gk_wl_features already ran the Gram prologue (square case):
                              // self similarities finished, column histogram on the host -- gk_gram then needs no
                              // host synchronisation before its launches
-  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper
+  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper, 5 = NeighborhoodHash
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
   // ---- columns / panel / diag
@@ -200,6 +200,13 @@ struct gk_handle {
   int gh_delta = 0;
   int gh_node_kernel = 0;  // GK_GH_LINEAR / GK_GH_GAUSSIAN / GK_GH_BRIDGE
   double gh_mu = 1.0;
+
+  // ---- NeighborhoodHash (feature_kind 5)
+  gk::DevBuf nh_codes, nh_valid;  // [(R + 1) V] u64 codes / u8 not-None flags: the initial labels, then levels 0 .. R-1
+  gk::DevBuf nh_blk;              // unary-expanded (graph, column) block of every level, nh_level_bytes apart
+  gk::DevBuf nh_lut, nh_tab, nh_ws, nh_cur, nh_C;
+  size_t nh_level_bytes = 0;
+  int nh_R = 0;
 
   // ---- GEMM
   gk::DevBuf tiles;  // int2 list

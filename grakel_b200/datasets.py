@@ -22,6 +22,7 @@ from . import _lib
 from .packing import Block
 
 _MODES = {"WL": 0, "VH": 0, "weisfeiler_lehman": 0, "vertex_histogram": 0, "subtree_wl": 0, "ST-WL": 0,
+          "NH": 0, "neighborhood_hash": 0,
           "SP": 1, "shortest_path": 1, "WL-OA": 1, "weisfeiler_lehman_optimal_assignment": 1}
 GK_TU_SYMMETRIC, GK_TU_ATTR_NODES, GK_TU_DEGREE_LABELS = 1, 2, 4
 

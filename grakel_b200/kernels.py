@@ -21,6 +21,7 @@ from numbers import Real
 import numpy as np
 from sklearn.base import BaseEstimator, TransformerMixin
 from sklearn.exceptions import NotFittedError
+from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from . import _lib
@@ -1056,3 +1057,200 @@ class GraphHopper(Kernel):
 
     def _device_features(self, eng):
         return eng.gh_features(*self._node_kernel)
+
+
+# ------------------------------------------------------------------------------
+_NH_ELEMENT_MSG = ("each element of X must be either a graph object or a list with at least a graph like object and "
+                   "node labels dict \n")
+
+
+class NeighborhoodHash(Kernel):
+    """Neighborhood hashing kernel (neighborhood_hash.py:14-570; Hido & Kashima 2009).
+
+    Every label gets a random code of `bits` bits at fit; each of the R levels rehashes every vertex from its own code
+    and its out-neighbours' codes ("simple": a rotation XOR-ed with the neighbours' codes, "count_sensitive": one
+    rotated term per run of equal codes after a stable sort of the neighbours by their low `bits` bits), and
+    K(G, G') = mean over the levels of c / (n + n' - c), c the number of vertex codes the two graphs share (a multiset
+    intersection) and n, n' their vertex counts.  The codes, the intersections (an exact integer Gram per level) and
+    the fp64 combine run on the device; K equals the reference's bit for bit.
+
+    As in the reference, K is never normalised (`normalize` is accepted and ignored) and `diagonal()` is 1.0.
+    Vertices are the symbols of the edge dictionary; the labels of every labelled vertex, also one outside every
+    edge, enter the code dictionary.  A label unseen at fit is None in `transform`, and so is every vertex that has it
+    or has a neighbour that is None at the previous level.  Deviations: bits > 64 and R > 64 raise
+    NotImplementedError; an element with a graph but no labels raises TypeError."""
+
+    _graph_format = "dictionary"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, random_state=None, R=3, nh_type="simple", bits=8):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.random_state = random_state
+        self.R = R
+        self.nh_type = nh_type
+        self.bits = bits
+        self._initialized.update({"random_state": False, "R": False, "nh_type": False, "bits": False})
+
+    def initialize(self):
+        """neighborhood_hash.py:61-89."""
+        super().initialize()
+        if not self._initialized["random_state"]:
+            self.random_state_ = check_random_state(self.random_state)
+            self._initialized["random_state"] = True
+        if not self._initialized["R"]:
+            if type(self.R) is not int or self.R <= 0:
+                raise TypeError("R must be an intger bigger than zero")
+            if self.R > 64:
+                raise NotImplementedError("NeighborhoodHash: at most R = 64 levels are supported")
+            self._initialized["R"] = True
+        if not self._initialized["nh_type"]:
+            if self.nh_type == "simple":
+                self._nh_code = _lib.GK_NH_SIMPLE
+            elif self.nh_type == "count_sensitive":
+                self._nh_code = _lib.GK_NH_COUNT_SENSITIVE
+            else:
+                raise TypeError("unrecognised neighborhood hashing type")
+            self._initialized["nh_type"] = True
+        if not self._initialized["bits"]:
+            if type(self.bits) is not int or self.bits <= 0:
+                raise TypeError("illegal number of bits for hashing")
+            if self.bits > 64:
+                raise NotImplementedError("NeighborhoodHash: codes are 64-bit on the device; bits > 64 is not supported")
+            self._max_number = 1 << self.bits
+            self._mask = self._max_number - 1
+            self._initialized["bits"] = True
+
+    # ---- input
+    @staticmethod
+    def _elements(X):
+        """[graph, node labels] of every element, with the reference's element checks (neighborhood_hash.py:123-151)."""
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            if not (is_iter and len(x) in (0, 1, 2, 3)):
+                raise TypeError(_NH_ELEMENT_MSG)
+            if len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            if len(x) == 1:
+                raise TypeError("Ignoring empty element on index: " + str(len(out)) + "\nLabels must be provided.")
+            if type(x[0]) is dict and x[0] and all(type(d) is list for d in x[0].values()) and not all(x[0].values()):
+                # {u: []}: u is a vertex without an edge-dictionary entry (graph.py:1634-1650, 849-855)
+                raise ValueError("vertex not inside edge dictionary")
+            out.append([x[0], x[1]])
+        return out
+
+    @staticmethod
+    def _from_packed(X):
+        """A read_tu(kernel="NH") block holds every labelled node (all of their labels enter the code dictionary);
+        the kernel's vertex set is the nodes that occur in an edge (graph.py:1613-1703).  The neighbour order of the
+        reference's edge sets (read_data builds Python sets, base.py:215-222) is not known here; `_nh_run` refuses a
+        count-sensitive result that depends on it."""
+        X.require("wl")
+        labels = np.asarray(X.labels)
+        gp0 = np.asarray(X.graph_ptr, dtype=np.int64)
+        values = [labels[gp0[g]:gp0[g + 1]].tolist() for g in range(X.n_graphs)]
+        rp = np.asarray(X.row_ptr, dtype=np.int64)
+        ci = np.asarray(X.col_idx, dtype=np.int64)
+        deg = np.diff(rp)
+        keep = deg > 0
+        keep[ci] = True
+        before = np.concatenate([[0], np.cumsum(keep)])
+        block = Block(before[gp0], np.concatenate([[0], np.cumsum(deg[keep])]), before[ci], None, labels[keep])
+        block.mode = "sp"
+        return block, values
+
+    def parse_input(self, X):
+        fit = self._method_calling in (1, 2)
+        if isinstance(X, Block):
+            block, values = self._from_packed(X)
+        else:
+            els = self._elements(X)
+            block = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_NH_ELEMENT_MSG,
+                         keep_edge_order=True)
+            values = [list(L.values()) for _, L in els]
+        if fit:  # neighborhood_hash.py:157-189: the label set and the draws, operation for operation
+            labels_hash_set = set()
+            for vals in values:
+                labels_hash_set |= set(vals)
+            if len(labels_hash_set) > self._max_number:
+                warnings.warn("Number of labels is smaller than"
+                              "the biggest possible.. "
+                              "Collisions will appear on the "
+                              "new labels.")
+                nl, nrl = list(), len(labels_hash_set)
+                while nrl > self._max_number:
+                    nl += self.random_state_.choice(self._max_number, self._max_number, replace=False).tolist()
+                    nrl -= self._max_number
+                if nrl > 0:
+                    nl += self.random_state_.choice(self._max_number, nrl, replace=False).tolist()
+            else:
+                nl = self.random_state_.choice(self._max_number, len(labels_hash_set), replace=False).tolist()
+            self._labels_hash_dict = dict(zip(labels_hash_set, nl))
+        ids, dictionary = label_ids(block.labels, None, sort_new=False)
+        hd = self._labels_hash_dict
+        fitted = Fitted(block, ids, dictionary)
+        fitted.order_known = not isinstance(X, Block)
+        fitted.codes = np.array([hd.get(l, 0) for l in dictionary], dtype=np.uint64)
+        fitted.valid = np.array([l in hd for l in dictionary], dtype=np.uint8)
+        return fitted
+
+    # ---- estimator protocol
+    def fit(self, X, y=None):
+        self._method_calling = 1
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        self.X = self.parse_input(X)
+        return self
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        b = self.X.block
+        if np.any(np.diff(b.graph_ptr) == 0):  # nh_compare_labels of two vertex-less graphs: 0 / 0
+            raise ZeroDivisionError("float division by zero")
+        return self._nh_run(b, self.X.ids, self.X.codes, self.X.valid, b.n_graphs, self.X.order_known)
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        Y = self.parse_input(X)
+        xb = self.X.block
+        if np.any(np.diff(xb.graph_ptr) == 0) and np.any(np.diff(Y.block.graph_ptr) == 0):
+            raise ZeroDivisionError("float division by zero")
+        K = self._nh_run(Block.concat(xb, Y.block), np.concatenate([self.X.ids, Y.ids + len(self.X.codes)]),
+                         np.concatenate([self.X.codes, Y.codes]), np.concatenate([self.X.valid, Y.valid]), xb.n_graphs,
+                         self.X.order_known and Y.order_known)
+        self._is_transformed = True
+        return K
+
+    def diagonal(self):
+        """neighborhood_hash.py:343-365: the kernel's self similarities are 1."""
+        if self._is_transformed:
+            return 1.0, 1.0
+        return 1.0
+
+    def _nh_run(self, block, ids, codes, valid, n_fit, order_known=True):
+        """pack -> gk_nh_features (R hash levels, per-level columns) -> gk_gram (per-level Grams, fp64 combine).
+        `order_known`: the block's rows list every vertex's neighbours in the reference's edge-dictionary order."""
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
+            self.stats_ = eng.nh_features(self.R, self._nh_code, self.bits, codes, valid)
+            if self.stats_.nh_order_dependent and not order_known:
+                raise NotImplementedError(
+                    "NeighborhoodHash(nh_type='count_sensitive'): a vertex has two different neighbour codes with equal "
+                    "low bits, so its code depends on the neighbour order of the reference's edge sets, which a packed "
+                    "block does not carry; pass the list of graphs instead")
+            K, _, _ = eng.gram(block.n_graphs, n_fit=n_fit, stats=self.stats_, want_diag=False)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K

@@ -220,7 +220,7 @@ _INT_TYPES = {int, np.int64, np.int32}
 _NUM_TYPES = {int, float, bool, np.float64, np.float32, np.int64, np.int32}
 
 
-def _fast_edge_dict(g, L, mode, need_labels):
+def _fast_edge_dict(g, L, mode, need_labels, keep_edge_order=False):
     """Vectorised packing of the common spelling {(u, v): w} with integer vertex symbols: every per-edge step
     runs inside C iterators (itertools / map / numpy.fromiter) instead of Python byte code.  Returns
     (n_vertices, src, dst, weights, label list) with the slow path's semantics, or None whenever anything is
@@ -263,7 +263,7 @@ def _fast_edge_dict(g, L, mode, need_labels):
                 lab_list = list(map(L.__getitem__, sv.tolist()))
             except KeyError:
                 return None
-    order = np.lexsort((dst, src))
+    order = np.argsort(src, kind="stable") if keep_edge_order else np.lexsort((dst, src))
     return n, src[order], dst[order], ww[order], lab_list
 
 
@@ -278,7 +278,7 @@ def _lengths_ok(X, len_ok):
 
 
 def pack(X, mode, need_labels=True, len_ok=lambda n: n in (2, 3), want_weights=False,
-         fw_zero_is_absent=False, attributes=False, type_error_msg=None):
+         fw_zero_is_absent=False, attributes=False, type_error_msg=None, keep_edge_order=False):
     """Pack an iterable of reference-style elements.
 
     mode = 'wl' : vertex set = the keys of the label dictionary (the reference walks
@@ -290,8 +290,11 @@ def pack(X, mode, need_labels=True, len_ok=lambda n: n in (2, 3), want_weights=F
                   adjacency input, the endpoints of the listed edges otherwise; labelled vertices
                   without any edge never reach the histogram
                   (weisfeiler_lehman_optimal_assignment.py:179, 203-209).
+
+    keep_edge_order: a vertex's neighbours stay in the order of the reference's edge dictionary (first listing of
+    each edge; ascending columns for adjacency input) instead of ascending vertex id.
     """
-    if (_fastpack is not None and type(X) is list and X and not attributes and not fw_zero_is_absent
+    if (_fastpack is not None and type(X) is list and X and not attributes and not fw_zero_is_absent and not keep_edge_order
             and _lengths_ok(X, len_ok)):
         # whole-input fast path: {(u, v): w} graphs with integer symbols, walked with the CPython API on several
         # threads; it declines (None) on anything unusual and the general loop below decides -- and raises -- as before
@@ -319,7 +322,7 @@ def pack(X, mode, need_labels=True, len_ok=lambda n: n in (2, 3), want_weights=F
         base = graph_ptr[-1]
         fast = None
         if type(g) is dict and not attributes and not fw_zero_is_absent:
-            fast = _fast_edge_dict(g, L, mode, need_labels)
+            fast = _fast_edge_dict(g, L, mode, need_labels, keep_edge_order)
         if fast is not None:
             all_adjacency = False
             verts_n, ii, jj, ww, lab_list = fast
@@ -417,7 +420,7 @@ def pack(X, mode, need_labels=True, len_ok=lambda n: n in (2, 3), want_weights=F
             ii = np.asarray(src, dtype=np.int64)
             jj = np.asarray(dst, dtype=np.int64)
             ww = np.asarray(ww, dtype=np.float64)
-            order = np.lexsort((jj, ii))
+            order = np.argsort(ii, kind="stable") if keep_edge_order else np.lexsort((jj, ii))
             ii, jj, ww = ii[order], jj[order], ww[order]
             counts = np.bincount(ii, minlength=verts_n) if len(ii) else np.zeros(verts_n, dtype=np.int64)
             rp_parts.append(deg_total + np.cumsum(counts))

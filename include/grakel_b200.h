@@ -104,7 +104,8 @@ typedef struct gk_stats {
   int64_t hash_retries;      /* WL: relabel passes repeated after a detected hash collision */
   int64_t gram_path;         /* 1 = wgmma tensor-core GEMM over the integer panel (u8 or bf16: gemm_elem_bytes), 2 = exact int64 CUDA-core Gram, 3 = no contracted columns,
                                 ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram,
-                                GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram */
+                                GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram,
+                                NeighborhoodHash: 7 = one exact integer Gram per level + the fp64 combine */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -112,6 +113,12 @@ typedef struct gk_stats {
   int64_t gemm_elem_bytes;   /* element bytes of the integer head panel the tensor-core GEMM (gram_path 1) read:
                                 1 = u8 (u8 x u8 -> s32 wgmma, every count <= 255), 2 = bf16 (a count of 256, or
                                 GRAKEL_B200_U8=0), 0 = no integer tensor-core GEMM ran */
+  /* NeighborhoodHash: gk_nh_features' hash levels and per-level columns + unary expansion; gk_gram's combine and
+     the integer Gram of every level */
+  float ms_hash, ms_columns, ms_combine;
+  float ms_level_gram[64];
+  int64_t nh_order_dependent; /* NeighborhoodHash, count sensitive: some vertex had two different neighbour codes with
+                                 equal low `bits` bits, so its code depended on the order of its neighbours */
 } gk_stats;
 
 int gk_version(void);
@@ -164,6 +171,25 @@ int gk_wl_oa_features(gk_handle* h, int32_t n_iter, gk_stats* stats);
 int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, gk_stats* stats);
 /* graph g's maps after gk_gh_features: out[n * delta * delta], M[v][a][b] at (v * delta + a) * delta + b */
 int gk_gh_node_maps(gk_handle* h, int64_t g, double* out);
+
+/* NeighborhoodHash (neighborhood_hash.py:14-570): R levels of neighbourhood hashing of u64 codes over the
+ * out-neighbours of the packed block, level 0 hashing the initial codes.  The packed label ids index
+ * code_of_label[n_labels] (the initial code of every label id) and label_valid[n_labels] (0 = None: a label unseen at
+ * fit; NULL = all valid).  bits in [1, 64] (masked rotations as in the reference's ROT).  A vertex whose code or any
+ * neighbour's code is None is None.  Count sensitive: runs of equal codes after a stable sort of each row by the low
+ * `bits` bits, as the reference's radix_sort_rot -- so each row must list its neighbours in the order of the
+ * reference's edge dictionary.  Every level's non-None codes become one unary-expanded count block of its own.
+ * stats: level_dims[r] = distinct codes of level r, n_columns = expanded columns of all levels, ms_hash / ms_columns.
+ * gk_gram then returns K_ij = sum(t_r) / R (CPython's float sum) with t_r = c_r / (n_i + n_j - c_r), c_r the multiset
+ * intersection of the two graphs' non-None level-r codes and n the graphs' vertex counts (gram_path 7): fp64 only,
+ * host or GK_OUT_DEVICE output, n_fit and row ranges; xdiag / ydiag are 1; GK_NORMALIZE has no effect; GK_DIST and
+ * row maps are GK_ERR_UNSUPPORTED.  flags must be 0. */
+#define GK_NH_SIMPLE 0
+#define GK_NH_COUNT_SENSITIVE 1
+int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const uint64_t* code_of_label,
+                   const uint8_t* label_valid, int64_t n_labels, int32_t flags, gk_stats* stats);
+/* codes of level `level` (0 .. R-1) of every packed vertex after gk_nh_features: out[V] u64, valid[V] (may be NULL) */
+int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid);
 
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
