@@ -22,6 +22,9 @@ GK_SP_WITH_LABELS, GK_SP_KEEP_DIST, GK_SP_DIJKSTRA_ORDER = 1, 2, 4
 GK_ERR_RANGE, GK_ERR_UNSUPPORTED = -4, -5
 GK_GH_LINEAR, GK_GH_GAUSSIAN, GK_GH_BRIDGE = 0, 1, 2
 GK_NH_SIMPLE, GK_NH_COUNT_SENSITIVE = 0, 1
+GK_RW_CG, GK_RW_SPECTRAL, GK_RW_SERIES = 0, 1, 2
+GK_RW_FINITE, GK_RW_EXP, GK_RW_INV = 0, 1, 2
+GK_RW_LABELED = 1
 
 
 class GkStats(C.Structure):
@@ -38,6 +41,7 @@ class GkStats(C.Structure):
         ("gemm_elem_bytes", C.c_int64),
         ("ms_hash", C.c_float), ("ms_columns", C.c_float), ("ms_combine", C.c_float),
         ("ms_level_gram", C.c_float * 64), ("nh_order_dependent", C.c_int64),
+        ("ms_rw", C.c_float), ("rw_cap_hits", C.c_int64),
     ]
 
     def as_dict(self):
@@ -69,6 +73,9 @@ _SYMBOLS = {
     "gk_gh_node_maps": (C.c_int, [_P, C.c_int64, _P]),
     "gk_nh_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_int64, C.c_int32, C.POINTER(GkStats)]),
     "gk_nh_labels": (C.c_int, [_P, C.c_int32, _P, _P]),
+    "gk_rw_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_double, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32,
+                                 C.POINTER(GkStats)]),
+    "gk_rw_iterations": (C.c_int, [_P, _P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -288,6 +295,28 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_nh_labels(self.h, int(level), _ptr(out), _ptr(valid)))
         return out, valid.astype(bool)
+
+    def rw_features(self, route, fn, lamda, coef=None, values=None, t_row_ptr=None, t_col_idx=None, t_values=None,
+                    q=None, w=None, labeled=False):
+        """Random walk route of the packed block (gk_rw_features); the next gram() runs it pair by pair."""
+        cf = None if coef is None else np.ascontiguousarray(coef, dtype=np.float64)
+        f64 = lambda a: None if a is None else np.ascontiguousarray(a, dtype=np.float64)
+        vals, tv, qq, ww = f64(values), f64(t_values), f64(q), f64(w)
+        trp = None if t_row_ptr is None else _i32(t_row_ptr)
+        tci = None if t_col_idx is None else _i32(t_col_idx)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_rw_features(self.h, int(route), int(fn), float(lamda), _ptr(cf),
+                                                0 if cf is None else len(cf), _ptr(vals), _ptr(trp), _ptr(tci), _ptr(tv),
+                                                _ptr(qq), _ptr(ww), GK_RW_LABELED if labeled else 0, C.byref(st)))
+        return st
+
+    def rw_iterations(self, rows, cols):
+        """CG iterations / series terms of every entry of the last random walk gram() (rows x cols u8)."""
+        out = np.empty((rows, cols), dtype=np.uint8)
+        with self._lock:
+            self._check(self.lib.gk_rw_iterations(self.h, _ptr(out)))
+        return out
 
     def gram(self, n_graphs, n_fit=None, normalize=False, nan_to_num=False, out=None, dtype=np.float64,
              row_range=None, simt=False, full_tiles=False, stats=None, want_diag=True, device_ptr=None, ld=0,

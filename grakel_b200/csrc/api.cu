@@ -27,6 +27,7 @@
 #include "wl_fused2.cuh"
 #include "wl_oa.cuh"
 #include "neighborhood_hash.cuh"
+#include "random_walk.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -325,7 +326,9 @@ int gk_destroy(gk_handle* h) {
                         &h->K, &h->K_stage, &h->wlf_buf, &h->row_map, &h->diag_rows, &h->oa_keys, &h->oa_cnt, &h->oa_colcnt, &h->wl_single,
                         &h->diag_frozen, &h->sp_lists, &h->wl_payload, &h->gram_dyn, &h->tb_cnt, &h->tb_ent, &h->tb_ovf,
                         &h->gh_M, &h->gh_ws, &h->gh_woff, &h->gh_gdiam, &h->gh_groups, &h->gh_pairs,
-                        &h->nh_codes, &h->nh_valid, &h->nh_blk, &h->nh_lut, &h->nh_tab, &h->nh_ws, &h->nh_cur, &h->nh_C};
+                        &h->nh_codes, &h->nh_valid, &h->nh_blk, &h->nh_lut, &h->nh_tab, &h->nh_ws, &h->nh_cur, &h->nh_C,
+                        &h->rw_val, &h->rw_trp, &h->rw_tci, &h->rw_tval, &h->rw_q, &h->rw_w, &h->rw_coef, &h->rw_ws,
+                        &h->rw_iters, &h->rw_cap};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -2171,6 +2174,212 @@ static int gram_nh(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin
 }
 
 // ---------------------------------------------------------------------------
+// Random walk kernels (random_walk.cuh).  gk_rw_features uploads what the route reads; gk_gram (gram_rw) runs one CTA
+// per graph pair.
+int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const double* coef, int32_t n_coef,
+                   const double* values, const int32_t* t_row_ptr, const int32_t* t_col_idx, const double* t_values,
+                   const double* q, const double* w, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_rw_features: no graphs packed");
+  if (route != GK_RW_CG && route != GK_RW_SPECTRAL && route != GK_RW_SERIES) return fail(GK_ERR_ARG, "gk_rw_features: unknown route");
+  if (fn != GK_RW_FINITE && fn != GK_RW_EXP && fn != GK_RW_INV) return fail(GK_ERR_ARG, "gk_rw_features: unknown fn");
+  if (flags & ~GK_RW_LABELED) return fail(GK_ERR_ARG, "gk_rw_features: unknown flags");
+  if ((flags & GK_RW_LABELED) && !h->has_labels) return fail(GK_ERR_ARG, "gk_rw_features: GK_RW_LABELED needs packed labels");
+  if (fn == GK_RW_FINITE && (!coef || n_coef < 1)) return fail(GK_ERR_ARG, "gk_rw_features: the finite series needs coefficients");
+  if (route == GK_RW_SPECTRAL && (!q || !w)) return fail(GK_ERR_ARG, "gk_rw_features: the spectral route needs q and w");
+  if (route == GK_RW_SPECTRAL && (flags & GK_RW_LABELED)) return fail(GK_ERR_UNSUPPORTED, "gk_rw_features: no labelled spectral route");
+  if (route == GK_RW_CG && fn != GK_RW_INV) return fail(GK_ERR_ARG, "gk_rw_features: conjugate gradients solve the geometric kernel (GK_RW_INV)");
+  if (route == GK_RW_SERIES && fn == GK_RW_INV) return fail(GK_ERR_UNSUPPORTED, "gk_rw_features: no series for the geometric inverse");
+  if (route != GK_RW_SPECTRAL && h->E > 0 && (!values || !t_row_ptr || !t_col_idx || !t_values))
+    return fail(GK_ERR_ARG, "gk_rw_features: edge values and the transposed CSR are required");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t V = h->V, E = h->E;
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  if (route != GK_RW_SPECTRAL) {
+    GK_TRY(h->rw_val.ensure(std::max<int64_t>(E, 1) * 8));
+    GK_TRY(h->rw_tval.ensure(std::max<int64_t>(E, 1) * 8));
+    GK_TRY(h->rw_tci.ensure(std::max<int64_t>(E, 1) * 4));
+    GK_TRY(h->rw_trp.ensure((V + 1) * 4));
+    if (t_row_ptr) {
+      if (t_row_ptr[0] != 0 || t_row_ptr[V] != E) return fail(GK_ERR_ARG, "gk_rw_features: transposed row_ptr does not match the packed block");
+      GK_CUDA(cudaMemcpyAsync(h->rw_trp.p, t_row_ptr, (V + 1) * 4, cudaMemcpyHostToDevice, h->stream));
+    } else {
+      GK_CUDA(cudaMemsetAsync(h->rw_trp.p, 0, (V + 1) * 4, h->stream));
+    }
+    if (E) {
+      GK_CUDA(cudaMemcpyAsync(h->rw_val.p, values, E * 8, cudaMemcpyHostToDevice, h->stream));
+      GK_CUDA(cudaMemcpyAsync(h->rw_tval.p, t_values, E * 8, cudaMemcpyHostToDevice, h->stream));
+      GK_CUDA(cudaMemcpyAsync(h->rw_tci.p, t_col_idx, E * 4, cudaMemcpyHostToDevice, h->stream));
+    }
+  } else {
+    GK_TRY(h->rw_q.ensure(std::max<int64_t>(V, 1) * 8));
+    GK_TRY(h->rw_w.ensure(std::max<int64_t>(V, 1) * 8));
+    if (V) {
+      GK_CUDA(cudaMemcpyAsync(h->rw_q.p, q, V * 8, cudaMemcpyHostToDevice, h->stream));
+      GK_CUDA(cudaMemcpyAsync(h->rw_w.p, w, V * 8, cudaMemcpyHostToDevice, h->stream));
+    }
+  }
+  h->rw_ncoef = fn == GK_RW_FINITE ? n_coef : 0;
+  if (h->rw_ncoef) {
+    GK_TRY(h->rw_coef.ensure((size_t)n_coef * 8));
+    GK_CUDA(cudaMemcpyAsync(h->rw_coef.p, coef, (size_t)n_coef * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  GK_TRY(h->rw_cap.ensure(8));
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffers may be reused once we return
+  h->rw_route = route; h->rw_fn = fn; h->rw_lamda = lamda;
+  h->rw_labeled = (flags & GK_RW_LABELED) != 0;
+  h->feature_kind = 6;
+  h->features_ready = true; h->feat_serial++;
+  if (stats) {
+    stats->n_graphs = h->N; stats->n_vertices = V; stats->n_edges = E;
+    stats->ms_h2d = ev_ms(h->tev[0], h->tev[1]);
+  }
+  return GK_OK;
+}
+
+int gk_rw_iterations(gk_handle* h, uint8_t* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_rw_iterations: null argument");
+  if (h->feature_kind != 6 || h->rw_iter_rows * h->rw_iter_cols == 0) return fail(GK_ERR_STATE, "gk_rw_iterations: no random walk Gram yet");
+  GK_CUDA(cudaSetDevice(h->dev));
+  GK_CUDA(cudaMemcpyAsync(out, h->rw_iters.p, (size_t)(h->rw_iter_rows * h->rw_iter_cols), cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+// Launch rw_pairs over `n_pairs` pairs: the iteration vectors in shared memory when `vec_elems` doubles fit, else in
+// a global workspace slice per CTA.
+static int rw_launch(gk_handle* h, RwParams p, size_t vec_elems) {
+  if (p.n_pairs <= 0) return GK_OK;
+  const size_t bytes = vec_elems * 8;
+  int grid;
+  size_t smem = 0;
+  if (bytes <= RW_SMEM_MAX) {
+    smem = bytes;
+    GK_CUDA(cudaFuncSetAttribute(rw_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
+    int per_sm = 0;
+    GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rw_pairs, RW_THREADS, smem));
+    grid = h->sm_count * std::max(per_sm, 1);
+    p.ws = nullptr;
+  } else {
+    grid = h->sm_count * 2;
+    GK_TRY(h->rw_ws.ensure((size_t)grid * bytes));
+    p.ws = h->rw_ws.as<double>();
+    p.ws_stride = (long long)vec_elems;
+  }
+  grid = (int)std::min<long long>(grid, p.n_pairs);
+  rw_pairs<<<grid, RW_THREADS, smem, h->stream>>>(p);
+  LAUNCH_CHECK(h);
+  return GK_OK;
+}
+
+// Gram of the random walk kernels (gram_path 8 conjugate gradients, 9 spectral, 10 power series): fp64, host or
+// GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges.  Self similarities come from the same pair kernel, so a
+// square K's diagonal equals them bit for bit.  The full square case computes the upper triangle and mirrors it.
+static int gram_rw(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
+                   int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
+  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "random walk Gram is fp64 only");
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N;
+  const bool square = n_fit == N;
+  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
+  if (row_end < 0) row_end = k_rows_total;
+  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
+  const int64_t k_rows = row_end - row_begin;
+  if (ld <= 0) ld = k_cols;
+  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
+  const bool dev_out = (flags & GK_OUT_DEVICE) != 0;
+  if (dev_out && !K_out) return fail(GK_ERR_ARG, "gk_gram: GK_OUT_DEVICE without a pointer");
+  const int64_t launches0 = h->launches;
+  double* d_out;
+  int64_t d_ld;
+  if (dev_out) {
+    d_out = reinterpret_cast<double*>(K_out);
+    d_ld = ld;
+  } else {
+    GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
+    h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
+    d_out = h->K.as<double>();
+    d_ld = k_cols;
+  }
+  GK_TRY(h->diag_f64.ensure((size_t)N * 8));
+  GK_TRY(h->rw_iters.ensure((size_t)std::max<int64_t>(k_rows * k_cols, 1)));
+  GK_CUDA(cudaMemsetAsync(h->rw_cap.p, 0, 8, h->stream));
+  // largest vertex count among the row graphs and among the column graphs: the vectors of the largest pair
+  const int64_t g_row0 = (square ? 0 : n_fit) + row_begin, g_row1 = (square ? 0 : n_fit) + row_end;
+  auto max_n = [&](int64_t g0, int64_t g1) {
+    int m = 0;
+    for (int64_t g = g0; g < g1; ++g) m = std::max(m, ex->graph_ptr[g + 1] - ex->graph_ptr[g]);
+    return (size_t)m;
+  };
+  const size_t nmax_all = max_n(0, N);
+  const int nvec = h->rw_route == GK_RW_CG ? 3 : h->rw_route == GK_RW_SERIES ? 2 : 0;
+  RwParams p;
+  memset(&p, 0, sizeof(p));
+  p.graph_ptr = h->graph_ptr.as<int>();
+  p.row_ptr = h->row_ptr.as<int>(); p.col_idx = h->col_idx.as<int>(); p.val = h->rw_val.as<double>();
+  p.trow_ptr = h->rw_trp.as<int>(); p.tcol_idx = h->rw_tci.as<int>(); p.tval = h->rw_tval.as<double>();
+  p.labels = h->rw_labeled ? h->labels0.as<int>() : nullptr;
+  p.q = h->rw_q.as<double>(); p.w = h->rw_w.as<double>();
+  p.coef = h->rw_coef.as<double>(); p.n_coef = h->rw_ncoef;
+  p.lamda = h->rw_lamda;
+  p.route = h->rw_route; p.fn = h->rw_fn;
+  p.cap_hits = h->rw_cap.as<unsigned long long>();
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  // self similarities of every graph
+  {
+    RwParams d = p;
+    d.pairs = RW_PAIRS_DIAG;
+    d.n_pairs = N;
+    d.out = h->diag_f64.as<double>();
+    GK_TRY(rw_launch(h, d, (size_t)nvec * nmax_all * nmax_all));
+  }
+  const bool mirror = square && row_begin == 0 && row_end == N && !(flags & GK_FULL_TILES);
+  if (k_rows > 0) {
+    RwParams k = p;
+    k.pairs = mirror ? RW_PAIRS_TRIANGLE : RW_PAIRS_RECT;
+    k.ordered = square ? 1 : 0;
+    k.n_pairs = mirror ? N * (N + 1) / 2 : k_rows * k_cols;
+    k.row_g0 = (int)g_row0;
+    k.rows = (int)k_rows; k.cols = (int)k_cols;
+    k.out = d_out; k.ld = d_ld;
+    k.iters = h->rw_iters.as<unsigned char>();
+    const size_t nr = mirror ? nmax_all : max_n(g_row0, g_row1), nc = max_n(0, n_fit);
+    GK_TRY(rw_launch(h, k, (size_t)nvec * nr * nc));
+    if (flags & GK_NORMALIZE) {
+      normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(k_rows, k_cols, d_out, d_ld,
+                                                                      h->diag_f64.as<double>() + g_row0,
+                                                                      h->diag_f64.as<double>(), (flags & GK_NAN_TO_NUM) ? 1 : 0);
+      LAUNCH_CHECK(h);
+    }
+  }
+  h->rw_iter_rows = k_rows; h->rw_iter_cols = k_cols;
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  if (K_out && !dev_out && k_rows > 0)
+    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, d_out, (size_t)d_ld * 8, (size_t)k_cols * 8, (size_t)k_rows,
+                              cudaMemcpyDeviceToHost, h->stream));
+  if (xdiag) GK_CUDA(cudaMemcpyAsync(xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (ydiag && !square)
+    GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
+  unsigned long long cap_hits = 0;
+  GK_CUDA(cudaMemcpyAsync(&cap_hits, h->rw_cap.p, 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[4], h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->gram_path = h->rw_route == GK_RW_CG ? 8 : h->rw_route == GK_RW_SPECTRAL ? 9 : 10;
+    stats->gemm_tiles = mirror ? N * (N + 1) / 2 : k_rows * k_cols;
+    stats->gemm_launches = h->launches - launches0;
+    stats->ms_rw = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_gemm = stats->ms_rw;
+    stats->ms_d2h = ev_ms(h->tev[3], h->tev[4]);
+    stats->ms_total = stats->ms_rw + stats->ms_d2h;
+    stats->rw_cap_hits = (int64_t)cap_hits;
+  }
+  return GK_OK;
+}
+
+// ---------------------------------------------------------------------------
 }  // extern "C"
 
 // ---------------------------------------------------------------------------
@@ -2303,6 +2512,12 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with NeighborhoodHash features");
     GK_CUDA(cudaSetDevice(h->dev));
     return gram_nh(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
+  }
+  if (h->feature_kind == 6) {
+    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with random walk features");
+    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with random walk features");
+    GK_CUDA(cudaSetDevice(h->dev));
+    return gram_rw(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
   }
   const bool square = n_fit == N;
   const int64_t k_rows_total = square ? N : N - n_fit;

@@ -161,7 +161,8 @@ struct gk_handle {
   int64_t pro_serial = -1;   // feat_serial for which gk_wl_features already ran the Gram prologue (square case):
                              // self similarities finished, column histogram on the host -- gk_gram then needs no
                              // host synchronisation before its launches
-  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper, 5 = NeighborhoodHash
+  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper, 5 = NeighborhoodHash,
+                         // 6 = random walk
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
   // ---- columns / panel / diag
@@ -207,6 +208,13 @@ struct gk_handle {
   gk::DevBuf nh_lut, nh_tab, nh_ws, nh_cur, nh_C;
   size_t nh_level_bytes = 0;
   int nh_R = 0;
+
+  // ---- random walk (feature_kind 6): edge values of the packed CSR, its transpose, eigen-data, coefficients
+  gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;
+  int rw_route = 0, rw_fn = 0, rw_ncoef = 0;
+  double rw_lamda = 0.0;
+  bool rw_labeled = false;
+  int64_t rw_iter_rows = 0, rw_iter_cols = 0;  // shape of the iteration counts of the last gk_gram
 
   // ---- GEMM
   gk::DevBuf tiles;  // int2 list

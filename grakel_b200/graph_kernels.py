@@ -177,6 +177,11 @@ class GraphKernel(BaseEstimator, TransformerMixin):
             params[key] = val
         entry = _REGISTRY.get(name)
         if entry is None:
+            if name in ("random_walk", "RW"):
+                # GraphKernel's set of names is part of this package's interface and does not include the random walk
+                # kernels; they run on the device as estimators of their own
+                raise NotImplementedError("GraphKernel does not dispatch '" + str(name) + "': use "
+                                          "grakel_b200.RandomWalk, or RandomWalkLabeled for with_labels=True")
             if name in _OUTSIDE:
                 raise NotImplementedError("kernel '" + str(name) + "' is outside the device hot path of grakel_b200")
             raise ValueError("Unsupported kernel: " + str(name))

@@ -1254,3 +1254,327 @@ class NeighborhoodHash(Kernel):
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K
+
+
+# ------------------------------------------------------------------------------
+def _stacked_by_size(mats, fn):
+    """fn over every matrix of `mats`, called once per vertex count on the stacked (k, n, n) array: numpy's LAPACK
+    gufuncs run the same routine matrix by matrix, so the results equal per-matrix calls bit for bit."""
+    out = [None] * len(mats)
+    groups = {}
+    for i, A in enumerate(mats):
+        groups.setdefault(A.shape[0], []).append(i)
+    for n, idx in groups.items():
+        if n == 0:
+            for i in idx:
+                out[i] = None
+            continue
+        res = fn(np.stack([mats[i] for i in idx]))
+        for k, i in enumerate(idx):
+            out[i] = tuple(r[k] for r in res) if isinstance(res, tuple) else res[k]
+    return out
+
+
+def spectral_radii(mats):
+    """random_walk.py:139-144 (largest |eigenvalue| of numpy.linalg.eigvals, 0 for an empty graph), stacked by size."""
+    ev = _stacked_by_size(mats, np.linalg.eigvals)
+    return [0.0 if e is None else float(np.max(np.absolute(e))) for e in ev]
+
+
+def _eigen_data(mats, symmetric):
+    """Per-vertex (q, w) of every graph, concatenated: (real(1^T V), real(w)) of numpy.linalg.eig as the reference's
+    `sd` (random_walk.py:548-553), or of numpy.linalg.eigh for the symmetric inverse."""
+    res = _stacked_by_size(mats, np.linalg.eigh if symmetric else np.linalg.eig)
+    qs, ws = [], []
+    for r in res:
+        if r is None:
+            continue
+        w, v = r
+        qs.append(np.real(np.sum(v, axis=0)))
+        ws.append(np.real(w))
+    if not qs:
+        return np.zeros(0), np.zeros(0)
+    return np.concatenate(qs), np.concatenate(ws)
+
+
+_RW_ELEMENT_MSG = "each element of X must be either a graph or an iterable with at least 1 and at most 3 elements\n"
+_RWL_ELEMENT_MSG = "each element of X must be either a graph or an iterable with at least 2 and at most 3 elements\n"
+
+
+class RandomWalk(Kernel):
+    """Random walk kernel (random_walk.py:28-341; Gaertner et al. 2003, Vishwanathan et al. 2010).
+
+    Same parameters, attributes (`mu_`, `_lamda`), errors and warnings as the reference, including the lowering of
+    lamda at fit time when the geometric series would diverge.  Every pair runs on the device in fp64:
+    method_type="fast" with the geometric kernel replays scipy's conjugate gradients per pair; the fast spectral
+    variants and the baseline geometric kernel on symmetric matrices sum over the eigen-pairs of both graphs (computed on
+    the host with numpy, as the reference does); the baseline finite series and exponential run as power series of
+    matvecs.  The baseline geometric kernel of a non-symmetric matrix raises NotImplementedError, as does the baseline
+    exponential kernel on a matrix with a negative entry."""
+
+    _graph_format = "adjacency"
+    _labeled = False
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, lamda=0.1, method_type="fast",
+                 kernel_type="geometric", p=None):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.method_type = method_type
+        self.kernel_type = kernel_type
+        self.p = p
+        self.lamda = lamda
+        self._initialized.update({"method_type": False, "kernel_type": False, "p": False, "lamda": False})
+
+    def initialize(self):
+        """random_walk.py:81-133, in its order: method_type, kernel_type, p (mu_), lamda."""
+        super().initialize()
+        if not self._initialized["method_type"]:
+            if self.method_type not in ("baseline", "fast"):
+                raise ValueError("unsupported method_type")
+            self._initialized["method_type"] = True
+        if not self._initialized["kernel_type"]:
+            if self.kernel_type not in ["geometric", "exponential"]:
+                raise ValueError('unsupported kernel type: either "geometric" or "exponential"')
+        if not self._initialized["p"]:
+            if self.p is not None:
+                if type(self.p) is int and self.p > 0:
+                    self.mu_ = [1]
+                    fact, power = 1, 1
+                    for k in range(1, self.p + 1):
+                        power *= self.lamda
+                        if self.kernel_type == "exponential":
+                            fact *= k
+                            self.mu_.append(power / fact)
+                        else:
+                            self.mu_.append(power)
+                else:
+                    raise TypeError("p must be a positive integer bigger than zero or nonetype")
+                self._initialized["kernel_type"] = True
+        if not self._initialized["lamda"]:
+            if self.lamda <= 0:
+                raise TypeError("lambda must be positive bigger than equal")
+            self._lamda = self.lamda
+            self._initialized["lamda"] = True
+
+    _lamda_safety = 0.9
+
+    def _tune_lamda(self, spectral_radii):
+        """random_walk.py:146-194: keep the geometric series convergent on the graphs given."""
+        if self.kernel_type != "geometric" or self.p is not None:
+            return
+        if not spectral_radii:
+            return
+        rho = max(spectral_radii)
+        if rho <= 0:
+            return
+        limit = 1.0 / (rho ** 2)
+        if self._method_calling in (1, 2):
+            if self.lamda >= limit:
+                self._lamda = self._lamda_safety * limit
+                warnings.warn(
+                    'lamda=' + repr(self.lamda) + ' makes the random walk '
+                    'series diverge on these graphs, whose largest spectral '
+                    'radius is ' + format(rho, '.4g') + ': convergence needs '
+                    'lamda < ' + format(limit, '.4g') + '. Using lamda=' +
+                    format(self._lamda, '.4g') + ' instead. Pass a smaller '
+                    'lamda, or p=<int> for a fixed number of steps, to '
+                    'silence this.', RuntimeWarning)
+        else:
+            if self._lamda >= limit:
+                warnings.warn(
+                    'the graphs passed to transform have a larger spectral '
+                    'radius (' + format(rho, '.4g') + ') than the fitted '
+                    'ones, so lamda=' + format(self._lamda, '.4g') + ' no '
+                    'longer converges on them (it needs to stay below ' +
+                    format(limit, '.4g') + '). Refit with a smaller lamda: it '
+                    'cannot be changed now without invalidating the fit.',
+                    RuntimeWarning)
+
+    def _warn_unnormalizable(self, *diagonals):
+        """kernel.py:206-234, with the negative-self-similarity message written for the random walk kernels."""
+        name = type(self).__name__
+        for d in diagonals:
+            d = np.asarray(d, dtype=float)
+            if np.any(d < 0):
+                warnings.warn(
+                    name + ' has negative self similarities, so normalizing '
+                    'it yields NaNs: k(G, G) < 0 means the kernel is not '
+                    'positive semi-definite on this input. For the random '
+                    'walk kernels this usually means the decay factor is too '
+                    'large for these graphs -- it has to stay below 1 over '
+                    'the largest eigenvalue of the product graph adjacency '
+                    'matrix. Either lower it or pass normalize=False.',
+                    RuntimeWarning)
+                break
+            if np.any(d == 0):
+                warnings.warn(
+                    name + ' has zero self similarities, so normalizing it '
+                    'yields NaNs: those graphs have no features this kernel '
+                    'can see. Either drop them or pass normalize=False.',
+                    RuntimeWarning)
+                break
+
+    # ---- route
+    def _route(self):
+        """(route, fn) of random_walk.py:272-341 (RandomWalkLabeled: :491-541)."""
+        fast, geo = self.method_type == "fast", self.kernel_type == "geometric"
+        if self._labeled:
+            if fast and geo and self.p is None:
+                return _lib.GK_RW_CG, _lib.GK_RW_INV
+            if self.p is not None:
+                return _lib.GK_RW_SERIES, _lib.GK_RW_FINITE
+            if not geo:
+                return _lib.GK_RW_SERIES, _lib.GK_RW_EXP
+            raise NotImplementedError("RandomWalkLabeled(method_type='baseline', kernel_type='geometric', p=None): the "
+                                      "inverse of the product graph matrix is not computed on the device")
+        if fast:
+            if self.p is None and geo:
+                return _lib.GK_RW_CG, _lib.GK_RW_INV
+            return _lib.GK_RW_SPECTRAL, (_lib.GK_RW_FINITE if self.p is not None else _lib.GK_RW_EXP)
+        if self.p is not None:
+            return _lib.GK_RW_SERIES, _lib.GK_RW_FINITE
+        if not geo:
+            return _lib.GK_RW_SERIES, _lib.GK_RW_EXP
+        return _lib.GK_RW_SPECTRAL, _lib.GK_RW_INV
+
+    # ---- input
+    def _elements(self, X):
+        """(adjacency matrix, labels in index order or None) of every element (random_walk.py:215-244, 423-448)."""
+        from .packing import adjacency_and_labels
+        if isinstance(X, Block):  # datasets.read_tu: the kernel's vertices are the nodes that occur in an edge
+            X.require("sp", labels=self._labeled)
+            out = []
+            gp, rp, ci = X.graph_ptr, X.row_ptr, X.col_idx
+            for g in range(X.n_graphs):
+                a, b = int(gp[g]), int(gp[g + 1])
+                A = np.zeros((b - a, b - a))
+                for u in range(a, b):
+                    e0, e1 = int(rp[u]), int(rp[u + 1])
+                    A[u - a, ci[e0:e1] - a] = 1.0 if X.weights is None else X.weights[e0:e1]
+                out.append((A, list(X.labels[a:b]) if self._labeled else None))
+            return out
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            ok = (1, 2, 3) if self._labeled else (0, 1, 2, 3)
+            if not (is_iter and len(x) in ok):
+                raise TypeError(_RWL_ELEMENT_MSG if self._labeled else _RW_ELEMENT_MSG)
+            if len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            out.append(adjacency_and_labels(x[0], x[1] if self._labeled else None))
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    def parse_input(self, X):
+        import time
+        els = self._elements(X)
+        mats = [A for A, _ in els]
+        t0 = time.perf_counter()
+        if self.kernel_type == "geometric" and self.p is None:
+            self._tune_lamda(spectral_radii(mats))
+        route, fn = self._route()
+        fitted = Fitted(None, None, {})
+        fitted.mats = mats
+        fitted.labels = [L for _, L in els]
+        fitted.q = fitted.w = None
+        if route == _lib.GK_RW_SPECTRAL:
+            symmetric = fn == _lib.GK_RW_INV
+            if symmetric and not all(np.array_equal(A, A.T) for A in mats):
+                raise NotImplementedError("RandomWalk(method_type='baseline', kernel_type='geometric', p=None) is "
+                                          "computed from the eigen-decomposition of symmetric adjacency matrices only")
+            fitted.q, fitted.w = _eigen_data(mats, symmetric)
+        elif route == _lib.GK_RW_SERIES and fn == _lib.GK_RW_EXP and any(np.any(A < 0) for A in mats):
+            raise NotImplementedError("the baseline exponential random walk kernel is summed as a power series, which "
+                                      "needs non-negative adjacency entries")
+        self.ms_host_eig_ = (time.perf_counter() - t0) * 1e3
+        return fitted
+
+    @staticmethod
+    def _concat(a, b):
+        out = Fitted(None, None, {})
+        out.mats = a.mats + b.mats
+        out.labels = a.labels + b.labels
+        out.q = None if a.q is None else np.concatenate([a.q, b.q])
+        out.w = None if a.w is None else np.concatenate([a.w, b.w])
+        return out
+
+    # ---- estimator protocol
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        K, xdiag, _ = self._rw_run(self.X, len(self.X.mats))
+        self._X_diag = xdiag
+        if self.normalize:
+            self._warn_unnormalizable(xdiag)
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        Y = self.parse_input(X)
+        K, xdiag, ydiag = self._rw_run(self._concat(self.X, Y), len(self.X.mats))
+        self._X_diag, self._Y_diag = xdiag, ydiag
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xdiag, ydiag)
+        return K
+
+    def diagonal(self):
+        check_is_fitted(self, ["X"])
+        try:
+            check_is_fitted(self, ["_X_diag"])
+        except NotFittedError:
+            _, self._X_diag, _ = self._rw_run(self.X, len(self.X.mats), want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
+
+    def _rw_run(self, data, n_fit, want_matrix=True, device_ptr=None):
+        """pack the structure -> gk_rw_features -> gk_gram.  Returns (K, xdiag, ydiag)."""
+        route, fn = self._route()
+        mats = data.mats
+        sizes = np.array([A.shape[0] for A in mats], dtype=np.int64)
+        gp = np.concatenate([[0], np.cumsum(sizes)])
+        rows, cols, vals, trows, tcols, tvals = [], [], [], [], [], []
+        for g, A in enumerate(mats):
+            ii, jj = np.nonzero(A)
+            rows.append(ii + gp[g]); cols.append(jj + gp[g]); vals.append(A[ii, jj])
+            ti, tj = np.nonzero(A.T)
+            trows.append(ti + gp[g]); tcols.append(tj + gp[g]); tvals.append(A.T[ti, tj])
+        cat = lambda parts, dt: np.concatenate(parts).astype(dt) if parts else np.zeros(0, dt)
+        V = int(gp[-1])
+        r, c, v = cat(rows, np.int64), cat(cols, np.int32), cat(vals, np.float64)
+        tr, tc, tv = cat(trows, np.int64), cat(tcols, np.int32), cat(tvals, np.float64)
+        rp = np.concatenate([[0], np.cumsum(np.bincount(r, minlength=V))])
+        trp = np.concatenate([[0], np.cumsum(np.bincount(tr, minlength=V))])
+        ids = None
+        if self._labeled:
+            ids, _ = label_ids([l for L in data.labels for l in L], None, sort_new=False)
+        coef = self.mu_ if fn == _lib.GK_RW_FINITE else None
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(gp, rp, c, ids, None, None)
+            eng.rw_features(route, fn, self._lamda, coef, v, trp, tc, tv, data.q, data.w, labeled=self._labeled)
+            self.stats_ = _lib.GkStats()
+            out = False if not want_matrix else None
+            K, xd, yd = eng.gram(len(mats), n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 out=out if device_ptr is None else None, device_ptr=device_ptr, stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd
+
+
+class RandomWalkLabeled(RandomWalk):
+    """Labelled random walk kernel (random_walk.py:343-541): walks of the product graph pair vertices with equal labels.
+    Conjugate gradients for the fast geometric kernel, power series for the finite and exponential variants; the
+    baseline geometric kernel with p=None raises NotImplementedError."""
+
+    _labeled = True

@@ -453,6 +453,32 @@ def pack(X, mode, need_labels=True, len_ok=lambda n: n in (2, 3), want_weights=F
     return out
 
 
+def adjacency_and_labels(g, L=None):
+    """The reference's `Graph(g, L, {}, "adjacency").get_adjacency_matrix()` as float64 and, when L is given,
+    `get_labels(purpose="adjacency")` in index order (graph.py:912-1053, 1156-1179, 689-772): an adjacency input is taken
+    as it is -- every non-zero entry is an edge with its weight, negative ones and self-loops included -- and an edge
+    dictionary becomes the matrix over its sorted vertex symbols, every listed symbol a vertex (also one without an
+    edge), a later duplicate overwriting an earlier one.  The random walk kernels use this, not pack()."""
+    kind = classify(g)
+    if kind is None:
+        raise ValueError("Unsupported input type. For more information check the documentation, concerning "
+                         "valid input types for graph type object.")
+    if kind == "adjacency":
+        A = np.array(_adjacency_array(g), dtype=np.float64)
+        order = range(A.shape[0])
+    else:
+        verts, edges = _edges_of(g, kind)
+        order = sorted(verts)
+        loc = {k: i for i, k in enumerate(order)}
+        A = np.zeros((len(order), len(order)))
+        for (u, v), w in edges.items():
+            A[loc[u], loc[v]] = w
+    labels = None
+    if L is not None:
+        labels = [L[k] for k in order]
+    return A, labels
+
+
 def label_ids(labels, known=None, sort_new=True):
     """Dense ids for Python label objects.
 

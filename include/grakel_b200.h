@@ -105,7 +105,8 @@ typedef struct gk_stats {
   int64_t gram_path;         /* 1 = wgmma tensor-core GEMM over the integer panel (u8 or bf16: gemm_elem_bytes), 2 = exact int64 CUDA-core Gram, 3 = no contracted columns,
                                 ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram,
                                 GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram,
-                                NeighborhoodHash: 7 = one exact integer Gram per level + the fp64 combine */
+                                NeighborhoodHash: 7 = one exact integer Gram per level + the fp64 combine,
+                                random walk: 8 = conjugate gradients, 9 = spectral pair sum, 10 = power series */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -119,6 +120,10 @@ typedef struct gk_stats {
   float ms_level_gram[64];
   int64_t nh_order_dependent; /* NeighborhoodHash, count sensitive: some vertex had two different neighbour codes with
                                  equal low `bits` bits, so its code depended on the order of its neighbours */
+  /* random walk: device time of gk_gram's pair kernels (self similarities included), and the Taylor pairs that
+     stopped at the term cap before converging */
+  float ms_rw;
+  int64_t rw_cap_hits;
 } gk_stats;
 
 int gk_version(void);
@@ -190,6 +195,33 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
                    const uint8_t* label_valid, int64_t n_labels, int32_t flags, gk_stats* stats);
 /* codes of level `level` (0 .. R-1) of every packed vertex after gk_nh_features: out[V] u64, valid[V] (may be NULL) */
 int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid);
+
+/* RandomWalk / RandomWalkLabeled (random_walk.py:28-541), one graph pair per CTA in fp64.  The packed CSR gives the
+ * structure (gk_pack_csr without weights; with labels for GK_RW_LABELED), `values[E]` the adjacency entries of its
+ * edges (any sign, self-loops included), `t_row_ptr[V+1]` / `t_col_idx[E]` / `t_values[E]` the same block transposed
+ * (in-edges, GLOBAL vertex ids).  Routes:
+ *   GK_RW_CG        fn GK_RW_INV: scipy's cg(I - lamda M, 1, rtol=1e-6, maxiter=20) per pair, K = sum(x) (gram_path 8);
+ *                   M p = Ax P Ay with P the Fortran-order reshape of p, masked as the reference's label-pair sum
+ *   GK_RW_SPECTRAL  sum_ab (q_a q'_b)^2 f(w_a w'_b), q[V] / w[V] the per-graph eigen-data from the host (gram_path 9);
+ *                   fn GK_RW_FINITE (coef[n_coef] = mu_0..mu_p, the reference's D *= Dij; S += mu_k D), GK_RW_EXP
+ *                   exp(lamda z), GK_RW_INV 1 / (1 - lamda z); unlabelled only
+ *   GK_RW_SERIES    sum_k c_k 1^T M^k 1 with M = D kron(Ax, Ay) D (gram_path 10): fn GK_RW_FINITE (c_k = coef[k]) or
+ *                   GK_RW_EXP (c_k = lamda^k / k!, non-negative entries; pairs that reach the term cap are counted in
+ *                   stats->rw_cap_hits)
+ * gk_gram: fp64 only, host or GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges; GK_DIST and row maps are
+ * GK_ERR_UNSUPPORTED.  gk_rw_iterations copies the CG iterations / series terms of every entry of the last K
+ * (rows x cols u8, row-major). */
+#define GK_RW_CG 0
+#define GK_RW_SPECTRAL 1
+#define GK_RW_SERIES 2
+#define GK_RW_FINITE 0
+#define GK_RW_EXP 1
+#define GK_RW_INV 2
+#define GK_RW_LABELED 1 /* gk_rw_features flag: RandomWalkLabeled (the packed labels mask the product graph) */
+int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const double* coef, int32_t n_coef,
+                   const double* values, const int32_t* t_row_ptr, const int32_t* t_col_idx, const double* t_values,
+                   const double* q, const double* w, int32_t flags, gk_stats* stats);
+int gk_rw_iterations(gk_handle* h, uint8_t* out);
 
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
