@@ -25,6 +25,7 @@ GK_NH_SIMPLE, GK_NH_COUNT_SENSITIVE = 0, 1
 GK_RW_CG, GK_RW_SPECTRAL, GK_RW_SERIES = 0, 1, 2
 GK_RW_FINITE, GK_RW_EXP, GK_RW_INV = 0, 1, 2
 GK_RW_LABELED = 1
+GK_PK_ATTR, GK_PK_SQRT, GK_PK_STORE_F32, GK_PK_STORE_INT, GK_PK_NEW_LABELS = 1, 2, 4, 8, 16
 
 
 class GkStats(C.Structure):
@@ -42,6 +43,7 @@ class GkStats(C.Structure):
         ("ms_hash", C.c_float), ("ms_columns", C.c_float), ("ms_combine", C.c_float),
         ("ms_level_gram", C.c_float * 64), ("nh_order_dependent", C.c_int64),
         ("ms_rw", C.c_float), ("rw_cap_hits", C.c_int64),
+        ("ms_propagate", C.c_float), ("pk_near_edge", C.c_int64),
     ]
 
     def as_dict(self):
@@ -76,6 +78,9 @@ _SYMBOLS = {
     "gk_rw_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_double, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_rw_iterations": (C.c_int, [_P, _P]),
+    "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
+                                 C.POINTER(GkStats)]),
+    "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -310,6 +315,27 @@ class Engine:
                                                 0 if cf is None else len(cf), _ptr(vals), _ptr(trp), _ptr(tci), _ptr(tv),
                                                 _ptr(qq), _ptr(ww), GK_RW_LABELED if labeled else 0, C.byref(st)))
         return st
+
+    def pk_features(self, t_max, w, u, b, dim, dim_orig, n_fit, t_values, p0=None, flags=0):
+        """Propagation bins of t_max levels and their (graph, column) counts (gk_pk_features).  u: [t_max, dim],
+        b: [t_max] or [t_max, dim] (GK_PK_ATTR), t_values[E]: the packed CSR's transition entries, p0: [V, dim]."""
+        u = np.ascontiguousarray(u, dtype=np.float64)
+        b = np.ascontiguousarray(b, dtype=np.float64)
+        tv = np.ascontiguousarray(t_values, dtype=np.float64)
+        p = None if p0 is None else np.ascontiguousarray(p0, dtype=np.float64)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_pk_features(self.h, int(t_max), float(w), _ptr(u), _ptr(b), int(dim), int(dim_orig),
+                                                int(n_fit), _ptr(tv), _ptr(p), int(flags), C.byref(st)))
+        return st
+
+    def pk_hashes(self, level, n_vertices, width=1):
+        """(bins [V, width] fp64, private flags [V] bool) of Propagation level `level`."""
+        out = np.empty((n_vertices, width), dtype=np.float64)
+        priv = np.empty(n_vertices, dtype=np.uint8)
+        with self._lock:
+            self._check(self.lib.gk_pk_hashes(self.h, int(level), _ptr(out), _ptr(priv)))
+        return out, priv.astype(bool)
 
     def rw_iterations(self, rows, cols):
         """CG iterations / series terms of every entry of the last random walk gram() (rows x cols u8)."""

@@ -28,6 +28,7 @@
 #include "wl_oa.cuh"
 #include "neighborhood_hash.cuh"
 #include "random_walk.cuh"
+#include "propagation.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -328,7 +329,8 @@ int gk_destroy(gk_handle* h) {
                         &h->gh_M, &h->gh_ws, &h->gh_woff, &h->gh_gdiam, &h->gh_groups, &h->gh_pairs,
                         &h->nh_codes, &h->nh_valid, &h->nh_blk, &h->nh_lut, &h->nh_tab, &h->nh_ws, &h->nh_cur, &h->nh_C,
                         &h->rw_val, &h->rw_trp, &h->rw_tci, &h->rw_tval, &h->rw_q, &h->rw_w, &h->rw_coef, &h->rw_ws,
-                        &h->rw_iters, &h->rw_cap};
+                        &h->rw_iters, &h->rw_cap,
+                        &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -2247,6 +2249,197 @@ int gk_rw_iterations(gk_handle* h, uint8_t* out) {
   return GK_OK;
 }
 
+// ---------------------------------------------------------------------------
+// Propagation (propagation.cuh).  The packed CSR is the sparsity pattern of the row-normalised transition matrices,
+// t_values[E] their entries; the features are the SP layout (feature_kind 7), so gk_gram's integer route runs them.
+int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const double* b, int32_t dim,
+                   int32_t dim_orig, int64_t n_fit, const double* t_values, const double* p0, int32_t flags,
+                   gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_pk_features: no graphs packed");
+  if (t_max < 1 || t_max > MAX_LEVELS) return fail(GK_ERR_ARG, "gk_pk_features: t_max out of range [1, 64]");
+  if (!(w != 0.0) || !std::isfinite(w)) return fail(GK_ERR_ARG, "gk_pk_features: w must be finite and non-zero");
+  if (flags & ~(GK_PK_ATTR | GK_PK_SQRT | GK_PK_STORE_F32 | GK_PK_STORE_INT | GK_PK_NEW_LABELS))
+    return fail(GK_ERR_ARG, "gk_pk_features: unknown flag");
+  const bool attr = flags & GK_PK_ATTR, split = flags & GK_PK_NEW_LABELS;
+  if ((flags & GK_PK_STORE_F32) && (flags & GK_PK_STORE_INT)) return fail(GK_ERR_ARG, "gk_pk_features: two storage modes");
+  if (attr && (split || (flags & GK_PK_SQRT))) return fail(GK_ERR_ARG, "gk_pk_features: GK_PK_SQRT / GK_PK_NEW_LABELS are for labels");
+  if (!attr && (flags & (GK_PK_STORE_F32 | GK_PK_STORE_INT))) return fail(GK_ERR_ARG, "gk_pk_features: storage modes are for attributes");
+  if (dim < 1 || dim_orig < 0 || dim_orig > dim || (!split && dim_orig != dim))
+    return fail(GK_ERR_ARG, "gk_pk_features: bad dim / dim_orig");
+  if (n_fit < 0 || n_fit > h->N) return fail(GK_ERR_ARG, "gk_pk_features: n_fit out of range");
+  if (!u || !b || (h->E && !t_values)) return fail(GK_ERR_ARG, "gk_pk_features: null argument");
+  if (attr && !p0 && h->V) return fail(GK_ERR_ARG, "gk_pk_features: attributes need p0");
+  if (!attr && !h->has_labels) return fail(GK_ERR_ARG, "gk_pk_features: vertex labels are required");
+  if (!attr && h->n_labels0 > dim) return fail(GK_ERR_ARG, "gk_pk_features: a label id is >= dim");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t N = h->N, V = h->V, E = h->E, V1 = std::max<int64_t>(V, 1);
+  const int K = attr ? dim : 1;
+  const int64_t launches0 = h->launches;
+  h->features_ready = false; h->feat_serial++;
+  h->pk_levels = 0;
+
+  // the dense P the reference also holds on the host: refuse clearly when it cannot fit
+  const size_t p_bytes = 2 * (size_t)V1 * dim * 8, bin_bytes = (size_t)t_max * V1 * K * 8;
+  size_t free_b = 0, total_b = 0;
+  GK_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  if (p_bytes + bin_bytes > free_b + h->pk_P.cap + h->pk_bins.cap)
+    return fail(GK_ERR_RANGE, "gk_pk_features: the dense V x D propagation matrix (" + std::to_string(p_bytes >> 20) +
+                                  " MiB double-buffered) and the bins (" + std::to_string(bin_bytes >> 20) +
+                                  " MiB) do not fit in device memory");
+  GK_TRY(h->pk_P.ensure(p_bytes));
+  GK_TRY(h->pk_bins.ensure(bin_bytes));
+  GK_TRY(h->pk_priv.ensure((size_t)t_max * V1));
+  GK_TRY(h->pk_tval.ensure((size_t)std::max<int64_t>(E, 1) * 8));
+  GK_TRY(h->pk_u.ensure((size_t)t_max * dim * 8));
+  GK_TRY(h->pk_b.ensure((size_t)t_max * K * 8));
+  GK_TRY(h->pk_cnt.ensure(24));  // [near-edge count u64 | NaN seen u32, pad | columns u64]
+  double* P0 = h->pk_P.as<double>();
+  double* P1 = P0 + (size_t)V1 * dim;
+  double* bins = h->pk_bins.as<double>();
+  unsigned char* priv = h->pk_priv.as<unsigned char>();
+  unsigned long long* near = h->pk_cnt.as<unsigned long long>();
+  unsigned* nan_seen = reinterpret_cast<unsigned*>(near + 1);
+  GK_CUDA(cudaMemsetAsync(h->pk_cnt.p, 0, 24, h->stream));
+  GK_CUDA(cudaMemsetAsync(priv, 0, (size_t)t_max * V1, h->stream));
+  if (E) GK_CUDA(cudaMemcpyAsync(h->pk_tval.p, t_values, (size_t)E * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->pk_u.p, u, (size_t)t_max * dim * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->pk_b.p, b, (size_t)t_max * K * 8, cudaMemcpyHostToDevice, h->stream));
+  if (attr) {
+    if (V) GK_CUDA(cudaMemcpyAsync(P0, p0, (size_t)V * dim * 8, cudaMemcpyHostToDevice, h->stream));
+  } else {
+    GK_CUDA(cudaMemsetAsync(P0, 0, (size_t)V1 * dim * 8, h->stream));
+    if (V) {
+      pk_onehot<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, dim, h->labels0.as<int>(), P0);
+      LAUNCH_CHECK(h);
+    }
+  }
+  const int store = (flags & GK_PK_STORE_F32) ? PK_STORE_F32 : (flags & GK_PK_STORE_INT) ? PK_STORE_INT : PK_STORE_F64;
+  HandleExtra* ex = extra_of(h);
+  const int v0 = ex->graph_ptr[n_fit];  // first vertex of the transformed graphs
+
+  // ---- levels: private flags, hash, propagate
+  std::vector<cudaEvent_t> pev(2 * (size_t)t_max, nullptr);
+  for (auto& e : pev) GK_CUDA(cudaEventCreate(&e));
+  struct EvGuard {
+    std::vector<cudaEvent_t>& v;
+    ~EvGuard() { for (auto e : v) if (e) cudaEventDestroy(e); }
+  } ev_guard{pev};
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  double* cur = P0;
+  double* nxt = P1;
+  const long long n_entries = (long long)V * dim;
+  const int prop_grid = (int)std::max<long long>(1, std::min<long long>(cdiv(n_entries, 256), (long long)h->sm_count * 16));
+  for (int t = 0; t < t_max && V; ++t) {
+    if (split) {
+      pk_private<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, v0, dim, dim_orig, t, h->labels0.as<int>(), cur,
+                                                      priv + (size_t)t * V);
+      LAUNCH_CHECK(h);
+    }
+    PkHashParams hp;
+    hp.V = (int)V; hp.D = dim; hp.attr = attr ? 1 : 0; hp.take_sqrt = (flags & GK_PK_SQRT) ? 1 : 0;
+    hp.dim_orig = dim_orig;
+    hp.P = cur;
+    hp.u = h->pk_u.as<double>() + (size_t)t * dim;
+    hp.b = h->pk_b.as<double>() + (size_t)t * K;
+    hp.w = w;
+    hp.priv = split ? priv + (size_t)t * V : nullptr;
+    hp.bins = bins + (size_t)t * V * K;
+    hp.near = near; hp.nan_seen = nan_seen;
+    pk_hash<<<cdiv(V, 256), 256, 0, h->stream>>>(hp);
+    LAUNCH_CHECK(h);
+    if (t + 1 < t_max) {
+      GK_CUDA(cudaEventRecord(pev[2 * t], h->stream));
+      pk_propagate<<<prop_grid, 256, 0, h->stream>>>(n_entries, dim, h->row_ptr.as<int>(), h->col_idx.as<int>(),
+                                                     h->pk_tval.as<double>(), cur, nxt, store, near);
+      LAUNCH_CHECK(h);
+      GK_CUDA(cudaEventRecord(pev[2 * t + 1], h->stream));
+      std::swap(cur, nxt);
+    }
+  }
+  GK_CUDA(cudaEventRecord(h->tev[5], h->stream));
+
+  // ---- per-level columns and (graph, column) counts
+  const size_t cap = std::max<size_t>(next_pow2((size_t)V1 * 2), 1024);
+  const size_t ft_cap = std::max<size_t>(next_pow2((size_t)t_max * (V1 + N) * 2), 1024);
+  if (ft_cap > (1ULL << 31)) return fail(GK_ERR_ARG, "gk_pk_features: feature table too large");
+  GK_TRY(h->pk_tab.ensure(cap * 8 + (size_t)V1 * 8));  // slot -> claiming vertex | slot -> column | vertex -> slot | ones
+  int* tab = h->pk_tab.as<int>();
+  int* colid = tab + cap;
+  int* slot_of = colid + cap;
+  unsigned char* ones = reinterpret_cast<unsigned char*>(slot_of + V1);
+  GK_TRY(h->ft_keys.ensure(ft_cap * 8));
+  GK_TRY(h->ft_cnt.ensure(ft_cap * 4));
+  h->ft_cap = ft_cap;
+  GK_TRY(init_scalars(h, 0));
+  const int nbv = cdiv(V1, 256);
+  FeatStats fst;
+  GK_TRY(reset_feature_stats(h, (int64_t)t_max * V1, 2LL * t_max * nbv, &fst));
+  GK_CUDA(cudaMemsetAsync(h->ft_keys.p, 0xFF, ft_cap * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->ft_cnt.p, 0, ft_cap * 4, h->stream));
+  GK_CUDA(cudaMemsetAsync(ones, 1, (size_t)V1, h->stream));
+  unsigned long long* n_cols_d = near + 2;
+  for (int t = 0; t < t_max && V; ++t) {
+    const double* bt = bins + (size_t)t * V * K;
+    const unsigned char* pt = split ? priv + (size_t)t * V : nullptr;
+    GK_CUDA(cudaMemsetAsync(tab, 0xFF, cap * 4, h->stream));
+    pk_code_insert<<<nbv, 256, 0, h->stream>>>((int)V, K, bt, pt, tab, (unsigned)(cap - 1), slot_of);
+    LAUNCH_CHECK(h);
+    nh_code_number<<<nbv, 256, 0, h->stream>>>((int)V, ones, tab, slot_of, colid, n_cols_d);
+    LAUNCH_CHECK(h);
+    pk_count<<<nbv, 256, 0, h->stream>>>((int)V, h->vgraph.as<int>(), h->graph_ptr.as<int>(), slot_of, colid,
+                                         h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
+                                         (unsigned)(ft_cap - 1), fst, t, split ? 1 : 0, (int)n_fit,
+                                         (size_t)t_max * nbv + (size_t)t * nbv);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  unsigned long long hc[3] = {0, 0, 0};
+  GK_CUDA(cudaMemcpyAsync(hc, h->pk_cnt.p, 24, cudaMemcpyDeviceToHost, h->stream));
+  DevScalars* hs;
+  GK_TRY(read_scalars(h, &hs));  // synchronises
+  if (hs->ft_overflow) return fail(GK_ERR_STATE, "gk_pk_features: feature table overflow");
+  if ((unsigned)hc[1]) return fail(GK_ERR_UNSUPPORTED, "gk_pk_features: a bin is NaN (sqrt of a negative entry, or a NaN "
+                                                       "input), which the reference cannot look up either");
+  h->n_columns = (int64_t)hc[2];
+  h->pk_levels = t_max;
+  h->pk_K = K;
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = 7;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
+    stats->n_levels = t_max;
+    stats->n_columns = h->n_columns;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_hash = ev_ms(h->tev[2], h->tev[5]);
+    stats->ms_columns = ev_ms(h->tev[5], h->tev[3]);
+    float mp = 0.f;
+    for (int t = 0; t + 1 < t_max && V; ++t) mp += ev_ms(pev[2 * t], pev[2 * t + 1]);
+    stats->ms_propagate = mp;
+    stats->pk_near_edge = (int64_t)hc[0];
+  }
+  return GK_OK;
+}
+
+int gk_pk_hashes(gk_handle* h, int32_t level, double* out, uint8_t* priv) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_pk_hashes: null argument");
+  if (h->feature_kind != 7 || !h->features_ready || level < 0 || level >= h->pk_levels)
+    return fail(GK_ERR_STATE, "gk_pk_hashes: no such level (run gk_pk_features first)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t V = (size_t)h->V, K = (size_t)h->pk_K;
+  if (V) {
+    GK_CUDA(cudaMemcpyAsync(out, h->pk_bins.as<double>() + (size_t)level * V * K, V * K * 8, cudaMemcpyDeviceToHost,
+                            h->stream));
+    if (priv)
+      GK_CUDA(cudaMemcpyAsync(priv, h->pk_priv.as<unsigned char>() + (size_t)level * V, V, cudaMemcpyDeviceToHost,
+                              h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  return GK_OK;
+}
+
 // Launch rw_pairs over `n_pairs` pairs: the iteration vectors in shared memory when `vec_elems` doubles fit, else in
 // a global workspace slice per CTA.
 static int rw_launch(gk_handle* h, RwParams p, size_t vec_elems) {
@@ -2518,6 +2711,10 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with random walk features");
     GK_CUDA(cudaSetDevice(h->dev));
     return gram_rw(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
+  }
+  if (h->feature_kind == 7) {  // Propagation: the generic integer route; the row map and distributed paths are untested
+    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with Propagation features");
+    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with Propagation features");
   }
   const bool square = n_fit == N;
   const int64_t k_rows_total = square ? N : N - n_fit;

@@ -162,7 +162,7 @@ struct gk_handle {
                              // self similarities finished, column histogram on the host -- gk_gram then needs no
                              // host synchronisation before its launches
   int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper, 5 = NeighborhoodHash,
-                         // 6 = random walk
+                         // 6 = random walk, 7 = Propagation (SP-layout integer features)
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
   // ---- columns / panel / diag
@@ -215,6 +215,11 @@ struct gk_handle {
   double rw_lamda = 0.0;
   bool rw_labeled = false;
   int64_t rw_iter_rows = 0, rw_iter_cols = 0;  // shape of the iteration counts of the last gk_gram
+
+  // ---- Propagation (feature_kind 7): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
+  // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]
+  gk::DevBuf pk_P, pk_bins, pk_priv, pk_tval, pk_u, pk_b, pk_tab, pk_cnt;
+  int pk_levels = 0, pk_K = 0;
 
   // ---- GEMM
   gk::DevBuf tiles;  // int2 list

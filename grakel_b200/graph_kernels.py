@@ -9,6 +9,7 @@ the kernels of the device hot path:
     "weisfeiler_lehman_optimal_assignment" / "WL-OA"
     "graph_hopper" / "GH"
     "neighborhood_hash" / "NH"
+    "propagation" / "PR"        (+ with_attributes: PropagationAttr)
 
 Any other reference kernel name raises NotImplementedError (not ValueError, which the reference reserves for
 unknown names).  The public surface (constructor parameters, `fit` / `transform` / `fit_transform`, the fitted
@@ -29,8 +30,8 @@ from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
-from .kernels import (EdgeHistogram, GraphHopper, NeighborhoodHash, ShortestPath, ShortestPathAttr, VertexHistogram,
-                      WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
+from .kernels import (EdgeHistogram, GraphHopper, NeighborhoodHash, Propagation, PropagationAttr, ShortestPath,
+                      ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
 
@@ -38,7 +39,11 @@ default_n_components = 100
 _OUTSIDE = frozenset((
     "random_walk", "RW", "graphlet_sampling", "GR", "subgraph_matching", "SM", "multiscale_laplacian", "ML",
     "lovasz_theta", "LOVT", "svm_theta", "SVMT", "neighborhood_subgraph_pairwise_distance",
-    "NSPD", "odd_sth", "ODD", "propagation", "PR", "pyramid_match", "PM", "hadamard_code", "HC"))
+    "NSPD", "odd_sth", "ODD", "pyramid_match", "PM", "hadamard_code", "HC"))
+
+
+def _propagation(params):
+    return (PropagationAttr if params.pop("with_attributes", False) else Propagation), params
 
 
 def _shortest_path(params):
@@ -54,6 +59,7 @@ for _names, _framework, _build in (
         (("shortest_path", "SP"), False, _shortest_path),
         (("graph_hopper", "GH"), False, lambda p: (GraphHopper, p)),
         (("neighborhood_hash", "NH"), False, lambda p: (NeighborhoodHash, p)),
+        (("propagation", "PR"), False, _propagation),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),
         (("core_framework", "CORE"), True, lambda p: (CoreFramework, p))):
     for _n in _names:
@@ -186,6 +192,9 @@ class GraphKernel(BaseEstimator, TransformerMixin):
                 raise NotImplementedError("kernel '" + str(name) + "' is outside the device hot path of grakel_b200")
             raise ValueError("Unsupported kernel: " + str(name))
         framework, build = entry
+        if name in ("propagation", "PR"):  # graph_kernels.py:486-489, 530-535
+            params["random_state"] = params.pop("random_state",
+                                                self.random_state_ if self.random_state is not None else None)
         if framework:
             if kernel_list:
                 params["base_graph_kernel"] = self.make_kernel_(kernel_list, {})

@@ -16,6 +16,8 @@ import copy
 import functools
 import warnings
 from collections.abc import Iterable
+from collections import Counter
+from itertools import chain, filterfalse
 from numbers import Real
 
 import numpy as np
@@ -1578,3 +1580,525 @@ class RandomWalkLabeled(RandomWalk):
     baseline geometric kernel with p=None raises NotImplementedError."""
 
     _labeled = True
+
+
+# ------------------------------------------------------------------------------
+def _pk_dot(x, y):
+    """propagation.py:23-24: the default metric, a dot product of two Counters."""
+    return sum(x[k] * y[k] for k in x)
+
+
+def row_normalized(mats):
+    """sklearn's normalize(T, axis=1, norm="l1") of every matrix (propagation.py:220, 568).  Dense matrices of one shape
+    and dtype go through one call on their vertical stack: the l1 norms and the division are row by row, so every block
+    of the result equals the per-matrix call bit for bit.  Only C-ordered matrices are stacked (numpy sums a strided
+    row in another order than a contiguous one); anything else is normalised matrix by matrix."""
+    from sklearn.preprocessing import normalize
+    out = [None] * len(mats)
+    groups = {}
+    for i, T in enumerate(mats):
+        if isinstance(T, np.ndarray) and T.ndim == 2 and T.shape[0] > 0 and T.flags.c_contiguous:
+            groups.setdefault((T.shape, T.dtype.str), []).append(i)
+        else:
+            out[i] = normalize(T, axis=1, norm="l1")
+    for (shape, _), idx in groups.items():
+        stacked = normalize(np.vstack([mats[i] for i in idx]), axis=1, norm="l1")
+        for k, i in enumerate(idx):
+            out[i] = stacked[k * shape[0]:(k + 1) * shape[0]]
+    return out
+
+
+_PK_ELEMENT_MSG = "Each element of X must be either a Graph or an iterable with at least 2 and at most 4 elements\n"
+
+
+class Propagation(Kernel):
+    """Propagation kernel for labelled graphs (propagation.py:27-423; Neumann et al. 2016).
+
+    Every vertex starts as the one-hot vector of its label; at each of t_max levels it is hashed into a bin,
+    floor((P_v . u_t + b_t) / w) with random u_t (Gaussian, or Cauchy for M="TV") and b_t drawn at fit, and every graph
+    then propagates P <- T P with its row-normalised transition matrix T (the adjacency matrix, or a matrix given as
+    the element's 4th entry).  K(G, G') = sum_t sum_c n_t(G, c) n_t(G', c), n_t(G, c) the vertices of G in bin c at
+    level t.  Propagation, hashing and the exact integer Gram run on the device; the label set, the draws and the
+    normalisation of T are the reference's own operations in its order.
+
+    Parameters, fitted attributes (`random_state_`, `_u`, `_b`, `_enum_labels`, `_parent_labels`) and errors are the
+    reference's, quirks included (a non-callable `metric` is not rejected; w < 0 is accepted).  A transform whose
+    graphs carry labels unseen at fit follows the reference's second branch: fresh draws per level for the new labels,
+    private bins for the vertices that hash with them, and the reference's inclusive count of each graph's successor's
+    first vertex.  `stats_.pk_near_edge` counts the hashes that lie within 2^-30 of their magnitude of a bin edge:
+    only those can fall into another bin than the reference's, whose summation order may differ.
+
+    A callable `metric` gets the reference's per-level Counters, built from the device bins with the reference's id
+    assignment, through the generic pairwise driver; `_hd` is built the same way on first access.
+
+    Deviations: w == 0 and t_max > 64 raise NotImplementedError; a NaN bin (M="H" over a negative entry) raises
+    KeyError as the reference does, but from the device check.  A sparse transition matrix raises the reference's
+    ValueError when t_max > 1."""
+
+    _graph_format = "adjacency"
+    attr_ = False
+
+    def __init__(self, n_jobs=None, verbose=False, normalize=False, random_state=None, metric=_pk_dot, M="TV", t_max=5,
+                 w=0.01):
+        super().__init__(n_jobs=n_jobs, verbose=verbose, normalize=normalize)
+        self.random_state = random_state
+        self.M = M
+        self.t_max = t_max
+        self.w = w
+        self.metric = metric
+        self._initialized.update({"M": False, "t_max": False, "w": False, "random_state": False, "metric": False})
+
+    def initialize(self):
+        """propagation.py:93-131, in its order and with its quirks."""
+        super().initialize()
+        if not self._initialized["random_state"]:
+            self.random_state_ = check_random_state(self.random_state)
+            self._initialized["random_state"] = True
+        if not self._initialized["metric"]:
+            if (type(self.M) is not str or (self.M not in ["H", "TV"] and not self.attr_)
+                    or (self.M not in ["L1", "L2"] and self.attr_)):
+                if self.attr_:
+                    raise TypeError('Metric type must be a str, one of "L1", "L2"')
+                raise TypeError('Metric type must be a str, one of "H", "TV"')
+            if not self.attr_:
+                self.take_sqrt_ = self.M == "H"
+            self.take_cauchy_ = self.M in ["TV", "L1"]
+            self._initialized["metric"] = True
+        if not self._initialized["t_max"]:
+            if type(self.t_max) is not int or self.t_max <= 0:
+                raise TypeError("The number of iterations must be a positive integer.")
+            if self.t_max > 64:
+                raise NotImplementedError(type(self).__name__ + ": at most t_max = 64 levels are supported")
+            self._initialized["t_max"] = True
+        if not self._initialized["w"]:
+            if not isinstance(self.w, Real) and self.w <= 0:
+                raise TypeError("The bin width must be a positive number.")
+            if self.w == 0:
+                raise NotImplementedError(type(self).__name__ + ": w = 0 puts every vertex into an infinite bin; "
+                                          "pass a non-zero bin width")
+            self._initialized["w"] = True
+        if not self._initialized["metric"]:
+            if not callable(self.metric):
+                raise TypeError("The base kernel must be callable.")
+            self._initialized["metric"] = True
+
+    # ---- input
+    def _elements(self, X, check=None):
+        """(adjacency matrix, labels / attributes in index order, T or None) of every element (propagation.py:169-226).
+        `check(lab)` validates an element's labels.  The reference normalises each element's T before checking its
+        labels, element by element; T is normalised in groups here, so an error raised for element k first lets the
+        normalisation of the elements before it (and of element k, for a label error) raise its own error."""
+        from .packing import adjacency_and_labels
+        if isinstance(X, Block):  # datasets.read_tu: the kernel's vertices are the nodes that occur in an edge
+            X.require("sp", labels=not self.attr_)
+            out = []
+            gp, rp, ci = X.graph_ptr, X.row_ptr, X.col_idx
+            for g in range(X.n_graphs):
+                a, b = int(gp[g]), int(gp[g + 1])
+                A = np.zeros((b - a, b - a))
+                for v in range(a, b):
+                    e0, e1 = int(rp[v]), int(rp[v + 1])
+                    A[v - a, ci[e0:e1] - a] = 1.0 if X.weights is None else X.weights[e0:e1]
+                lab = list(np.asarray(X.attrs)[a:b]) if self.attr_ else list(X.labels[a:b])
+                if check:
+                    check(lab)
+                out.append((A, lab, None))
+            return out
+        if not isinstance(X, Iterable):
+            raise ValueError("input must be an iterable\n")
+        out = []
+
+        def normalised_first(err, upto):
+            row_normalized([A if T is None else T for A, _, T in out[:upto]])
+            raise err
+
+        for idx, x in enumerate(iter(X)):
+            is_iter = isinstance(x, Iterable)
+            if is_iter and not isinstance(x, Graph):
+                x = list(x)
+            if is_iter and not isinstance(x, Graph) and len(x) in [0, 2, 3, 4]:
+                if len(x) == 0:
+                    warnings.warn("Ignoring empty element on " + "index: " + str(idx))
+                    continue
+                if len(x) == 2 and isinstance(x[0], Graph):
+                    el, T = x[0].as_element(), x[1]
+                else:
+                    el, T = x, (x[3] if len(x) == 4 else None)
+            elif isinstance(x, Graph):
+                el, T = x.as_element(), None
+            else:
+                normalised_first(ValueError("Each element of X must be either a " + "Graph or an iterable with at "
+                                            "least 2 " + "and at most 4 elements\n"), len(out))
+            try:
+                A, lab = adjacency_and_labels(el[0], el[1])
+                if T is not None:
+                    if T.shape[0] != T.shape[1]:
+                        raise TypeError("Transition matrix on index" + " " + str(idx) + "must be " +
+                                        "a square matrix.")
+                    if T.shape[0] != A.shape[0]:
+                        raise TypeError("Propagation matrix must " + "have the same dimension " +
+                                        "as the number of vertices.")
+            except Exception as e:  # noqa: BLE001
+                normalised_first(e, len(out))
+            out.append((A, lab, T))
+            if check:
+                try:
+                    check(lab)
+                except Exception as e:  # noqa: BLE001
+                    normalised_first(e, len(out))
+        return out
+
+    def _transitions(self, els):
+        """Row-normalised T of every element as dense float64 (the values numpy's dot reads), and whether one of them
+        is a scipy sparse matrix (numpy's dot cannot propagate it: propagation.py:292 raises at the first step)."""
+        normed = row_normalized([A if T is None else T for A, _, T in els])
+        out, sparse = [], False
+        for T in normed:
+            if not isinstance(T, np.ndarray):
+                sparse = True
+                T = T.toarray()
+            out.append(np.asarray(T, dtype=np.float64))
+        return out, sparse
+
+    def _sparse_step_error(self, data):
+        """The reference's error at its first propagation step over a sparse T, raised where it raises it: after the
+        draws of the fit, or after the first level's draws of a transform with new labels."""
+        if data.sparse and self.t_max > 1:
+            raise ValueError("setting an array element with a sequence.")
+
+    def parse_input(self, X):
+        """propagation.py:149-294: the label set, the enumeration and the draws, operation for operation."""
+        labels = set()
+
+        def check(lab):
+            nonlocal labels
+            try:
+                labels |= set(lab)
+            except TypeError:
+                raise TypeError("For a non attributed kernel, labels should be hashable.")
+
+        els = self._elements(X, check)
+        if not els:
+            raise ValueError("Parsed input is empty")
+        data = Fitted(None, None, {})
+        data.T, data.sparse = self._transitions(els)
+        data.sizes = np.array([len(lab) for _, lab, _ in els], dtype=np.int64)
+        data.u_full = None
+        if self._method_calling == 1:
+            enum_labels = {l: i for (i, l) in enumerate(list(labels))}
+            self._enum_labels = enum_labels
+            self._parent_labels = labels
+        else:
+            new_elements = labels - self._parent_labels
+            if len(new_elements) > 0:
+                new_enum_labels = iter((l, i) for (i, l) in enumerate(list(new_elements), len(self._enum_labels)))
+                enum_labels = dict(chain(self._enum_labels.items(), new_enum_labels))
+            else:
+                enum_labels = self._enum_labels
+        data.ids = np.array([enum_labels[l] for _, lab, _ in els for l in lab], dtype=np.int32)
+        data.dim = len(enum_labels)
+        dim_orig = len(self._enum_labels)
+        if self._method_calling == 1:
+            self._u, self._b = list(), list()
+            for t in range(self.t_max):
+                u = self.random_state_.randn(len(enum_labels))
+                if self.take_cauchy_:
+                    u = np.divide(u, self.random_state_.randn(len(enum_labels)))
+                self._u.append(u)
+                self._b.append(self.w * self.random_state_.rand())
+            self._hd_cache = None
+        elif dim_orig < len(enum_labels):  # :353-359, drawn level by level at transform time
+            nnv = len(enum_labels) - dim_orig
+            data.u_full = []
+            for t in range(self.t_max if not (data.sparse and self.t_max > 1) else 1):
+                u = self.random_state_.randn(nnv)
+                if self.take_cauchy_:
+                    u = np.divide(u, self.random_state_.randn(nnv))
+                data.u_full.append(np.hstack((self._u[t], u)))
+        self._sparse_step_error(data)
+        return data
+
+    # ---- estimator protocol
+    def _default_metric(self):
+        return self.metric is _pk_dot
+
+    def pairwise_operation(self, x, y):
+        """propagation.py:133-147: the metric summed over the levels' Counters."""
+        return sum(self.metric(x[t], y[t]) for t in range(self.t_max))
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        if not self._default_metric():
+            return self._metric_fit_transform()
+        K, xdiag, _ = self._pk_run(self.X, None, want_matrix=True)
+        self._X_diag = xdiag
+        if self.normalize:
+            self._warn_unnormalizable(xdiag)
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        Y = self.parse_input(X)
+        if not self._default_metric():
+            return self._metric_transform(Y)
+        K, xdiag, ydiag = self._pk_run(self.X, Y, want_matrix=True)
+        self._X_diag, self._Y_diag = xdiag, ydiag
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xdiag, ydiag)
+        return K
+
+    def diagonal(self):
+        check_is_fitted(self, ["X"])
+        if not self._default_metric():
+            return self._with_phi(self._pairwise_diagonal)
+        try:
+            check_is_fitted(self, ["_X_diag"])
+        except NotFittedError:
+            _, self._X_diag, _ = self._pk_run(self.X, None, want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
+
+    # ---- callable metric: the reference's Counters from the device bins, through the generic pairwise driver
+    @property
+    def _hd(self):
+        """The fit's per-level bin -> id dictionaries (propagation.py:280, 615), built lazily from the device bins of
+        the fitted graphs with the reference's id assignment."""
+        check_is_fitted(self, ["X"])
+        if getattr(self, "_hd_cache", None) is None:
+            levels = self._device_bins(self.X, None)
+            self._hd_cache = [self._fit_ids(b)[0] for b, _ in levels]
+        return self._hd_cache
+
+    def _device_bins(self, X, Y):
+        """Per level (bins [V, K], private flags [V]) of the joint X || Y block."""
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            self.stats_, V, _, _ = self._pk_features(eng, X, Y)
+            width = self._dim if self.attr_ else 1
+            return [eng.pk_hashes(t, V, width) for t in range(self.t_max)]
+
+    def _fit_ids(self, bins):
+        """(hd, ids) of one level at fit (propagation.py:279-282; attributes :613-618)."""
+        if self.attr_:
+            hashes = bins.tolist()
+            hd = {j: i for i, j in enumerate({tuple(l) for l in hashes})}
+            return hd, np.array([hd[tuple(l)] for l in hashes])
+        hashes = bins[:, 0]
+        hd = dict((j, i) for i, j in enumerate(set(np.unique(hashes))))
+        return hd, np.vectorize(lambda i: hd[i])(hashes)
+
+    def _transform_ids(self, hd_fit, bins, otypes=None):
+        """ids of one level's transformed bins: the fit's ids, then fresh ids in the reference's order
+        (propagation.py:301-314, 338-351; attributes :638-653)."""
+        if self.attr_:
+            hashes = bins.tolist()
+            new = filterfalse(lambda x: x in hd_fit, {tuple(l) for l in hashes})
+            hd = dict(chain(hd_fit.items(), ((j, i) for i, j in enumerate(new, len(hd_fit)))))
+            return hd, np.array([hd[tuple(l)] for l in hashes])
+        hashes = bins[:, 0]
+        new = filterfalse(lambda x: x in hd_fit, np.unique(hashes))
+        hd = dict(chain(hd_fit.items(), ((j, i) for i, j in enumerate(new, len(hd_fit)))))
+        if len(hashes) == 0:
+            return hd, np.zeros(0, dtype=int)
+        return hd, np.vectorize(lambda i: hd[i], otypes=otypes)(hashes)
+
+    def _phi(self, levels, sizes, offset, hd_fit=None, split=False):
+        """The reference's per-graph {level: Counter} of the graphs whose vertices start at `offset`: ids assigned as at
+        fit (hd_fit None) or as at transform, `split` for a transform with labels unseen at fit (ordinary and private
+        vertices, propagation.py:328-395)."""
+        idx = np.concatenate([[0], np.cumsum(sizes)])
+        n, V = len(sizes), int(idx[-1])
+        phi = [dict() for _ in range(n)]
+        for t, (bins, priv) in enumerate(levels):
+            b, pv = bins[offset:offset + V], priv[offset:offset + V]
+            if hd_fit is None:
+                _, features = self._fit_ids(b)
+            elif not split:
+                _, features = self._transform_ids(hd_fit[t], b)
+            else:
+                vertices, vertices_p = np.where(~pv)[0], np.where(pv)[0]
+                hd, features = self._transform_ids(hd_fit[t], b[vertices], otypes=[int])
+                hashes = b[vertices_p, 0]
+                hd = dict(chain(hd.items(), ((j, i) for i, j in enumerate(hashes, len(hd)))))
+                features_p = np.vectorize(lambda i: hd[i], otypes=[int])(hashes) if len(hashes) else \
+                    np.zeros(0, dtype=int)
+                for k in range(n):
+                    A = Counter(features[np.logical_and(idx[k] <= vertices, vertices <= idx[k + 1])])
+                    B = Counter(features_p[np.logical_and(idx[k] <= vertices_p, vertices_p <= idx[k + 1])])
+                    phi[k][t] = A + B
+                continue
+            for k in range(n):
+                phi[k][t] = Counter(features[idx[k]:idx[k + 1]])
+        return phi
+
+    def _with_phi(self, fn, *args):
+        """Run a generic-driver method with `self.X` / `self._Y` holding the per-graph Counters."""
+        data = self.X
+        self.X = self._phi_X
+        try:
+            return fn(*args)
+        finally:
+            self.X = data
+
+    def _metric_fit_transform(self):
+        levels = self._device_bins(self.X, None)
+        self._hd_cache = [self._fit_ids(b)[0] for b, _ in levels]
+        self._phi_X = self._phi(levels, self.X.sizes, 0)
+        km = self._with_phi(self._calculate_kernel_matrix)
+        self._X_diag = np.diagonal(km)
+        if self.normalize:  # kernel.py:196-203
+            self._warn_unnormalizable(self._X_diag)
+            with np.errstate(invalid="ignore", divide="ignore"):
+                return km / np.sqrt(np.outer(self._X_diag, self._X_diag))
+        return km
+
+    def _metric_transform(self, Y):
+        levels = self._device_bins(self.X, Y)
+        hd_fit = [self._fit_ids(b[:int(np.sum(self.X.sizes))])[0] for b, _ in levels]
+        self._hd_cache = hd_fit
+        self._phi_X = self._phi(levels, self.X.sizes, 0)
+        phi_Y = self._phi(levels, Y.sizes, int(np.sum(self.X.sizes)), hd_fit, split=Y.u_full is not None)
+        km = self._with_phi(self._calculate_kernel_matrix, phi_Y)
+        self._Y = phi_Y
+        self._is_transformed = True
+        if self.normalize:  # kernel.py:155-164
+            X_diag, Y_diag = self._with_phi(self._pairwise_diagonal)
+            self._warn_unnormalizable(X_diag, Y_diag)
+            with np.errstate(invalid="ignore", divide="ignore"):
+                km /= np.sqrt(np.outer(Y_diag, X_diag))
+        return km
+
+    # ---- device side
+    def _pk_inputs(self, X, Y):
+        """(graph sizes, T list, label ids, P0 or None, u [t_max, dim], b, dim, dim_orig, flags) of the joint X || Y run."""
+        parts = [X] if Y is None else [X, Y]
+        sizes = np.concatenate([p.sizes for p in parts])
+        mats = [T for p in parts for T in p.T]
+        ids = np.concatenate([p.ids for p in parts])
+        dim = parts[-1].dim
+        dim_orig = len(self._enum_labels)
+        flags = _lib.GK_PK_SQRT if self.take_sqrt_ else 0
+        if Y is not None and Y.u_full is not None:
+            u = np.stack(Y.u_full)
+            flags |= _lib.GK_PK_NEW_LABELS
+        else:
+            u = np.stack(self._u)
+            dim_orig = dim
+        return sizes, mats, ids, None, u, np.asarray(self._b, dtype=np.float64), dim, dim_orig, flags
+
+    def _pk_features(self, eng, X, Y):
+        """Pack T's pattern and run gk_pk_features on `eng` for the joint X || Y block.  Returns (stats, V, n_graphs,
+        n_fit)."""
+        sizes, mats, ids, p0, u, b, dim, dim_orig, flags = self._pk_inputs(X, Y)
+        gp = np.concatenate([[0], np.cumsum(sizes)])
+        rows, cols, vals = [], [], []
+        for g, T in enumerate(mats):
+            ii, jj = np.nonzero(T)
+            rows.append(ii + gp[g]); cols.append(jj + gp[g]); vals.append(T[ii, jj])
+        V = int(gp[-1])
+        r = np.concatenate(rows).astype(np.int64) if rows else np.zeros(0, np.int64)
+        c = np.concatenate(cols).astype(np.int32) if cols else np.zeros(0, np.int32)
+        v = np.concatenate(vals).astype(np.float64) if vals else np.zeros(0)
+        rp = np.concatenate([[0], np.cumsum(np.bincount(r, minlength=V))])
+        n_fit = len(X.sizes)
+        eng.pack(gp, rp, c, None if self.attr_ else ids, None, None)
+        try:
+            st = eng.pk_features(self.t_max, self.w, u, b, dim, dim_orig, n_fit, v, p0, flags)
+        except NotImplementedError as e:
+            if "NaN" in str(e):  # the reference's hash dictionary cannot look a NaN bin up (propagation.py:282)
+                raise KeyError(np.float64(np.nan)) from e
+            raise
+        return st, V, len(sizes), n_fit
+
+    def _pk_run(self, X, Y, want_matrix=True, device_ptr=None):
+        """gk_pk_features -> gk_gram.  Returns (K, xdiag, ydiag)."""
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            self.stats_, _, n_graphs, n_fit = self._pk_features(eng, X, Y)
+            out = False if not want_matrix else None
+            K, xd, yd = eng.gram(n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 out=out if device_ptr is None else None, device_ptr=device_ptr, stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd
+
+
+class PropagationAttr(Propagation):
+    """Propagation kernel for attributed graphs (propagation.py:426-689).
+
+    P starts as the vertex attributes, in the dtype numpy's vstack gives them, and keeps that dtype: every propagation
+    step is rounded to float32, or truncated toward zero for integer attributes, as the reference's assignment into P
+    does.  A vertex's bin at level t is the tuple floor((P_v * u_t + b_t) / w) (element-wise, u_t Gaussian or Cauchy for
+    M="L1", b_t = w * randn(d)).  Only the plain transform exists, as in the reference.  Deviations as for
+    Propagation; attributes of a dtype other than float64, float32 or signed integers, a float32 T over float32
+    attributes, and transform attributes of another dtype than the fitted ones raise NotImplementedError."""
+
+    _graph_format = "adjacency"
+    attr_ = True
+
+    def __init__(self, n_jobs=None, verbose=False, normalize=False, random_state=None, metric=_pk_dot, M="L1", t_max=5,
+                 w=4):
+        super().__init__(n_jobs=n_jobs, verbose=verbose, normalize=normalize, random_state=random_state, metric=metric,
+                         M=M, t_max=t_max, w=w)
+
+    def initialize(self):
+        super().initialize()
+
+    def parse_input(self, X):
+        """propagation.py:496-608: attributes, their dimension and the draws."""
+        Attr = []
+        els = self._elements(X, lambda lab: Attr.append(np.array([lab[j] for j in range(len(lab))])))
+        data = Fitted(None, None, {})
+        data.T, data.sparse = self._transitions(els)
+        try:
+            P = np.vstack(Attr)
+        except ValueError:
+            raise ValueError("Attribute dimensions should be the same, for all graphs")
+        if self._method_calling == 1:
+            self._dim = P.shape[1]
+        elif self._dim != P.shape[1]:
+            raise ValueError("transform attribute vectors should have the same dimension as in fit")
+        if not els:
+            raise ValueError("Parsed input is empty")
+        if P.dtype == np.float64:
+            data.store = 0
+        elif P.dtype == np.float32:
+            data.store = _lib.GK_PK_STORE_F32
+        elif P.dtype.kind == "i":
+            data.store = _lib.GK_PK_STORE_INT
+        else:
+            raise NotImplementedError("PropagationAttr: attributes of dtype " + str(P.dtype) + " are not supported "
+                                      "(float64, float32 or signed integers)")
+        if data.store == _lib.GK_PK_STORE_F32 and any(isinstance(T, np.ndarray) and T.dtype == np.float32
+                                                      for _, _, T in els):
+            raise NotImplementedError("PropagationAttr: a float32 transition matrix over float32 attributes is "
+                                      "propagated in float32 by numpy; only float64 propagation runs on the device")
+        data.P = P
+        data.sizes = np.array([len(lab) for _, lab, _ in els], dtype=np.int64)
+        data.ids = None
+        data.u_full = None  # no new-label branch for attributes
+        if self._method_calling == 1:
+            self._u, self._b = list(), list()
+            for t in range(self.t_max):
+                u = self.random_state_.randn(self._dim)
+                if self.take_cauchy_:
+                    u = np.divide(u, self.random_state_.randn(self._dim))
+                self._u.append(u)
+                self._b.append(self.w * self.random_state_.randn(self._dim))
+            self._hd_cache = None
+        self._sparse_step_error(data)
+        return data
+
+    def _pk_inputs(self, X, Y):
+        parts = [X] if Y is None else [X, Y]
+        if len({p.store for p in parts}) != 1:
+            raise NotImplementedError("PropagationAttr: fit and transform attributes of different dtypes")
+        sizes = np.concatenate([p.sizes for p in parts])
+        mats = [T for p in parts for T in p.T]
+        p0 = np.concatenate([np.asarray(p.P, dtype=np.float64) for p in parts])
+        return (sizes, mats, None, p0, np.stack(self._u), np.stack(self._b), self._dim, self._dim,
+                _lib.GK_PK_ATTR | parts[0].store)

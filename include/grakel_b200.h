@@ -124,6 +124,11 @@ typedef struct gk_stats {
      stopped at the term cap before converging */
   float ms_rw;
   int64_t rw_cap_hits;
+  /* Propagation: device time of the P <- T P steps (inside ms_hash, which covers propagation + hashing), and the
+     hashes (or float32 / integer stores of P) within 2^-30 of their magnitude of a bin edge, where a different
+     summation order could move a vertex to the neighbouring bin */
+  float ms_propagate;
+  int64_t pk_near_edge;
 } gk_stats;
 
 int gk_version(void);
@@ -222,6 +227,35 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
                    const double* values, const int32_t* t_row_ptr, const int32_t* t_col_idx, const double* t_values,
                    const double* q, const double* w, int32_t flags, gk_stats* stats);
 int gk_rw_iterations(gk_handle* h, uint8_t* out);
+
+/* Propagation / PropagationAttr (propagation.py:27-689).  The packed CSR (gk_pack_csr without weights; with the
+ * label ids for the labelled kernel) is the sparsity pattern of every graph's row-normalised transition matrix T,
+ * t_values[E] its entries.  P (V x dim, fp64) starts one-hot from the packed label ids or as p0[V * dim] (GK_PK_ATTR).
+ * Level t = 0 .. t_max-1 hashes every vertex with u[t * dim ..] and b, then P <- T P (each entry one FMA chain over
+ * the row's entries in ascending column order):
+ *   labelled     bin = floor((dot(P_v, u_t) + b[t]) / w), sqrt(P) first with GK_PK_SQRT (M = "H")
+ *   GK_PK_ATTR   bin = the dim-tuple floor((P_vj u_tj + b[t * dim + j]) / w); P is stored back rounded to float32
+ *                (GK_PK_STORE_F32) or truncated toward zero (GK_PK_STORE_INT), as numpy's assignment into P does
+ * GK_PK_NEW_LABELS (labels unseen at fit, propagation.py:328-395): the vertices of graphs >= n_fit that have a label
+ * id >= dim_orig (level 0), or whose columns >= dim_orig are all positive (later levels), hash the full row with
+ * u_t; every other vertex uses the columns < dim_orig.  Those private bins never equal a bin of another vertex kind,
+ * and each of them also counts in the transformed graph before its own when it is that graph's successor's first
+ * vertex (the reference's inclusive upper bound).  Without the flag dim_orig must equal dim.
+ * Every level's bins become columns of their own and (graph, column) counts an SP-layout feature block: gk_gram's
+ * integer route gives K = sum_t Phi_t Phi_t^T (fp32 / fp64, normalisation, n_fit, row ranges, GK_OUT_DEVICE); row maps
+ * and GK_DIST are GK_ERR_UNSUPPORTED.  A NaN bin is GK_ERR_UNSUPPORTED; a P that does not fit is GK_ERR_RANGE.
+ * stats: n_columns, ms_hash (propagate + hash), ms_propagate, ms_columns, pk_near_edge.  t_max in [1, 64], w != 0. */
+#define GK_PK_ATTR 1
+#define GK_PK_SQRT 2
+#define GK_PK_STORE_F32 4
+#define GK_PK_STORE_INT 8
+#define GK_PK_NEW_LABELS 16
+int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const double* b, int32_t dim,
+                   int32_t dim_orig, int64_t n_fit, const double* t_values, const double* p0, int32_t flags,
+                   gk_stats* stats);
+/* bins of level `level` after gk_pk_features: out[V * K] (K = dim for GK_PK_ATTR, else 1; -0.0 stored as 0.0), and
+ * priv[V] (may be NULL) = 1 where the vertex hashed as a private (new-label) vertex */
+int gk_pk_hashes(gk_handle* h, int32_t level, double* out, uint8_t* priv);
 
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
