@@ -180,6 +180,20 @@ def host_matrix(rows, cols, dtype=np.float64):
     return np.asarray(block).view(dt).reshape(rows, cols)
 
 
+def _gram_out(out, device_ptr, shape, dt):
+    """(K, pointer, GK_OUT_DEVICE or 0) of a Gram's output: the raw device pointer `device_ptr`, the caller's host array
+    `out`, no matrix (`out=False`) or a fresh host matrix."""
+    if device_ptr is not None:
+        return None, C.c_void_p(int(device_ptr)), GK_OUT_DEVICE
+    if out is False:
+        return None, None, 0
+    if out is not None:
+        assert out.dtype == dt and out.flags.c_contiguous and out.shape == shape
+        return out, _ptr(out), 0
+    K = host_matrix(*shape, dt)
+    return K, _ptr(K), 0
+
+
 class Engine:
     """One device context (opaque gk_handle + CUDA stream).  Not picklable on
     purpose: estimators keep only host-side state and fetch an engine lazily."""
@@ -358,19 +372,8 @@ class Engine:
         flags = (GK_NORMALIZE if normalize else 0) | (GK_NAN_TO_NUM if nan_to_num else 0)
         flags |= (GK_GRAM_SIMT if simt else 0) | (GK_FULL_TILES if full_tiles else 0) | (GK_DENSE_ALL if dense_all else 0)
         flags |= (GK_DIST if dist else 0) | (GK_DIST_GATHER if gather else 0)
-        K = None
-        kptr = None
-        if device_ptr is not None:
-            flags |= GK_OUT_DEVICE
-            kptr = C.c_void_p(int(device_ptr))
-        elif out is not None:
-            if out is not False:
-                K = out
-                assert K.dtype == dt and K.flags.c_contiguous and K.shape == (re_ - rb, n_fit)
-                kptr = _ptr(K)
-        else:
-            K = host_matrix(re_ - rb, n_fit, dt)
-            kptr = _ptr(K)
+        K, kptr, oflags = _gram_out(out, device_ptr, (re_ - rb, n_fit), dt)
+        flags |= oflags
         xd = np.empty(n_fit, dtype=np.float64) if want_diag else None
         yd = np.empty(n_graphs - n_fit, dtype=np.float64) if (want_diag and not square) else None
         st = stats if stats is not None else GkStats()
@@ -442,18 +445,8 @@ class Engine:
         dt = np.dtype(dtype)
         code = GK_F64 if dt == np.float64 else GK_F32
         flags = GK_DENSE_ALL if dense_all else 0
-        K, kptr = None, None
-        if device_ptr is not None:
-            flags |= GK_OUT_DEVICE
-            kptr = C.c_void_p(int(device_ptr))
-        elif out is not None:
-            if out is not False:
-                K = out
-                assert K.dtype == dt and K.flags.c_contiguous and K.shape == (n, n)
-                kptr = _ptr(K)
-        else:
-            K = host_matrix(n, n, dt)
-            kptr = _ptr(K)
+        K, kptr, oflags = _gram_out(out, device_ptr, (n, n), dt)
+        flags |= oflags
         xd = np.empty(n, dtype=np.float64) if want_diag else None
         st = stats if stats is not None else GkStats()
         with self._lock:

@@ -403,7 +403,7 @@ int gk_pack_csr(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const 
   h->attr_dim = attrs ? attr_dim : 0;
   h->max_graph_size = max_n;
   h->features_ready = false; h->feat_serial++;
-  h->feature_kind = 0;
+  h->feature_kind = FK_NONE;
   h->n_rows = 0;  // a new block starts without a row map
   HandleExtra* ex = extra_of(h);
   ex->wl_tiles_valid = false;
@@ -897,7 +897,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
   DevScalars* hs = h->h_scalars.as<DevScalars>();
   h->n_columns = hs->level_base[L];
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 1;
+  h->feature_kind = FK_WL;
   if (pro_enqueued) {
     HandleExtra* ex = extra_of(h);
     ex->pro_hist = *h->h_colstats.as<ColStats>();
@@ -1005,7 +1005,7 @@ static int wl_densify(gk_handle* h, int level, int* dst) {
 
 int gk_wl_labels(gk_handle* h, int32_t level, int32_t* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_wl_labels: null argument");
-  if (h->feature_kind != 1 || level < 0 || level >= h->n_levels) return fail(GK_ERR_STATE, "gk_wl_labels: no such level");
+  if (h->feature_kind != FK_WL || level < 0 || level >= h->n_levels) return fail(GK_ERR_STATE, "gk_wl_labels: no such level");
   GK_CUDA(cudaSetDevice(h->dev));
   const int* src = h->labels_all.as<int>() + (size_t)level * h->V;
   if (h->wl_sparse_ids && level >= 1) {
@@ -1272,7 +1272,7 @@ static int sp_features_impl(gk_handle* h, int32_t flags, int32_t wl_iter, gk_sta
   DevScalars* hs = h->h_scalars.as<DevScalars>();
   h->n_columns = (int64_t)dict_cap;  // column id = dictionary slot
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 2;
+  h->feature_kind = FK_SP;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = h->N; stats->n_vertices = h->V; stats->n_edges = h->E;
@@ -1294,7 +1294,7 @@ int gk_wl_sp_features(gk_handle* h, int32_t n_iter, int32_t flags, gk_stats* sta
 
 int gk_sp_distances(gk_handle* h, int64_t g, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_sp_distances: null argument");
-  if (h->feature_kind == 3 && h->sp_dist_esz) {
+  if (h->feature_kind == FK_SPATTR && h->sp_dist_esz) {
     // after gk_spattr_features: the APSP matrices of every graph are still in sp_dist (u16 with the saturated
     // value 0x3FFF for "no path", or fp64 with +inf)
     if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_sp_distances: bad graph index");
@@ -1312,7 +1312,7 @@ int gk_sp_distances(gk_handle* h, int64_t g, double* out) {
     }
     return GK_OK;
   }
-  if (h->feature_kind != 2 || !(h->sp_flags & GK_SP_KEEP_DIST)) return fail(GK_ERR_STATE, "gk_sp_distances: run gk_sp_features with GK_SP_KEEP_DIST (or gk_spattr_features) first");
+  if (h->feature_kind != FK_SP || !(h->sp_flags & GK_SP_KEEP_DIST)) return fail(GK_ERR_STATE, "gk_sp_distances: run gk_sp_features with GK_SP_KEEP_DIST (or gk_spattr_features) first");
   if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_sp_distances: bad graph index");
   HandleExtra* ex = extra_of(h);
   const long long off = ex->sp_goff[g], cnt = ex->sp_goff[g + 1] - off;
@@ -1455,7 +1455,7 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
   h->fattr_signed = *h_negative != 0;
   h->n_columns = Dfeat;
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 3;
+  h->feature_kind = FK_SPATTR;
   h->sp_dist_esz = (int)esz;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
@@ -1472,28 +1472,157 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
 
 static void build_tiles(std::vector<int2>& tiles, int a0, int a1, int b0, int b1, bool upper_only, int bm);
 
-// Gram of the dense fp64 SP-attr feature matrix (feature_kind == 3).  Non-negative features: the wgmma kernel with
+// ---------------------------------------------------------------------------
+// One gk_gram request, checked by gram_request and handed to the route of the feature kind.
+struct GramReq {
+  int64_t N;           // rows of the feature block (gk_set_row_map)
+  const int* row_map;  // packed graph -> row of the block, null for the identity
+  int64_t n_fit, k_rows, k_cols, row_begin, row_end;
+  int a0, a1;          // K's rows are the block's rows [a0, a1)
+  bool square, full_square, dev_out;
+  int64_t ld;          // resolved: >= k_cols
+  int32_t flags, out_dtype;
+  void* K_out;
+  double *xdiag, *ydiag;
+};
+
+// What each feature kind's route accepts besides fp64 host output of a row range of K.
+struct GramRules {
+  const char* name;
+  bool f32_out, dev_out, row_map, dist;
+};
+static const GramRules GRAM_RULES[] = {
+    /* FK_NONE   */ {"integer", true, true, true, true},
+    /* FK_WL     */ {"WL", true, true, true, true},
+    /* FK_SP     */ {"ShortestPath", true, true, true, true},
+    /* FK_SPATTR */ {"ShortestPathAttr", false, false, false, false},
+    /* FK_GH     */ {"GraphHopper", false, false, false, false},
+    /* FK_NH     */ {"NeighborhoodHash", false, true, false, false},
+    /* FK_RW     */ {"random walk", false, true, false, false},
+    /* FK_PK     */ {"Propagation", true, true, false, false},
+};
+
+static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
+                        int64_t row_end, void* K_out, int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag,
+                        GramReq* q) {
+  const GramRules& r = GRAM_RULES[kind];
+  if (out_dtype != GK_F32 && out_dtype != GK_F64) return fail(GK_ERR_ARG, "gk_gram: bad out_dtype");
+  const int64_t N = h->n_rows > 0 ? h->n_rows : h->N;
+  if (n_fit <= 0 || n_fit > N) return fail(GK_ERR_ARG, "gk_gram: n_fit out of range");
+  const bool dist = (flags & (GK_DIST | GK_DIST_GATHER)) != 0;
+  if (h->n_rows > 0 && !r.row_map) return fail(GK_ERR_UNSUPPORTED, std::string("gk_gram: row map with ") + r.name + " features");
+  if (dist && !r.dist) return fail(GK_ERR_UNSUPPORTED, std::string("gk_gram: GK_DIST with ") + r.name + " features");
+  if (out_dtype != GK_F64 && !r.f32_out) return fail(GK_ERR_UNSUPPORTED, std::string(r.name) + " Gram is fp64 only");
+  if ((flags & GK_OUT_DEVICE) && !r.dev_out)
+    return fail(GK_ERR_UNSUPPORTED, std::string(r.name) + " Gram: device output not supported");
+  const bool square = n_fit == N;
+  const int64_t k_rows_total = square ? N : N - n_fit;
+  if (row_end < 0) row_end = k_rows_total;
+  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
+  if (ld <= 0) ld = n_fit;
+  if (ld < n_fit) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
+  if (dist) {  // multi-GPU row tiling of the integer Gram (collective)
+    if (!h->comm) return fail(GK_ERR_STATE, "gk_gram: GK_DIST without gk_comm_init");
+    if (!square || h->n_rows > 0) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST needs the square fit_transform case without a row map");
+    if (flags & GK_OUT_DEVICE) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST results are library-owned (gk_result_device / gk_fetch / host K_out)");
+    int64_t rb = 0, re = 0;
+    GK_TRY(gk_comm_rows(h, N, &rb, &re));
+    if (row_begin != rb || row_end != re) return fail(GK_ERR_ARG, "gk_gram: GK_DIST row range must be the one gk_comm_rows returns");
+  }
+  if ((flags & GK_OUT_DEVICE) && !K_out) return fail(GK_ERR_ARG, "gk_gram: GK_OUT_DEVICE without a pointer");
+  q->N = N;
+  q->row_map = h->n_rows > 0 ? h->row_map.as<int>() : nullptr;
+  q->n_fit = n_fit; q->k_cols = n_fit;
+  q->row_begin = row_begin; q->row_end = row_end; q->k_rows = row_end - row_begin;
+  q->a0 = (int)((square ? 0 : n_fit) + row_begin); q->a1 = (int)((square ? 0 : n_fit) + row_end);
+  q->square = square; q->full_square = square && row_begin == 0 && row_end == N;
+  q->dev_out = (flags & GK_OUT_DEVICE) != 0;
+  q->ld = ld;
+  q->flags = flags; q->out_dtype = out_dtype;
+  q->K_out = K_out;
+  q->xdiag = xdiag; q->ydiag = ydiag;
+  return GK_OK;
+}
+
+// The integer feature block gram_int reads: the handle's own (block_of) or one NeighborhoodHash level (gram_nh).
+struct IntBlock {
+  unsigned long long* keys;  // (graph, column) -> count hash table of `cap` slots
+  unsigned* cnt;
+  size_t cap;
+  unsigned* colcnt;          // graphs per column: col_cap entries, the first n_columns in use
+  int64_t col_cap, n_columns;
+  unsigned long long* diag;  // self similarities, finished with the n_part per-CTA partials of the feature kernels
+  unsigned *part_max, *part_new;
+  int64_t n_part;
+  bool prologue_on_host;     // gk_wl_features already ran the square Gram prologue of this block
+};
+
+static IntBlock block_of(gk_handle* h) {
+  IntBlock b;
+  b.keys = h->ft_keys.as<unsigned long long>(); b.cnt = h->ft_cnt.as<unsigned>(); b.cap = h->ft_cap;
+  b.colcnt = h->colcnt.as<unsigned>(); b.col_cap = h->col_cap; b.n_columns = h->n_columns;
+  b.diag = h->diag_u64.as<unsigned long long>();
+  b.part_max = h->part_max.as<unsigned>(); b.part_new = h->part_new.as<unsigned>(); b.n_part = h->n_part;
+  b.prologue_on_host = h->pro_serial == h->feat_serial;
+  return b;
+}
+
+static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats* stats);
+
+// Where an fp64 route writes K: the caller's device buffer, else the library-owned h->K with unpitched rows.
+struct F64Out {
+  double* p;
+  int64_t ld;
+};
+
+static int f64_target(gk_handle* h, const GramReq& q, F64Out* out) {
+  if (q.dev_out) {
+    *out = {reinterpret_cast<double*>(q.K_out), q.ld};
+    return GK_OK;
+  }
+  GK_TRY(h->K.ensure((size_t)std::max<int64_t>(q.k_rows, 1) * q.k_cols * 8));
+  h->K_rows = q.k_rows; h->K_cols = q.k_cols; h->K_ld = q.k_cols; h->K_dtype = GK_F64;
+  *out = {h->K.as<double>(), q.k_cols};
+  return GK_OK;
+}
+
+// The end of an fp64 route: GK_NORMALIZE by the self similarities in diag_f64 (when the route normalises), ev_d2h,
+// the pitched copy of K into the caller's host array, xdiag / ydiag from diag_f64, ev_done (if given), and the
+// synchronisation after which the caller's buffers hold the result.
+static int f64_deliver(gk_handle* h, const GramReq& q, const F64Out& out, bool normalize, cudaEvent_t ev_d2h,
+                       cudaEvent_t ev_done = nullptr) {
+  const double* diag = h->diag_f64.as<double>();
+  if (normalize && (q.flags & GK_NORMALIZE) && q.k_rows > 0) {
+    normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(q.k_rows, q.k_cols, out.p, out.ld, diag + q.a0, diag,
+                                                                    (q.flags & GK_NAN_TO_NUM) ? 1 : 0);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(ev_d2h, h->stream));
+  if (q.K_out && !q.dev_out && q.k_rows > 0)
+    GK_CUDA(cudaMemcpy2DAsync(q.K_out, (size_t)q.ld * 8, out.p, (size_t)out.ld * 8, (size_t)q.k_cols * 8,
+                              (size_t)q.k_rows, cudaMemcpyDeviceToHost, h->stream));
+  if (q.xdiag) GK_CUDA(cudaMemcpyAsync(q.xdiag, diag, q.n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (q.ydiag && !q.square)
+    GK_CUDA(cudaMemcpyAsync(q.ydiag, diag + q.n_fit, (q.N - q.n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (ev_done) GK_CUDA(cudaEventRecord(ev_done, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+// Gram of the dense fp64 SP-attr feature matrix (FK_SPATTR).  Non-negative features: the wgmma kernel with
 // tf32 operands on a hi/lo split of the features (3xTF32: hi hi^T + hi lo^T + lo hi^T, fp32 accumulation in
 // registers, k range processed in chunks and summed in fp64), self similarities exact in fp64.  Its error is a small
 // multiple of 2^-22 times sum_k |phi_ik| |phi_jk| (measured on an H100: below 1e-6 of it), which for non-negative
 // features is K_ij itself: every entry within 1e-5 relative.  A feature map with a negative entry (attributes of
 // mixed sign) can have entries that cancel far below that scale, so it takes the fp64 CUDA-core Gram (1e-9).
 // GRAKEL_B200_SPATTR_F64=1 forces the fp64 Gram, =0 the tensor-core Gram.
-static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
-                       int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
-  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "ShortestPathAttr Gram is fp64 only");
-  if (flags & GK_OUT_DEVICE) return fail(GK_ERR_UNSUPPORTED, "ShortestPathAttr Gram: device output not supported");
-  const int64_t N = h->N;
-  const bool square = n_fit == N;
-  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
-  if (row_end < 0) row_end = k_rows_total;
-  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
-  const int64_t k_rows = row_end - row_begin;
-  if (ld <= 0) ld = k_cols;
+static int gram_spattr(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
+  const bool square = q.square;
+  const int a0 = q.a0, a1 = q.a1;
   const int64_t launches0 = h->launches;
-  GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
-  h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
-  const int a0 = (int)((square ? 0 : n_fit) + row_begin), a1 = (int)((square ? 0 : n_fit) + row_end);
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
   GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
   const char* e_f64 = getenv("GRAKEL_B200_SPATTR_F64");
   const bool use_f64 = (e_f64 && *e_f64) ? atoi(e_f64) != 0 : h->fattr_signed;
@@ -1504,7 +1633,7 @@ static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_b
     float* P2 = P1 + (size_t)N * W;
     spattr_split_tf32<<<h->sm_count * 8, 256, 0, h->stream>>>(h->fattr.as<double>(), D, Dp, (int)N, P1, P2);
     LAUNCH_CHECK(h);
-    const bool sym = square && row_begin == 0 && row_end == N;
+    const bool sym = q.full_square;
     std::vector<int2> tiles;
     build_tiles(tiles, a0, a1, 0, (int)n_fit, sym, BM);
     GK_TRY(h->h_tiles.ensure(tiles.size() * sizeof(int2)));
@@ -1521,7 +1650,7 @@ static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_b
     p.n_tiles = (int)tiles.size();
     p.a_row_end = a1; p.b_row_end = (int)n_fit;
     p.c_row0 = a0; p.c_col0 = 0;
-    p.out = h->K.p; p.ld = k_cols;
+    p.out = out.p; p.ld = out.ld;
     p.mirror = 0;  // the symmetric case mirrors the upper triangle once, after all chunks (mirror_upper_f64)
     p.diag = h->diag_f64.as<double>();
     // The tensor core's fp32 accumulate truncates, so no accumulator sums more than `chunk` k-blocks x 4 MMAs: the
@@ -1539,36 +1668,20 @@ static int gram_spattr(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_b
     gram_tc_kernel<double, false, 1><<<grid, GEMM_THREADS, GEMM_SMEM, h->stream>>>(tmA, tmB, tmC, p);
     LAUNCH_CHECK(h);
     if (sym) {
-      mirror_upper_f64<<<h->sm_count * 8, 256, 0, h->stream>>>((int)N, h->K.as<double>(), k_cols);
+      mirror_upper_f64<<<h->sm_count * 8, 256, 0, h->stream>>>((int)N, out.p, out.ld);
       LAUNCH_CHECK(h);
     }
     if (square) {  // exact self similarities
-      set_diag_f64<<<cdiv(k_rows, 256), 256, 0, h->stream>>>(a0, a1, 0, (int)n_fit, h->diag_f64.as<double>(), h->K.as<double>(), k_cols);
+      set_diag_f64<<<cdiv(k_rows, 256), 256, 0, h->stream>>>(a0, a1, 0, (int)n_fit, h->diag_f64.as<double>(), out.p, out.ld);
       LAUNCH_CHECK(h);
     }
   }
-  if (k_rows > 0) {
-    if (use_f64) {
-      dim3 grid(cdiv(k_cols, 64), cdiv(k_rows, 64));
-      gram_f64_kernel<<<grid, 256, 0, h->stream>>>(h->fattr.as<double>(), h->fattr_dim, a0, a1, 0, (int)n_fit,
-                                                   h->K.as<double>(), k_cols);
-      LAUNCH_CHECK(h);
-    }
-    if (flags & GK_NORMALIZE) {
-      normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(k_rows, k_cols, h->K.as<double>(), k_cols,
-                                                                      h->diag_f64.as<double>() + a0,
-                                                                      h->diag_f64.as<double>(), (flags & GK_NAN_TO_NUM) ? 1 : 0);
-      LAUNCH_CHECK(h);
-    }
+  if (k_rows > 0 && use_f64) {
+    dim3 grid(cdiv(k_cols, 64), cdiv(k_rows, 64));
+    gram_f64_kernel<<<grid, 256, 0, h->stream>>>(h->fattr.as<double>(), h->fattr_dim, a0, a1, 0, (int)n_fit, out.p, out.ld);
+    LAUNCH_CHECK(h);
   }
-  GK_CUDA(cudaEventRecord(h->tev[7], h->stream));
-  if (K_out && k_rows > 0)
-    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, h->K.p, (size_t)k_cols * 8, (size_t)k_cols * 8, (size_t)k_rows,
-                              cudaMemcpyDeviceToHost, h->stream));
-  if (xdiag) GK_CUDA(cudaMemcpyAsync(xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (ydiag && !square)
-    GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
-  GK_CUDA(cudaStreamSynchronize(h->stream));
+  GK_TRY(f64_deliver(h, q, out, true, h->tev[7]));
   if (stats) {
     stats->gram_path = use_f64 ? 5 : 4;
     stats->gemm_launches = h->launches - launches0;
@@ -1704,7 +1817,7 @@ int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, 
   h->gh_mu = mu;
   h->n_columns = n_columns;
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 4;
+  h->feature_kind = FK_GH;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
@@ -1720,7 +1833,7 @@ int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, 
 
 int gk_gh_node_maps(gk_handle* h, int64_t g, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_gh_node_maps: null argument");
-  if (h->feature_kind != 4 || !h->features_ready) return fail(GK_ERR_STATE, "gk_gh_node_maps: run gk_gh_features first");
+  if (h->feature_kind != FK_GH || !h->features_ready) return fail(GK_ERR_STATE, "gk_gh_node_maps: run gk_gh_features first");
   if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_gh_node_maps: bad graph index");
   HandleExtra* ex = extra_of(h);
   const int delta = h->gh_delta;
@@ -1757,23 +1870,14 @@ static void gh_groups(const std::vector<int>& gp, int g0, int g1, std::vector<in
 
 // Gram of the node-pair kernels (gaussian / bridge): gh_nodepair_gram over graph-group pairs, self similarities from
 // gh_nodepair_diag.  fp64, host output, GK_NORMALIZE, n_fit / row ranges as in gram_spattr.
-static int gram_gh_nodepair(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
-                            int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
-  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "GraphHopper Gram is fp64 only");
-  if (flags & GK_OUT_DEVICE) return fail(GK_ERR_UNSUPPORTED, "GraphHopper Gram: device output not supported");
+static int gram_gh_nodepair(gk_handle* h, const GramReq& q, gk_stats* stats) {
   HandleExtra* ex = extra_of(h);
-  const int64_t N = h->N;
-  const bool square = n_fit == N;
-  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
-  if (row_end < 0) row_end = k_rows_total;
-  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
-  const int64_t k_rows = row_end - row_begin;
-  if (ld <= 0) ld = k_cols;
-  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
+  const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows;
+  const bool square = q.square;
+  const int a0 = q.a0, a1 = q.a1;
   const int64_t launches0 = h->launches;
-  GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
-  h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
-  const int a0 = (int)((square ? 0 : n_fit) + row_begin), a1 = (int)((square ? 0 : n_fit) + row_end);
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
   // groups: over all graphs (square) or over Y rows and X columns; the same groups whatever the row range, so a
   // row block reproduces the full matrix's entries bit for bit
   std::vector<int> rgroups, cgroups;
@@ -1807,8 +1911,8 @@ static int gram_gh_nodepair(gk_handle* h, int64_t n_fit, int32_t flags, int64_t 
     p.cgroups = h->gh_groups.as<int>() + rgroups.size();
     p.square = square ? 1 : 0;
     p.a0 = a0; p.a1 = a1; p.row0 = a0;
-    p.out = h->K.as<double>();
-    p.ld = k_cols;
+    p.out = out.p;
+    p.ld = out.ld;
     if (!pairs.empty()) {
       if (h->gh_node_kernel == GK_GH_GAUSSIAN) {
         GK_CUDA(cudaFuncSetAttribute(gh_nodepair_gram<GH_NK_GAUSSIAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GH_GRAM_SMEM));
@@ -1820,24 +1924,12 @@ static int gram_gh_nodepair(gk_handle* h, int64_t n_fit, int32_t flags, int64_t 
       LAUNCH_CHECK(h);
     }
     if (square) {
-      set_diag_f64<<<cdiv(k_rows, 256), 256, 0, h->stream>>>(a0, a1, 0, (int)n_fit, h->diag_f64.as<double>(), h->K.as<double>(), k_cols);
-      LAUNCH_CHECK(h);
-    }
-    if (flags & GK_NORMALIZE) {
-      normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(k_rows, k_cols, h->K.as<double>(), k_cols,
-                                                                      h->diag_f64.as<double>() + a0,
-                                                                      h->diag_f64.as<double>(), (flags & GK_NAN_TO_NUM) ? 1 : 0);
+      set_diag_f64<<<cdiv(k_rows, 256), 256, 0, h->stream>>>(a0, a1, 0, (int)n_fit, h->diag_f64.as<double>(), out.p, out.ld);
       LAUNCH_CHECK(h);
     }
   }
-  GK_CUDA(cudaEventRecord(h->tev[7], h->stream));
-  if (K_out && k_rows > 0)
-    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, h->K.p, (size_t)k_cols * 8, (size_t)k_cols * 8, (size_t)k_rows,
-                              cudaMemcpyDeviceToHost, h->stream));
-  if (xdiag) GK_CUDA(cudaMemcpyAsync(xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (ydiag && !square)
-    GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
-  GK_CUDA(cudaStreamSynchronize(h->stream));  // also keeps the host group / pair lists alive for their copies
+  // its synchronisation also keeps the host group / pair lists alive for their copies
+  GK_TRY(f64_deliver(h, q, out, true, h->tev[7]));
   if (stats) {
     stats->gram_path = 6;
     stats->gemm_tiles = (int64_t)pairs.size();
@@ -1851,27 +1943,26 @@ static int gram_gh_nodepair(gk_handle* h, int64_t n_fit, int32_t flags, int64_t 
 // NeighborhoodHash (neighborhood_hash.cuh).  Level r's expanded block lives at nh_blk + r * nh_level_bytes:
 // keys [V] u64 | counts [V] u32 | graphs per column [V + 1] u32 | self similarities [N] u64 (at most one unary entry
 // per non-None vertex, so V entries and V columns bound every level).
-struct NhLevel {
-  unsigned long long* keys;
-  unsigned* cnt;
-  unsigned* colcnt;
-  unsigned long long* diag;
-};
-
 static size_t nh_level_bytes(int64_t V, int64_t N) {
   const size_t V1 = (size_t)std::max<int64_t>(V, 1);
   const size_t diag_off = (16 * V1 + 4 + 7) / 8 * 8;
   return (diag_off + 8 * (size_t)std::max<int64_t>(N, 1) + 255) / 256 * 256;
 }
 
-static NhLevel nh_level(gk_handle* h, int r) {
+// Level r's block as an integer feature block; its self similarities are one partial (part_max / part_new, uploaded
+// by gram_nh), its column count is set by gram_nh.
+static IntBlock nh_level(gk_handle* h, int r) {
   const size_t V1 = (size_t)std::max<int64_t>(h->V, 1);
   char* b = h->nh_blk.as<char>() + (size_t)r * h->nh_level_bytes;
-  NhLevel L;
+  IntBlock L;
   L.keys = reinterpret_cast<unsigned long long*>(b);
   L.cnt = reinterpret_cast<unsigned*>(b + 8 * V1);
+  L.cap = V1;
   L.colcnt = reinterpret_cast<unsigned*>(b + 12 * V1);
+  L.col_cap = (int64_t)V1 + 1; L.n_columns = 0;
   L.diag = reinterpret_cast<unsigned long long*>(b + (16 * V1 + 4 + 7) / 8 * 8);
+  L.part_max = h->part_max.as<unsigned>(); L.part_new = h->part_new.as<unsigned>(); L.n_part = 1;
+  L.prologue_on_host = false;
   return L;
 }
 
@@ -1963,7 +2054,7 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
   GK_CUDA(cudaMemsetAsync(h->nh_cur.p, 0, cur_bytes, h->stream));
   GK_CUDA(cudaMemsetAsync(h->nh_blk.p, 0, (size_t)R * h->nh_level_bytes, h->stream));
   for (int r = 0; r < R; ++r) {
-    const NhLevel lv = nh_level(h, r);
+    const IntBlock lv = nh_level(h, r);
     GK_CUDA(cudaMemsetAsync(lv.keys, 0xFF, (size_t)V1 * 8, h->stream));
     if (!V) continue;
     const unsigned long long* c_r = codes + (size_t)(r + 1) * V;
@@ -2012,7 +2103,7 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
   h->nh_R = R;
   h->n_columns = n_cols;
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 5;
+  h->feature_kind = FK_NH;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
@@ -2031,7 +2122,7 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
 
 int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_nh_labels: null argument");
-  if (h->feature_kind != 5 || !h->features_ready || level < 0 || level >= h->nh_R)
+  if (h->feature_kind != FK_NH || !h->features_ready || level < 0 || level >= h->nh_R)
     return fail(GK_ERR_STATE, "gk_nh_labels: no such level (run gk_nh_features first)");
   GK_CUDA(cudaSetDevice(h->dev));
   const size_t V = (size_t)h->V;
@@ -2054,71 +2145,41 @@ int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid) {
 // normalises this kernel, and its self similarities are 1.
 constexpr size_t NH_C_BUDGET = (size_t)8 << 30;
 
-static int gram_nh(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
-                   int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
-  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "NeighborhoodHash Gram is fp64 only");
+static int gram_nh(gk_handle* h, const GramReq& q, gk_stats* stats) {
   HandleExtra* ex = extra_of(h);
-  const int64_t N = h->N;
+  const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
   const int R = h->nh_R;
-  const bool square = n_fit == N;
-  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
-  if (row_end < 0) row_end = k_rows_total;
-  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
-  const int64_t k_rows = row_end - row_begin;
-  if (ld <= 0) ld = k_cols;
-  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
-  const bool dev_out = (flags & GK_OUT_DEVICE) != 0;
-  if (dev_out && !K_out) return fail(GK_ERR_ARG, "gk_gram: GK_OUT_DEVICE without a pointer");
+  const bool square = q.square;
   const int64_t launches0 = h->launches;
-  double* d_out;
-  int64_t d_ld;
-  if (dev_out) {
-    d_out = reinterpret_cast<double*>(K_out);
-    d_ld = ld;
-  } else {
-    GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
-    h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
-    d_out = h->K.as<double>();
-    d_ld = k_cols;
-  }
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
   const int64_t ldc = (k_cols + 7) / 8 * 8;  // 32-byte rows: TMA stores of the Gram epilogue
   size_t c_budget = NH_C_BUDGET;
   if (const char* e = getenv("GRAKEL_B200_NH_C_BUDGET")) c_budget = std::max<size_t>(1, strtoull(e, nullptr, 10));
   const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(std::max<int64_t>(k_rows, 1),
                                                                 (int64_t)(c_budget / ((size_t)R * ldc * 4))));
   GK_TRY(h->nh_C.ensure((size_t)R * chunk * ldc * 4));
-  const int32_t gflags = (flags & (GK_GRAM_SIMT | GK_DENSE_ALL | GK_FULL_TILES)) | GK_OUT_DEVICE;
-  const size_t V1 = (size_t)std::max<int64_t>(h->V, 1);
+  const int32_t gflags = (q.flags & (GK_GRAM_SIMT | GK_DENSE_ALL | GK_FULL_TILES)) | GK_OUT_DEVICE;
   GK_TRY(h->part_max.ensure(4));
   GK_TRY(h->part_new.ensure(4));
   std::vector<float> ms_level(R, 0.f);
   float ms_combine = 0.f;
   gk_stats st;
   int64_t max_T = 0, gram_launches = 0, elem_bytes = 0;
-  for (int64_t cb = row_begin; cb < row_end; cb += chunk) {
-    const int64_t ce = std::min<int64_t>(row_end, cb + chunk), rows = ce - cb;
+  for (int64_t cb = q.row_begin; cb < q.row_end; cb += chunk) {
+    const int64_t ce = std::min<int64_t>(q.row_end, cb + chunk), rows = ce - cb;
     for (int r = 0; r < R; ++r) {
-      // install level r as the handle's integer feature block, run the Gram, put the handle's own buffers back
-      const NhLevel lv = nh_level(h, r);
+      // the integer Gram of level r's expanded block: its rows [cb, ce) as fp32 counts into nh_C
+      IntBlock fb = nh_level(h, r);
+      fb.n_columns = ex->nh_cols[r];
       const unsigned part[2] = {ex->nh_entries[r] ? 1u : 0u, (unsigned)ex->nh_entries[r]};
       GK_CUDA(cudaMemcpyAsync(h->part_max.p, &part[0], 4, cudaMemcpyHostToDevice, h->stream));
       GK_CUDA(cudaMemcpyAsync(h->part_new.p, &part[1], 4, cudaMemcpyHostToDevice, h->stream));
-      const DevBuf s_keys = h->ft_keys, s_cnt = h->ft_cnt, s_colcnt = h->colcnt, s_diag = h->diag_u64;
-      const size_t s_ftcap = h->ft_cap;
-      const int64_t s_colcap = h->col_cap, s_ncols = h->n_columns, s_npart = h->n_part;
-      h->ft_keys.p = lv.keys; h->ft_keys.cap = V1 * 8;
-      h->ft_cnt.p = lv.cnt; h->ft_cnt.cap = V1 * 4;
-      h->colcnt.p = lv.colcnt; h->colcnt.cap = (V1 + 1) * 4;
-      h->diag_u64.p = lv.diag; h->diag_u64.cap = (size_t)N * 8;
-      h->ft_cap = V1; h->col_cap = (int64_t)V1 + 1; h->n_columns = ex->nh_cols[r]; h->n_part = 1;
-      h->feature_kind = 1;
+      GramReq lq;
+      GK_TRY(gram_request(h, FK_WL, n_fit, gflags, cb, ce, h->nh_C.as<float>() + (size_t)r * chunk * ldc, GK_F32, ldc,
+                          nullptr, nullptr, &lq));
       memset(&st, 0, sizeof(st));
-      const int rc = gk_gram(h, n_fit, gflags, cb, ce, h->nh_C.as<float>() + (size_t)r * chunk * ldc, GK_F32, ldc, nullptr,
-                             nullptr, &st);
-      h->ft_keys = s_keys; h->ft_cnt = s_cnt; h->colcnt = s_colcnt; h->diag_u64 = s_diag;
-      h->ft_cap = s_ftcap; h->col_cap = s_colcap; h->n_columns = s_ncols; h->n_part = s_npart;
-      h->feature_kind = 5;
-      if (rc != GK_OK) return rc;
+      GK_TRY(gram_int(h, lq, fb, &st));
       ms_level[r] += st.ms_total;
       max_T = std::max<int64_t>(max_T, st.threshold);
       gram_launches += st.gemm_launches;
@@ -2134,9 +2195,9 @@ static int gram_nh(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin
       p.row_g0 = (int)((square ? 0 : n_fit) + cb);
       p.rows = (int)rows;
       p.cols = (int)k_cols;
-      p.mirror = square && cb == 0 && ce == N && !(flags & GK_FULL_TILES) ? 1 : 0;
-      p.out = d_out + (size_t)(cb - row_begin) * d_ld;
-      p.ld = d_ld;
+      p.mirror = square && cb == 0 && ce == N && !(q.flags & GK_FULL_TILES) ? 1 : 0;
+      p.out = out.p + (size_t)(cb - q.row_begin) * out.ld;
+      p.ld = out.ld;
       const long long nbi = (rows + NH_TILE - 1) / NH_TILE, nbj = (k_cols + NH_TILE - 1) / NH_TILE;
       const long long grid = p.mirror ? nbj * (nbj + 1) / 2 : nbi * nbj;
       GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
@@ -2149,14 +2210,11 @@ static int gram_nh(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin
       ms_combine += ev_ms(h->tev[0], h->tev[1]);
     }
   }
-  GK_CUDA(cudaEventRecord(h->ev[14], h->stream));
-  if (K_out && !dev_out && k_rows > 0)
-    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, d_out, (size_t)d_ld * 8, (size_t)k_cols * 8, (size_t)k_rows,
-                              cudaMemcpyDeviceToHost, h->stream));
-  GK_CUDA(cudaEventRecord(h->ev[15], h->stream));
-  GK_CUDA(cudaStreamSynchronize(h->stream));
-  if (xdiag) for (int64_t i = 0; i < n_fit; ++i) xdiag[i] = 1.0;
-  if (ydiag && !square) for (int64_t i = 0; i < N - n_fit; ++i) ydiag[i] = 1.0;
+  GramReq kq = q;  // the self similarities are 1, written on the host
+  kq.xdiag = kq.ydiag = nullptr;
+  GK_TRY(f64_deliver(h, kq, out, false, h->ev[14], h->ev[15]));
+  if (q.xdiag) for (int64_t i = 0; i < n_fit; ++i) q.xdiag[i] = 1.0;
+  if (q.ydiag && !square) for (int64_t i = 0; i < N - n_fit; ++i) q.ydiag[i] = 1.0;
   if (stats) {
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
     stats->n_levels = R;
@@ -2231,7 +2289,7 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
   GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffers may be reused once we return
   h->rw_route = route; h->rw_fn = fn; h->rw_lamda = lamda;
   h->rw_labeled = (flags & GK_RW_LABELED) != 0;
-  h->feature_kind = 6;
+  h->feature_kind = FK_RW;
   h->features_ready = true; h->feat_serial++;
   if (stats) {
     stats->n_graphs = h->N; stats->n_vertices = V; stats->n_edges = E;
@@ -2242,7 +2300,7 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
 
 int gk_rw_iterations(gk_handle* h, uint8_t* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_rw_iterations: null argument");
-  if (h->feature_kind != 6 || h->rw_iter_rows * h->rw_iter_cols == 0) return fail(GK_ERR_STATE, "gk_rw_iterations: no random walk Gram yet");
+  if (h->feature_kind != FK_RW || h->rw_iter_rows * h->rw_iter_cols == 0) return fail(GK_ERR_STATE, "gk_rw_iterations: no random walk Gram yet");
   GK_CUDA(cudaSetDevice(h->dev));
   GK_CUDA(cudaMemcpyAsync(out, h->rw_iters.p, (size_t)(h->rw_iter_rows * h->rw_iter_cols), cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
@@ -2251,7 +2309,7 @@ int gk_rw_iterations(gk_handle* h, uint8_t* out) {
 
 // ---------------------------------------------------------------------------
 // Propagation (propagation.cuh).  The packed CSR is the sparsity pattern of the row-normalised transition matrices,
-// t_values[E] their entries; the features are the SP layout (feature_kind 7), so gk_gram's integer route runs them.
+// t_values[E] their entries; the features are the SP layout (FK_PK), so gk_gram's integer route runs them.
 int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const double* b, int32_t dim,
                    int32_t dim_orig, int64_t n_fit, const double* t_values, const double* p0, int32_t flags,
                    gk_stats* stats) {
@@ -2405,7 +2463,7 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
   h->pk_levels = t_max;
   h->pk_K = K;
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 7;
+  h->feature_kind = FK_PK;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
@@ -2425,7 +2483,7 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
 
 int gk_pk_hashes(gk_handle* h, int32_t level, double* out, uint8_t* priv) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_pk_hashes: null argument");
-  if (h->feature_kind != 7 || !h->features_ready || level < 0 || level >= h->pk_levels)
+  if (h->feature_kind != FK_PK || !h->features_ready || level < 0 || level >= h->pk_levels)
     return fail(GK_ERR_STATE, "gk_pk_hashes: no such level (run gk_pk_features first)");
   GK_CUDA(cudaSetDevice(h->dev));
   const size_t V = (size_t)h->V, K = (size_t)h->pk_K;
@@ -2469,37 +2527,17 @@ static int rw_launch(gk_handle* h, RwParams p, size_t vec_elems) {
 // Gram of the random walk kernels (gram_path 8 conjugate gradients, 9 spectral, 10 power series): fp64, host or
 // GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges.  Self similarities come from the same pair kernel, so a
 // square K's diagonal equals them bit for bit.  The full square case computes the upper triangle and mirrors it.
-static int gram_rw(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
-                   int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
-  if (out_dtype != GK_F64) return fail(GK_ERR_UNSUPPORTED, "random walk Gram is fp64 only");
+static int gram_rw(gk_handle* h, const GramReq& q, gk_stats* stats) {
   HandleExtra* ex = extra_of(h);
-  const int64_t N = h->N;
-  const bool square = n_fit == N;
-  const int64_t k_rows_total = square ? N : N - n_fit, k_cols = n_fit;
-  if (row_end < 0) row_end = k_rows_total;
-  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
-  const int64_t k_rows = row_end - row_begin;
-  if (ld <= 0) ld = k_cols;
-  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
-  const bool dev_out = (flags & GK_OUT_DEVICE) != 0;
-  if (dev_out && !K_out) return fail(GK_ERR_ARG, "gk_gram: GK_OUT_DEVICE without a pointer");
+  const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
+  const bool square = q.square;
   const int64_t launches0 = h->launches;
-  double* d_out;
-  int64_t d_ld;
-  if (dev_out) {
-    d_out = reinterpret_cast<double*>(K_out);
-    d_ld = ld;
-  } else {
-    GK_TRY(h->K.ensure((size_t)std::max<int64_t>(k_rows, 1) * k_cols * 8));
-    h->K_rows = k_rows; h->K_cols = k_cols; h->K_ld = k_cols; h->K_dtype = GK_F64;
-    d_out = h->K.as<double>();
-    d_ld = k_cols;
-  }
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
   GK_TRY(h->diag_f64.ensure((size_t)N * 8));
   GK_TRY(h->rw_iters.ensure((size_t)std::max<int64_t>(k_rows * k_cols, 1)));
   GK_CUDA(cudaMemsetAsync(h->rw_cap.p, 0, 8, h->stream));
   // largest vertex count among the row graphs and among the column graphs: the vectors of the largest pair
-  const int64_t g_row0 = (square ? 0 : n_fit) + row_begin, g_row1 = (square ? 0 : n_fit) + row_end;
   auto max_n = [&](int64_t g0, int64_t g1) {
     int m = 0;
     for (int64_t g = g0; g < g1; ++g) m = std::max(m, ex->graph_ptr[g + 1] - ex->graph_ptr[g]);
@@ -2527,36 +2565,23 @@ static int gram_rw(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin
     d.out = h->diag_f64.as<double>();
     GK_TRY(rw_launch(h, d, (size_t)nvec * nmax_all * nmax_all));
   }
-  const bool mirror = square && row_begin == 0 && row_end == N && !(flags & GK_FULL_TILES);
+  const bool mirror = q.full_square && !(q.flags & GK_FULL_TILES);
   if (k_rows > 0) {
     RwParams k = p;
     k.pairs = mirror ? RW_PAIRS_TRIANGLE : RW_PAIRS_RECT;
     k.ordered = square ? 1 : 0;
     k.n_pairs = mirror ? N * (N + 1) / 2 : k_rows * k_cols;
-    k.row_g0 = (int)g_row0;
+    k.row_g0 = q.a0;
     k.rows = (int)k_rows; k.cols = (int)k_cols;
-    k.out = d_out; k.ld = d_ld;
+    k.out = out.p; k.ld = out.ld;
     k.iters = h->rw_iters.as<unsigned char>();
-    const size_t nr = mirror ? nmax_all : max_n(g_row0, g_row1), nc = max_n(0, n_fit);
+    const size_t nr = mirror ? nmax_all : max_n(q.a0, q.a1), nc = max_n(0, n_fit);
     GK_TRY(rw_launch(h, k, (size_t)nvec * nr * nc));
-    if (flags & GK_NORMALIZE) {
-      normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(k_rows, k_cols, d_out, d_ld,
-                                                                      h->diag_f64.as<double>() + g_row0,
-                                                                      h->diag_f64.as<double>(), (flags & GK_NAN_TO_NUM) ? 1 : 0);
-      LAUNCH_CHECK(h);
-    }
   }
   h->rw_iter_rows = k_rows; h->rw_iter_cols = k_cols;
-  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
-  if (K_out && !dev_out && k_rows > 0)
-    GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * 8, d_out, (size_t)d_ld * 8, (size_t)k_cols * 8, (size_t)k_rows,
-                              cudaMemcpyDeviceToHost, h->stream));
-  if (xdiag) GK_CUDA(cudaMemcpyAsync(xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (ydiag && !square)
-    GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_TRY(f64_deliver(h, q, out, true, h->tev[3], h->tev[4]));
   unsigned long long cap_hits = 0;
   GK_CUDA(cudaMemcpyAsync(&cap_hits, h->rw_cap.p, 8, cudaMemcpyDeviceToHost, h->stream));
-  GK_CUDA(cudaEventRecord(h->tev[4], h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
   if (stats) {
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
@@ -2677,54 +2702,13 @@ static int comm_share_K(gk_handle* h, size_t bytes) {
   return GK_OK;
 }
 
-extern "C" {
-
-int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
-            int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (!h->features_ready) return fail(GK_ERR_STATE, "gk_gram: no feature block (call gk_wl_features / gk_sp_features)");
-  if (out_dtype != GK_F32 && out_dtype != GK_F64) return fail(GK_ERR_ARG, "gk_gram: bad out_dtype");
-  const int64_t N = h->n_rows > 0 ? h->n_rows : h->N;  // rows of the feature block (gk_set_row_map)
-  const int* d_row_map = h->n_rows > 0 ? h->row_map.as<int>() : nullptr;
-  if (n_fit <= 0 || n_fit > N) return fail(GK_ERR_ARG, "gk_gram: n_fit out of range");
-  if (h->feature_kind == 3) {
-    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with ShortestPathAttr features");
-    GK_CUDA(cudaSetDevice(h->dev));
-    return gram_spattr(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
-  }
-  if (h->feature_kind == 4) {
-    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with GraphHopper features");
-    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with GraphHopper features");
-    GK_CUDA(cudaSetDevice(h->dev));
-    if (h->gh_node_kernel == GK_GH_LINEAR)
-      return gram_spattr(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
-    return gram_gh_nodepair(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
-  }
-  if (h->feature_kind == 5) {
-    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with NeighborhoodHash features");
-    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with NeighborhoodHash features");
-    GK_CUDA(cudaSetDevice(h->dev));
-    return gram_nh(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
-  }
-  if (h->feature_kind == 6) {
-    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with random walk features");
-    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with random walk features");
-    GK_CUDA(cudaSetDevice(h->dev));
-    return gram_rw(h, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, stats);
-  }
-  if (h->feature_kind == 7) {  // Propagation: the generic integer route; the row map and distributed paths are untested
-    if (d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: row map with Propagation features");
-    if (flags & (GK_DIST | GK_DIST_GATHER)) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST with Propagation features");
-  }
-  const bool square = n_fit == N;
-  const int64_t k_rows_total = square ? N : N - n_fit;
-  const int64_t k_cols = n_fit;
-  if (row_end < 0) row_end = k_rows_total;
-  if (row_begin < 0 || row_begin > row_end || row_end > k_rows_total) return fail(GK_ERR_ARG, "gk_gram: bad row range");
-  const int64_t k_rows = row_end - row_begin;
-  if (ld <= 0) ld = k_cols;
-  if (ld < k_cols) return fail(GK_ERR_ARG, "gk_gram: ld smaller than the row length");
-  GK_CUDA(cudaSetDevice(h->dev));
+// The integer Gram of the counts in `fb` (gram_path 1 tensor cores, 2 CUDA cores, 3 no shared column), with the
+// head/tail split of its columns, fp32 or fp64 output, GK_NORMALIZE, a row map and GK_DIST.
+static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats* stats) {
+  const int64_t N = q.N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols, row_begin = q.row_begin, row_end = q.row_end;
+  const int32_t flags = q.flags, out_dtype = q.out_dtype;
+  const bool square = q.square;
+  const int* d_row_map = q.row_map;
   const int64_t launches0 = h->launches;
   const bool normalize = flags & GK_NORMALIZE;
   const size_t esz = out_dtype == GK_F64 ? 8 : 4;
@@ -2732,17 +2716,17 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
 
   GK_CUDA(cudaEventRecord(h->tev[4], h->stream));
   // ---- column statistics were maintained by the feature kernels; finish the self similarities
-  const int64_t D = std::max<int64_t>(h->n_columns, 1);
-  if (D > h->col_cap) return fail(GK_ERR_STATE, "gk_gram: column statistics missing");
+  const int64_t D = std::max<int64_t>(fb.n_columns, 1);
+  if (D > fb.col_cap) return fail(GK_ERR_STATE, "gk_gram: column statistics missing");
   const int nbc = cdiv(D, 256);
   GK_TRY(h->colslot.ensure(D * 4));
   GK_TRY(h->colstats.ensure(sizeof(ColStats)));
   GK_TRY(h->h_colstats.ensure(sizeof(ColStats)));
   GK_TRY(h->diag_f64.ensure(N * 8));
   HandleExtra* hx = extra_of(h);
-  const bool pro = square && !d_row_map && h->pro_serial == h->feat_serial && D <= h->col_cap;  // prologue already on the host
+  const bool pro = square && !d_row_map && fb.prologue_on_host && D <= fb.col_cap;
   if (!pro) GK_CUDA(cudaMemsetAsync(&sc->n_entries, 0, sizeof(unsigned long long) * 3 + sizeof(long long), h->stream));
-  const unsigned long long* d_diag_u64 = h->diag_u64.as<unsigned long long>();
+  const unsigned long long* d_diag_u64 = fb.diag;
   if (d_row_map) {
     GK_TRY(h->diag_rows.ensure(N * 8));
     GK_CUDA(cudaMemsetAsync(h->diag_rows.p, 0, N * 8, h->stream));
@@ -2752,8 +2736,8 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   }
   if (!pro) {
     diag_finish<<<cdiv(N, 256), 256, 0, h->stream>>>((int)N, d_diag_u64,
-                                                     h->diag_f64.as<double>(), (int)h->n_part,
-                                                     h->part_max.as<unsigned>(), h->part_new.as<unsigned>(), sc);
+                                                     h->diag_f64.as<double>(), (int)fb.n_part, fb.part_max,
+                                                     fb.part_new, sc);
     LAUNCH_CHECK(h);
   }
   if (!square) {  // which columns occur on both the X and the Y side
@@ -2761,7 +2745,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     GK_TRY(h->colmax.ensure(D * 4));
     GK_CUDA(cudaMemsetAsync(h->colmin.p, 0x7F, D * 4, h->stream));
     GK_CUDA(cudaMemsetAsync(h->colmax.p, 0xFF, D * 4, h->stream));
-    feat_minmax<<<h->sm_count * 16, 256, 0, h->stream>>>(h->ft_cap, h->ft_keys.as<unsigned long long>(), d_row_map,
+    feat_minmax<<<h->sm_count * 16, 256, 0, h->stream>>>(fb.cap, fb.keys, d_row_map,
                                                          h->colmin.as<int>(), h->colmax.as<int>());
     LAUNCH_CHECK(h);
   }
@@ -2783,7 +2767,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     max_count = hx->pro_max_count; max_diag = hx->pro_max_diag; n_entries = hx->pro_n_entries;
   } else {
     GK_CUDA(cudaMemsetAsync(cs, 0, sizeof(ColStats), h->stream));
-    col_hist<<<nbc, 256, 0, h->stream>>>(D, square ? 1 : 0, (int)n_fit, h->colcnt.as<unsigned>(), h->colmin.as<int>(),
+    col_hist<<<nbc, 256, 0, h->stream>>>(D, square ? 1 : 0, (int)n_fit, fb.colcnt, h->colmin.as<int>(),
                                          h->colmax.as<int>(), cs);
     LAUNCH_CHECK(h);
     GK_CUDA(cudaMemcpyAsync(h->h_colstats.p, cs, sizeof(ColStats), cudaMemcpyDeviceToHost, h->stream));
@@ -2841,7 +2825,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   GK_TRY(h->tail_cur.ensure((size_t)std::max<int64_t>(n_tail_cols, 1) * 4));
   unsigned* col_counters = reinterpret_cast<unsigned*>(cs);  // the histogram has been read: reuse its first words
   GK_CUDA(cudaMemsetAsync(col_counters, 0, 16, h->stream));
-  col_classify<<<nbc, 256, 0, h->stream>>>(D, square ? 1 : 0, (int)n_fit, h->colcnt.as<unsigned>(), h->colmin.as<int>(),
+  col_classify<<<nbc, 256, 0, h->stream>>>(D, square ? 1 : 0, (int)n_fit, fb.colcnt, h->colmin.as<int>(),
                                            h->colmax.as<int>(), T, h->colslot.as<int>(), h->tail_desc.as<int2>(),
                                            h->tail_cur.as<unsigned>(), col_counters);
   LAUNCH_CHECK(h);
@@ -2856,7 +2840,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   // by host threads while the next band is in flight (host_deliver.h).  GRAKEL_B200_WIDEN=0 restores the
   // plain fp64 D2H copy of a device-side fp64 result.
   const char* widen_env = getenv("GRAKEL_B200_WIDEN");
-  const bool widen_on_host = K_out && !(flags & GK_OUT_DEVICE) && out_dtype == GK_F64 && path != 2 &&
+  const bool widen_on_host = q.K_out && !(flags & GK_OUT_DEVICE) && out_dtype == GK_F64 && path != 2 &&
                              !(widen_env && atoi(widen_env) == 0);
   const bool host_norm = widen_on_host && normalize;
   const int32_t dev_dtype = widen_on_host ? GK_F32 : out_dtype;
@@ -2867,14 +2851,6 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   // row block with full tiles (the decision depends on replicated data only, so all ranks take the same branch).
   Comm* comm = reinterpret_cast<Comm*>(h->comm);
   const bool dist_req = (flags & (GK_DIST | GK_DIST_GATHER)) != 0;
-  if (dist_req) {
-    if (!comm) return fail(GK_ERR_STATE, "gk_gram: GK_DIST without gk_comm_init");
-    if (!square || d_row_map) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST needs the square fit_transform case without a row map");
-    if (flags & GK_OUT_DEVICE) return fail(GK_ERR_UNSUPPORTED, "gk_gram: GK_DIST results are library-owned (gk_result_device / gk_fetch / host K_out)");
-    int64_t rb = 0, re = 0;
-    GK_TRY(gk_comm_rows(h, N, &rb, &re));
-    if (row_begin != rb || row_end != re) return fail(GK_ERR_ARG, "gk_gram: GK_DIST row range must be the one gk_comm_rows returns");
-  }
   // GRAKEL_B200_DIST_SHARE=0: no tile sharing -- every rank computes its row block with full tiles (twice the SYRK
   // flops, no peer stores, no barriers): the round-1 scheme, kept for A/B measurements
   const char* e_share = getenv("GRAKEL_B200_DIST_SHARE");
@@ -2886,8 +2862,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   // ---- output buffer
   void* d_out = nullptr;
   if (flags & GK_OUT_DEVICE) {
-    if (!K_out) return fail(GK_ERR_ARG, "gk_gram: GK_OUT_DEVICE without a pointer");
-    d_out = K_out;
+    d_out = q.K_out;
   } else {
     // library-owned K: rows padded to a multiple of 8 elements so that every row is 32-byte aligned
     // (TMA / 256-bit stores in the GEMM epilogue for any n_fit, e.g. 14 142 graphs on 2 GPUs)
@@ -2903,12 +2878,12 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     }
     h->K_rows = k_rows; h->K_cols = k_cols; h->K_dtype = dev_dtype;
   }
-  const long long d_ld = (flags & GK_OUT_DEVICE) ? ld : h->K_ld;
+  const long long d_ld = (flags & GK_OUT_DEVICE) ? q.ld : h->K_ld;
 
   // panel-row ranges: A rows index K rows, B rows index K columns
-  const int a0 = (int)((square ? 0 : n_fit) + row_begin), a1 = (int)((square ? 0 : n_fit) + row_end);
+  const int a0 = q.a0, a1 = q.a1;
   const int b0 = 0, b1 = (int)n_fit;
-  const bool full_square = square && row_begin == 0 && row_end == N;
+  const bool full_square = q.full_square;
   const bool mirror = (full_square && !(flags & GK_FULL_TILES)) || dist;
   const bool has_tail = path != 2 && n_tail_cols > 0;
   const bool norm_in_epilogue = normalize && !has_tail && !host_norm;
@@ -2943,13 +2918,13 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
       if (Dc) GK_CUDA(cudaMemsetAsync(h->panel.p, 0, panel_bytes, h->stream));
       if (Dc || has_tail) {
         if (elem_bytes == 1)
-          feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
-              h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), d_row_map,
+          feat_scatter<<<cdiv((long long)fb.cap, 256), 256, 0, h->stream>>>(
+              fb.cap, fb.keys, fb.cnt, h->colslot.as<int>(), d_row_map,
               h->panel.as<uint8_t>(), h->Dc_pad, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(),
               h->tail_ent.as<int2>());
         else
-          feat_scatter<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
-              h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), d_row_map,
+          feat_scatter<<<cdiv((long long)fb.cap, 256), 256, 0, h->stream>>>(
+              fb.cap, fb.keys, fb.cnt, h->colslot.as<int>(), d_row_map,
               h->panel.as<__nv_bfloat16>(), h->Dc_pad, h->tail_cur.as<unsigned>(), h->tail_desc.as<int2>(),
               h->tail_ent.as<int2>());
         LAUNCH_CHECK(h);
@@ -3033,8 +3008,8 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
       const size_t panel_bytes = (size_t)N * std::max<int64_t>(Dc, 1) * 4;
       GK_TRY(h->panel.ensure(panel_bytes));
       GK_CUDA(cudaMemsetAsync(h->panel.p, 0, panel_bytes, h->stream));
-      feat_fill_panel_u32<<<cdiv((long long)h->ft_cap, 256), 256, 0, h->stream>>>(
-          h->ft_cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colslot.as<int>(), d_row_map,
+      feat_fill_panel_u32<<<cdiv((long long)fb.cap, 256), 256, 0, h->stream>>>(
+          fb.cap, fb.keys, fb.cnt, h->colslot.as<int>(), d_row_map,
           h->panel.as<unsigned>(), std::max<int64_t>(Dc, 1));
       LAUNCH_CHECK(h);
       GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
@@ -3089,30 +3064,30 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
 
   // ---- results to the host
   GK_CUDA(cudaEventRecord(h->ev[14], h->stream));
-  if (K_out && !(flags & GK_OUT_DEVICE) && k_rows > 0) {
+  if (q.K_out && !(flags & GK_OUT_DEVICE) && k_rows > 0) {
     if (widen_on_host) {
       const float* d_k = reinterpret_cast<const float*>(d_out);
-      double* dst = reinterpret_cast<double*>(K_out);
+      double* dst = reinterpret_cast<double*>(q.K_out);
       DeviceCopier cp{h};
       if (host_norm) {
         GK_TRY(h->h_diag.ensure((size_t)N * 8));
         GK_CUDA(cudaMemcpyAsync(h->h_diag.p, h->diag_f64.p, (size_t)N * 8, cudaMemcpyDeviceToHost, h->stream));
         GK_CUDA(cudaStreamSynchronize(h->stream));
-        GK_TRY(deliver_rows(cp, d_k, d_ld, k_rows, k_cols, dst, ld, h->h_diag.as<double>() + a0, h->h_diag.as<double>() + b0,
+        GK_TRY(deliver_rows(cp, d_k, d_ld, k_rows, k_cols, dst, q.ld, h->h_diag.as<double>() + a0, h->h_diag.as<double>() + b0,
                             p.nan_to_num));
       } else if (full_square && !getenv("GRAKEL_B200_NO_TRI")) {
-        GK_TRY(deliver_square(h, d_k, d_ld, k_rows, dst, ld, max_diag));
+        GK_TRY(deliver_square(h, d_k, d_ld, k_rows, dst, q.ld, max_diag));
       } else {
-        GK_TRY(deliver_rows(cp, d_k, d_ld, k_rows, k_cols, dst, ld, nullptr, nullptr, 0));
+        GK_TRY(deliver_rows(cp, d_k, d_ld, k_rows, k_cols, dst, q.ld, nullptr, nullptr, 0));
       }
     } else {
-      GK_CUDA(cudaMemcpy2DAsync(K_out, (size_t)ld * esz, d_out, (size_t)d_ld * esz, (size_t)k_cols * esz,
+      GK_CUDA(cudaMemcpy2DAsync(q.K_out, (size_t)q.ld * esz, d_out, (size_t)d_ld * esz, (size_t)k_cols * esz,
                                 (size_t)k_rows, cudaMemcpyDeviceToHost, h->stream));
     }
   }
-  if (xdiag) GK_CUDA(cudaMemcpyAsync(xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
-  if (ydiag && !square)
-    GK_CUDA(cudaMemcpyAsync(ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (q.xdiag) GK_CUDA(cudaMemcpyAsync(q.xdiag, h->diag_f64.p, n_fit * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (q.ydiag && !square)
+    GK_CUDA(cudaMemcpyAsync(q.ydiag, h->diag_f64.as<double>() + n_fit, (N - n_fit) * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaEventRecord(h->ev[15], h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
   if (stats) {
@@ -3135,6 +3110,24 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     stats->ms_total = ev_ms(h->tev[4], h->ev[15]);
   }
   return GK_OK;
+}
+
+extern "C" {
+
+int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
+            int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (!h->features_ready) return fail(GK_ERR_STATE, "gk_gram: no feature block (call gk_wl_features / gk_sp_features)");
+  GramReq q;
+  GK_TRY(gram_request(h, h->feature_kind, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, &q));
+  GK_CUDA(cudaSetDevice(h->dev));
+  switch (h->feature_kind) {
+    case FK_SPATTR: return gram_spattr(h, q, stats);
+    case FK_GH: return h->gh_node_kernel == GK_GH_LINEAR ? gram_spattr(h, q, stats) : gram_gh_nodepair(h, q, stats);
+    case FK_NH: return gram_nh(h, q, stats);
+    case FK_RW: return gram_rw(h, q, stats);
+    default: return gram_int(h, q, block_of(h), stats);
+  }
 }
 
 int gk_set_row_map(gk_handle* h, int64_t n_rows, const int32_t* row_of_graph) {
@@ -3471,7 +3464,7 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   // ---- state as gk_wl_features + gk_gram leave it
   h->n_columns = hd.n_columns;
   h->features_ready = true; h->feat_serial++;
-  h->feature_kind = 1;
+  h->feature_kind = FK_WL;
   h->Dc = hd.Dc; h->Dc_pad = hd.Dc_pad;
   if (force_T < 0) hx->head_row_bytes = (long long)hd.Dc_pad * elem_bytes;
   hx->last_max_count = (long long)hd.max_count;

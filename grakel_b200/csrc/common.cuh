@@ -110,6 +110,18 @@ struct DevScalars {
 
 static_assert(sizeof(DevScalars) % 8 == 0, "cleared as 64-bit words");
 
+// What the handle's feature block holds, i.e. which gk_gram route computes K from it.
+enum FeatureKind : int {
+  FK_NONE = 0,
+  FK_WL = 1,      // WL / WL-OA / VertexHistogram / EdgeHistogram (graph, column) counts: the integer Gram
+  FK_SP = 2,      // ShortestPath (lu, lv, d) counts: the integer Gram
+  FK_SPATTR = 3,  // ShortestPathAttr dense fp64 feature matrix
+  FK_GH = 4,      // GraphHopper per-vertex maps
+  FK_NH = 5,      // NeighborhoodHash per-level expanded blocks
+  FK_RW = 6,      // random walk edge values
+  FK_PK = 7,      // Propagation counts in the SP layout: the integer Gram
+};
+
 }  // namespace gk
 
 // The opaque handle of the C-ABI.
@@ -161,8 +173,7 @@ struct gk_handle {
   int64_t pro_serial = -1;   // feat_serial for which gk_wl_features already ran the Gram prologue (square case):
                              // self similarities finished, column histogram on the host -- gk_gram then needs no
                              // host synchronisation before its launches
-  int feature_kind = 0;  // 1 = WL, 2 = SP, 3 = SP-attr (dense fp32 features), 4 = GraphHopper, 5 = NeighborhoodHash,
-                         // 6 = random walk, 7 = Propagation (SP-layout integer features)
+  gk::FeatureKind feature_kind = gk::FK_NONE;
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
   // ---- columns / panel / diag
@@ -196,27 +207,27 @@ struct gk_handle {
   int64_t fattr_dim = 0;
   bool fattr_signed = false;  // some feature is negative: entries of K may cancel (gram_spattr takes the fp64 Gram)
 
-  // ---- GraphHopper (feature_kind 4): per-vertex maps M [V][delta (delta + 1) / 2] fp64
+  // ---- GraphHopper (FK_GH): per-vertex maps M [V][delta (delta + 1) / 2] fp64
   gk::DevBuf gh_M, gh_ws, gh_woff, gh_gdiam, gh_groups, gh_pairs;
   int gh_delta = 0;
   int gh_node_kernel = 0;  // GK_GH_LINEAR / GK_GH_GAUSSIAN / GK_GH_BRIDGE
   double gh_mu = 1.0;
 
-  // ---- NeighborhoodHash (feature_kind 5)
+  // ---- NeighborhoodHash (FK_NH)
   gk::DevBuf nh_codes, nh_valid;  // [(R + 1) V] u64 codes / u8 not-None flags: the initial labels, then levels 0 .. R-1
   gk::DevBuf nh_blk;              // unary-expanded (graph, column) block of every level, nh_level_bytes apart
   gk::DevBuf nh_lut, nh_tab, nh_ws, nh_cur, nh_C;
   size_t nh_level_bytes = 0;
   int nh_R = 0;
 
-  // ---- random walk (feature_kind 6): edge values of the packed CSR, its transpose, eigen-data, coefficients
+  // ---- random walk (FK_RW): edge values of the packed CSR, its transpose, eigen-data, coefficients
   gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;
   int rw_route = 0, rw_fn = 0, rw_ncoef = 0;
   double rw_lamda = 0.0;
   bool rw_labeled = false;
   int64_t rw_iter_rows = 0, rw_iter_cols = 0;  // shape of the iteration counts of the last gk_gram
 
-  // ---- Propagation (feature_kind 7): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
+  // ---- Propagation (FK_PK): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
   // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]
   gk::DevBuf pk_P, pk_bins, pk_priv, pk_tval, pk_u, pk_b, pk_tab, pk_cnt;
   int pk_levels = 0, pk_K = 0;
