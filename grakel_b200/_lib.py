@@ -26,6 +26,7 @@ GK_RW_CG, GK_RW_SPECTRAL, GK_RW_SERIES = 0, 1, 2
 GK_RW_FINITE, GK_RW_EXP, GK_RW_INV = 0, 1, 2
 GK_RW_LABELED = 1
 GK_PK_ATTR, GK_PK_SQRT, GK_PK_STORE_F32, GK_PK_STORE_INT, GK_PK_NEW_LABELS = 1, 2, 4, 8, 16
+GK_PM_LABELS, GK_PM_WL_LABELS = 1, 2
 
 
 class GkStats(C.Structure):
@@ -81,6 +82,9 @@ _SYMBOLS = {
     "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
+    "gk_pm_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, C.c_int32,
+                                 C.POINTER(GkStats)]),
+    "gk_pm_cells": (C.c_int, [_P, C.c_int32, C.c_int32, _P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -350,6 +354,26 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_pk_hashes(self.h, int(level), _ptr(out), _ptr(priv)))
         return out, priv.astype(bool)
+
+    def pm_features(self, L, d, U, n_cols, n_iter=0, flags=0, skip=None):
+        """PyramidMatch level blocks (gk_pm_features).  U: [n_sets, V, d] fp64 embeddings, n_cols: [n_sets, N] column
+        counts; flags GK_PM_LABELS (packed label ids) or GK_PM_WL_LABELS (WL level s after wl_features(n_iter));
+        skip: [V] flags of the vertices without entries, or None."""
+        U = np.ascontiguousarray(U, dtype=np.float64)
+        nc = np.ascontiguousarray(n_cols, dtype=np.int32)
+        sk = None if skip is None else np.ascontiguousarray(skip, dtype=np.uint8)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_pm_features(self.h, int(n_iter), int(L), int(d), _ptr(U), _ptr(nc), _ptr(sk),
+                                                nc.shape[0], int(flags), C.byref(st)))
+        return st
+
+    def pm_cells(self, s, level, n_vertices, d):
+        """[V, d] int64 cells of embedding set s at level `level` (-1 past a graph's column count)."""
+        out = np.empty((n_vertices, d), dtype=np.int64)
+        with self._lock:
+            self._check(self.lib.gk_pm_cells(self.h, int(s), int(level), _ptr(out)))
+        return out
 
     def rw_iterations(self, rows, cols):
         """CG iterations / series terms of every entry of the last random walk gram() (rows x cols u8)."""

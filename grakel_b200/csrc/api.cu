@@ -29,6 +29,7 @@
 #include "neighborhood_hash.cuh"
 #include "random_walk.cuh"
 #include "propagation.cuh"
+#include "pyramid_match.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -330,7 +331,8 @@ int gk_destroy(gk_handle* h) {
                         &h->nh_codes, &h->nh_valid, &h->nh_blk, &h->nh_lut, &h->nh_tab, &h->nh_ws, &h->nh_cur, &h->nh_C,
                         &h->rw_val, &h->rw_trp, &h->rw_tci, &h->rw_tval, &h->rw_q, &h->rw_w, &h->rw_coef, &h->rw_ws,
                         &h->rw_iters, &h->rw_cap,
-                        &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt};
+                        &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt,
+                        &h->pm_U, &h->pm_ncols, &h->pm_skip};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1500,6 +1502,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_NH     */ {"NeighborhoodHash", false, true, false, false},
     /* FK_RW     */ {"random walk", false, true, false, false},
     /* FK_PK     */ {"Propagation", true, true, false, false},
+    /* FK_PM     */ {"PyramidMatch", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -1941,18 +1944,19 @@ static int gram_gh_nodepair(gk_handle* h, const GramReq& q, gk_stats* stats) {
 
 // ---------------------------------------------------------------------------
 // NeighborhoodHash (neighborhood_hash.cuh).  Level r's expanded block lives at nh_blk + r * nh_level_bytes:
-// keys [V] u64 | counts [V] u32 | graphs per column [V + 1] u32 | self similarities [N] u64 (at most one unary entry
-// per non-None vertex, so V entries and V columns bound every level).
-static size_t nh_level_bytes(int64_t V, int64_t N) {
-  const size_t V1 = (size_t)std::max<int64_t>(V, 1);
+// keys [M] u64 | counts [M] u32 | graphs per column [M + 1] u32 | self similarities [N] u64, M = nh_level_cap (at
+// most one unary entry per non-None vertex, so V entries and V columns bound every NeighborhoodHash level;
+// PyramidMatch has d entries per vertex).
+static size_t nh_level_bytes(int64_t M, int64_t N) {
+  const size_t V1 = (size_t)std::max<int64_t>(M, 1);
   const size_t diag_off = (16 * V1 + 4 + 7) / 8 * 8;
   return (diag_off + 8 * (size_t)std::max<int64_t>(N, 1) + 255) / 256 * 256;
 }
 
 // Level r's block as an integer feature block; its self similarities are one partial (part_max / part_new, uploaded
-// by gram_nh), its column count is set by gram_nh.
+// by gram_levels), its column count is set by gram_levels.
 static IntBlock nh_level(gk_handle* h, int r) {
-  const size_t V1 = (size_t)std::max<int64_t>(h->V, 1);
+  const size_t V1 = (size_t)std::max<int64_t>(h->nh_level_cap, 1);
   char* b = h->nh_blk.as<char>() + (size_t)r * h->nh_level_bytes;
   IntBlock L;
   L.keys = reinterpret_cast<unsigned long long*>(b);
@@ -1964,6 +1968,97 @@ static IntBlock nh_level(gk_handle* h, int r) {
   L.part_max = h->part_max.as<unsigned>(); L.part_new = h->part_new.as<unsigned>(); L.n_part = 1;
   L.prologue_on_host = false;
   return L;
+}
+
+// The per-level column pipeline NeighborhoodHash and PyramidMatch share: every level's M entries (codes + valid
+// flags) are numbered by distinct code (nh_code_insert / nh_code_number), counted per (graph, column) (nh_count, entry
+// e belongs to vertex e / per) and unary-expanded into level block r (oa_colmax / oa_colbase / oa_expand), so that the
+// integer Gram of block r gives the levels' multiset intersections.
+struct LevelScratch {
+  size_t cap, cur_bytes;
+  OaCursors* cur;
+  unsigned long long* dims;
+  int *tab, *colid, *slot_of;
+};
+
+static int level_setup(gk_handle* h, int64_t M, int n_blocks, LevelScratch* ls) {
+  const int64_t M1 = std::max<int64_t>(M, 1);
+  const size_t cap = std::max<size_t>(next_pow2((size_t)M1 * 2), 1024);
+  h->nh_level_cap = M1;
+  h->nh_level_bytes = nh_level_bytes(M, h->N);
+  GK_TRY(h->nh_blk.ensure((size_t)n_blocks * h->nh_level_bytes));
+  GK_TRY(h->nh_tab.ensure(cap * 8 + (size_t)M1 * 4));  // slot -> claiming entry | slot -> column | entry -> slot
+  GK_TRY(h->ft_keys.ensure(cap * 8));                 // (graph, column) -> count scratch table
+  GK_TRY(h->ft_cnt.ensure(cap * 4));
+  GK_TRY(h->colmin.ensure((size_t)M1 * 4));  // largest count of every column
+  GK_TRY(h->colmax.ensure((size_t)M1 * 4));  // first expanded column of every column
+  ls->cap = cap;
+  ls->cur_bytes = (size_t)n_blocks * (sizeof(OaCursors) + 8);
+  GK_TRY(h->nh_cur.ensure(ls->cur_bytes));
+  GK_TRY(h->h_colstats.ensure(std::max(ls->cur_bytes, sizeof(ColStats))));
+  ls->cur = h->nh_cur.as<OaCursors>();
+  ls->dims = reinterpret_cast<unsigned long long*>(ls->cur + n_blocks);
+  ls->tab = h->nh_tab.as<int>();
+  ls->colid = ls->tab + cap;
+  ls->slot_of = ls->colid + cap;
+  GK_CUDA(cudaMemsetAsync(h->nh_cur.p, 0, ls->cur_bytes, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->nh_blk.p, 0, (size_t)n_blocks * h->nh_level_bytes, h->stream));
+  return GK_OK;
+}
+
+static int level_columns(gk_handle* h, const LevelScratch& ls, int r, int64_t M, int per, const unsigned long long* c_r,
+                         const unsigned char* v_r) {
+  const int64_t M1 = h->nh_level_cap;
+  const size_t cap = ls.cap;
+  const IntBlock lv = nh_level(h, r);
+  GK_CUDA(cudaMemsetAsync(lv.keys, 0xFF, (size_t)M1 * 8, h->stream));
+  if (!M) return GK_OK;
+  GK_CUDA(cudaMemsetAsync(ls.tab, 0xFF, cap * 4, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->ft_keys.p, 0xFF, cap * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->ft_cnt.p, 0, cap * 4, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->colmin.p, 0, (size_t)M1 * 4, h->stream));
+  nh_code_insert<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, c_r, v_r, ls.tab, (unsigned)(cap - 1), ls.slot_of);
+  LAUNCH_CHECK(h);
+  nh_code_number<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, v_r, ls.tab, ls.slot_of, ls.colid, ls.dims + r);
+  LAUNCH_CHECK(h);
+  nh_count<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, per, v_r, h->vgraph.as<int>(), ls.slot_of, ls.colid,
+                                                h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
+                                                (unsigned)(cap - 1));
+  LAUNCH_CHECK(h);
+  oa_colmax<<<h->sm_count * 8, 256, 0, h->stream>>>(cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
+                                                    h->colmin.as<unsigned>());
+  LAUNCH_CHECK(h);
+  oa_colbase<<<cdiv(M1, OA_THREADS), OA_THREADS, 0, h->stream>>>(M1, h->colmin.as<unsigned>(), h->colmax.as<unsigned>(),
+                                                                 ls.cur + r);
+  LAUNCH_CHECK(h);
+  oa_expand<<<cdiv((long long)cap, OA_THREADS), OA_THREADS, 0, h->stream>>>(
+      cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colmax.as<unsigned>(), (size_t)M1, lv.keys,
+      lv.cnt, ls.cur + r, lv.colcnt, lv.diag, h->scalars.as<DevScalars>());
+  LAUNCH_CHECK(h);
+  return GK_OK;
+}
+
+// Reads the levels' column statistics back (synchronises) into the handle's per-level tables.
+static int level_finish(gk_handle* h, const LevelScratch& ls, int n_blocks, const char* who, DevScalars** hs,
+                        int64_t* n_cols, int64_t* n_ent) {
+  HandleExtra* ex = extra_of(h);
+  GK_CUDA(cudaMemcpyAsync(h->h_colstats.p, h->nh_cur.p, ls.cur_bytes, cudaMemcpyDeviceToHost, h->stream));
+  GK_TRY(read_scalars(h, hs));  // synchronises
+  if ((*hs)->ft_overflow) return fail(GK_ERR_STATE, std::string(who) + ": expanded feature block overflow");
+  const OaCursors* hc = h->h_colstats.as<OaCursors>();
+  const unsigned long long* hdims = reinterpret_cast<const unsigned long long*>(hc + n_blocks);
+  ex->nh_dims.assign(n_blocks, 0);
+  ex->nh_cols.assign(n_blocks, 0);
+  ex->nh_entries.assign(n_blocks, 0);
+  *n_cols = *n_ent = 0;
+  for (int r = 0; r < n_blocks; ++r) {
+    ex->nh_dims[r] = (long long)hdims[r];
+    ex->nh_cols[r] = (long long)hc[r].n_cols;
+    ex->nh_entries[r] = (long long)hc[r].n_entries;
+    *n_cols += ex->nh_cols[r];
+    *n_ent += ex->nh_entries[r];
+  }
+  return GK_OK;
 }
 
 int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const uint64_t* code_of_label,
@@ -2035,71 +2130,14 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
   GK_CUDA(cudaEventRecord(h->tev[5], h->stream));
 
   // ---- per-level columns, counts and unary expansion
-  const size_t cap = std::max<size_t>(next_pow2((size_t)V1 * 2), 1024);
-  h->nh_level_bytes = nh_level_bytes(V, N);
-  GK_TRY(h->nh_blk.ensure((size_t)R * h->nh_level_bytes));
-  GK_TRY(h->nh_tab.ensure(cap * 8 + (size_t)V1 * 4));  // slot -> claiming vertex | slot -> column | vertex -> slot
-  GK_TRY(h->ft_keys.ensure(cap * 8));                 // (graph, column) -> count scratch table
-  GK_TRY(h->ft_cnt.ensure(cap * 4));
-  GK_TRY(h->colmin.ensure((size_t)V1 * 4));  // largest count of every column
-  GK_TRY(h->colmax.ensure((size_t)V1 * 4));  // first expanded column of every column
-  const size_t cur_bytes = (size_t)R * (sizeof(OaCursors) + 8);
-  GK_TRY(h->nh_cur.ensure(cur_bytes));
-  GK_TRY(h->h_colstats.ensure(std::max(cur_bytes, sizeof(ColStats))));
-  OaCursors* cur = h->nh_cur.as<OaCursors>();
-  unsigned long long* dims = reinterpret_cast<unsigned long long*>(cur + R);
-  int* tab = h->nh_tab.as<int>();
-  int* colid = tab + cap;
-  int* slot_of = colid + cap;
-  GK_CUDA(cudaMemsetAsync(h->nh_cur.p, 0, cur_bytes, h->stream));
-  GK_CUDA(cudaMemsetAsync(h->nh_blk.p, 0, (size_t)R * h->nh_level_bytes, h->stream));
-  for (int r = 0; r < R; ++r) {
-    const IntBlock lv = nh_level(h, r);
-    GK_CUDA(cudaMemsetAsync(lv.keys, 0xFF, (size_t)V1 * 8, h->stream));
-    if (!V) continue;
-    const unsigned long long* c_r = codes + (size_t)(r + 1) * V;
-    const unsigned char* v_r = valid + (size_t)(r + 1) * V;
-    GK_CUDA(cudaMemsetAsync(tab, 0xFF, cap * 4, h->stream));
-    GK_CUDA(cudaMemsetAsync(h->ft_keys.p, 0xFF, cap * 8, h->stream));
-    GK_CUDA(cudaMemsetAsync(h->ft_cnt.p, 0, cap * 4, h->stream));
-    GK_CUDA(cudaMemsetAsync(h->colmin.p, 0, (size_t)V1 * 4, h->stream));
-    nh_code_insert<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, c_r, v_r, tab, (unsigned)(cap - 1), slot_of);
-    LAUNCH_CHECK(h);
-    nh_code_number<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, v_r, tab, slot_of, colid, dims + r);
-    LAUNCH_CHECK(h);
-    nh_count<<<cdiv(V, 256), 256, 0, h->stream>>>((int)V, v_r, h->vgraph.as<int>(), slot_of, colid,
-                                                  h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
-                                                  (unsigned)(cap - 1));
-    LAUNCH_CHECK(h);
-    oa_colmax<<<h->sm_count * 8, 256, 0, h->stream>>>(cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(),
-                                                      h->colmin.as<unsigned>());
-    LAUNCH_CHECK(h);
-    oa_colbase<<<cdiv(V1, OA_THREADS), OA_THREADS, 0, h->stream>>>(V1, h->colmin.as<unsigned>(), h->colmax.as<unsigned>(),
-                                                                   cur + r);
-    LAUNCH_CHECK(h);
-    oa_expand<<<cdiv((long long)cap, OA_THREADS), OA_THREADS, 0, h->stream>>>(
-        cap, h->ft_keys.as<unsigned long long>(), h->ft_cnt.as<unsigned>(), h->colmax.as<unsigned>(), (size_t)V1, lv.keys,
-        lv.cnt, cur + r, lv.colcnt, lv.diag, h->scalars.as<DevScalars>());
-    LAUNCH_CHECK(h);
-  }
+  LevelScratch ls;
+  GK_TRY(level_setup(h, V, R, &ls));
+  for (int r = 0; r < R; ++r)
+    GK_TRY(level_columns(h, ls, r, V, 1, codes + (size_t)(r + 1) * V, valid + (size_t)(r + 1) * V));
   GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
-  GK_CUDA(cudaMemcpyAsync(h->h_colstats.p, h->nh_cur.p, cur_bytes, cudaMemcpyDeviceToHost, h->stream));
   DevScalars* hs;
-  GK_TRY(read_scalars(h, &hs));  // synchronises
-  if (hs->ft_overflow) return fail(GK_ERR_STATE, "gk_nh_features: expanded feature block overflow");
-  const OaCursors* hc = h->h_colstats.as<OaCursors>();
-  const unsigned long long* hdims = reinterpret_cast<const unsigned long long*>(hc + R);
-  ex->nh_dims.assign(R, 0);
-  ex->nh_cols.assign(R, 0);
-  ex->nh_entries.assign(R, 0);
   int64_t n_cols = 0, n_ent = 0;
-  for (int r = 0; r < R; ++r) {
-    ex->nh_dims[r] = (long long)hdims[r];
-    ex->nh_cols[r] = (long long)hc[r].n_cols;
-    ex->nh_entries[r] = (long long)hc[r].n_entries;
-    n_cols += ex->nh_cols[r];
-    n_ent += ex->nh_entries[r];
-  }
+  GK_TRY(level_finish(h, ls, R, "gk_nh_features", &hs, &n_cols, &n_ent));
   h->nh_R = R;
   h->n_columns = n_cols;
   h->features_ready = true; h->feat_serial++;
@@ -2137,39 +2175,51 @@ int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid) {
   return GK_OK;
 }
 
-// Gram of NeighborhoodHash features (gram_path 7): for every level, gk_gram's exact integer Gram of the level's
-// expanded block gives the intersection counts c_r as fp32 in nh_C; nh_combine turns the R count matrices into the
-// fp64 K.  Rows go in chunks when R count matrices of the whole request would exceed NH_C_BUDGET bytes
-// (GRAKEL_B200_NH_C_BUDGET=<bytes> lowers it, so that tests reach the chunked route; a chunk of
-// the square case then computes full rows instead of mirroring).  GK_NORMALIZE changes nothing: the reference never
-// normalises this kernel, and its self similarities are 1.
-constexpr size_t NH_C_BUDGET = (size_t)8 << 30;
+// The per-level Gram driver of NeighborhoodHash (gram_path 7) and PyramidMatch (gram_path 11): for every one of the
+// n_blocks level blocks, gram_int's exact integer Gram of the block gives the intersection counts as fp32 in nh_C;
+// `combine` turns the n_blocks count matrices of a row chunk into the fp64 K.  Rows go in chunks when the count
+// matrices of the whole request would exceed LEVEL_C_BUDGET bytes (GRAKEL_B200_NH_C_BUDGET=<bytes> lowers it, so that
+// tests reach the chunked route; a chunk of the square case then computes full rows instead of mirroring).
+}  // extern "C" (a template driver follows)
 
-static int gram_nh(gk_handle* h, const GramReq& q, gk_stats* stats) {
+constexpr size_t LEVEL_C_BUDGET = (size_t)8 << 30;
+
+struct LevelChunk {  // what a combine kernel reads and writes for rows [cb, cb + rows) of the request
+  const float* C;    // n_blocks matrices [rows x ldc], block r at C + r * stride
+  long long stride, ldc;
+  int row_g0;        // packed graph of the chunk's first row
+  int rows, cols;
+  int mirror;        // the full square matrix: compute upper tiles and mirror them
+  double* out;
+  long long ld;
+};
+
+struct LevelTimes {
+  std::vector<float> ms_block;
+  float ms_combine = 0.f;
+  int64_t max_T = 0, gram_launches = 0, elem_bytes = 0;
+};
+
+template <class Combine>
+static int gram_levels(gk_handle* h, const GramReq& q, int n_blocks, const F64Out& out, Combine combine, LevelTimes* t) {
   HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
-  const int R = h->nh_R;
   const bool square = q.square;
-  const int64_t launches0 = h->launches;
-  F64Out out;
-  GK_TRY(f64_target(h, q, &out));
   const int64_t ldc = (k_cols + 7) / 8 * 8;  // 32-byte rows: TMA stores of the Gram epilogue
-  size_t c_budget = NH_C_BUDGET;
+  size_t c_budget = LEVEL_C_BUDGET;
   if (const char* e = getenv("GRAKEL_B200_NH_C_BUDGET")) c_budget = std::max<size_t>(1, strtoull(e, nullptr, 10));
   const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(std::max<int64_t>(k_rows, 1),
-                                                                (int64_t)(c_budget / ((size_t)R * ldc * 4))));
-  GK_TRY(h->nh_C.ensure((size_t)R * chunk * ldc * 4));
+                                                                (int64_t)(c_budget / ((size_t)n_blocks * ldc * 4))));
+  GK_TRY(h->nh_C.ensure((size_t)n_blocks * chunk * ldc * 4));
   const int32_t gflags = (q.flags & (GK_GRAM_SIMT | GK_DENSE_ALL | GK_FULL_TILES)) | GK_OUT_DEVICE;
   GK_TRY(h->part_max.ensure(4));
   GK_TRY(h->part_new.ensure(4));
-  std::vector<float> ms_level(R, 0.f);
-  float ms_combine = 0.f;
+  t->ms_block.assign(n_blocks, 0.f);
   gk_stats st;
-  int64_t max_T = 0, gram_launches = 0, elem_bytes = 0;
   for (int64_t cb = q.row_begin; cb < q.row_end; cb += chunk) {
     const int64_t ce = std::min<int64_t>(q.row_end, cb + chunk), rows = ce - cb;
-    for (int r = 0; r < R; ++r) {
-      // the integer Gram of level r's expanded block: its rows [cb, ce) as fp32 counts into nh_C
+    for (int r = 0; r < n_blocks; ++r) {
+      // the integer Gram of level block r: its rows [cb, ce) as fp32 counts into nh_C
       IntBlock fb = nh_level(h, r);
       fb.n_columns = ex->nh_cols[r];
       const unsigned part[2] = {ex->nh_entries[r] ? 1u : 0u, (unsigned)ex->nh_entries[r]};
@@ -2180,36 +2230,66 @@ static int gram_nh(gk_handle* h, const GramReq& q, gk_stats* stats) {
                           nullptr, nullptr, &lq));
       memset(&st, 0, sizeof(st));
       GK_TRY(gram_int(h, lq, fb, &st));
-      ms_level[r] += st.ms_total;
-      max_T = std::max<int64_t>(max_T, st.threshold);
-      gram_launches += st.gemm_launches;
-      elem_bytes = std::max<int64_t>(elem_bytes, st.gemm_elem_bytes);  // 0 when no tensor-core GEMM ran
+      t->ms_block[r] += st.ms_total;
+      t->max_T = std::max<int64_t>(t->max_T, st.threshold);
+      t->gram_launches += st.gemm_launches;
+      t->elem_bytes = std::max<int64_t>(t->elem_bytes, st.gemm_elem_bytes);  // 0 when no tensor-core GEMM ran
     }
     if (rows > 0) {
-      NhCombineParams p;
-      p.C = h->nh_C.as<float>();
-      p.stride = chunk * ldc;
-      p.ldc = ldc;
-      p.R = R;
-      p.graph_ptr = h->graph_ptr.as<int>();
-      p.row_g0 = (int)((square ? 0 : n_fit) + cb);
-      p.rows = (int)rows;
-      p.cols = (int)k_cols;
-      p.mirror = square && cb == 0 && ce == N && !(q.flags & GK_FULL_TILES) ? 1 : 0;
-      p.out = out.p + (size_t)(cb - q.row_begin) * out.ld;
-      p.ld = out.ld;
-      const long long nbi = (rows + NH_TILE - 1) / NH_TILE, nbj = (k_cols + NH_TILE - 1) / NH_TILE;
-      const long long grid = p.mirror ? nbj * (nbj + 1) / 2 : nbi * nbj;
+      LevelChunk c;
+      c.C = h->nh_C.as<float>();
+      c.stride = chunk * ldc;
+      c.ldc = ldc;
+      c.row_g0 = (int)((square ? 0 : n_fit) + cb);
+      c.rows = (int)rows;
+      c.cols = (int)k_cols;
+      c.mirror = square && cb == 0 && ce == N && !(q.flags & GK_FULL_TILES) ? 1 : 0;
+      c.out = out.p + (size_t)(cb - q.row_begin) * out.ld;
+      c.ld = out.ld;
       GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
-      if (grid > 0) {
-        nh_combine<<<(unsigned)grid, NH_TILE * 8, 0, h->stream>>>(p);
-        LAUNCH_CHECK(h);
-      }
+      GK_TRY(combine(c));
       GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
       GK_CUDA(cudaEventSynchronize(h->tev[1]));
-      ms_combine += ev_ms(h->tev[0], h->tev[1]);
+      t->ms_combine += ev_ms(h->tev[0], h->tev[1]);
     }
   }
+  return GK_OK;
+}
+
+extern "C" {
+
+// Gram of NeighborhoodHash features (gram_path 7): gram_levels with nh_combine.  GK_NORMALIZE changes nothing: the
+// reference never normalises this kernel, and its self similarities are 1.
+static int gram_nh(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const int64_t N = h->N, n_fit = q.n_fit, k_cols = q.k_cols;
+  const int R = h->nh_R;
+  const bool square = q.square;
+  const int64_t launches0 = h->launches;
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  LevelTimes lt;
+  GK_TRY(gram_levels(h, q, R, out, [&](const LevelChunk& c) {
+    NhCombineParams p;
+    p.C = c.C;
+    p.stride = c.stride;
+    p.ldc = c.ldc;
+    p.R = R;
+    p.graph_ptr = h->graph_ptr.as<int>();
+    p.row_g0 = c.row_g0;
+    p.rows = c.rows;
+    p.cols = c.cols;
+    p.mirror = c.mirror;
+    p.out = c.out;
+    p.ld = c.ld;
+    const long long nbi = (c.rows + NH_TILE - 1) / NH_TILE, nbj = (k_cols + NH_TILE - 1) / NH_TILE;
+    const long long grid = p.mirror ? nbj * (nbj + 1) / 2 : nbi * nbj;
+    if (grid > 0) {
+      nh_combine<<<(unsigned)grid, NH_TILE * 8, 0, h->stream>>>(p);
+      LAUNCH_CHECK(h);
+    }
+    return GK_OK;
+  }, &lt));
+  const float ms_combine = lt.ms_combine;
   GramReq kq = q;  // the self similarities are 1, written on the host
   kq.xdiag = kq.ydiag = nullptr;
   GK_TRY(f64_deliver(h, kq, out, false, h->ev[14], h->ev[15]));
@@ -2219,14 +2299,208 @@ static int gram_nh(gk_handle* h, const GramReq& q, gk_stats* stats) {
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
     stats->n_levels = R;
     stats->gram_path = 7;
-    stats->threshold = max_T;
+    stats->threshold = lt.max_T;
     stats->max_count = 1;
-    stats->gemm_launches = gram_launches + (h->launches - launches0);
-    stats->gemm_elem_bytes = elem_bytes;
+    stats->gemm_launches = lt.gram_launches + (h->launches - launches0);
+    stats->gemm_elem_bytes = lt.elem_bytes;
     float tot = ms_combine;
-    for (int r = 0; r < R; ++r) { stats->ms_level_gram[r] = ms_level[r]; tot += ms_level[r]; }
+    for (int r = 0; r < R; ++r) { stats->ms_level_gram[r] = lt.ms_block[r]; tot += lt.ms_block[r]; }
     stats->ms_gemm = tot - ms_combine;
     stats->ms_combine = ms_combine;
+    stats->ms_d2h = ev_ms(h->ev[14], h->ev[15]);
+    stats->ms_total = tot + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
+// ---------------------------------------------------------------------------
+// PyramidMatch (pyramid_match.cuh).  The host hands over n_sets embedding sets U [n_sets][V][d] fp64 (|U| of every
+// vertex, zero past its graph's column count) and the column counts [n_sets][N]; each set's L levels become level
+// blocks s * L + j of the NeighborhoodHash layout.  Histogram rows come from the packed label ids (GK_PM_LABELS), from
+// WL level s of a preceding gk_wl_features (GK_PM_WL_LABELS: one set per WL level) or are the dimension alone.
+static int pm_keys(gk_handle* h, int s, int j, unsigned long long* keys, unsigned char* valid) {
+  const int64_t V = h->V, N = h->N, M = V * h->pm_d;
+  if (!M) return GK_OK;
+  const int* labels = nullptr;
+  if (h->pm_flags & GK_PM_WL_LABELS) labels = h->labels_all.as<int>() + (size_t)s * V;
+  else if (h->pm_flags & GK_PM_LABELS) labels = h->labels0.as<int>();
+  pm_cells<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, h->pm_d, j, h->pm_U.as<double>() + (size_t)s * M,
+                                                h->pm_ncols.as<int>() + (size_t)s * N, h->vgraph.as<int>(), labels,
+                                                h->pm_has_skip ? h->pm_skip.as<unsigned char>() : nullptr, keys, valid);
+  LAUNCH_CHECK(h);
+  return GK_OK;
+}
+
+int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const double* U, const int32_t* n_cols,
+                   const uint8_t* skip, int32_t n_sets, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_pm_features: no graphs packed");
+  if (L < 0) return fail(GK_ERR_ARG, "gk_pm_features: L < 0");
+  if (L > MAX_LEVELS) return fail(GK_ERR_UNSUPPORTED, "gk_pm_features: at most L = 64 levels are supported");
+  if (d < 1 || n_sets < 1) return fail(GK_ERR_ARG, "gk_pm_features: d and n_sets must be positive");
+  if (flags & ~(GK_PM_LABELS | GK_PM_WL_LABELS)) return fail(GK_ERR_ARG, "gk_pm_features: unknown flags");
+  if (!n_cols || (!U && h->V)) return fail(GK_ERR_ARG, "gk_pm_features: null embeddings or column counts");
+  const bool wl = flags & GK_PM_WL_LABELS;
+  if (wl && (h->feature_kind != FK_WL || !h->features_ready || h->n_levels != n_iter + 1 || n_sets != n_iter + 1))
+    return fail(GK_ERR_STATE, "gk_pm_features: GK_PM_WL_LABELS needs gk_wl_features(n_iter) first and n_iter + 1 sets");
+  if (!wl && n_sets != 1 && (flags & GK_PM_LABELS)) return fail(GK_ERR_ARG, "gk_pm_features: one set per label source");
+  if ((flags & GK_PM_LABELS) && !wl && !h->has_labels) return fail(GK_ERR_ARG, "gk_pm_features: vertex labels are required");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t N = h->N, V = h->V, M = V * (int64_t)d;
+  if (M >= (1LL << 31)) return fail(GK_ERR_UNSUPPORTED, "gk_pm_features: V * d must stay below 2^31");
+  // the level Grams count in fp32: exact while every intersection (<= d * n_max) stays below 2^24
+  if ((int64_t)h->max_graph_size * d >= (1LL << 24))
+    return fail(GK_ERR_UNSUPPORTED, "gk_pm_features: d * (largest graph) must stay below 2^24");
+  // (row, cell) keys: row < n_lab * d, cell < 2^(L-1), row << (L-1) must fit 64 bits
+  const int64_t n_lab = wl ? std::max<int64_t>(h->n_labels0, V) : (flags & GK_PM_LABELS) ? h->n_labels0 : 1;
+  if (L > 0) {
+    const unsigned long long rows = (unsigned long long)std::max<int64_t>(n_lab, 1) * (unsigned long long)d;
+    int bits = 0;
+    while (bits < 64 && (rows - 1) >> bits) ++bits;
+    if (bits + (L - 1) > 64) return fail(GK_ERR_UNSUPPORTED, "gk_pm_features: a (histogram row, cell) key does not fit 64 bits");
+  }
+  for (int64_t i = 0; i < (int64_t)n_sets * N; ++i)
+    if (n_cols[i] < 0 || n_cols[i] > d) return fail(GK_ERR_ARG, "gk_pm_features: a column count is outside [0, d]");
+  // every used u must lie in [0, 1 + 2^-(L-1)): a NaN or negative u has no cell, and a larger one would give a cell
+  // past the clamp 2^j - 1 that runs into the next row's keys
+  if (L > 0 && V) {
+    const std::vector<int>& gp = extra_of(h)->graph_ptr;
+    const double top = ldexp(1.0, L - 1);
+    for (int s = 0; s < n_sets; ++s)
+      for (int64_t g = 0; g < N; ++g)
+        for (int64_t v = gp[g]; v < gp[g + 1]; ++v) {
+          if (skip && skip[v]) continue;
+          const double* u = U + ((size_t)s * V + v) * d;
+          for (int q = 0; q < n_cols[(size_t)s * N + g]; ++q)
+            if (!(u[q] >= 0.0) || floor(u[q] * top) > top)
+              return fail(GK_ERR_ARG, "gk_pm_features: an embedding value is NaN, negative or >= 1 + 2^-(L-1)");
+        }
+  }
+  const int64_t launches0 = h->launches;
+  h->features_ready = false; h->feat_serial++;
+  HandleExtra* ex = extra_of(h);
+  GK_TRY(init_scalars(h, 0));  // clears ft_overflow
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  if (wl && h->wl_sparse_ids) {  // the histogram rows are indexed by dense label ids
+    for (int lv = 1; lv <= n_iter; ++lv) GK_TRY(wl_densify(h, lv, h->labels_all.as<int>() + (size_t)lv * V));
+    h->wl_sparse_ids = false;
+  }
+  GK_TRY(h->pm_U.ensure((size_t)n_sets * std::max<int64_t>(M, 1) * 8));
+  GK_TRY(h->pm_ncols.ensure((size_t)n_sets * N * 4));
+  if (M) GK_CUDA(cudaMemcpyAsync(h->pm_U.p, U, (size_t)n_sets * M * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->pm_ncols.p, n_cols, (size_t)n_sets * N * 4, cudaMemcpyHostToDevice, h->stream));
+  h->pm_has_skip = skip != nullptr && V > 0;
+  if (h->pm_has_skip) {
+    GK_TRY(h->pm_skip.ensure((size_t)V));
+    GK_CUDA(cudaMemcpyAsync(h->pm_skip.p, skip, (size_t)V, cudaMemcpyHostToDevice, h->stream));
+  }
+  h->pm_S = n_sets; h->pm_L = L; h->pm_d = d; h->pm_flags = flags;
+  const int n_blocks = n_sets * L;
+  GK_TRY(h->nh_codes.ensure((size_t)std::max<int64_t>(M, 1) * 8));
+  GK_TRY(h->nh_valid.ensure((size_t)std::max<int64_t>(M, 1)));
+  unsigned long long* keys = h->nh_codes.as<unsigned long long>();
+  unsigned char* valid = h->nh_valid.as<unsigned char>();
+  LevelScratch ls;
+  GK_TRY(level_setup(h, M, std::max(n_blocks, 1), &ls));
+  for (int s = 0; s < n_sets; ++s)
+    for (int j = 0; j < L; ++j) {
+      GK_TRY(pm_keys(h, s, j, keys, valid));
+      GK_TRY(level_columns(h, ls, s * L + j, M, d, keys, valid));
+    }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  DevScalars* hs;
+  int64_t n_col = 0, n_ent = 0;
+  GK_TRY(level_finish(h, ls, n_blocks, "gk_pm_features", &hs, &n_col, &n_ent));
+  h->nh_R = n_blocks;
+  h->n_columns = n_col;
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = FK_PM;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
+    stats->n_levels = n_blocks;
+    for (int r = 0; r < std::min(n_blocks, MAX_LEVELS); ++r) stats->level_dims[r] = ex->nh_dims[r];
+    stats->n_columns = n_col;
+    stats->n_entries = n_ent;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_columns = stats->ms_features;
+  }
+  return GK_OK;
+}
+
+int gk_pm_cells(gk_handle* h, int32_t set, int32_t level, int64_t* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_pm_cells: null argument");
+  if (h->feature_kind != FK_PM || !h->features_ready || set < 0 || set >= h->pm_S || level < 0 || level >= h->pm_L)
+    return fail(GK_ERR_STATE, "gk_pm_cells: no such set / level (run gk_pm_features first)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t M = (size_t)h->V * h->pm_d;
+  if (!M) return GK_OK;
+  // the level's keys are recomputed into the scratch of gk_pm_features (its level blocks are not touched)
+  GK_TRY(pm_keys(h, set, level, h->nh_codes.as<unsigned long long>(), h->nh_valid.as<unsigned char>()));
+  std::vector<unsigned long long> keys(M);
+  std::vector<unsigned char> valid(M);
+  GK_CUDA(cudaMemcpyAsync(keys.data(), h->nh_codes.p, M * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaMemcpyAsync(valid.data(), h->nh_valid.p, M, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  const unsigned long long mask = level == 0 ? 0ULL : (level >= 64 ? ~0ULL : (1ULL << level) - 1ULL);
+  for (size_t e = 0; e < M; ++e) out[e] = valid[e] ? (int64_t)(keys[e] & mask) : -1;
+  return GK_OK;
+}
+
+// Gram of PyramidMatch features (gram_path 11): gram_levels with pm_combine; self similarities from pm_diag, so
+// GK_NORMALIZE divides by sqrt(K_ii K_jj) as the reference's base class does.
+static int gram_pm(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const int64_t N = h->N, k_cols = q.k_cols;
+  const int S = h->pm_S, L = h->pm_L, n_blocks = S * L;
+  const int64_t launches0 = h->launches;
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  LevelTimes lt;
+  if (n_blocks == 0) {  // L = 0: the reference's k stays 0
+    if (q.k_rows > 0) GK_CUDA(cudaMemset2DAsync(out.p, (size_t)out.ld * 8, 0, (size_t)k_cols * 8, (size_t)q.k_rows, h->stream));
+  } else {
+    GK_TRY(gram_levels(h, q, n_blocks, out, [&](const LevelChunk& c) {
+      PmCombineParams p;
+      p.C = c.C;
+      p.stride = c.stride;
+      p.ldc = c.ldc;
+      p.S = S;
+      p.L = L;
+      p.rows = c.rows;
+      p.cols = c.cols;
+      p.mirror = c.mirror;
+      p.out = c.out;
+      p.ld = c.ld;
+      const long long nbi = (c.rows + PM_TILE - 1) / PM_TILE, nbj = (k_cols + PM_TILE - 1) / PM_TILE;
+      const long long grid = p.mirror ? nbj * (nbj + 1) / 2 : nbi * nbj;
+      if (grid > 0) {
+        pm_combine<<<(unsigned)grid, PM_TILE * 8, 0, h->stream>>>(p);
+        LAUNCH_CHECK(h);
+      }
+      return GK_OK;
+    }, &lt));
+  }
+  // after the level Grams: gram_int leaves each level block's own self similarities in diag_f64
+  GK_TRY(h->diag_f64.ensure((size_t)N * 8));
+  pm_diag<<<cdiv(N, 256), 256, 0, h->stream>>>((int)N, S, L, h->graph_ptr.as<int>(), h->pm_ncols.as<int>(),
+                                               h->pm_has_skip ? h->pm_skip.as<unsigned char>() : nullptr,
+                                               h->diag_f64.as<double>());
+  LAUNCH_CHECK(h);
+  GK_TRY(f64_deliver(h, q, out, true, h->ev[14], h->ev[15]));
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->n_levels = L;
+    stats->gram_path = 11;
+    stats->threshold = lt.max_T;
+    stats->max_count = 1;
+    stats->gemm_launches = lt.gram_launches + (h->launches - launches0);
+    stats->gemm_elem_bytes = lt.elem_bytes;
+    float tot = lt.ms_combine;
+    for (int j = 0; j < L; ++j) stats->ms_level_gram[j] = 0.f;
+    for (int r = 0; r < n_blocks; ++r) { stats->ms_level_gram[r % L] += lt.ms_block[r]; tot += lt.ms_block[r]; }
+    stats->ms_gemm = tot - lt.ms_combine;
+    stats->ms_combine = lt.ms_combine;
     stats->ms_d2h = ev_ms(h->ev[14], h->ev[15]);
     stats->ms_total = tot + stats->ms_d2h;
   }
@@ -3125,6 +3399,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_SPATTR: return gram_spattr(h, q, stats);
     case FK_GH: return h->gh_node_kernel == GK_GH_LINEAR ? gram_spattr(h, q, stats) : gram_gh_nodepair(h, q, stats);
     case FK_NH: return gram_nh(h, q, stats);
+    case FK_PM: return gram_pm(h, q, stats);
     case FK_RW: return gram_rw(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }

@@ -120,6 +120,7 @@ enum FeatureKind : int {
   FK_NH = 5,      // NeighborhoodHash per-level expanded blocks
   FK_RW = 6,      // random walk edge values
   FK_PK = 7,      // Propagation counts in the SP layout: the integer Gram
+  FK_PM = 8,      // PyramidMatch per-level expanded blocks (the NeighborhoodHash layout)
 };
 
 }  // namespace gk
@@ -218,7 +219,15 @@ struct gk_handle {
   gk::DevBuf nh_blk;              // unary-expanded (graph, column) block of every level, nh_level_bytes apart
   gk::DevBuf nh_lut, nh_tab, nh_ws, nh_cur, nh_C;
   size_t nh_level_bytes = 0;
+  int64_t nh_level_cap = 0;       // entries (and columns) one level's expanded block can hold
   int nh_R = 0;
+
+  // ---- PyramidMatch (FK_PM): the levels live in the NeighborhoodHash buffers above (nh_codes / nh_valid hold the
+  // current level's keys, nh_blk the expanded blocks, pm_S * pm_L of them); the embeddings [S][V][d] fp64 and the
+  // column counts [S][N] stay for gk_pm_cells and the self similarities
+  gk::DevBuf pm_U, pm_ncols, pm_skip;  // pm_skip: [V] u8, vertices without entries (when has_skip)
+  int pm_S = 0, pm_L = 0, pm_d = 0, pm_flags = 0;
+  bool pm_has_skip = false;
 
   // ---- random walk (FK_RW): edge values of the packed CSR, its transpose, eigen-data, coefficients
   gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;

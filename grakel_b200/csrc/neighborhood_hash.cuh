@@ -214,13 +214,15 @@ nh_code_number(int V, const unsigned char* __restrict__ valid, const int* __rest
   if (tab[s] == v) colid[s] = (int)atomicAdd(n_cols, 1ULL);
 }
 
-// pass 3: (graph, column) -> count, the (graph << 32 | column) element layout of the SP / WL feature tables
+// pass 3: (graph, column) -> count, the (graph << 32 | column) element layout of the SP / WL feature tables.
+// Entry v belongs to vertex v / per (NeighborhoodHash: one entry per vertex; PyramidMatch: d per vertex).
 __global__ void __launch_bounds__(256)
-nh_count(int V, const unsigned char* __restrict__ valid, const int* __restrict__ vgraph, const int* __restrict__ slot_of,
-         const int* __restrict__ colid, unsigned long long* __restrict__ keys, unsigned* __restrict__ cnt, unsigned mask) {
+nh_count(int V, int per, const unsigned char* __restrict__ valid, const int* __restrict__ vgraph,
+         const int* __restrict__ slot_of, const int* __restrict__ colid, unsigned long long* __restrict__ keys,
+         unsigned* __restrict__ cnt, unsigned mask) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= V || !valid[v]) return;
-  const unsigned long long key = ((unsigned long long)(unsigned)vgraph[v] << 32) | (unsigned)colid[slot_of[v]];
+  const unsigned long long key = ((unsigned long long)(unsigned)vgraph[v / per] << 32) | (unsigned)colid[slot_of[v]];
   unsigned s = (unsigned)mix64(key) & mask;
   for (;;) {
     unsigned long long cur = keys[s];

@@ -10,6 +10,7 @@ the kernels of the device hot path:
     "graph_hopper" / "GH"
     "neighborhood_hash" / "NH"
     "propagation" / "PR"        (+ with_attributes: PropagationAttr)
+    "pyramid_match" / "PM"      (+ with_labels, L, d)
 
 Any other reference kernel name raises NotImplementedError (not ValueError, which the reference reserves for
 unknown names).  The public surface (constructor parameters, `fit` / `transform` / `fit_transform`, the fitted
@@ -30,8 +31,8 @@ from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
-from .kernels import (EdgeHistogram, GraphHopper, NeighborhoodHash, Propagation, PropagationAttr, ShortestPath,
-                      ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
+from .kernels import (EdgeHistogram, GraphHopper, NeighborhoodHash, Propagation, PropagationAttr, PyramidMatch,
+                      ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
 
@@ -39,7 +40,7 @@ default_n_components = 100
 _OUTSIDE = frozenset((
     "random_walk", "RW", "graphlet_sampling", "GR", "subgraph_matching", "SM", "multiscale_laplacian", "ML",
     "lovasz_theta", "LOVT", "svm_theta", "SVMT", "neighborhood_subgraph_pairwise_distance",
-    "NSPD", "odd_sth", "ODD", "pyramid_match", "PM", "hadamard_code", "HC"))
+    "NSPD", "odd_sth", "ODD", "hadamard_code", "HC"))
 
 
 def _propagation(params):
@@ -60,6 +61,7 @@ for _names, _framework, _build in (
         (("graph_hopper", "GH"), False, lambda p: (GraphHopper, p)),
         (("neighborhood_hash", "NH"), False, lambda p: (NeighborhoodHash, p)),
         (("propagation", "PR"), False, _propagation),
+        (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),
         (("core_framework", "CORE"), True, lambda p: (CoreFramework, p))):
     for _n in _names:

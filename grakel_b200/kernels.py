@@ -442,10 +442,12 @@ class WeisfeilerLehman(Kernel):
                     raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
                                      "parameters names and values")
                 params.pop("normalize", None)
-            if base not in (VertexHistogram, EdgeHistogram, ShortestPath):
+            if base not in (VertexHistogram, EdgeHistogram, ShortestPath, PyramidMatch):
                 raise NotImplementedError("grakel_b200 runs WeisfeilerLehman over VertexHistogram (the subtree kernel), "
-                                          "EdgeHistogram or ShortestPath; other base kernels are outside the device "
-                                          "hot path")
+                                          "EdgeHistogram, ShortestPath or PyramidMatch; other base kernels are outside "
+                                          "the device hot path")
+            if base is PyramidMatch:  # the base kernel's own checks (pyramid_match.py:62-81)
+                PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
             if base is ShortestPath:
                 if not params.get("with_labels", True):
                     raise NotImplementedError("WeisfeilerLehman over ShortestPath(with_labels=False) ignores the WL "
@@ -484,6 +486,9 @@ class WeisfeilerLehman(Kernel):
             sizes = np.concatenate([[0], np.cumsum([len(v) for v in values])])
             return Block(sizes, np.zeros(int(sizes[-1]) + 1, dtype=np.int64), np.zeros(0, dtype=np.int64), None,
                          [l for v in values for l in v])
+        if base is PyramidMatch and isinstance(X, Block):
+            raise NotImplementedError("WeisfeilerLehman over PyramidMatch embeds every graph's adjacency matrix; pass "
+                                      "the list of graphs")
         if base is ShortestPath:
             # the base kernel receives the edge DICTIONARY of every graph (weisfeiler_lehman.py:188, 218):
             # Dijkstra semantics whatever the input spelling; labels are the WL vertex set
@@ -496,16 +501,66 @@ class WeisfeilerLehman(Kernel):
                 delattr(self, "_X_diag")
             if not isinstance(X, (Iterable, Block)):
                 raise TypeError("input must be an iterable\n")
+            if self._base_graph_kernel is PyramidMatch and not isinstance(X, Block):
+                X = list(X)
             block = self._pack_for_base(X, lambda n: n >= 2)  # weisfeiler_lehman.py:152
             self._nx = block.n_graphs
             ids, dictionary = label_ids(block.labels, None, sort_new=True)  # :199-206
             self._inv_labels = _LevelDictionaries(dictionary, self)
-            return Fitted(block, ids, dictionary)
+            fitted = Fitted(block, ids, dictionary)
+            fitted.pm = self._pm_embed(X, block)
+            return fitted
         if self._method_calling != 3:
             raise ValueError("method call must be called either from fit or fit-transform")
+        if self._base_graph_kernel is PyramidMatch and not isinstance(X, Block):
+            X = list(X)
         block = self._pack_for_base(X, lambda n: n in (2, 3))  # :367
         ids, _ = label_ids(block.labels, self._inv_labels[0], sort_new=True)  # :417-418
-        return Fitted(block, ids, self._inv_labels[0])
+        fitted = Fitted(block, ids, self._inv_labels[0])
+        fitted.pm = self._pm_embed(X, block)
+        return fitted
+
+    def _pm_embed(self, X, block):
+        """PyramidMatch base: the embeddings of every level's fresh base kernel (weisfeiler_lehman.py:260-270,
+        478-482): n_iter + 1 passes over the graphs, level-major, each one eigs / eig call per graph.  The base kernel
+        sees every graph's edge DICTIONARY: its vertices are those of the element's adjacency matrix (range(n), or the
+        sorted symbols of the edge dictionary), each with its own label.  The packed WL block lists a graph's vertices
+        in the order of its labels dictionary and also holds labelled vertices outside the edge dictionary; so every
+        embedding row is moved to its vertex's packed position, and the vertices the base kernel does not see are
+        skipped (they never change another vertex's WL label)."""
+        if self._base_graph_kernel is not PyramidMatch:
+            return None
+        from .packing import adjacency_and_order
+        import time
+        d, L = self._params.get("d", 6), self._params.get("L", 4)
+        mats, src = [], []
+        n_pm = 0
+        for x in X:
+            if isinstance(x, Graph):
+                x = x.as_element()
+            x = list(x)
+            if len(x) == 0:
+                continue
+            A, order = adjacency_and_order(x[0])
+            loc = {k: i for i, k in enumerate(order)}
+            rows = [loc.get(k, -1) for k in x[1].keys()]  # the packed vertices, in the pack's order
+            if sum(r >= 0 for r in rows) != len(order):
+                raise NotImplementedError("WeisfeilerLehman over PyramidMatch: a vertex of a graph's edge dictionary "
+                                          "has no label")
+            src.extend(r + n_pm if r >= 0 else -1 for r in rows)
+            mats.append(A)
+            n_pm += A.shape[0]
+        src = np.asarray(src, dtype=np.int64)
+        if len(src) != block.n_vertices:
+            raise NotImplementedError("WeisfeilerLehman over PyramidMatch: the packed vertices are not the labelled ones")
+        t0 = time.perf_counter()
+        U_pm, n_cols = pm_embed_sets(mats, d, self._n_iter)
+        self.ms_host_embed_ = (time.perf_counter() - t0) * 1e3
+        pm_check_cells(U_pm, n_cols, np.array([A.shape[0] for A in mats]), L)
+        seen = src >= 0
+        U = np.zeros((self._n_iter, len(src), d))
+        U[:, seen] = U_pm[:, src[seen]]
+        return _PmData(np.diff(np.asarray(block.graph_ptr)), U, n_cols, None, skip=None if seen.all() else ~seen)
 
     def fit_transform(self, X, y=None):
         self._method_calling = 2
@@ -535,6 +590,7 @@ class WeisfeilerLehman(Kernel):
         if not isinstance(X, (Iterable, Block)):
             raise ValueError("input must be an iterable\n")
         Y = self.parse_input(X)
+        self._pm_y = Y.pm
         K, xdiag, ydiag = self._run(Block.concat(self.X.block, Y.block), np.concatenate([self.X.ids, Y.ids]),
                                     n_fit=self._nx)
         self._X_diag = xdiag
@@ -545,6 +601,15 @@ class WeisfeilerLehman(Kernel):
     def _device_features(self, eng):
         if self._base_graph_kernel is ShortestPath:
             return eng.wl_sp_features(self._n_iter - 1, dijkstra_order=True)  # the base kernel gets edge dictionaries
+        if self._base_graph_kernel is PyramidMatch:
+            # every WL level's classes label a PyramidMatch of its own; the joint relabel of X and Y gives classes
+            # unseen at fit columns no fitted graph has (the reference's row cut)
+            p = self._params
+            pm = self.X.pm if eng.n_graphs == self._nx else _PmData.concat(self.X.pm, self._pm_y)
+            with_labels = p.get("with_labels", True)
+            eng.wl_features(self._n_iter - 1)
+            return eng.pm_features(p.get("L", 4), p.get("d", 6), pm.U, pm.n_cols, n_iter=self._n_iter - 1,
+                                   flags=_lib.GK_PM_WL_LABELS if with_labels else 0, skip=pm.skip)
         return eng.wl_features(self._n_iter - 1)
 
     def _run(self, block, ids, n_fit, want_matrix=True):
@@ -1299,6 +1364,22 @@ def _eigen_data(mats, symmetric):
     return np.concatenate(qs), np.concatenate(ws)
 
 
+def _block_adjacency(X, labeled):
+    """(adjacency matrix, labels or None) of every graph of a datasets.read_tu block: the kernel's vertices are the
+    nodes that occur in an edge (the reference's adjacency matrix of an edge-set graph)."""
+    X.require("sp", labels=labeled)
+    out = []
+    gp, rp, ci = X.graph_ptr, X.row_ptr, X.col_idx
+    for g in range(X.n_graphs):
+        a, b = int(gp[g]), int(gp[g + 1])
+        A = np.zeros((b - a, b - a))
+        for u in range(a, b):
+            e0, e1 = int(rp[u]), int(rp[u + 1])
+            A[u - a, ci[e0:e1] - a] = 1.0 if X.weights is None else X.weights[e0:e1]
+        out.append((A, list(X.labels[a:b]) if labeled else None))
+    return out
+
+
 _RW_ELEMENT_MSG = "each element of X must be either a graph or an iterable with at least 1 and at most 3 elements\n"
 _RWL_ELEMENT_MSG = "each element of X must be either a graph or an iterable with at least 2 and at most 3 elements\n"
 
@@ -1442,18 +1523,8 @@ class RandomWalk(Kernel):
     def _elements(self, X):
         """(adjacency matrix, labels in index order or None) of every element (random_walk.py:215-244, 423-448)."""
         from .packing import adjacency_and_labels
-        if isinstance(X, Block):  # datasets.read_tu: the kernel's vertices are the nodes that occur in an edge
-            X.require("sp", labels=self._labeled)
-            out = []
-            gp, rp, ci = X.graph_ptr, X.row_ptr, X.col_idx
-            for g in range(X.n_graphs):
-                a, b = int(gp[g]), int(gp[g + 1])
-                A = np.zeros((b - a, b - a))
-                for u in range(a, b):
-                    e0, e1 = int(rp[u]), int(rp[u + 1])
-                    A[u - a, ci[e0:e1] - a] = 1.0 if X.weights is None else X.weights[e0:e1]
-                out.append((A, list(X.labels[a:b]) if self._labeled else None))
-            return out
+        if isinstance(X, Block):
+            return _block_adjacency(X, self._labeled)
         if not isinstance(X, Iterable):
             raise TypeError("input must be an iterable\n")
         out = []
@@ -2102,3 +2173,254 @@ class PropagationAttr(Propagation):
         p0 = np.concatenate([np.asarray(p.P, dtype=np.float64) for p in parts])
         return (sizes, mats, None, p0, np.stack(self._u), np.stack(self._b), self._dim, self._dim,
                 _lib.GK_PK_ATTR | parts[0].store)
+
+
+# ------------------------------------------------------------------------------
+# The embedding calls of PyramidMatch, by module-level name: `eigs` for graphs of more than d + 1 vertices, `eig` for
+# the others, with the reference's arguments.  scipy's eigs draws its start vector from OS entropy unless it is given an
+# `rng`, so the reference's K is not reproducible; substituting a seeded `eigs` here (tests) makes both deterministic.
+from scipy.sparse import csr_matrix as _csr_matrix  # noqa: E402
+from scipy.sparse.linalg import eigs  # noqa: E402
+
+eig = np.linalg.eig
+
+_PM_ELEMENT_MSG = ("each element of X must be either a graph object or a list with at least a graph like object and "
+                   "node labels dict \n")
+
+
+def pm_embedding(A, d):
+    """|U| of one graph's adjacency matrix A as pyramid_match.py:135-147 makes it: the d eigenvectors of eigs (n > d + 1)
+    or the first d columns of eig, ordered by descending eigenvalue (numpy's argsort, complex for directed graphs)."""
+    if A.shape[0] > d + 1:
+        Lambda, U = eigs(_csr_matrix(A, dtype=float), k=d, ncv=10 * d)
+        U = U[:, Lambda.argsort()[::-1]]
+    else:
+        Lambda, U = eig(A)
+        U = U[:, Lambda.argsort()[::-1]]
+        U = U[:, :d]
+    return np.absolute(U)
+
+
+def _pm_empty_error(g, with_labels):
+    """The error the reference meets on a graph without vertices (inside Graph or its own unpacking)."""
+    if isinstance(g, dict):
+        return TypeError("cannot unpack non-iterable NoneType object")
+    if isinstance(g, (list, tuple)):
+        return IndexError("tuple index out of range")
+    if with_labels:
+        return ValueError("Graph does not have any labels for vertices.")
+    return ValueError("not enough values to unpack (expected 2, got 1)")
+
+
+class _PmData:
+    """Host state of a PyramidMatch input: per embedding set the |U| of every vertex ([S, V, d], zero past a graph's
+    column count) and the column counts [S, N]; graph sizes; per-vertex labels (or None)."""
+
+    def __init__(self, sizes, U, n_cols, labels, skip=None):
+        self.sizes = np.asarray(sizes, dtype=np.int64)
+        self.U = U
+        self.n_cols = n_cols
+        self.labels = labels
+        self.skip = skip  # [V] bool: packed vertices without embedding (outside the base kernel's graph), or None
+
+    def __len__(self):
+        return len(self.sizes)
+
+    @staticmethod
+    def concat(a, b):
+        labels = None if a.labels is None else list(a.labels) + list(b.labels)
+        skip = None
+        if a.skip is not None or b.skip is not None:
+            skip = np.concatenate([np.zeros(a.U.shape[1], bool) if a.skip is None else a.skip,
+                                   np.zeros(b.U.shape[1], bool) if b.skip is None else b.skip])
+        return _PmData(np.concatenate([a.sizes, b.sizes]), np.concatenate([a.U, b.U], axis=1),
+                       np.concatenate([a.n_cols, b.n_cols], axis=1), labels, skip)
+
+
+def pm_embed_sets(mats, d, n_sets):
+    """(U [n_sets, V, d], n_cols [n_sets, N]) of the adjacency matrices `mats`: n_sets embedding passes, set-major
+    (WeisfeilerLehman over PyramidMatch fits a fresh kernel per level, each of which embeds every graph again)."""
+    sizes = np.array([A.shape[0] for A in mats], dtype=np.int64)
+    gp = np.concatenate([[0], np.cumsum(sizes)])
+    U = np.zeros((n_sets, int(gp[-1]), d))
+    n_cols = np.zeros((n_sets, len(mats)), dtype=np.int32)
+    for s in range(n_sets):
+        for g, A in enumerate(mats):
+            u = pm_embedding(A, d)
+            U[s, gp[g]:gp[g + 1], :u.shape[1]] = u
+            n_cols[s, g] = u.shape[1]
+    return U, n_cols
+
+
+def pm_check_cells(U, n_cols, sizes, L):
+    """The reference's own failures while binning (pyramid_match.py:213-221): int() of a NaN cell, a cell past the
+    clamp (u >= 1 + 2^-j) as an index out of range."""
+    if L == 0 or U.size == 0:
+        return
+    gp = np.concatenate([[0], np.cumsum(sizes)])
+    mask = np.arange(U.shape[2])[None, None, :] < np.repeat(n_cols, np.diff(gp), axis=1)[:, :, None]
+    u = U[mask]
+    if np.isnan(u).any():
+        raise ValueError("cannot convert float NaN to integer")
+    umax = float(u.max()) if u.size else 0.0
+    for j in range(L):
+        k = 2 ** j
+        if np.floor(umax * k) > k:
+            raise IndexError("index %d is out of bounds for axis 1 with size %d" % (int(np.floor(umax * k)), k))
+
+
+class PyramidMatch(Kernel):
+    """Pyramid match kernel (pyramid_match.py:18-285; Nikolentzos et al. 2017).
+
+    Every vertex is embedded by the absolute values of d eigenvectors of its graph's adjacency matrix; level j < L
+    splits the unit hypercube into 2^j cells per dimension, and K sums the levels' histogram intersections with the
+    reference's weights.  The embedding runs on the host with the reference's own scipy / numpy calls (`eigs`, `eig`
+    above); the cells, the per-level intersections (an exact integer Gram per level) and the fp64 combine run on the
+    device.  Given the same embeddings, K equals the reference's bit for bit, including its combine, whose two
+    statements sit inside the level loop (a graph's self similarity at L = 2 is 1.5 times its vertex-dimension count).
+
+    Deviations: L > 64, d * (largest graph) >= 2^24 and V * d >= 2^31 raise NotImplementedError, as does a
+    (label, dimension, cell) key that does not fit 64 bits."""
+
+    _graph_format = "adjacency"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, with_labels=True, L=4, d=6):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.with_labels = with_labels
+        self.L = L
+        self.d = d
+        self._initialized.update({"d": False, "L": False, "with_labels": False})
+
+    def initialize(self):
+        """pyramid_match.py:62-81."""
+        super().initialize()
+        if not self._initialized["with_labels"]:
+            if type(self.with_labels) != bool:
+                raise TypeError("with labels must be a boolean variable")
+            self._initialized["with_labels"] = True
+        if not self._initialized["L"]:
+            if type(self.L) is not int or self.L < 0:
+                raise TypeError("L: the number of levels must be an integer bigger equal to 0")
+            self._initialized["L"] = True
+        if not self._initialized["d"]:
+            if type(self.d) is not int or self.d < 1:
+                raise TypeError("d: hypercube dimension must be an integer bigger than 1")
+            self._initialized["d"] = True
+
+    # ---- input
+    def _elements(self, X):
+        """(adjacency matrix, labels in index order or None) of every element (pyramid_match.py:102-153); the
+        embedding calls are made afterwards, in input order."""
+        from .packing import adjacency_and_labels
+        if isinstance(X, Block):  # datasets.read_tu
+            out = _block_adjacency(X, self.with_labels)
+            if any(A.shape[0] == 0 for A, _ in out):
+                raise ValueError("Graph does not have any labels for vertices." if self.with_labels else
+                                 "not enough values to unpack (expected 2, got 1)")
+            if not out:
+                raise ValueError("parsed input is empty")
+            return out
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            if not (is_iter and (len(x) == 0 or (len(x) >= 1 and not self.with_labels) or
+                                 (len(x) >= 2 and self.with_labels))):
+                raise TypeError(_PM_ELEMENT_MSG)
+            if len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            if isinstance(x[0], (list, tuple)) and len(x[0]) == 0:
+                raise _pm_empty_error(x[0], self.with_labels)
+            A, labels = adjacency_and_labels(x[0], x[1] if self.with_labels else None)
+            if A.shape[0] == 0:
+                raise _pm_empty_error(x[0], self.with_labels)
+            out.append((A, labels))
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    def parse_input(self, X):
+        import time
+        els = self._elements(X)
+        t0 = time.perf_counter()
+        U, n_cols = pm_embed_sets([A for A, _ in els], self.d, 1)
+        self.ms_host_embed_ = (time.perf_counter() - t0) * 1e3
+        data = _PmData([A.shape[0] for A, _ in els], U, n_cols, None)
+        pm_check_cells(U, n_cols, data.sizes, self.L)
+        if self.with_labels:
+            data.labels = [l for _, L in els for l in L]
+            if self._method_calling in (1, 2):  # pyramid_match.py:158-165
+                labels = set()
+                for _, L in els:
+                    labels |= set(L)
+                self._num_labels = len(labels)
+                self._labels = {l: i for (i, l) in enumerate(labels)}
+        return data
+
+    def _label_ids(self, data, n_fit):
+        """Packed label ids: the fit enumeration, labels unseen at fit after it (pyramid_match.py:167-174) -- their rows
+        never meet a fitted graph's, as the reference's row cut `yp[:xp.shape[0]]` has it."""
+        known = dict(self._labels)
+        ids = np.empty(len(data.labels), dtype=np.int32)
+        for i, l in enumerate(data.labels):
+            v = known.get(l)
+            if v is None:
+                v = known[l] = len(known)
+            ids[i] = v
+        return ids
+
+    # ---- estimator protocol
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        K, xdiag, _ = self._pm_run(self.X, len(self.X))
+        self._X_diag = xdiag
+        if self.normalize:
+            self._warn_unnormalizable(xdiag)
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        Y = self.parse_input(X)
+        K, xdiag, ydiag = self._pm_run(_PmData.concat(self.X, Y), len(self.X))
+        self._X_diag, self._Y_diag = xdiag, ydiag
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xdiag, ydiag)
+        return K
+
+    def diagonal(self):
+        check_is_fitted(self, ["X"])
+        try:
+            check_is_fitted(self, ["_X_diag"])
+        except NotFittedError:
+            _, self._X_diag, _ = self._pm_run(self.X, len(self.X), want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
+
+    def _pm_run(self, data, n_fit, want_matrix=True, device_ptr=None):
+        """pack the vertex sets -> gk_pm_features (cells, per-level columns) -> gk_gram (per-level Grams, fp64 combine).
+        Returns (K, xdiag, ydiag)."""
+        ids = self._label_ids(data, n_fit) if self.with_labels else None
+        gp = np.concatenate([[0], np.cumsum(data.sizes)])
+        V = int(gp[-1])
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(gp, np.zeros(V + 1, dtype=np.int32), np.zeros(0, dtype=np.int32), ids, None, None)
+            self.stats_ = eng.pm_features(self.L, self.d, data.U, data.n_cols,
+                                          flags=_lib.GK_PM_LABELS if self.with_labels else 0, skip=data.skip)
+            out = False if not want_matrix else None
+            K, xd, yd = eng.gram(len(data), n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 out=out if device_ptr is None else None, device_ptr=device_ptr, stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd

@@ -459,24 +459,30 @@ def adjacency_and_labels(g, L=None):
     as it is -- every non-zero entry is an edge with its weight, negative ones and self-loops included -- and an edge
     dictionary becomes the matrix over its sorted vertex symbols, every listed symbol a vertex (also one without an
     edge), a later duplicate overwriting an earlier one.  The random walk kernels use this, not pack()."""
+    A, order = adjacency_and_order(g)
+    labels = None
+    if L is not None:
+        labels = [L[k] for k in order]
+    return A, labels
+
+
+def adjacency_and_order(g):
+    """(the matrix of `adjacency_and_labels`, the vertex symbol of each of its rows): range(n) for an adjacency input,
+    the sorted symbols of an edge dictionary."""
     kind = classify(g)
     if kind is None:
         raise ValueError("Unsupported input type. For more information check the documentation, concerning "
                          "valid input types for graph type object.")
     if kind == "adjacency":
         A = np.array(_adjacency_array(g), dtype=np.float64)
-        order = range(A.shape[0])
-    else:
-        verts, edges = _edges_of(g, kind)
-        order = sorted(verts)
-        loc = {k: i for i, k in enumerate(order)}
-        A = np.zeros((len(order), len(order)))
-        for (u, v), w in edges.items():
-            A[loc[u], loc[v]] = w
-    labels = None
-    if L is not None:
-        labels = [L[k] for k in order]
-    return A, labels
+        return A, range(A.shape[0])
+    verts, edges = _edges_of(g, kind)
+    order = sorted(verts)
+    loc = {k: i for i, k in enumerate(order)}
+    A = np.zeros((len(order), len(order)))
+    for (u, v), w in edges.items():
+        A[loc[u], loc[v]] = w
+    return A, order
 
 
 def label_ids(labels, known=None, sort_new=True):

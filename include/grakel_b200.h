@@ -106,7 +106,8 @@ typedef struct gk_stats {
                                 ShortestPathAttr: 4 = 3xTF32 wgmma GEMM (non-negative features), 5 = fp64 CUDA-core Gram,
                                 GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram,
                                 NeighborhoodHash: 7 = one exact integer Gram per level + the fp64 combine,
-                                random walk: 8 = conjugate gradients, 9 = spectral pair sum, 10 = power series */
+                                random walk: 8 = conjugate gradients, 9 = spectral pair sum, 10 = power series,
+                                PyramidMatch: 11 = one exact integer Gram per level + the fp64 combine */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -256,6 +257,30 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
 /* bins of level `level` after gk_pk_features: out[V * K] (K = dim for GK_PK_ATTR, else 1; -0.0 stored as 0.0), and
  * priv[V] (may be NULL) = 1 where the vertex hashed as a private (new-label) vertex */
 int gk_pk_hashes(gk_handle* h, int32_t level, double* out, uint8_t* priv);
+
+/* PyramidMatch (pyramid_match.py:18-285) and WeisfeilerLehman over it.  The vertex embeddings are made on the host
+ * (the reference's eigs / numpy.linalg.eig calls, absolute values): U[n_sets * V * d] fp64, vertex v's row at
+ * (s * V + v) * d, and n_cols[n_sets * N] the column count of every graph's embedding (min(n, d) on the eig branch);
+ * entries past a graph's column count are ignored, and so is every vertex with skip[v] != 0 (skip[V] may be NULL: a
+ * vertex of the packed block that the base kernel's graph does not contain).  Every used value must lie in
+ * [0, 1 + 2^-(L-1)) -- the |U| of unit eigenvectors do -- else GK_ERR_ARG.  Level j < L puts every entry (v, q < n_cols) into cell
+ * floor(u * 2^j) (2^j clamped to 2^j - 1) of histogram row label(v) * d + q:
+ *   GK_PM_LABELS     label = the packed label id (one set)
+ *   GK_PM_WL_LABELS  label = WL level s of the gk_wl_features(n_iter) call just before (n_sets = n_iter + 1)
+ *   neither          row = q
+ * Every (set, level) becomes a unary-expanded count block of its own (the NeighborhoodHash layout).  gk_gram then
+ * returns, per set, the reference's fp64 combine of the level intersections I_j = sum min(cnt, cnt') replayed in its
+ * order, summed over the sets in set order (gram_path 11): fp64 only, host or GK_OUT_DEVICE output, GK_NORMALIZE,
+ * n_fit and row ranges; xdiag / ydiag are the same replay of I_j = n * n_cols (n without the skipped vertices).  GK_DIST and row maps are
+ * GK_ERR_UNSUPPORTED, as are L > 64, V * d >= 2^31, d * (largest graph) >= 2^24 (fp32 counts) and keys whose row
+ * << (L - 1) does not fit 64 bits.  stats: n_levels = n_sets * L blocks, level_dims = distinct cells per block,
+ * n_columns, ms_columns.  gk_pm_cells writes the cell of every entry e = v * d + q of one set and level (-1 for
+ * q >= n_cols or a skipped vertex): out[V * d]. */
+#define GK_PM_LABELS 1
+#define GK_PM_WL_LABELS 2
+int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const double* U, const int32_t* n_cols,
+                   const uint8_t* skip, int32_t n_sets, int32_t flags, gk_stats* stats);
+int gk_pm_cells(gk_handle* h, int32_t set, int32_t level, int64_t* out);
 
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
