@@ -27,6 +27,7 @@ GK_RW_FINITE, GK_RW_EXP, GK_RW_INV = 0, 1, 2
 GK_RW_LABELED = 1
 GK_PK_ATTR, GK_PK_SQRT, GK_PK_STORE_F32, GK_PK_STORE_INT, GK_PK_NEW_LABELS = 1, 2, 4, 8, 16
 GK_PM_LABELS, GK_PM_WL_LABELS = 1, 2
+GK_HC_SP = 8
 
 
 class GkStats(C.Structure):
@@ -85,6 +86,9 @@ _SYMBOLS = {
     "gk_pm_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pm_cells": (C.c_int, [_P, C.c_int32, C.c_int32, _P]),
+    "gk_hc_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_hc_vectors": (C.c_int, [_P, C.c_int32, _P]),
+    "gk_selftest_hc_collision": (C.c_int, [_P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -374,6 +378,29 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_pm_cells(self.h, int(s), int(level), _ptr(out)))
         return out
+
+    def hc_features(self, n_iter, width, skip=None, sp=False, dijkstra_order=False):
+        """HadamardCode levels of the packed block (gk_hc_features): n_iter levels of width-`width` vectors, classes per
+        level, and the VertexHistogram (sp=False) or ShortestPath (sp=True) block of all levels.  skip: [V] flags of the
+        vertices absent from the levels >= 1, or None."""
+        sk = None if skip is None else np.ascontiguousarray(skip, dtype=np.uint8)
+        flags = (GK_HC_SP if sp else 0) | (GK_SP_DIJKSTRA_ORDER if dijkstra_order else 0)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_hc_features(self.h, int(n_iter), int(width), _ptr(sk), flags, C.byref(st)))
+        return st
+
+    def hc_vectors(self, level, n_vertices, width):
+        """[V, W] int64 vectors of HadamardCode level `level` of the last hc_features call."""
+        out = np.empty((n_vertices, width), dtype=np.int64)
+        with self._lock:
+            self._check(self.lib.gk_hc_vectors(self.h, int(level), _ptr(out)))
+        return out
+
+    def selftest_hc_collision(self):
+        """Tests only: the next hc_features starts with a degenerate hash, so it must detect collisions and retry."""
+        with self._lock:
+            self._check(self.lib.gk_selftest_hc_collision(self.h))
 
     def rw_iterations(self, rows, cols):
         """CG iterations / series terms of every entry of the last random walk gram() (rows x cols u8)."""

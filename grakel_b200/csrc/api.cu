@@ -30,6 +30,7 @@
 #include "random_walk.cuh"
 #include "propagation.cuh"
 #include "pyramid_match.cuh"
+#include "hadamard_code.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -332,7 +333,7 @@ int gk_destroy(gk_handle* h) {
                         &h->rw_val, &h->rw_trp, &h->rw_tci, &h->rw_tval, &h->rw_q, &h->rw_w, &h->rw_coef, &h->rw_ws,
                         &h->rw_iters, &h->rw_cap,
                         &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt,
-                        &h->pm_U, &h->pm_ncols, &h->pm_skip};
+                        &h->pm_U, &h->pm_ncols, &h->pm_skip, &h->hc_S, &h->hc_z, &h->hc_skip};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -407,6 +408,7 @@ int gk_pack_csr(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const 
   h->features_ready = false; h->feat_serial++;
   h->feature_kind = FK_NONE;
   h->n_rows = 0;  // a new block starts without a row map
+  h->hc_W = 0;    // ... and without HadamardCode vectors
   HandleExtra* ex = extra_of(h);
   ex->wl_tiles_valid = false;
   ex->graph_ptr.assign(graph_ptr, graph_ptr + N + 1);
@@ -1020,34 +1022,30 @@ int gk_wl_labels(gk_handle* h, int32_t level, int32_t* out) {
 }
 
 // ---------------------------------------------------------------------------
-// Shortest-path features.  wl_iter < 0: the ShortestPath kernel on the packed labels.
-// wl_iter >= 0: WeisfeilerLehman(base_graph_kernel=ShortestPath) -- the graphs are relabelled for
-// wl_iter rounds first (gk_wl_features), then the labelled path histogram of EVERY level goes into one
-// feature block: label ids are made level-unique (id + first column of the level), so the levels use
-// disjoint columns and one Gram equals the reference's sum of per-level matrices
-// (weisfeiler_lehman.py:260-270 with shortest_path.py:370-410 as the base kernel).
-static int sp_features_impl(gk_handle* h, int32_t flags, int32_t wl_iter, gk_stats* stats) {
+// Shortest-path features.  Without a level label source: the ShortestPath kernel on the packed labels.
+// With one (WeisfeilerLehman or HadamardCode over ShortestPath): the graphs were relabelled first, and the labelled
+// path histogram of EVERY level goes into one feature block: label ids are made level-unique (id + first column of
+// the level), so the levels use disjoint columns and one Gram equals the reference's sum of per-level matrices
+// (weisfeiler_lehman.py:260-270, hadamard_code.py:217-236, with shortest_path.py:370-410 as the base kernel).
+struct SpLabels {
+  int n_pass = 1;
+  const int* labels = nullptr;            // [n_pass][V] dense label ids of every level; null = the packed labels
+  std::vector<long long> level_base{0};   // first label id of each level (n_pass + 1 entries)
+};
+
+static int sp_check(gk_handle* h, int32_t flags) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
   if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sp_features: no graphs packed");
   GK_CUDA(cudaSetDevice(h->dev));
+  if ((flags & GK_SP_WITH_LABELS) && !h->has_labels) return fail(GK_ERR_ARG, "gk_sp_features: vertex labels are required");
+  return GK_OK;
+}
+
+static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk_stats* stats) {
   const bool with_labels = flags & GK_SP_WITH_LABELS;
-  if (with_labels && !h->has_labels) return fail(GK_ERR_ARG, "gk_sp_features: vertex labels are required");
-  std::vector<long long> level_base(1, 0);  // first label id of each pass
-  int n_pass = 1;
-  long long n_labels_total = h->n_labels0;
-  if (wl_iter >= 0) {
-    if (!with_labels) return fail(GK_ERR_ARG, "gk_wl_sp_features: the base kernel needs vertex labels");
-    gk_stats wst;
-    GK_TRY(gk_wl_features(h, wl_iter, &wst));
-    if (h->wl_sparse_ids) {  // the base kernel's counters are indexed by dense label ids
-      for (int lv = 1; lv <= wl_iter; ++lv) GK_TRY(wl_densify(h, lv, h->labels_all.as<int>() + (size_t)lv * h->V));
-      h->wl_sparse_ids = false;
-    }
-    n_pass = wl_iter + 1;
-    level_base.assign(n_pass + 1, 0);
-    for (int l = 0; l < n_pass; ++l) level_base[l + 1] = level_base[l] + wst.level_dims[l];
-    n_labels_total = level_base[n_pass];
-  }
+  const std::vector<long long>& level_base = lab.level_base;
+  const int n_pass = lab.n_pass;
+  const long long n_labels_total = lab.labels ? level_base[n_pass] : h->n_labels0;
   if (with_labels && n_labels_total >= (1 << 20)) return fail(GK_ERR_UNSUPPORTED, "gk_sp_features: more than 2^20 distinct labels");
   const bool use_u16 = (!h->has_weights || h->unit_weights) && h->max_graph_size < 16000;
   const size_t esz = use_u16 ? 2 : 8;
@@ -1150,8 +1148,8 @@ static int sp_features_impl(gk_handle* h, int32_t flags, int32_t wl_iter, gk_sta
     p.st = fst;
     p.gdist = h->sp_dist.p;
     for (int pass = 0; pass < n_pass; ++pass) {
-    if (wl_iter >= 0) {
-      p.labels = h->labels_all.as<int>() + (size_t)pass * h->V;
+    if (lab.labels) {
+      p.labels = lab.labels + (size_t)pass * h->V;
       p.label_offset = (int)level_base[pass];
     }
     if (real_mode) {
@@ -1287,11 +1285,202 @@ static int sp_features_impl(gk_handle* h, int32_t flags, int32_t wl_iter, gk_sta
   return GK_OK;
 }
 
-int gk_sp_features(gk_handle* h, int32_t flags, gk_stats* stats) { return sp_features_impl(h, flags, -1, stats); }
+int gk_sp_features(gk_handle* h, int32_t flags, gk_stats* stats) {
+  GK_TRY(sp_check(h, flags));
+  return sp_features_impl(h, flags, SpLabels(), stats);
+}
 
 int gk_wl_sp_features(gk_handle* h, int32_t n_iter, int32_t flags, gk_stats* stats) {
   if (n_iter < 0) return fail(GK_ERR_ARG, "gk_wl_sp_features: n_iter out of range");
-  return sp_features_impl(h, flags | GK_SP_WITH_LABELS, n_iter, stats);
+  flags |= GK_SP_WITH_LABELS;
+  GK_TRY(sp_check(h, flags));
+  gk_stats wst;
+  GK_TRY(gk_wl_features(h, n_iter, &wst));
+  if (h->wl_sparse_ids) {  // the base kernel's counters are indexed by dense label ids
+    for (int lv = 1; lv <= n_iter; ++lv) GK_TRY(wl_densify(h, lv, h->labels_all.as<int>() + (size_t)lv * h->V));
+    h->wl_sparse_ids = false;
+  }
+  SpLabels lab;
+  lab.n_pass = n_iter + 1;
+  lab.labels = h->labels_all.as<int>();
+  lab.level_base.assign(lab.n_pass + 1, 0);
+  for (int l = 0; l < lab.n_pass; ++l) lab.level_base[l + 1] = lab.level_base[l] + wst.level_dims[l];
+  return sp_features_impl(h, flags, lab, stats);
+}
+
+// ---------------------------------------------------------------------------
+// HadamardCode (hadamard_code.cuh): the vectors of levels 0 .. upto into the two halves of hc_S (level i in half i & 1).
+// With `fst`, every level's classes are resolved into dense ids in labels_all, and with `count` also counted into the
+// per-level sub-tables of the feature block.
+static int hc_run_levels(gk_handle* h, int upto, const FeatStats* fst, bool count, size_t ft_level_cap) {
+  const int V = (int)h->V;
+  int lgW = 0;
+  while ((1 << lgW) < h->hc_W) ++lgW;
+  HcShape s;
+  s.V = V; s.lgW = lgW; s.lgT = std::min(lgW, 5);
+  const int nbT = cdiv((long long)V << s.lgT, HC_THREADS), nb = cdiv(V, 256);
+  unsigned long long* S[2] = {h->hc_S.as<unsigned long long>(), h->hc_S.as<unsigned long long>() + ((size_t)V << lgW)};
+  const unsigned long long* z = h->hc_z.as<unsigned long long>();
+  const unsigned char* skip = h->hc_has_skip ? h->hc_skip.as<unsigned char>() : nullptr;
+  unsigned long long* keys = fst ? h->ht_keys.as<unsigned long long>() : nullptr;
+  int* rep = h->ht_rep.as<int>();
+  const unsigned mask = (unsigned)(h->ht_cap - 1);
+  DevScalars* sc = h->scalars.as<DevScalars>();
+  for (int lv = 0; lv <= upto; ++lv) {
+    if (fst) {
+      GK_CUDA(cudaMemsetAsync(h->ht_keys.p, 0xFF, h->ht_cap * 8, h->stream));
+      GK_CUDA(cudaMemsetAsync(h->ht_rep.p, 0x7F, h->ht_cap * 4, h->stream));
+    }
+    if (lv == 0)
+      hc_level0<<<nbT, HC_THREADS, 0, h->stream>>>(s, h->labels0.as<int>(), z, S[0], keys, rep, mask, h->slot_of.as<int>(), sc);
+    else
+      hc_step<<<nbT, HC_THREADS, 0, h->stream>>>(s, h->row_ptr.as<int>(), h->col_idx.as<int>(), skip, z, S[(lv - 1) & 1],
+                                                  S[lv & 1], keys, rep, mask, h->slot_of.as<int>(), sc);
+    LAUNCH_CHECK(h);
+    if (!fst) continue;
+    const unsigned char* lv_skip = lv ? skip : nullptr;  // level 0 holds every labelled vertex
+    hc_verify<<<nbT, HC_THREADS, 0, h->stream>>>(s, lv_skip, S[lv & 1], rep, h->slot_of.as<int>(), h->flags.as<int>(), sc);
+    LAUNCH_CHECK(h);
+    hc_flag_sums<<<nb, 256, 0, h->stream>>>(V, h->flags.as<int>(), h->block_sums.as<int>());
+    LAUNCH_CHECK(h);
+    int* lab_out = h->labels_all.as<int>() + (size_t)lv * V;
+    wl_assign<<<nb, 256, 0, h->stream>>>(V, lv, h->flags.as<int>(), h->block_sums.as<int>(), lab_out, sc);
+    LAUNCH_CHECK(h);
+    hc_gather_insert<<<nb, 256, 0, h->stream>>>(V, lv, lv_skip, h->slot_of.as<int>(), lab_out, h->vgraph.as<int>(), *fst,
+                                                count ? h->ft_keys.as<unsigned long long>() : nullptr,
+                                                h->ft_cnt.as<unsigned>(), (unsigned)(ft_level_cap - 1));
+    LAUNCH_CHECK(h);
+  }
+  return GK_OK;
+}
+
+int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* skip, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_hc_features: no graphs packed");
+  if (!h->has_labels || h->V == 0) return fail(GK_ERR_ARG, "gk_hc_features: vertex labels are required");
+  if (n_iter < 1 || n_iter >= MAX_LEVELS) return fail(GK_ERR_ARG, "gk_hc_features: n_iter out of range [1, 64)");
+  if (width < 1 || (width & (width - 1))) return fail(GK_ERR_ARG, "gk_hc_features: width must be a power of two");
+  if (h->n_labels0 > width) return fail(GK_ERR_ARG, "gk_hc_features: a packed label is >= width");
+  if (flags & ~(GK_HC_SP | GK_SP_DIJKSTRA_ORDER)) return fail(GK_ERR_ARG, "gk_hc_features: unknown flags");
+  const bool sp = flags & GK_HC_SP;
+  const int64_t V = h->V;
+  if (sp && skip)
+    for (int64_t v = 0; v < V; ++v)
+      if (skip[v]) return fail(GK_ERR_ARG, "gk_hc_features: the ShortestPath base needs a label for every vertex at every level");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const double need = 2.0 * (double)V * (double)width * 8.0;
+  {
+    size_t free_b = 0, total_b = 0;
+    GK_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    if (need > (double)free_b + (double)h->hc_S.cap)
+      return fail(GK_ERR_UNSUPPORTED, "gk_hc_features: the two level buffers of V x W x 8 bytes need " +
+                                          std::to_string((long long)(need / 1048576.0)) + " MiB, " +
+                                          std::to_string((long long)((free_b + h->hc_S.cap) / 1048576)) + " MiB are available");
+  }
+  const int L = n_iter;
+  const int nb = cdiv(V, 256);
+  const int64_t launches0 = h->launches;
+  h->features_ready = false; h->feat_serial++;
+  h->hc_W = 0;
+  GK_TRY(h->hc_S.ensure((size_t)need));
+  GK_TRY(h->hc_z.ensure((size_t)width * 8));
+  h->hc_has_skip = skip != nullptr;
+  if (skip) {
+    GK_TRY(h->hc_skip.ensure((size_t)V));
+    GK_CUDA(cudaMemcpyAsync(h->hc_skip.p, skip, (size_t)V, cudaMemcpyHostToDevice, h->stream));
+  }
+  GK_TRY(h->labels_all.ensure((size_t)L * V * 4));
+  GK_TRY(h->slot_of.ensure(V * 4));
+  GK_TRY(h->flags.ensure(V * 4));
+  GK_TRY(h->block_sums.ensure((size_t)nb * 4));
+  h->ht_cap = std::max<size_t>(next_pow2((size_t)V * 2), 1024);
+  GK_TRY(h->ht_keys.ensure(h->ht_cap * 8));
+  GK_TRY(h->ht_rep.ensure(h->ht_cap * 4));
+  const size_t ft_level_cap = std::max<size_t>(next_pow2((size_t)V * 2), 1024);
+  if (!sp) {
+    if (ft_level_cap * (size_t)L > (1ULL << 31)) return fail(GK_ERR_ARG, "gk_hc_features: feature table too large");
+    h->ft_cap = ft_level_cap * (size_t)L;
+    GK_TRY(h->ft_keys.ensure(h->ft_cap * 8));
+    GK_TRY(h->ft_cnt.ensure(h->ft_cap * 4));
+  }
+  h->hc_W = width;
+  h->hc_levels = L;
+  std::vector<unsigned long long> z((size_t)width);
+  int retries = 0;
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  for (;; ++retries) {
+    if (retries > 8) return fail(GK_ERR_STATE, "gk_hc_features: repeated hash collisions");
+    const unsigned long long seed = mix64(0x2545F4914F6CDD1DULL + 0x9E3779B97F4A7C15ULL * (unsigned long long)retries);
+    const bool degenerate = retries == 0 && h->hc_degenerate_once;
+    for (int c = 0; c < width; ++c) z[c] = degenerate ? 0ULL : (mix64(seed + 0xD1B54A32D192ED03ULL * (unsigned long long)(c + 1)) | 1ULL);
+    GK_CUDA(cudaMemcpyAsync(h->hc_z.p, z.data(), (size_t)width * 8, cudaMemcpyHostToDevice, h->stream));
+    GK_TRY(init_scalars(h, 0));  // (synchronises: z may be rewritten by the next attempt)
+    FeatStats fst;
+    GK_TRY(reset_feature_stats(h, V * (int64_t)L + 1, (int64_t)nb * L, &fst));
+    if (!sp) {
+      GK_CUDA(cudaMemsetAsync(h->ft_keys.p, 0xFF, h->ft_cap * 8, h->stream));
+      GK_CUDA(cudaMemsetAsync(h->ft_cnt.p, 0, h->ft_cap * 4, h->stream));
+    }
+    GK_TRY(hc_run_levels(h, L - 1, &fst, !sp, ft_level_cap));
+    DevScalars* hs;
+    GK_TRY(read_scalars(h, &hs));
+    if (hs->ft_overflow) return fail(GK_ERR_STATE, "gk_hc_features: hash table overflow");
+    if (!hs->collision) break;
+  }
+  h->hc_degenerate_once = false;
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_CUDA(cudaEventSynchronize(h->tev[3]));
+  const float ms_relabel = ev_ms(h->tev[2], h->tev[3]);
+  const DevScalars hs = *h->h_scalars.as<DevScalars>();
+  h->n_levels = L;
+  h->wl_sparse_ids = false;
+  if (sp) {
+    SpLabels lab;
+    lab.n_pass = L;
+    lab.labels = h->labels_all.as<int>();
+    lab.level_base.assign(hs.level_base, hs.level_base + L + 1);
+    GK_TRY(sp_features_impl(h, GK_SP_WITH_LABELS | (flags & GK_SP_DIJKSTRA_ORDER), lab, stats));
+    if (stats) {
+      stats->hash_retries = retries;
+      stats->ms_hash = ms_relabel;
+      stats->kernel_launches = h->launches - launches0;
+    }
+    return GK_OK;
+  }
+  h->n_columns = hs.level_base[L];
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = FK_WL;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = h->N; stats->n_vertices = V; stats->n_edges = h->E;
+    stats->n_levels = L;
+    for (int i = 0; i < L; ++i) stats->level_dims[i] = hs.level_dims[i];
+    stats->n_columns = h->n_columns;
+    stats->hash_retries = retries;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ms_relabel;
+    stats->ms_hash = ms_relabel;
+  }
+  return GK_OK;
+}
+
+int gk_hc_vectors(gk_handle* h, int32_t level, int64_t* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_hc_vectors: null argument");
+  if (h->hc_W <= 0 || level < 0 || level >= h->hc_levels)
+    return fail(GK_ERR_STATE, "gk_hc_vectors: no such level (run gk_hc_features on the packed block first)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  GK_TRY(hc_run_levels(h, level, nullptr, false, 0));
+  const size_t n = (size_t)h->V * (size_t)h->hc_W;
+  GK_CUDA(cudaMemcpyAsync(out, h->hc_S.as<unsigned long long>() + (size_t)(level & 1) * n, n * 8, cudaMemcpyDeviceToHost,
+                          h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+int gk_selftest_hc_collision(gk_handle* h) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  h->hc_degenerate_once = true;
+  return GK_OK;
 }
 
 int gk_sp_distances(gk_handle* h, int64_t g, double* out) {

@@ -229,6 +229,13 @@ struct gk_handle {
   int pm_S = 0, pm_L = 0, pm_d = 0, pm_flags = 0;
   bool pm_has_skip = false;
 
+  // ---- HadamardCode (an FK_WL or FK_SP block): the two level buffers of V x W u64 vectors, the hash multipliers, the
+  // skip flags and the shape of the last gk_hc_features call (gk_hc_vectors recomputes its levels from them)
+  gk::DevBuf hc_S, hc_z, hc_skip;
+  int hc_W = 0, hc_levels = 0;
+  bool hc_has_skip = false;
+  bool hc_degenerate_once = false;  // gk_selftest_hc_collision: the next pass starts with all z_c = 0
+
   // ---- random walk (FK_RW): edge values of the packed CSR, its transpose, eigen-data, coefficients
   gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;
   int rw_route = 0, rw_fn = 0, rw_ncoef = 0;

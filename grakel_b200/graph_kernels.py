@@ -6,6 +6,7 @@ the kernels of the device hot path:
     "shortest_path" / "SP"      (+ with_labels, algorithm_type, as_attributes)
     "edge_histogram" / "EH"
     "core_framework" / "CORE"   (framework; base "shortest_path" or "weisfeiler_lehman" ...)
+    "hadamard_code" / "HC"      (framework; base "vertex_histogram", "shortest_path" or "edge_histogram")
     "weisfeiler_lehman_optimal_assignment" / "WL-OA"
     "graph_hopper" / "GH"
     "neighborhood_hash" / "NH"
@@ -31,7 +32,7 @@ from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
-from .kernels import (EdgeHistogram, GraphHopper, NeighborhoodHash, Propagation, PropagationAttr, PyramidMatch,
+from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, Propagation, PropagationAttr, PyramidMatch,
                       ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
@@ -40,7 +41,7 @@ default_n_components = 100
 _OUTSIDE = frozenset((
     "random_walk", "RW", "graphlet_sampling", "GR", "subgraph_matching", "SM", "multiscale_laplacian", "ML",
     "lovasz_theta", "LOVT", "svm_theta", "SVMT", "neighborhood_subgraph_pairwise_distance",
-    "NSPD", "odd_sth", "ODD", "hadamard_code", "HC"))
+    "NSPD", "odd_sth", "ODD"))
 
 
 def _propagation(params):
@@ -63,6 +64,7 @@ for _names, _framework, _build in (
         (("propagation", "PR"), False, _propagation),
         (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),
+        (("hadamard_code", "HC"), True, lambda p: (HadamardCode, p)),
         (("core_framework", "CORE"), True, lambda p: (CoreFramework, p))):
     for _n in _names:
         _REGISTRY[_n] = (_framework, _build)

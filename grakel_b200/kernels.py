@@ -2424,3 +2424,328 @@ class PyramidMatch(Kernel):
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
+
+
+# ------------------------------------------------------------------------------
+def hc_width(n_labels):
+    """Columns of the reference's Hadamard matrix, `2 ** ceil(log2(nl))` (hadamard_code.py:187), in integers."""
+    return 1 if n_labels <= 1 else 1 << (int(n_labels) - 1).bit_length()
+
+
+def hc_edge_keys(g):
+    """The keys of the reference's edge dictionary of graph-like `g` (graph.py:1182-1204): None for an adjacency
+    input (every vertex is a key), else the endpoints of the listed edges plus the keys of a dict-of-dicts, where
+    `{u: {}}` keeps u (graph.py:1660-1667); `{u: []}` does not."""
+    from .packing import classify
+    kind = classify(g)
+    if kind is None:
+        raise ValueError("Unsupported input type. For more information check the documentation, concerning valid input "
+                         "types for graph type object.")
+    if kind == "adjacency":
+        return None
+    if kind == "dict_tuple":
+        return set(chain.from_iterable(g))
+    if kind == "dict_list":
+        return {u for u, lst in g.items() if lst}.union(chain.from_iterable(g.values()))
+    if kind == "dict_dict":
+        return set(g).union(chain.from_iterable(g.values()))
+    return set(chain.from_iterable((t[0], t[1]) for t in g))
+
+
+def hc_enumerate(label_dicts, labels_enum=None):
+    """The reference's label enumeration (hadamard_code.py:178-181): graph by graph, `for v in set(label.values())`,
+    new labels numbered on from the fitted enumeration.  Returns a new dict."""
+    enum = {} if labels_enum is None else dict(labels_enum)
+    for L in label_dicts:
+        for v in set(L.values()):
+            if v not in enum:
+                enum[v] = len(enum)
+    return enum
+
+
+def _enum_ids(labels, enum):
+    """Enumeration id of every packed vertex label."""
+    if isinstance(labels, np.ndarray):
+        uniq, inv = np.unique(labels, return_inverse=True)
+        lut = np.fromiter((enum[int(u)] for u in uniq.tolist()), dtype=np.int32, count=len(uniq))
+        return lut[inv.reshape(-1)]
+    return np.fromiter((enum[l] for l in labels), dtype=np.int32, count=len(labels))
+
+
+class _HcData:
+    """One parsed input of HadamardCode: the packed block, its enumeration ids, the skip flags of the levels >= 1."""
+
+    def __init__(self, block, ids, skip):
+        self.block, self.ids, self.skip = block, ids, skip
+
+    def __len__(self):
+        return self.block.n_graphs
+
+    @staticmethod
+    def concat(a, b):
+        skip = None
+        if a.skip is not None or b.skip is not None:
+            fa = a.skip if a.skip is not None else np.zeros(a.block.n_vertices, dtype=bool)
+            fb = b.skip if b.skip is not None else np.zeros(b.block.n_vertices, dtype=bool)
+            skip = np.concatenate([fa, fb])
+        return _HcData(Block.concat(a.block, b.block), np.concatenate([a.ids, b.ids]), skip)
+
+
+class HadamardCode(Kernel):
+    """Hadamard code kernel (hadamard_code.py:24-391): K = sum over n_iter levels of the base kernel on the vertices'
+    Hadamard-code vectors.  Level 0 gives every labelled vertex row `enumeration id` of the W x W Sylvester Hadamard
+    matrix (W = 2^ceil(log2 nl)); level i adds every edge-dictionary key's out-neighbour vectors to its own, in int64
+    arithmetic that wraps.  The vectors, their exact classes and the per-level base-kernel features are computed on
+    the device (gk_hc_features); the host replays the reference's label enumeration, so the device vectors are the
+    reference's tuples entry for entry.
+
+    Base kernels: VertexHistogram (default), ShortestPath(with_labels=True) and EdgeHistogram.  Labelled vertices that
+    are not keys of the edge dictionary count at level 0 only, as in the reference."""
+
+    _graph_format = "auto"
+    _nan_to_num = True
+
+    def __init__(self, n_jobs=None, verbose=False, normalize=False, n_iter=5, base_graph_kernel=None):
+        super().__init__(n_jobs=n_jobs, verbose=verbose, normalize=normalize)
+        self.n_iter = n_iter
+        self.base_graph_kernel = base_graph_kernel
+        self._initialized.update({"n_iter": False, "base_graph_kernel": False})
+
+    def initialize(self):
+        if not self._initialized["n_jobs"]:  # kernel.py:386-399: validated, then one device job
+            if type(self.n_jobs) is not int and self.n_jobs is not None:
+                raise ValueError("n_jobs parameter must be an int indicating the number of jobs as in joblib or None")
+            self._parallel = None
+            self._initialized["n_jobs"] = True
+        if not self._initialized["base_graph_kernel"]:  # hadamard_code.py:68-97
+            base = self.base_graph_kernel
+            if base is None:
+                base, params = VertexHistogram, dict()
+            elif type(base) is type and issubclass(base, Kernel):
+                params = dict()
+            else:
+                try:
+                    base, params = base
+                except Exception:
+                    raise TypeError("Base kernel was not formulated in the correct way. Check documentation.")
+                if not (type(base) is type and issubclass(base, Kernel)):
+                    raise TypeError("The first argument must be a valid grakel.kernel.kernel Object")
+                if type(params) is not dict:
+                    raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
+                                     "parameters names and values")
+                params.pop("normalize", None)
+            if base not in (VertexHistogram, ShortestPath, EdgeHistogram):
+                raise NotImplementedError("grakel_b200 runs HadamardCode over VertexHistogram, ShortestPath or "
+                                          "EdgeHistogram; other base kernels are outside the device hot path")
+            if base is ShortestPath:
+                if not params.get("with_labels", True):
+                    raise NotImplementedError("HadamardCode over ShortestPath(with_labels=False) ignores the Hadamard "
+                                              "codes; use n_iter * ShortestPath(with_labels=False)")
+                if params.get("algorithm_type", "auto") not in ("auto", "floyd_warshall", "dijkstra"):
+                    raise ValueError('Unsupported "algorithm_type"')
+            params["normalize"] = False
+            params["verbose"] = self.verbose
+            params["n_jobs"] = None
+            self.base_graph_kernel_ = (base, params)
+            self._initialized["base_graph_kernel"] = True
+        if not self._initialized["n_iter"]:  # :99-102
+            if type(self.n_iter) is not int or self.n_iter <= 0:
+                raise TypeError("'n_iter' must be a positive integer")
+            self._initialized["n_iter"] = True
+
+    # ---- host parsing -----------------------------------------------------------
+    def _elements(self, X):
+        """[graph, labels] or [graph, labels, edge labels] per kept element, with the reference's element checks
+        (hadamard_code.py:142-176)."""
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            is_iter = False
+            if isinstance(x, Iterable):
+                x, is_iter = list(x), True
+            if is_iter and (len(x) == 0 or len(x) >= 2):
+                if len(x) == 0:
+                    warnings.warn("Ignoring empty element on index: " + str(idx))
+                    continue
+                out.append(x[:3])
+            elif type(x) is Graph:
+                el = x.as_element()
+                out.append(el if x.edge_labels else el[:2])
+            else:
+                raise TypeError("each element of X must be either a graph object or a list with at least a graph like "
+                                "object and node labels dict \n")
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    def _parse(self, X, labels_enum):
+        """(_HcData, extended enumeration) of one input."""
+        base = self.base_graph_kernel_[0]
+        if isinstance(X, Block):  # packed input (datasets.read_tu): integer labels
+            if base is EdgeHistogram:
+                raise NotImplementedError("packed blocks carry no edge-label entries; pass the list of graphs")
+            block = X.require("wl", "sp")
+            gp = np.asarray(block.graph_ptr)
+            labels = np.asarray(block.labels)
+            enum = {} if labels_enum is None else dict(labels_enum)
+            for g in range(block.n_graphs):
+                for v in set(labels[gp[g]:gp[g + 1]].tolist()):
+                    if v not in enum:
+                        enum[v] = len(enum)
+            skip = None
+            if block.mode == "wl" and self.n_iter > 1:  # the edge-dictionary keys are the endpoints of the edges
+                rp = np.asarray(block.row_ptr)
+                key = np.diff(rp) > 0
+                key[np.asarray(block.col_idx)] = True
+                skip = None if key.all() else ~key
+            elif block.mode == "sp" and base is not ShortestPath:
+                raise ValueError("this block was packed for another kernel (vertex set 'sp', needed 'wl'): see "
+                                 "grakel_b200.datasets.read_tu(kernel=...)")
+            return _HcData(block, _enum_ids(labels, enum), skip), enum
+        els = self._elements(X)
+        enum = hc_enumerate((x[1] for x in els), labels_enum)
+        if base is EdgeHistogram:
+            values = _edge_label_values(els)
+            sizes = np.concatenate([[0], np.cumsum([len(v) for v in values])])
+            block = Block(sizes, np.zeros(int(sizes[-1]) + 1, dtype=np.int64), np.zeros(0, dtype=np.int64), None,
+                          [l for v in values for l in v])
+            return _HcData(block, None, None), enum
+        if base is ShortestPath:
+            # the base kernel receives every element's own graph object (hadamard_code.py:175, 197): its vertices, and
+            # Floyd-Warshall or Dijkstra path sums as the element's format implies (_path_sum_order).  Its vertices
+            # outside the edge dictionary's keys have no edge, so their labels never reach a path feature.
+            block = pack([x[:2] for x in els], "sp", want_weights=True,
+                         fw_zero_is_absent=self.base_graph_kernel_[1].get("algorithm_type") == "floyd_warshall",
+                         type_error_msg="each element of X must have at least one and at most 3 elements\n")
+            return _HcData(block, _enum_ids(block.labels, enum), None), enum
+        if self.n_iter == 1:  # level 0 only: the label multisets
+            labels = [l for x in els for l in x[1].values()]
+            sizes = np.concatenate([[0], np.cumsum([len(x[1]) for x in els])])
+            block = Block(sizes, np.zeros(int(sizes[-1]) + 1, dtype=np.int64), np.zeros(0, dtype=np.int64), None, labels)
+            return _HcData(block, _enum_ids(labels, enum), None), enum
+        # packed vertices: the keys of every labels dictionary, in its order ('wl' packing)
+        skip = []
+        for x in els:
+            keys = hc_edge_keys(x[0])
+            if keys is None:
+                skip.append(np.zeros(len(x[1]), dtype=bool))
+                continue
+            missing = keys.difference(x[1])
+            if missing:  # the reference's old_label[k] (hadamard_code.py:209)
+                raise KeyError(next(iter(missing)))
+            skip.append(np.fromiter((k not in keys for k in x[1]), dtype=bool, count=len(x[1])))
+        skip = np.concatenate(skip)
+        block = pack([x[:2] for x in els], "wl", len_ok=lambda n: n >= 2)
+        return _HcData(block, _enum_ids(block.labels, enum), skip if skip.any() else None), enum
+
+    def _eh_ids(self, data, known):
+        ids, new = label_ids(data.block.labels, known, sort_new=False)
+        data.ids = ids
+        return new
+
+    # ---- estimator protocol -----------------------------------------------------
+    def fit(self, X, y=None):
+        self._is_transformed = False
+        self._method_calling = 1
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        self._fit(X)
+        return self
+
+    def _fit(self, X):
+        if hasattr(self, "_X_diag"):
+            delattr(self, "_X_diag")
+        data, enum = self._parse(X, None)
+        if self.base_graph_kernel_[0] is EdgeHistogram:
+            self._eh_labels = self._eh_ids(data, None)
+            self._width = hc_width(len(self._eh_labels))
+        else:
+            self._width = hc_width(len(enum))
+        self.X = data
+        self._labels_enum = enum
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("transform input cannot be None")
+        self._fit(X)
+        K, xdiag, _ = self._run(self.X, len(self.X), self._width)
+        self._X_diag = xdiag
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("transform input cannot be None")
+        Y, enum = self._parse(X, self._labels_enum)
+        n_x, n_y = len(self.X), len(Y)
+        if self.base_graph_kernel_[0] is EdgeHistogram:
+            new = self._eh_ids(Y, self._eh_labels)
+            width = hc_width(len(self._eh_labels) + len(new))
+        else:
+            width = hc_width(len(enum))
+        if width == self._width or self.base_graph_kernel_[0] is EdgeHistogram:
+            K, xdiag, ydiag = self._run(_HcData.concat(self.X, Y), n_x, width)
+        else:
+            # the vectors of Y are longer than every fitted vector: no label is shared (hadamard_code.py:187, 235) and
+            # every Y graph is only similar to itself, at its own width
+            _, ydiag, _ = self._run(Y, n_y, width, want_matrix=False)
+            try:
+                check_is_fitted(self, ["_X_diag"])
+                xdiag = self._X_diag
+            except NotFittedError:
+                _, xdiag, _ = self._run(self.X, n_x, self._width, want_matrix=False)
+            K = np.zeros((n_y, n_x))
+        self._X_diag = xdiag
+        self._Y_diag = ydiag
+        self._is_transformed = True
+        return K
+
+    def diagonal(self):
+        check_is_fitted(self, ["X"])
+        try:
+            check_is_fitted(self, ["_X_diag"])
+        except NotFittedError:
+            _, self._X_diag, _ = self._run(self.X, len(self.X), self._width, want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
+
+    # ---- device -----------------------------------------------------------------
+    def _dijkstra_order(self, block):
+        return _path_sum_order(block, self.base_graph_kernel_[1].get("algorithm_type", "auto"))
+
+    def _run(self, data, n_fit, width, want_matrix=True):
+        """pack -> gk_hc_features -> gk_gram.  Returns (K, xdiag, ydiag)."""
+        block = data.block
+        base = self.base_graph_kernel_[0]
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids,
+                     block.weights if base is ShortestPath else None, None)
+            if base is ShortestPath:
+                self.stats_ = eng.hc_features(self.n_iter, width, sp=True, dijkstra_order=self._dijkstra_order(block))
+            else:
+                self.stats_ = eng.hc_features(self.n_iter, width, skip=data.skip)
+            K, xd, yd = eng.gram(block.n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 nan_to_num=True, out=None if want_matrix else False, stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd
+
+    def hc_vectors(self, X, level):
+        """[V, W] int64 Hadamard-code vectors of every packed vertex of X at `level` (zeros where a vertex is absent
+        from the level), as the fitted estimator's relabelling computes them; rows follow each labels dictionary's
+        key order."""
+        check_is_fitted(self, ["X"])
+        data, enum = self._parse(X, self._labels_enum)
+        width = hc_width(len(enum))
+        block = data.block
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
+            eng.hc_features(self.n_iter, width, skip=data.skip)
+            return eng.hc_vectors(level, block.n_vertices, width)

@@ -282,6 +282,30 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
                    const uint8_t* skip, int32_t n_sets, int32_t flags, gk_stats* stats);
 int gk_pm_cells(gk_handle* h, int32_t set, int32_t level, int64_t* out);
 
+/* HadamardCode (hadamard_code.py:24-391) over VertexHistogram or ShortestPath.  Every vertex carries a vector of
+ * `width` (W, a power of two) int64 entries: at level 0 row `label` of Sylvester's Hadamard matrix,
+ * H[r, c] = (-1)^popcount(r & c), for the packed label id r (< W: the reference's label enumeration); at level i >= 1
+ * its own level-(i-1) vector plus those of its out-neighbours, wrapping modulo 2^64 like numpy's int64 additions.
+ * Vertices with skip[v] != 0 (skip[V] may be NULL) are absent from the levels >= 1: labelled vertices that are not
+ * keys of the reference's edge dictionary.  n_iter in [1, 64) levels (level 0 included).  Classes of a level are
+ * exact vector equality (hashed, then verified vector by vector; a collision repeats the pass with another seed).
+ *   flags 0          VertexHistogram: the (graph, level column) counts of every level in one FK_WL block, so gk_gram
+ *                    returns the reference's sum of per-level matrices, with everything gk_gram supports for WL
+ *   GK_HC_SP         ShortestPath(with_labels=True): the labelled path histogram of every level in one FK_SP block
+ *                    (as gk_wl_sp_features); GK_SP_DIJKSTRA_ORDER selects the path-sum order of real weights.  No
+ *                    vertex may be skipped.
+ * GK_ERR_ARG for a packed label >= width, a width that is not a power of two or n_iter out of range;
+ * GK_ERR_UNSUPPORTED when the two V x W x 8-byte level buffers do not fit in device memory.
+ * stats: level_dims = classes per level, hash_retries, ms_hash = the relabel (vectors, classes, VH counts).
+ * gk_hc_vectors recomputes the vectors of one level of the last gk_hc_features call on the packed block:
+ * out[V * W], vertex v's vector at v * W (zeros for a skipped vertex at levels >= 1).
+ * gk_selftest_hc_collision (tests only): the next gk_hc_features starts with a degenerate hash (every z_c = 0), so its
+ * verification must see collisions and its retry must give the right classes. */
+#define GK_HC_SP 8
+int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* skip, int32_t flags, gk_stats* stats);
+int gk_hc_vectors(gk_handle* h, int32_t level, int64_t* out);
+int gk_selftest_hc_collision(gk_handle* h);
+
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
  *   n_fit <  n_graphs : K is [(n_graphs-n_fit) x n_fit], rows = Y graphs (transform)
