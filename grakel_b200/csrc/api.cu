@@ -1111,7 +1111,12 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
   }
 
   size_t dict_cap = std::max<size_t>(h->sp_dict_cap, 1 << 16);
-  size_t dkey_cap = 1 << 18;
+  // distance dictionary of real mode: its slot is the 24-bit distance field of a feature key, so it holds at most
+  // 2^24 lengths (GRAKEL_B200_SP_DKEY_CAP=<slots> lowers the starting size, so that tests reach the regrowth)
+  const size_t DKEY_CAP_MAX = (size_t)1 << 24;
+  size_t dkey_cap = (size_t)1 << 18;
+  if (const char* e = getenv("GRAKEL_B200_SP_DKEY_CAP"))
+    dkey_cap = std::min(DKEY_CAP_MAX, next_pow2(std::max<size_t>(16, strtoull(e, nullptr, 10))));
   bool real_mode = false;
   size_t ft_cap = std::max<size_t>(next_pow2((size_t)std::max<int64_t>(h->V, 1024) * 16 * (size_t)std::min(n_pass, 4)), 1 << 20);
   DevScalars* sc = h->scalars.as<DevScalars>();
@@ -1257,10 +1262,12 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
     DevScalars* hs;
     GK_TRY(read_scalars(h, &hs));
     if (hs->sp_nonint && !real_mode) { real_mode = true; --attempt; continue; }  // switch to exact float keys
-    if (real_mode && (hs->ft_overflow & 2u) && dkey_cap < (1u << 24)) {
-      // either dictionary may have overflowed; grow the distance dictionary first
-      dkey_cap *= 8;
-      if (dkey_cap > (1u << 24)) dkey_cap = 1u << 24;
+    if (hs->ft_overflow & 8u) {  // real mode: the distance dictionary is full (features of this attempt incomplete)
+      if (dkey_cap >= DKEY_CAP_MAX)
+        return fail(GK_ERR_UNSUPPORTED, "gk_sp_features: more than 2^24 distinct real-valued path lengths");
+      dkey_cap = std::min(dkey_cap * 8, DKEY_CAP_MAX);
+      if (hs->ft_overflow & 2u) dict_cap *= 8;
+      continue;
     }
     if (hs->ft_overflow & 2u) { dict_cap *= 8; continue; }
     if (hs->ft_overflow & 1u) { ft_cap *= 4; continue; }
@@ -1595,7 +1602,9 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
   GK_CUDA(cudaMemcpyAsync(keys.data(), h->sp_dict_keys.p, dict_cap * 8, cudaMemcpyDeviceToHost, h->stream));
   DevScalars* hs;
   GK_TRY(read_scalars(h, &hs));
-  if (hs->ft_overflow) return fail(GK_ERR_UNSUPPORTED, "gk_spattr_features: more than 32768 distinct path lengths");
+  // block ids are 16-bit in spattr_accumulate; a full 65536-slot dictionary is past that limit as well
+  if (hs->ft_overflow || hs->sp_dkey_size > 32768)
+    return fail(GK_ERR_UNSUPPORTED, "gk_spattr_features: more than 32768 distinct path lengths");
   std::vector<std::pair<double, int>> found;
   for (size_t i = 0; i < dict_cap; ++i)
     if (keys[i] != EMPTY64) {

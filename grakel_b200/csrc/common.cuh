@@ -106,6 +106,8 @@ struct DevScalars {
   unsigned int sp_nonint;                // SP: a non-integer / out-of-range distance was met
   unsigned int fattr_negative;           // SP-attr: the feature map has a negative entry
   unsigned int nh_order_dep;             // NeighborhoodHash: a count-sensitive result depended on the neighbour order
+  unsigned int sp_dkey_size;             // SP real mode / SP-attr: number of distinct path-length bit patterns
+  unsigned int pad0;
 };
 
 static_assert(sizeof(DevScalars) % 8 == 0, "cleared as 64-bit words");

@@ -73,21 +73,40 @@ __device__ __forceinline__ void sp_feature_add(const SpParams& p, int g, int col
   if (is_new) atomicAdd(&p.st.part_new[blockIdx.x], 1u);
 }
 
-// global (lu,lv,d) dictionary: the slot index IS the column id
-__device__ __forceinline__ int sp_dict_slot(unsigned long long* keys, unsigned mask, unsigned long long key,
-                                            DevScalars* sc) {
+// open-addressing insert into a global key table: returns the key's slot; a new key adds 1 to *size.  A table that is
+// full -- or has a probe chain longer than SP_TABLE_PROBES, which the host's load limit of one half makes vanishingly
+// rare -- sets `ovf_bit` in ft_overflow and returns 0: the host grows that table and repeats the call.  Once the bit
+// is set the attempt is void, so later inserts return at once instead of sweeping a full table each.
+constexpr unsigned SP_TABLE_PROBES = 4096;
+__device__ __forceinline__ int sp_table_slot(unsigned long long* keys, unsigned mask, unsigned long long key,
+                                             unsigned* size, DevScalars* sc, unsigned ovf_bit) {
+  if (__ldcg(&sc->ft_overflow) & ovf_bit) return 0;
   unsigned slot = (unsigned)(mix64(key) >> 13) & mask;
-  for (unsigned probe = 0; probe <= mask; ++probe) {
+  const unsigned probes = mask < SP_TABLE_PROBES ? mask + 1 : SP_TABLE_PROBES;
+  for (unsigned probe = 0; probe < probes; ++probe) {
     unsigned long long prev = __ldcg(&keys[slot]);
     if (prev == EMPTY64) {
       prev = atomicCAS(&keys[slot], EMPTY64, key);
-      if (prev == EMPTY64) { atomicAdd(&sc->sp_dict_size, 1u); return (int)slot; }
+      if (prev == EMPTY64) { atomicAdd(size, 1u); return (int)slot; }
     }
     if (prev == key) return (int)slot;
     slot = (slot + 1) & mask;
   }
-  atomicOr(&sc->ft_overflow, 2u);
+  atomicOr(&sc->ft_overflow, ovf_bit);
   return 0;
+}
+
+// global (lu,lv,d) dictionary: the slot index IS the column id
+__device__ __forceinline__ int sp_dict_slot(unsigned long long* keys, unsigned mask, unsigned long long key,
+                                            DevScalars* sc) {
+  return sp_table_slot(keys, mask, key, &sc->sp_dict_size, sc, 2u);
+}
+
+// global dictionary of distinct path lengths (real mode, SP-attr): counted apart from the feature columns, and with
+// an overflow bit of its own (8) so that only the table that overflowed is grown
+__device__ __forceinline__ int sp_dkey_slot(unsigned long long* keys, unsigned mask, unsigned long long key,
+                                            DevScalars* sc) {
+  return sp_table_slot(keys, mask, key, &sc->sp_dkey_size, sc, 8u);
 }
 
 // CTA-local (key -> count) aggregation shared by the SP feature kernels; falls through to

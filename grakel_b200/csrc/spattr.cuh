@@ -64,7 +64,7 @@ spattr_apsp(SpParams p) {
     unsigned long long key;
     if constexpr (sizeof(T) == 2) key = (unsigned long long)d;
     else key = (unsigned long long)__double_as_longlong((double)d);  // exact-equality key (shortest_path.py:159)
-    sp_dict_slot(p.dict_keys, p.dict_mask, key, p.sc);
+    sp_dkey_slot(p.dict_keys, p.dict_mask, key, p.sc);
   }
 }
 
@@ -122,13 +122,15 @@ sp_dijkstra_order_apsp(SpParams p) {
     if (!p.dist_in_global) gout[i] = __longlong_as_double((long long)d);
     const int u = (int)(i / n), w = (int)(i - (long long)u * n);
     if (u == w || d >= INF) continue;
-    sp_dict_slot(p.dict_keys, p.dict_mask, d, p.sc);  // exact-equality key = the bit pattern
+    sp_dkey_slot(p.dict_keys, p.dict_mask, d, p.sc);  // exact-equality key = the bit pattern
   }
 }
 
 // Real-valued edge weights: histogram of (l(u), l(v), id(d(u,v))) from distance matrices kept
 // in global memory, where id() is the slot of the distance's bit pattern in the global distance
-// dictionary filled by spattr_apsp<double> (exact float equality, shortest_path.py:472, 511).
+// dictionary filled by spattr_apsp<double> (exact float equality, shortest_path.py:472, 511).  A distance that is not
+// in the dictionary (it overflowed while being filled) sets bit 8 of ft_overflow and is skipped: the lookup stops at
+// an empty slot or after one full sweep, so a full table cannot make it spin; the host grows the table and repeats.
 __global__ void __launch_bounds__(SP_THREADS)
 sp_hist_from_dist(SpParams p, const unsigned long long* __restrict__ dkeys, unsigned dmask) {
   extern __shared__ __align__(16) unsigned char sp_smem[];
@@ -150,7 +152,14 @@ sp_hist_from_dist(SpParams p, const unsigned long long* __restrict__ dkeys, unsi
     if (u == w || !(d < 1.0e300)) continue;
     const unsigned long long dk = (unsigned long long)__double_as_longlong(d);
     unsigned slot = (unsigned)(mix64(dk) >> 13) & dmask;
-    while (dkeys[slot] != dk) slot = (slot + 1) & dmask;
+    bool found = false;
+    for (unsigned probe = 0; probe <= dmask; ++probe) {
+      const unsigned long long k = dkeys[slot];
+      if (k == dk) { found = true; break; }
+      if (k == EMPTY64) break;
+      slot = (slot + 1) & dmask;
+    }
+    if (!found) { atomicOr(&p.sc->ft_overflow, 8u); continue; }
     const unsigned long long lu = p.labels ? (unsigned long long)(unsigned)(p.labels[v0 + u] + p.label_offset) : 0ULL;
     const unsigned long long lv = p.labels ? (unsigned long long)(unsigned)(p.labels[v0 + w] + p.label_offset) : 0ULL;
     sp_local_add(lkeys, lcnt, p, g, (lu << 44) | (lv << 24) | (unsigned long long)slot);

@@ -459,7 +459,8 @@ def test_config3_small_and_large_graph_path():
     sp = k.ShortestPath()
     _same(sp.fit_transform(gen(40, 60, 0, as_adj=True)), ref["K"])
     assert int(sp.stats_.n_columns) == int(ref["D"])
-    # graphs whose distance matrix does not fit shared memory use the global-memory path
+    # unit-weight graphs of up to 512 vertices take the bitmask BFS (W = 8 words at 420); the global-memory
+    # Floyd-Warshall routes are covered by test_gpu_sp_routes.py
     X = gen(3, 420, 9, as_adj=True) + gen(5, 30, 9, as_adj=True)
     _same(k.ShortestPath().fit_transform(X), SPOracle().fit_transform(X))
     _same(k.ShortestPath(with_labels=False).fit_transform(X), SPOracle(with_labels=False).fit_transform(X))
