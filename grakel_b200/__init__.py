@@ -2,12 +2,13 @@
 
 Hot path only: WeisfeilerLehman (subtree, or over EdgeHistogram / ShortestPath), VertexHistogram,
 EdgeHistogram, ShortestPath, ShortestPathAttr, WeisfeilerLehmanOptimalAssignment, GraphHopper, NeighborhoodHash, RandomWalk,
-RandomWalkLabeled, Propagation, PropagationAttr, PyramidMatch, HadamardCode, CoreFramework
+RandomWalkLabeled, Propagation, PropagationAttr, PyramidMatch, HadamardCode, NeighborhoodSubgraphPairwiseDistance, CoreFramework
 (`fit` / `transform` / `fit_transform` / `diagonal`), plus the `GraphKernel` name dispatcher.  All kernel matrices are computed by
 hand-written sm_90a CUDA (`libgrakel_b200.so`, C-ABI in include/grakel_b200.h); there is no CPU path.
 """
 from .packing import Graph
-from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, Kernel, NeighborhoodHash, Propagation, PropagationAttr, PyramidMatch,
+from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, Kernel, NeighborhoodHash,
+                      NeighborhoodSubgraphPairwiseDistance, Propagation, PropagationAttr, PyramidMatch,
                       RandomWalk,
                       RandomWalkLabeled, ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman,
                       WeisfeilerLehmanOptimalAssignment)
@@ -19,5 +20,5 @@ __version__ = "0.1.0"
 __all__ = ["Graph", "Kernel", "GraphKernel", "WeisfeilerLehman", "VertexHistogram", "ShortestPath",
            "ShortestPathAttr", "EdgeHistogram", "CoreFramework", "WeisfeilerLehmanOptimalAssignment", "GraphHopper",
            "NeighborhoodHash", "RandomWalk", "RandomWalkLabeled", "Propagation", "PropagationAttr", "PyramidMatch",
-           "HadamardCode", "set_default_device",
+           "HadamardCode", "NeighborhoodSubgraphPairwiseDistance", "set_default_device",
            "default_device"]

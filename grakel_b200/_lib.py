@@ -89,6 +89,10 @@ _SYMBOLS = {
     "gk_hc_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_hc_vectors": (C.c_int, [_P, C.c_int32, _P]),
     "gk_selftest_hc_collision": (C.c_int, [_P]),
+    "gk_nspd_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int32, _P, _P, _P,
+                                   C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_nspd_hashes": (C.c_int, [_P, C.c_int32, _P]),
+    "gk_selftest_nspd_set_order": (C.c_int, [C.c_int64, _P, _P, _P]),
     "gk_gram": (C.c_int, [_P, C.c_int64, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P,
                           C.POINTER(GkStats)]),
     "gk_fetch": (C.c_int, [_P, _P, C.c_int32, C.c_int64]),
@@ -156,6 +160,18 @@ def _ptr(a):
 
 def _i32(a):
     return np.ascontiguousarray(a, dtype=np.int32)
+
+
+def nspd_set_order(h0, h1):
+    """Host only: iteration order of CPython's set after inserting the distinct pairs with element hashes
+    (h0[k], h1[k]) in order k = 0 .. n-1 (the emulation NeighborhoodSubgraphPairwiseDistance runs on the device)."""
+    a = np.ascontiguousarray(h0, dtype=np.int64)
+    b = np.ascontiguousarray(h1, dtype=np.int64)
+    out = np.empty(len(a), dtype=np.int64)
+    lib = load_library()
+    if lib.gk_selftest_nspd_set_order(len(a), _ptr(a), _ptr(b), _ptr(out)) != 0:
+        raise GrakelB200Error(lib.gk_last_error().decode())
+    return out
 
 
 class _HostBlock:
@@ -401,6 +417,28 @@ class Engine:
         """Tests only: the next hc_features starts with a degenerate hash, so it must detect collisions and retry."""
         with self._lock:
             self._check(self.lib.gk_selftest_hc_collision(self.h))
+
+    def nspd_features(self, r, d, sym_hash, edge_label, tokens):
+        """NeighborhoodSubgraphPairwiseDistance hashes and per-level count tables (gk_nspd_features).  `tokens` is
+        the NspdTokens of kernels.py.  Returns (stats, per-graph masks of the distances with pairs)."""
+        sh = np.ascontiguousarray(sym_hash, dtype=np.int64)
+        el = _i32(edge_label)
+        t = tokens
+        mask = np.zeros(self.n_graphs, dtype=np.uint64)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_nspd_features(
+                self.h, int(r), int(d), _ptr(sh), _ptr(el), _ptr(t.tok_rank), int(t.n_labels), _ptr(t.rank_off),
+                _ptr(t.rank_bytes), _ptr(t.rank_cp), int(t.n_ranks), _ptr(t.el_off), _ptr(t.el_bytes), _ptr(t.el_cp),
+                int(t.n_elabels), _ptr(mask), 0, C.byref(st)))
+        return st, mask
+
+    def nspd_hashes(self, radius, n_vertices):
+        """H[radius][v] (u32) of every packed vertex after nspd_features."""
+        out = np.empty(n_vertices, dtype=np.uint32)
+        with self._lock:
+            self._check(self.lib.gk_nspd_hashes(self.h, int(radius), _ptr(out)))
+        return out
 
     def rw_iterations(self, rows, cols):
         """CG iterations / series terms of every entry of the last random walk gram() (rows x cols u8)."""

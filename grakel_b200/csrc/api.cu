@@ -31,6 +31,7 @@
 #include "propagation.cuh"
 #include "pyramid_match.cuh"
 #include "hadamard_code.cuh"
+#include "nspd.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -169,6 +170,10 @@ struct HandleExtra {
                                  // unless it was 256 (a count of 256 repeats through the synchronous route once)
   // NeighborhoodHash: per level, distinct codes, columns and entries of the unary-expanded block
   std::vector<long long> nh_dims, nh_cols, nh_entries;
+  // NeighborhoodSubgraphPairwiseDistance: per level (delta-major), its table's byte offset in nspd_blk, slots, pairs
+  // and columns; per graph, the mask of the distances it has pairs at
+  std::vector<long long> nspd_off, nspd_cap, nspd_M, nspd_cols;
+  std::vector<unsigned long long> nspd_mask;
 };
 static std::vector<std::pair<gk_handle*, HandleExtra*>> g_extra;
 static HandleExtra* extra_of(gk_handle* h) {
@@ -333,7 +338,9 @@ int gk_destroy(gk_handle* h) {
                         &h->rw_val, &h->rw_trp, &h->rw_tci, &h->rw_tval, &h->rw_q, &h->rw_w, &h->rw_coef, &h->rw_ws,
                         &h->rw_iters, &h->rw_cap,
                         &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt,
-                        &h->pm_U, &h->pm_ncols, &h->pm_skip, &h->hc_S, &h->hc_z, &h->hc_skip};
+                        &h->pm_U, &h->pm_ncols, &h->pm_skip, &h->hc_S, &h->hc_z, &h->hc_skip,
+                        &h->nspd_lvl, &h->nspd_q, &h->nspd_H, &h->nspd_aux, &h->nspd_ws, &h->nspd_pairs, &h->nspd_blk,
+                        &h->nspd_tab, &h->nspd_keys, &h->nspd_C};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1701,6 +1708,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_RW     */ {"random walk", false, true, false, false},
     /* FK_PK     */ {"Propagation", true, true, false, false},
     /* FK_PM     */ {"PyramidMatch", false, true, false, false},
+    /* FK_NSPD   */ {"NeighborhoodSubgraphPairwiseDistance", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -3584,6 +3592,387 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
   return GK_OK;
 }
 
+// ---------------------------------------------------------------------------
+// NeighborhoodSubgraphPairwiseDistance (nspd.cuh).  Level l = delta * (r + 1) + rho has its (graph, column) -> count
+// table at nspd_blk + nspd_off[l]: keys [cap] u64 | counts [cap] u32 | graphs per column [M + 1] u32 | self
+// similarities [N] u64 | largest count, entries (u32 x 2).
+struct NspdLevel {
+  unsigned long long* keys;
+  unsigned* cnt;
+  unsigned* colcnt;
+  unsigned long long* diag;
+  unsigned* part;
+};
+
+static size_t nspd_level_bytes(long long cap, long long M, long long N) {
+  const size_t b = (size_t)cap * 12 + ((size_t)(M + 1) * 4 + 7) / 8 * 8 + (size_t)std::max<long long>(N, 1) * 8 + 8;
+  return (b + 255) / 256 * 256;
+}
+
+static NspdLevel nspd_level(gk_handle* h, int l) {
+  HandleExtra* ex = extra_of(h);
+  char* b = h->nspd_blk.as<char>() + ex->nspd_off[l];
+  const long long cap = ex->nspd_cap[l], M = ex->nspd_M[l];
+  NspdLevel L;
+  L.keys = reinterpret_cast<unsigned long long*>(b);
+  L.cnt = reinterpret_cast<unsigned*>(b + cap * 8);
+  L.colcnt = reinterpret_cast<unsigned*>(b + cap * 12);
+  L.diag = reinterpret_cast<unsigned long long*>(b + cap * 12 + ((M + 1) * 4 + 7) / 8 * 8);
+  L.part = reinterpret_cast<unsigned*>(L.diag + std::max<long long>(h->N, 1));
+  return L;
+}
+
+// Host tables of gk_nspd_features, packed one after another (8-byte aligned) into nspd_aux.
+struct NspdAux {
+  std::vector<char> host;
+  size_t add(const void* p, size_t bytes) {
+    const size_t at = (host.size() + 7) / 8 * 8;
+    host.resize(at + bytes);
+    if (bytes) memcpy(host.data() + at, p, bytes);
+    return at;
+  }
+};
+
+static int nspd_build_params(gk_handle* h, const int64_t* sym_hash, const int32_t* edge_label, const int32_t* tok_rank,
+                             int64_t n_labels, const int64_t* rank_off, const uint8_t* rank_bytes, const int32_t* rank_cp,
+                             int32_t n_ranks, const int64_t* el_off, const uint8_t* el_bytes, const int32_t* el_cp,
+                             int32_t n_elabels, NspdParams* p, std::vector<long long>* lvl_off_h) {
+  const int64_t N = h->N, V = h->V, E = h->E;
+  HandleExtra* ex = extra_of(h);
+  const std::vector<int>& gp = ex->graph_ptr;
+  lvl_off_h->assign(N + 1, 0);
+  for (int64_t g = 0; g < N; ++g) {
+    const long long n = gp[g + 1] - gp[g];
+    (*lvl_off_h)[g + 1] = (*lvl_off_h)[g] + n * n;
+  }
+  NspdAux a;
+  const size_t o_sym = a.add(sym_hash, (size_t)V * 8);
+  const size_t o_el = a.add(edge_label, (size_t)E * 4);
+  const size_t o_tok = a.add(tok_rank, (size_t)(h->nspd_d + 1) * n_labels * 4);
+  const size_t o_roff = a.add(rank_off, (size_t)(n_ranks + 1) * 8);
+  const size_t o_rb = a.add(rank_bytes, (size_t)rank_off[n_ranks]);
+  const size_t o_rcp = a.add(rank_cp, (size_t)n_ranks * 4);
+  const size_t o_eoff = a.add(el_off, (size_t)(n_elabels + 1) * 8);
+  const size_t o_eb = a.add(el_bytes, (size_t)el_off[n_elabels]);
+  const size_t o_ecp = a.add(el_cp, (size_t)n_elabels * 4);
+  const size_t o_loff = a.add(lvl_off_h->data(), (size_t)(N + 1) * 8);
+  std::vector<unsigned char> loop(std::max<int64_t>(V, 1), 0);
+  {
+    std::vector<int> rp(V + 1), ci(std::max<int64_t>(E, 1));
+    GK_CUDA(cudaMemcpy(rp.data(), h->row_ptr.p, (V + 1) * 4, cudaMemcpyDeviceToHost));
+    if (E) GK_CUDA(cudaMemcpy(ci.data(), h->col_idx.p, E * 4, cudaMemcpyDeviceToHost));
+    for (int64_t v = 0; v < V; ++v)
+      for (int k = rp[v]; k < rp[v + 1]; ++k)
+        if (ci[k] == v) loop[v] = 1;
+  }
+  const size_t o_loop = a.add(loop.data(), (size_t)V);
+  GK_TRY(h->nspd_aux.ensure(a.host.size() + 8));
+  GK_CUDA(cudaMemcpy(h->nspd_aux.p, a.host.data(), a.host.size(), cudaMemcpyHostToDevice));
+  char* d = h->nspd_aux.as<char>();
+  memset(p, 0, sizeof(*p));
+  p->N = (int)N; p->r = h->nspd_r; p->d = h->nspd_d; p->n_labels = (int)n_labels;
+  p->graph_ptr = h->graph_ptr.as<int>(); p->row_ptr = h->row_ptr.as<int>(); p->col_idx = h->col_idx.as<int>();
+  p->labels = h->labels0.as<int>();
+  p->edge_label = reinterpret_cast<const int*>(d + o_el);
+  p->sym_hash = reinterpret_cast<const long long*>(d + o_sym);
+  p->lvl_off = reinterpret_cast<const long long*>(d + o_loff);
+  p->tok_rank = reinterpret_cast<const int*>(d + o_tok);
+  p->rank_off = reinterpret_cast<const long long*>(d + o_roff);
+  p->rank_bytes = reinterpret_cast<const unsigned char*>(d + o_rb);
+  p->rank_cp = reinterpret_cast<const int*>(d + o_rcp);
+  p->el_off = reinterpret_cast<const long long*>(d + o_eoff);
+  p->el_bytes = reinterpret_cast<const unsigned char*>(d + o_eb);
+  p->el_cp = reinterpret_cast<const int*>(d + o_ecp);
+  p->selfloop = reinterpret_cast<const unsigned char*>(d + o_loop);
+  return GK_OK;
+}
+
+extern "C" {
+
+int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash, const int32_t* edge_label,
+                     const int32_t* tok_rank, int64_t n_labels, const int64_t* rank_off, const uint8_t* rank_bytes,
+                     const int32_t* rank_cp, int32_t n_ranks, const int64_t* el_off, const uint8_t* el_bytes,
+                     const int32_t* el_cp, int32_t n_elabels, uint64_t* delta_mask, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_nspd_features: no graphs packed");
+  if (!h->has_labels) return fail(GK_ERR_ARG, "gk_nspd_features: vertex labels are required");
+  if (r < 0 || d < 0) return fail(GK_ERR_ARG, "gk_nspd_features: r and d must be >= 0");
+  if ((int64_t)(r + 1) * (d + 1) > MAX_LEVELS)
+    return fail(GK_ERR_UNSUPPORTED, "gk_nspd_features: (r + 1)(d + 1) levels exceed 64");
+  if (flags != 0) return fail(GK_ERR_ARG, "gk_nspd_features: no flags are defined");
+  if (!sym_hash || (!edge_label && h->E) || !tok_rank || !rank_off || !rank_cp || !el_off || (!el_cp && n_elabels))
+    return fail(GK_ERR_ARG, "gk_nspd_features: null table");
+  if (n_labels < h->n_labels0) return fail(GK_ERR_ARG, "gk_nspd_features: a token is needed for every label id");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t N = h->N, V = h->V, E = h->E;
+  const int64_t launches0 = h->launches;
+  HandleExtra* ex = extra_of(h);
+  h->features_ready = false; h->feat_serial++;
+  h->nspd_r = r; h->nspd_d = d;
+  GK_TRY(init_scalars(h, 0));
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  NspdParams p;
+  std::vector<long long> loff;
+  GK_TRY(nspd_build_params(h, sym_hash, edge_label, tok_rank, n_labels, rank_off, rank_bytes, rank_cp, n_ranks, el_off,
+                           el_bytes, el_cp, n_elabels, &p, &loff));
+  const long long P = loff[N];
+  const std::vector<int>& gp = ex->graph_ptr;
+  long long max_n = 1, max_e = 1;
+  for (int64_t g = 0; g < N; ++g) {
+    max_n = std::max<long long>(max_n, gp[g + 1] - gp[g]);
+    max_e = std::max<long long>(max_e, ex->graph_eptr[g + 1] - ex->graph_eptr[g]);
+  }
+  // ---- BFS levels
+  GK_TRY(h->nspd_lvl.ensure((size_t)std::max<long long>(P, 1)));
+  GK_TRY(h->nspd_q.ensure((size_t)std::max<long long>(P, 1) * 4));
+  p.lvl = h->nspd_lvl.as<unsigned char>();
+  const int max_level = r > 0 ? std::max(r, d) : 0;
+  nspd_bfs<<<cdiv(V, 128), 128, 0, h->stream>>>((int)V, (int)N, p.graph_ptr, p.row_ptr, p.col_idx, p.lvl_off, max_level,
+                                                h->nspd_lvl.as<unsigned char>(), h->nspd_q.as<int>());
+  LAUNCH_CHECK(h);
+  // ---- hashes: one slot per vertex, fewer under the workspace budget (GRAKEL_B200_NSPD_WS_BUDGET=<bytes>)
+  GK_TRY(h->nspd_H.ensure((size_t)(r + 1) * std::max<int64_t>(V, 1) * 4));
+  p.H = h->nspd_H.as<unsigned>();
+  p.set_cap = (long long)nspd_set_cap(max_e);
+  p.max_e = max_e;
+  p.max_n = max_n;
+  p.ball = r > 0 ? max_n + 1 : 1;
+  if (p.ball * p.ball >= (1LL << 32))  // label offsets are u32
+    return fail(GK_ERR_UNSUPPORTED, "gk_nspd_features: r > 0 with a graph of 65535 or more vertices");
+  p.slot_words = nspd_slot_words(p.set_cap, max_e, max_n, p.ball);
+  size_t budget = (size_t)4 << 30;
+  if (const char* e = getenv("GRAKEL_B200_NSPD_WS_BUDGET")) budget = std::max<size_t>(1, strtoull(e, nullptr, 10));
+  const long long slots = std::max<long long>(1, std::min<long long>(V, (long long)(budget / ((size_t)p.slot_words * 4))));
+  p.n_slots = (int)slots;
+  GK_TRY(h->nspd_ws.ensure((size_t)slots * p.slot_words * 4));
+  p.ws = h->nspd_ws.as<unsigned>();
+  nspd_hash<<<cdiv(slots, 64), 64, 0, h->stream>>>(p, (int)V);
+  LAUNCH_CHECK(h);
+  GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
+  // ---- pairs of every distance: count, then fill
+  const int D1 = d + 1;
+  GK_TRY(h->nspd_keys.ensure((size_t)(3 * D1 + N) * 8 + 64));
+  unsigned long long* cnt = h->nspd_keys.as<unsigned long long>();
+  unsigned long long* cursor = cnt + D1;
+  unsigned long long* base = cursor + D1;
+  unsigned long long* mask = base + D1;
+  GK_CUDA(cudaMemsetAsync(cnt, 0, (size_t)(3 * D1 + N) * 8, h->stream));
+  const int pgrid = (int)std::min<int64_t>(N, (int64_t)h->sm_count * 16);
+  nspd_pairs<<<pgrid, 256, 0, h->stream>>>((int)N, r, d, p.graph_ptr, p.lvl_off, p.lvl, p.selfloop, 0, cnt, cursor, base,
+                                           nullptr, nullptr, mask);
+  LAUNCH_CHECK(h);
+  std::vector<unsigned long long> hc(D1 + N);
+  GK_CUDA(cudaMemcpyAsync(hc.data(), cnt, D1 * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaMemcpyAsync(hc.data() + D1, mask, N * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  std::vector<unsigned long long> hb(D1, 0);
+  unsigned long long tot = 0, Mmax = 1;
+  for (int t = 0; t < D1; ++t) { hb[t] = tot; tot += hc[t]; Mmax = std::max(Mmax, hc[t]); }
+  if (tot >= (1ULL << 31)) return fail(GK_ERR_UNSUPPORTED, "gk_nspd_features: 2^31 or more vertex pairs");
+  ex->nspd_mask.assign(hc.begin() + D1, hc.end());
+  if (delta_mask) memcpy(delta_mask, ex->nspd_mask.data(), N * 8);
+  GK_TRY(h->nspd_pairs.ensure((size_t)std::max<unsigned long long>(tot, 1) * 8));
+  unsigned* A = h->nspd_pairs.as<unsigned>();
+  unsigned* Bv = A + std::max<unsigned long long>(tot, 1);
+  GK_CUDA(cudaMemcpyAsync(base, hb.data(), D1 * 8, cudaMemcpyHostToDevice, h->stream));
+  nspd_pairs<<<pgrid, 256, 0, h->stream>>>((int)N, r, d, p.graph_ptr, p.lvl_off, p.lvl, p.selfloop, 1, cnt, cursor, base,
+                                           A, Bv, mask);
+  LAUNCH_CHECK(h);
+  // ---- per-level tables (delta-major), numbered with the NeighborhoodHash column passes
+  const int n_lev = D1 * (r + 1);
+  ex->nspd_off.assign(n_lev, 0); ex->nspd_cap.assign(n_lev, 0); ex->nspd_M.assign(n_lev, 0); ex->nspd_cols.assign(n_lev, 0);
+  size_t blk = 0;
+  for (int l = 0; l < n_lev; ++l) {
+    const long long M = (long long)hc[l / (r + 1)];
+    ex->nspd_M[l] = M;
+    ex->nspd_cap[l] = (long long)std::max<size_t>(next_pow2((size_t)std::max<long long>(M, 1) * 2), 1024);
+    ex->nspd_off[l] = (long long)blk;
+    blk += nspd_level_bytes(ex->nspd_cap[l], M, N);
+  }
+  GK_TRY(h->nspd_blk.ensure(blk));
+  const size_t tcap = std::max<size_t>(next_pow2((size_t)Mmax * 2), 1024);
+  GK_TRY(h->nspd_tab.ensure(tcap * 8 + (size_t)Mmax * 4));
+  int* tab = h->nspd_tab.as<int>();
+  int* colid = tab + tcap;
+  int* slot_of = colid + tcap;
+  GK_TRY(h->nspd_C.ensure((size_t)Mmax * 13 + (size_t)n_lev * 8 + 64));  // keys | entry graphs | valid | columns
+  unsigned long long* keys = h->nspd_C.as<unsigned long long>();
+  int* egraph = reinterpret_cast<int*>(keys + Mmax);
+  unsigned char* valid = reinterpret_cast<unsigned char*>(egraph + Mmax);
+  unsigned long long* dims = reinterpret_cast<unsigned long long*>(h->nspd_C.as<char>() + ((size_t)Mmax * 13 + 7) / 8 * 8);
+  GK_CUDA(cudaMemsetAsync(valid, 1, Mmax, h->stream));
+  GK_CUDA(cudaMemsetAsync(dims, 0, (size_t)n_lev * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->nspd_blk.p, 0, blk, h->stream));
+  for (int l = 0; l < n_lev; ++l) {
+    const int delta = l / (r + 1), rho = l % (r + 1);
+    const long long M = ex->nspd_M[l];
+    const size_t cap = (size_t)ex->nspd_cap[l];
+    NspdLevel L = nspd_level(h, l);
+    GK_CUDA(cudaMemsetAsync(L.keys, 0xFF, cap * 8, h->stream));
+    if (!M) continue;
+    nspd_keys<<<cdiv(M, 256), 256, 0, h->stream>>>(M, A + hb[delta], Bv + hb[delta], p.H + (size_t)rho * V,
+                                                   h->vgraph.as<int>(), keys, egraph);
+    LAUNCH_CHECK(h);
+    GK_CUDA(cudaMemsetAsync(tab, 0xFF, tcap * 4, h->stream));
+    nh_code_insert<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, keys, valid, tab, (unsigned)(tcap - 1), slot_of);
+    LAUNCH_CHECK(h);
+    nh_code_number<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, valid, tab, slot_of, colid, dims + l);
+    LAUNCH_CHECK(h);
+    nh_count<<<cdiv(M, 256), 256, 0, h->stream>>>((int)M, 1, valid, egraph, slot_of, colid, L.keys, L.cnt,
+                                                  (unsigned)(cap - 1));
+    LAUNCH_CHECK(h);
+    nspd_level_stats<<<cdiv((long long)cap, 256), 256, 0, h->stream>>>(cap, L.keys, L.cnt, L.colcnt, L.diag, L.part);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  std::vector<unsigned long long> hd(n_lev);
+  GK_CUDA(cudaMemcpyAsync(hd.data(), dims, n_lev * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  int64_t n_cols = 0;
+  for (int l = 0; l < n_lev; ++l) { ex->nspd_cols[l] = (long long)hd[l]; n_cols += (int64_t)hd[l]; }
+  h->n_columns = n_cols;
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = FK_NSPD;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
+    stats->n_levels = n_lev;
+    for (int l = 0; l < n_lev; ++l) stats->level_dims[l] = ex->nspd_cols[l];
+    stats->n_columns = n_cols;
+    stats->n_entries = (int64_t)tot;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_hash = ev_ms(h->tev[2], h->tev[6]);
+    stats->ms_columns = ev_ms(h->tev[6], h->tev[3]);
+  }
+  return GK_OK;
+}
+
+int gk_nspd_hashes(gk_handle* h, int32_t radius, uint32_t* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_nspd_hashes: null argument");
+  if (h->feature_kind != FK_NSPD || !h->features_ready || radius < 0 || radius > h->nspd_r)
+    return fail(GK_ERR_STATE, "gk_nspd_hashes: no such radius (run gk_nspd_features first)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  if (h->V) {
+    GK_CUDA(cudaMemcpyAsync(out, h->nspd_H.as<unsigned>() + (size_t)radius * h->V, (size_t)h->V * 4,
+                            cudaMemcpyDeviceToHost, h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  return GK_OK;
+}
+
+// CPython's set on n distinct pairs inserted in order (element hashes h0[k], h1[k]); order[] = iteration order.
+int gk_selftest_nspd_set_order(int64_t n, const int64_t* h0, const int64_t* h1, int64_t* order) {
+  if (n < 0 || (n && (!h0 || !h1 || !order))) return fail(GK_ERR_ARG, "gk_selftest_nspd_set_order: bad argument");
+  const unsigned long long cap = nspd_set_cap(n);
+  std::vector<unsigned> buf(2 * cap);
+  NspdSet s;
+  s.buf[0] = buf.data();
+  s.buf[1] = buf.data() + cap;
+  nspd_set_clear(s);
+  auto hash_of = [&](unsigned id) { return nspd_tuple_hash(h0[id], h1[id]); };
+  for (int64_t k = 0; k < n; ++k) nspd_set_add(s, (unsigned)k, hash_of((unsigned)k), hash_of);
+  int64_t m = 0;
+  for (unsigned long long k = 0; k <= s.mask; ++k)
+    if (s.buf[s.cur][k] != NSPD_EMPTY) order[m++] = s.buf[s.cur][k];
+  return m == n ? GK_OK : fail(GK_ERR_STATE, "gk_selftest_nspd_set_order: lost an item");
+}
+
+}  // extern "C"
+
+// Gram of NeighborhoodSubgraphPairwiseDistance features (gram_path 12): per level, in the reference's order, the
+// exact integer Gram of its count table as fp64 counts, folded into K at once (one count matrix live).  The levels
+// are those the fitted graphs have (square case) or that both sides have (transform); GK_NORMALIZE divides by the
+// number of fitted levels, or by sqrt(levels of Y x levels of X).  Rows go in chunks when one level's count matrix of
+// the whole request would exceed 8 GiB (GRAKEL_B200_NSPD_C_BUDGET=<bytes> lowers it).
+static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
+  const bool square = q.square;
+  const int r1 = h->nspd_r + 1;
+  const int64_t launches0 = h->launches;
+  auto maxd = [&](int64_t a, int64_t b) {
+    int m = -1;
+    for (int64_t g = a; g < b; ++g)
+      if (ex->nspd_mask[g]) m = std::max(m, 63 - __builtin_clzll(ex->nspd_mask[g]));
+    return m;
+  };
+  const int mx = maxd(0, n_fit), my = square ? mx : maxd(n_fit, N);
+  const int m_use = std::min(mx, my);
+  const long long nlx = (long long)r1 * (mx + 1), nly = (long long)r1 * (my + 1);
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  const int64_t ldc = (k_cols + 7) / 8 * 8;
+  size_t c_budget = (size_t)8 << 30;
+  if (const char* e = getenv("GRAKEL_B200_NSPD_C_BUDGET")) c_budget = std::max<size_t>(1, strtoull(e, nullptr, 10));
+  const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(std::max<int64_t>(k_rows, 1), (int64_t)(c_budget / ((size_t)ldc * 8))));
+  GK_TRY(h->nh_C.ensure((size_t)chunk * ldc * 8));
+  double* C = h->nh_C.as<double>();
+  const int32_t gflags = (q.flags & (GK_GRAM_SIMT | GK_DENSE_ALL)) | GK_FULL_TILES | GK_OUT_DEVICE;
+  std::vector<float> ms_level(64, 0.f);
+  float ms_fold = 0.f;
+  int64_t max_T = 0, gram_launches = 0, elem_bytes = 0;
+  for (int64_t cb = q.row_begin; cb < q.row_end; cb += chunk) {
+    const int64_t ce = std::min<int64_t>(q.row_end, cb + chunk), rows = ce - cb;
+    double* o = out.p + (size_t)(cb - q.row_begin) * out.ld;
+    GK_CUDA(cudaMemset2DAsync(o, (size_t)out.ld * 8, 0, (size_t)k_cols * 8, (size_t)rows, h->stream));
+    for (int delta = 0; delta <= m_use; ++delta)
+      for (int rho = 0; rho < r1; ++rho) {
+        const int l = delta * r1 + rho;
+        NspdLevel L = nspd_level(h, l);
+        IntBlock fb;
+        fb.keys = L.keys; fb.cnt = L.cnt; fb.cap = (size_t)ex->nspd_cap[l];
+        fb.colcnt = L.colcnt; fb.col_cap = ex->nspd_M[l] + 1; fb.n_columns = ex->nspd_cols[l];
+        fb.diag = L.diag; fb.part_max = L.part; fb.part_new = L.part + 1; fb.n_part = 1;
+        fb.prologue_on_host = false;
+        GramReq lq;
+        GK_TRY(gram_request(h, FK_WL, n_fit, gflags, cb, ce, C, GK_F64, ldc, nullptr, nullptr, &lq));
+        gk_stats st;
+        memset(&st, 0, sizeof(st));
+        GK_TRY(gram_int(h, lq, fb, &st));
+        ms_level[l] += st.ms_total;
+        max_T = std::max<int64_t>(max_T, st.threshold);
+        gram_launches += st.gemm_launches;
+        elem_bytes = std::max<int64_t>(elem_bytes, st.gemm_elem_bytes);
+        if (rows > 0) {
+          GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+          nspd_fold<<<cdiv(rows * k_cols, 256), 256, 0, h->stream>>>((int)rows, (int)k_cols, C, ldc,
+                                                                     (int)((square ? 0 : n_fit) + cb), L.diag,
+                                                                     square ? 1 : 0, o, out.ld);
+          LAUNCH_CHECK(h);
+          GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+          GK_CUDA(cudaEventSynchronize(h->tev[1]));
+          ms_fold += ev_ms(h->tev[0], h->tev[1]);
+        }
+      }
+    if ((q.flags & GK_NORMALIZE) && rows > 0) {
+      const double div = square ? (double)nlx : sqrt((double)nly * (double)nlx);
+      nspd_scale<<<cdiv(rows * k_cols, 256), 256, 0, h->stream>>>((int)rows, (int)k_cols, div, o, out.ld);
+      LAUNCH_CHECK(h);
+    }
+  }
+  GramReq kq = q;  // diagonal(): the number of levels of each side, written on the host
+  kq.xdiag = kq.ydiag = nullptr;
+  GK_TRY(f64_deliver(h, kq, out, false, h->ev[14], h->ev[15]));
+  if (q.xdiag) for (int64_t i = 0; i < n_fit; ++i) q.xdiag[i] = (double)nlx;
+  if (q.ydiag && !square) for (int64_t i = 0; i < N - n_fit; ++i) q.ydiag[i] = (double)nly;
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->n_levels = (int64_t)r1 * (m_use + 1);
+    stats->gram_path = 12;
+    stats->threshold = max_T;
+    stats->gemm_launches = gram_launches + (h->launches - launches0);
+    stats->gemm_elem_bytes = elem_bytes;
+    float tot = ms_fold;
+    for (int l = 0; l < 64; ++l) { stats->ms_level_gram[l] = ms_level[l]; tot += ms_level[l]; }
+    stats->ms_gemm = tot - ms_fold;
+    stats->ms_combine = ms_fold;
+    stats->ms_d2h = ev_ms(h->ev[14], h->ev[15]);
+    stats->ms_total = tot + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
 extern "C" {
 
 int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
@@ -3598,6 +3987,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_GH: return h->gh_node_kernel == GK_GH_LINEAR ? gram_spattr(h, q, stats) : gram_gh_nodepair(h, q, stats);
     case FK_NH: return gram_nh(h, q, stats);
     case FK_PM: return gram_pm(h, q, stats);
+    case FK_NSPD: return gram_nspd(h, q, stats);
     case FK_RW: return gram_rw(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }

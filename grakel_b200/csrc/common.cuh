@@ -123,6 +123,7 @@ enum FeatureKind : int {
   FK_RW = 6,      // random walk edge values
   FK_PK = 7,      // Propagation counts in the SP layout: the integer Gram
   FK_PM = 8,      // PyramidMatch per-level expanded blocks (the NeighborhoodHash layout)
+  FK_NSPD = 9,    // NeighborhoodSubgraphPairwiseDistance per-(radius, distance) count tables
 };
 
 }  // namespace gk
@@ -237,6 +238,12 @@ struct gk_handle {
   int hc_W = 0, hc_levels = 0;
   bool hc_has_skip = false;
   bool hc_degenerate_once = false;  // gk_selftest_hc_collision: the next pass starts with all z_c = 0
+
+  // ---- NeighborhoodSubgraphPairwiseDistance (FK_NSPD): BFS level matrices [sum n_g^2] u8 and their queue, hashes
+  // [(r + 1) V] u32, the host tables (aux), the hashing slots, the pairs of every distance, the per-level (graph,
+  // column) count tables and the fp64 count matrix of one level
+  gk::DevBuf nspd_lvl, nspd_q, nspd_H, nspd_aux, nspd_ws, nspd_pairs, nspd_blk, nspd_tab, nspd_keys, nspd_C;
+  int nspd_r = 0, nspd_d = 0;
 
   // ---- random walk (FK_RW): edge values of the packed CSR, its transpose, eigen-data, coefficients
   gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;

@@ -10,6 +10,7 @@ the kernels of the device hot path:
     "weisfeiler_lehman_optimal_assignment" / "WL-OA"
     "graph_hopper" / "GH"
     "neighborhood_hash" / "NH"
+    "neighborhood_subgraph_pairwise_distance" / "NSPD"  (+ r, d)
     "propagation" / "PR"        (+ with_attributes: PropagationAttr)
     "pyramid_match" / "PM"      (+ with_labels, L, d)
 
@@ -32,7 +33,8 @@ from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
-from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, Propagation, PropagationAttr, PyramidMatch,
+from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, NeighborhoodSubgraphPairwiseDistance,
+                      Propagation, PropagationAttr, PyramidMatch,
                       ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
@@ -40,8 +42,7 @@ default_n_components = 100
 # reference names outside the hot path (graph_kernels.py:38-64)
 _OUTSIDE = frozenset((
     "random_walk", "RW", "graphlet_sampling", "GR", "subgraph_matching", "SM", "multiscale_laplacian", "ML",
-    "lovasz_theta", "LOVT", "svm_theta", "SVMT", "neighborhood_subgraph_pairwise_distance",
-    "NSPD", "odd_sth", "ODD"))
+    "lovasz_theta", "LOVT", "svm_theta", "SVMT", "odd_sth", "ODD"))
 
 
 def _propagation(params):
@@ -61,6 +62,8 @@ for _names, _framework, _build in (
         (("shortest_path", "SP"), False, _shortest_path),
         (("graph_hopper", "GH"), False, lambda p: (GraphHopper, p)),
         (("neighborhood_hash", "NH"), False, lambda p: (NeighborhoodHash, p)),
+        (("neighborhood_subgraph_pairwise_distance", "NSPD"), False,
+         lambda p: (NeighborhoodSubgraphPairwiseDistance, p)),
         (("propagation", "PR"), False, _propagation),
         (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),

@@ -27,7 +27,7 @@ from sklearn.utils import check_random_state
 from sklearn.utils.validation import check_is_fitted
 
 from . import _lib
-from .packing import Block, Graph, label_ids, pack
+from .packing import Block, Graph, adjacency_and_order, label_ids, pack
 
 
 class Fitted:
@@ -2749,3 +2749,191 @@ class HadamardCode(Kernel):
             eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
             eng.hc_features(self.n_iter, width, skip=data.skip)
             return eng.hc_vectors(level, block.n_vertices, width)
+
+
+# ------------------------------------------------------------------------------
+_NSPD_ELEMENT_MSG = ("each element of X must have either a graph with labels for node and edge or 3 elements "
+                     "consisting of a graph type object, labels for vertices and labels for edges.")
+
+
+def _nspd_graph(g, node_labels, edge_labels):
+    """One graph as the reference sees it after change_format("adjacency") then ("dictionary") (graph.py:912-1053):
+    the spelling is read by packing.classify (graph.py's is_adjacency / is_edge_dictionary), the vertices are the
+    indices 0 .. n-1 of an adjacency matrix or of the sorted symbols of an edge dictionary, and an edge survives when
+    its adjacency entry is > 0.  Missing vertex or edge labels raise get_labels' ValueError (graph.py:750-770).
+    Returns (n, sorted (i, j) edge list, vertex label strings, edge label strings)."""
+    if not node_labels:
+        raise ValueError("Graph does not have any labels for vertices.")
+    if not edge_labels:
+        raise ValueError("Graph does not have any labels for edges.")
+    A, order = adjacency_and_order(g)
+    order = list(order)
+    ii, jj = np.nonzero(A > 0)
+    edges = sorted(zip(ii.tolist(), jj.tolist()))
+    vl = [str(node_labels[s]) for s in order]
+    el = [str(edge_labels[(order[i], order[j])]) for i, j in edges]
+    return len(order), edges, vl, el
+
+
+class _NspdTokens:
+    """str(delta) + "," + str(label) for every delta <= d and label string, ranked by Python's string order, with
+    UTF-8 bytes and code-point lengths; the same for the edge label strings."""
+
+    def __init__(self, d, labels, elabels):
+        self.n_labels = len(labels)
+        toks = [str(t) + "," + s for t in range(d + 1) for s in labels]
+        uniq = sorted(set(toks))
+        rank = {s: i for i, s in enumerate(uniq)}
+        self.tok_rank = np.array([rank[s] for s in toks] or [0], dtype=np.int32)  # padded: never a null pointer
+        self.rank_off, self.rank_bytes, self.rank_cp = self._strings(uniq)
+        self.el_off, self.el_bytes, self.el_cp = self._strings(elabels)
+
+        self.n_ranks = len(uniq)
+        self.n_elabels = len(elabels)
+
+    @staticmethod
+    def _strings(strs):
+        """(offsets [n + 1], UTF-8 bytes, code points [n]); the byte and code-point arrays are padded by one entry so
+        that no pointer is null when n = 0 (the counts passed on are n_ranks / n_elabels, never the padded lengths)."""
+        bs = [s.encode("utf-8") for s in strs]
+        off = np.zeros(len(bs) + 1, dtype=np.int64)
+        off[1:] = np.cumsum([len(b) for b in bs]) if bs else []
+        data = np.frombuffer(b"".join(bs) + b"\0", dtype=np.uint8).copy()
+        return off, data, np.array([len(s) for s in strs] + [0], dtype=np.int32)
+
+
+class NeighborhoodSubgraphPairwiseDistance(Kernel):
+    """Neighborhood subgraph pairwise distance kernel (neighborhood_subgraph_pairwise_distance.py; Costa & De Grave
+    2010).  For every radius rho <= r and distance delta <= d, the pairs of vertices at distance delta are counted by
+    the pair of hashes of their radius-rho neighbourhood subgraphs; K is the sum over the levels (rho, delta) of the
+    cosine-normalised level Grams.  The BFS levels, the hashes (CPython's set order of the sub-edge sets emulated on
+    the device, the APHash of each encoding streamed from sorted token ranks), the per-level columns, the exact
+    integer Gram of every level and the reference's fp64 fold run on the device; K equals the reference's bit for
+    bit.
+
+    As in the reference, the neighbourhood of level l has BFS radius 2^(l - 1) (produce_neighborhoods unites the
+    level-l balls of the level-l ball), `diagonal()` is the number of levels and the vertices are the indices of the
+    sorted symbols.  Deviations: (r + 1)(d + 1) > 64 levels raise NotImplementedError, as do a datasets.read_tu
+    block (it carries no edge labels) and r > 0 with a graph of 65 535 or more vertices."""
+
+    _graph_format = "dictionary"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, r=3, d=4):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.r = r
+        self.d = d
+        self._initialized.update({"r": False, "d": False})
+
+    def initialize(self):
+        if not self._initialized["n_jobs"]:
+            if self.n_jobs is not None:
+                warnings.warn("no implemented parallelization for NeighborhoodSubgraphPairwiseDistance")
+            self._initialized["n_jobs"] = True
+        if not self._initialized["r"]:
+            if type(self.r) is not int or self.r < 0:
+                raise ValueError("r must be a positive integer")
+            self._initialized["r"] = True
+        if not self._initialized["d"]:
+            if type(self.d) is not int or self.d < 0:
+                raise ValueError("d must be a positive integer")
+            self._initialized["d"] = True
+        if (self.r + 1) * (self.d + 1) > 64:
+            raise NotImplementedError("NeighborhoodSubgraphPairwiseDistance: at most (r + 1)(d + 1) = 64 levels are "
+                                      "supported")
+
+    def parse_input(self, X):
+        """The graphs of X as (n, edges, vertex label strings, edge label strings), with the reference's element
+        checks."""
+        if isinstance(X, Block):
+            raise NotImplementedError("packed blocks carry no edge-label entries; pass the list of graphs")
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()  # labels it lacks are {}: _nspd_graph raises get_labels' error
+            elif isinstance(x, Iterable):
+                x = list(x)
+                if len(x) == 0:
+                    warnings.warn("Ignoring empty element on index: " + str(idx))
+                    continue
+                if len(x) != 3:
+                    raise TypeError(_NSPD_ELEMENT_MSG)
+            else:
+                raise TypeError(_NSPD_ELEMENT_MSG)
+            out.append(_nspd_graph(x[0], x[1], x[2]))
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    def fit(self, X, y=None):
+        self._method_calling = 1
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        self.X = self.parse_input(X)
+        for a in ("_X_diag", "_Y", "_ngy"):
+            self.__dict__.pop(a, None)
+        self._ngx = len(self.X)
+        return self
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        K, xd, _ = self._nspd_run(self.X, len(self.X))
+        self._X_diag = xd
+        return K
+
+    def transform(self, X, y=None):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("transform input cannot be None")
+        Y = self.parse_input(X)
+        K, xd, yd = self._nspd_run(self.X + Y, len(self.X))
+        self._X_diag, self._Y_diag = xd, yd
+        self._ngy = len(Y)
+        self._Y = True
+        self._is_transformed = True
+        return K
+
+    def diagonal(self):
+        """The number of levels of each side (the reference's constant self similarity)."""
+        check_is_fitted(self, ["X"])
+        if getattr(self, "_X_diag", None) is None:
+            self._nspd_run(self.X, len(self.X), want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
+
+    def _pack(self, graphs):
+        gp, rp, ci, lab, el, sh = [0], [0], [], [], [], []
+        lstr, estr = {}, {}
+        for n, edges, vl, elab in graphs:
+            v0 = gp[-1]
+            deg = np.zeros(n, dtype=np.int64)
+            for (i, j), s in zip(edges, elab):
+                deg[i] += 1
+                ci.append(v0 + j)
+                el.append(estr.setdefault(s, len(estr)))
+            rp.extend((rp[-1] + np.cumsum(deg)).tolist())
+            lab.extend(lstr.setdefault(s, len(lstr)) for s in vl)
+            sh.extend(hash(i) for i in range(n))
+            gp.append(v0 + n)
+        tokens = _NspdTokens(self.d, list(lstr), list(estr))
+        return (np.array(gp), np.array(rp), np.array(ci, dtype=np.int64), np.array(lab, dtype=np.int64),
+                np.array(el, dtype=np.int64), np.array(sh, dtype=np.int64), tokens)
+
+    def _nspd_run(self, graphs, n_fit, want_matrix=True, device_ptr=None, row_range=None, simt=False):
+        gp, rp, ci, lab, el, sh, tokens = self._pack(graphs)
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(gp, rp, ci, lab, None, None)
+            self.stats_, self.delta_mask_ = eng.nspd_features(self.r, self.d, sh, el, tokens)
+            K, xd, yd = eng.gram(len(graphs), n_fit=n_fit, normalize=self.normalize, stats=self.stats_,
+                                 out=None if want_matrix else False, device_ptr=device_ptr, row_range=row_range,
+                                 simt=simt)
+        self._X_diag = xd
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd

@@ -107,7 +107,8 @@ typedef struct gk_stats {
                                 GraphHopper node-pair kernels: 6 = fused fp64 CUDA-core node-pair Gram,
                                 NeighborhoodHash: 7 = one exact integer Gram per level + the fp64 combine,
                                 random walk: 8 = conjugate gradients, 9 = spectral pair sum, 10 = power series,
-                                PyramidMatch: 11 = one exact integer Gram per level + the fp64 combine */
+                                PyramidMatch: 11 = one exact integer Gram per level + the fp64 combine,
+                                NeighborhoodSubgraphPairwiseDistance: 12 = one exact integer Gram per level + the fp64 fold */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -201,6 +202,30 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
                    const uint8_t* label_valid, int64_t n_labels, int32_t flags, gk_stats* stats);
 /* codes of level `level` (0 .. R-1) of every packed vertex after gk_nh_features: out[V] u64, valid[V] (may be NULL) */
 int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid);
+
+/* NeighborhoodSubgraphPairwiseDistance (neighborhood_subgraph_pairwise_distance.py).  The packed block lists every
+ * graph's vertices in the reference's sorted-symbol order with ascending CSR columns (directed edges kept); labels
+ * are vertex label ids.  sym_hash[V] = hash() of every vertex symbol, edge_label[E] = edge label id of every CSR
+ * edge.  Tokens: tok_rank[(d + 1) * n_labels] is the rank of str(delta) + "," + str(label) in Python's string order;
+ * rank_off[n_ranks + 1] / rank_bytes / rank_cp give every rank's UTF-8 bytes and code points, el_off[n_elabels + 1] /
+ * el_bytes / el_cp those of str(edge label).  Builds the hashes H[rho][v] (BFS levels, CPython set order of the
+ * sub-edge sets, APHash over the first code-point-count bytes of the encoding) and one (graph, column) count table
+ * per level (delta, rho), levels numbered delta * (r + 1) + rho.  delta_mask[N] (may be NULL) receives the distances
+ * every graph has pairs at.  (r + 1)(d + 1) > 64 is GK_ERR_UNSUPPORTED.  stats: level_dims = columns per level,
+ * ms_hash (BFS levels + hashes) / ms_columns.  gk_gram (gram_path 12) then returns the reference's fp64 sum
+ * of cosine-normalised level Grams over the fitted levels (square) or the levels both sides have (transform);
+ * GK_NORMALIZE divides by the number of fitted levels, or sqrt(levels of Y x levels of X); xdiag / ydiag are those
+ * level counts.  fp64 only, host or GK_OUT_DEVICE output, n_fit and row ranges; GK_DIST and row maps are
+ * GK_ERR_UNSUPPORTED.  flags must be 0. */
+int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash, const int32_t* edge_label,
+                     const int32_t* tok_rank, int64_t n_labels, const int64_t* rank_off, const uint8_t* rank_bytes,
+                     const int32_t* rank_cp, int32_t n_ranks, const int64_t* el_off, const uint8_t* el_bytes,
+                     const int32_t* el_cp, int32_t n_elabels, uint64_t* delta_mask, int32_t flags, gk_stats* stats);
+/* H[radius][v] of every packed vertex after gk_nspd_features: out[V] */
+int gk_nspd_hashes(gk_handle* h, int32_t radius, uint32_t* out);
+/* host only: the iteration order of CPython's set after inserting the n distinct pairs (h0[k], h1[k]) (element
+ * hashes) in order k = 0 .. n-1 */
+int gk_selftest_nspd_set_order(int64_t n, const int64_t* h0, const int64_t* h1, int64_t* order);
 
 /* RandomWalk / RandomWalkLabeled (random_walk.py:28-541), one graph pair per CTA in fp64.  The packed CSR gives the
  * structure (gk_pack_csr without weights; with labels for GK_RW_LABELED), `values[E]` the adjacency entries of its
