@@ -89,6 +89,7 @@ _SYMBOLS = {
     "gk_hc_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_hc_vectors": (C.c_int, [_P, C.c_int32, _P]),
     "gk_selftest_hc_collision": (C.c_int, [_P]),
+    "gk_selftest_wl_collision": (C.c_int, [_P, C.c_int32, C.c_int32]),
     "gk_nspd_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int32, _P, _P, _P,
                                    C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_nspd_hashes": (C.c_int, [_P, C.c_int32, _P]),
@@ -417,6 +418,13 @@ class Engine:
         """Tests only: the next hc_features starts with a degenerate hash, so it must detect collisions and retry."""
         with self._lock:
             self._check(self.lib.gk_selftest_hc_collision(self.h))
+
+    def selftest_wl_collision(self, attempts, from_level=1):
+        """Tests only: the next `attempts` WL relabel attempts (each wl_features retry, the asynchronous pass of wl_gram)
+        hash the levels >= from_level by (own label, degree) alone, so only the signature verification separates
+        classes and every such attempt must detect a collision and be repeated."""
+        with self._lock:
+            self._check(self.lib.gk_selftest_wl_collision(self.h, int(attempts), int(from_level)))
 
     def nspd_features(self, r, d, sym_hash, edge_label, tokens):
         """NeighborhoodSubgraphPairwiseDistance hashes and per-level count tables (gk_nspd_features).  `tokens` is

@@ -1,6 +1,7 @@
 // C-ABI of the grakel_b200 engine (see include/grakel_b200.h for the contract and
 // the reference file:line each entry point replaces).  sm_90a (H100) only.
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <condition_variable>
@@ -497,10 +498,10 @@ int gk_pack_csr(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const 
 }  // extern "C"
 
 template <int G>
-static void launch_sig_small(gk_handle* h, const int* lab_in, unsigned long long seed) {
+static void launch_sig_small(gk_handle* h, const int* lab_in, unsigned long long seed, int degen) {
   const long long threads = (long long)h->V * G;
   wl_sig_small<G><<<cdiv(threads, 256), 256, 0, h->stream>>>(
-      (int)h->V, h->row_ptr.as<int>(), h->col_idx.as<int>(), lab_in, h->sig_nbr.as<int>(), seed,
+      (int)h->V, h->row_ptr.as<int>(), h->col_idx.as<int>(), lab_in, h->sig_nbr.as<int>(), seed, degen,
       h->ht_keys.as<unsigned long long>(), h->ht_rep.as<int>(), (unsigned)(h->ht_cap - 1), h->slot_of.as<int>());
 }
 
@@ -540,6 +541,14 @@ static int init_scalars(gk_handle* h, int n_labels0) {
   // the pinned struct is reused for read-back; make sure the upload has consumed it
   GK_CUDA(cudaStreamSynchronize(h->stream));
   return GK_OK;
+}
+
+// gk_selftest_wl_collision: the level from which this relabel attempt hashes (own label, degree) only, INT_MAX for a
+// normal attempt.  Every attempt (each iteration of gk_wl_features' retry loop, the asynchronous pass) takes one.
+static int wl_take_degen(gk_handle* h) {
+  if (h->wl_degen_attempts <= 0) return INT_MAX;
+  --h->wl_degen_attempts;
+  return h->wl_degen_from;
 }
 
 // What gk_wl_features decides and allocates before its first launch (shared with the asynchronous pass, gk_wl_gram)
@@ -635,7 +644,8 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
 }
 
 // prepare + wl_fused2 on the handle's stream; no synchronisation
-static int wl_launch_v2(gk_handle* h, const WlPlan& pl, unsigned long long seed, const FeatStats& fst, bool prof) {
+static int wl_launch_v2(gk_handle* h, const WlPlan& pl, unsigned long long seed, int degen_from, const FeatStats& fst,
+                        bool prof) {
   const int64_t V = h->V, E = h->E;
   const int L = pl.L, G = pl.G, n_tiles = pl.n_tiles;
   DevScalars* sc = h->scalars.as<DevScalars>();
@@ -679,7 +689,7 @@ static int wl_launch_v2(gk_handle* h, const WlPlan& pl, unsigned long long seed,
       fp.table = h->ht_keys.as<unsigned long long>();
       fp.ht_mask = (unsigned)(h->ht_cap - 1);
       fp.coo_keys = h->ft_keys.as<unsigned long long>(); fp.coo_cnt = h->ft_cnt.as<unsigned>();
-      fp.seed = seed; fp.st = fst; fp.sc = sc;
+      fp.seed = seed; fp.degen_from = degen_from; fp.st = fst; fp.sc = sc;
       fp.diag_frozen = h->diag_frozen.as<unsigned long long>();
       if (prof) {
         GK_TRY(h->K_stage.ensure((size_t)G * L * 128));
@@ -725,6 +735,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
       return fail(GK_ERR_STATE, "gk_wl_features: repeated hash collisions (level mask 0x" +
                                     [&] { char b[16]; snprintf(b, sizeof(b), "%x", h->h_scalars.as<DevScalars>()->collision); return std::string(b); }() + ")");
     const unsigned long long seed = mix64(0x5851F42D4C957F2DULL + 0x9E3779B97F4A7C15ULL * (unsigned long long)retries);
+    const int degen_from = wl_take_degen(h);
     const char* e_v1 = getenv("GRAKEL_B200_WL_V1");
     const bool wl_v2 = fused && !(e_v1 && atoi(e_v1) != 0);
     FeatStats fst;
@@ -734,7 +745,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
     used_v2 = wl_v2;
     if (wl_v2) {
       const bool prof = getenv("GRAKEL_B200_PROF") != nullptr;
-      GK_TRY(wl_launch_v2(h, pl, seed, fst, prof));
+      GK_TRY(wl_launch_v2(h, pl, seed, degen_from, fst, prof));
       h->wl_sparse_ids = L > 1;
       GK_CUDA(cudaEventRecord(h->tev[3], h->stream));  // end of the feature stage
       if (!prof) {
@@ -813,7 +824,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
       fp.table = h->ht_keys.as<unsigned long long>();
       fp.ht_mask = (unsigned)(h->ht_cap - 1);
       fp.coo_keys = h->ft_keys.as<unsigned long long>(); fp.coo_cnt = h->ft_cnt.as<unsigned>();
-      fp.seed = seed; fp.st = fst; fp.sc = sc;
+      fp.seed = seed; fp.degen_from = degen_from; fp.st = fst; fp.sc = sc;
       const bool prof = getenv("GRAKEL_B200_PROF") != nullptr;
       if (prof) {
         GK_TRY(h->K_stage.ensure((size_t)G * L * 128));
@@ -865,22 +876,23 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
     for (int lv = 1; lv < L; ++lv) {
       const int* lab_in = labels_all + (size_t)(lv - 1) * V;
       int* lab_out = labels_all + (size_t)lv * V;
+      const int degen = lv >= degen_from ? 1 : 0;
       GK_CUDA(cudaMemsetAsync(h->ht_keys.p, 0xFF, h->ht_cap * 8, h->stream));
       GK_CUDA(cudaMemsetAsync(h->ht_rep.p, 0x7F, h->ht_cap * 4, h->stream));
       if (h->group_width <= 8) {
         wl_sig_thread8<<<nb, 256, 0, h->stream>>>((int)V, h->row_ptr.as<int>(), h->col_idx.as<int>(), lab_in,
-                                                  h->sig_nbr.as<int>(), seed, h->ht_keys.as<unsigned long long>(),
+                                                  h->sig_nbr.as<int>(), seed, degen, h->ht_keys.as<unsigned long long>(),
                                                   h->ht_rep.as<int>(), (unsigned)(h->ht_cap - 1), h->slot_of.as<int>());
       } else if (h->group_width == 16) {
-        launch_sig_small<16>(h, lab_in, seed);
+        launch_sig_small<16>(h, lab_in, seed, degen);
       } else {
-        launch_sig_small<32>(h, lab_in, seed);
+        launch_sig_small<32>(h, lab_in, seed, degen);
       }
       LAUNCH_CHECK(h);
       if (h->n_large) {
         wl_sig_large<<<cdiv(h->n_large * 32, 256), 256, 0, h->stream>>>(
             (int)h->n_large, h->large_list.as<int>(), h->row_ptr.as<int>(), h->col_idx.as<int>(), lab_in,
-            h->sig_nbr.as<int>(), seed, h->ht_keys.as<unsigned long long>(), h->ht_rep.as<int>(),
+            h->sig_nbr.as<int>(), seed, degen, h->ht_keys.as<unsigned long long>(), h->ht_rep.as<int>(),
             (unsigned)(h->ht_cap - 1), h->slot_of.as<int>());
         LAUNCH_CHECK(h);
       }
@@ -1494,6 +1506,14 @@ int gk_hc_vectors(gk_handle* h, int32_t level, int64_t* out) {
 int gk_selftest_hc_collision(gk_handle* h) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
   h->hc_degenerate_once = true;
+  return GK_OK;
+}
+
+int gk_selftest_wl_collision(gk_handle* h, int32_t attempts, int32_t from_level) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (attempts < 0 || from_level < 1) return fail(GK_ERR_ARG, "gk_selftest_wl_collision: bad arguments");
+  h->wl_degen_attempts = attempts;
+  h->wl_degen_from = from_level;
   return GK_OK;
 }
 
@@ -4164,7 +4184,7 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   GK_CUDA(cudaMemsetAsync(cs, 0, sizeof(ColStats), h->stream));
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   const unsigned long long seed = mix64(0x5851F42D4C957F2DULL);
-  GK_TRY(wl_launch_v2(h, pl, seed, fst, false));
+  GK_TRY(wl_launch_v2(h, pl, seed, wl_take_degen(h), fst, false));
   h->wl_sparse_ids = L > 1;
   GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
   // ---- the panel (full row pitch) is zeroed on the side stream while the column statistics run (the WL kernel itself

@@ -238,6 +238,9 @@ struct gk_handle {
   int hc_W = 0, hc_levels = 0;
   bool hc_has_skip = false;
   bool hc_degenerate_once = false;  // gk_selftest_hc_collision: the next pass starts with all z_c = 0
+  // gk_selftest_wl_collision: the next wl_degen_attempts WL relabel attempts hash (own label, degree) only at the levels
+  // >= wl_degen_from
+  int wl_degen_attempts = 0, wl_degen_from = 1;
 
   // ---- NeighborhoodSubgraphPairwiseDistance (FK_NSPD): BFS level matrices [sum n_g^2] u8 and their queue, hashes
   // [(r + 1) V] u32, the host tables (aux), the hashing slots, the pairs of every distance, the per-level (graph,

@@ -55,10 +55,12 @@ __device__ __forceinline__ unsigned ht_insert(unsigned long long* keys, int* rep
 // K1a: G lanes per vertex, degree <= G.  Coalesced read of the neighbour list,
 // label gather (cache-resident: a graph's vertices are contiguous), bitonic sort
 // in registers via shuffles, positional 64-bit hash, table insert.
+// degen != 0 (tests, gk_selftest_wl_collision): the key leaves the neighbour terms out, so vertices with equal own label
+// and degree share a slot and only wl_resolve's verification can separate their classes.
 template <int G>
 __global__ void __launch_bounds__(256)
 wl_sig_small(int V, const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
-             const int* __restrict__ lab_in, int* __restrict__ sig_nbr, unsigned long long seed,
+             const int* __restrict__ lab_in, int* __restrict__ sig_nbr, unsigned long long seed, int degen,
              unsigned long long* ht_keys, int* ht_rep, unsigned ht_mask, int* __restrict__ slot_of) {
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
   const int v = tid / G;
@@ -90,7 +92,7 @@ wl_sig_small(int V, const int* __restrict__ row_ptr, const int* __restrict__ col
 #pragma unroll
   for (int j = G >> 1; j > 0; j >>= 1) t += __shfl_xor_sync(0xffffffffu, t, j);
   if (active && lane == 0) {
-    unsigned long long key = sig_final(t, lab_in[v], deg, seed);
+    unsigned long long key = sig_final(degen ? 0ULL : t, lab_in[v], deg, seed);
     slot_of[v] = (int)ht_insert(ht_keys, ht_rep, ht_mask, key, v);
   }
 }
@@ -103,7 +105,7 @@ wl_sig_small(int V, const int* __restrict__ row_ptr, const int* __restrict__ col
 #define GK_CSWAP(a, b) { const int _lo = min(a, b); const int _hi = max(a, b); a = _lo; b = _hi; }
 __global__ void __launch_bounds__(256)
 wl_sig_thread8(int V, const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
-               const int* __restrict__ lab_in, int* __restrict__ sig_nbr, unsigned long long seed,
+               const int* __restrict__ lab_in, int* __restrict__ sig_nbr, unsigned long long seed, int degen,
                unsigned long long* ht_keys, int* ht_rep, unsigned ht_mask, int* __restrict__ slot_of) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= V) return;
@@ -140,7 +142,7 @@ wl_sig_thread8(int V, const int* __restrict__ row_ptr, const int* __restrict__ c
       t += sig_term(xs[i], i, seed);
     }
   }
-  const unsigned long long key = sig_final(t, own, deg, seed);
+  const unsigned long long key = sig_final(degen ? 0ULL : t, own, deg, seed);
   slot_of[v] = (int)ht_insert(ht_keys, ht_rep, ht_mask, key, v);
 }
 
@@ -150,7 +152,7 @@ wl_sig_thread8(int V, const int* __restrict__ row_ptr, const int* __restrict__ c
 __global__ void __launch_bounds__(256)
 wl_sig_large(int n_large, const int* __restrict__ large_list, const int* __restrict__ row_ptr,
              const int* __restrict__ col_idx, const int* __restrict__ lab_in, int* sig_nbr,
-             unsigned long long seed, unsigned long long* ht_keys, int* ht_rep, unsigned ht_mask,
+             unsigned long long seed, int degen, unsigned long long* ht_keys, int* ht_rep, unsigned ht_mask,
              int* __restrict__ slot_of) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -206,7 +208,7 @@ wl_sig_large(int n_large, const int* __restrict__ large_list, const int* __restr
 #pragma unroll
   for (int j = 16; j > 0; j >>= 1) t += __shfl_xor_sync(0xffffffffu, t, j);
   if (lane == 0) {
-    unsigned long long key = sig_final(t, lab_in[v], deg, seed);
+    unsigned long long key = sig_final(degen ? 0ULL : t, lab_in[v], deg, seed);
     slot_of[v] = (int)ht_insert(ht_keys, ht_rep, ht_mask, key, v);
   }
 }

@@ -59,6 +59,7 @@ struct WlFusedParams {
   unsigned* coo_cnt;
   unsigned* barrier;  // zeroed by the host before the launch
   unsigned long long seed;
+  int degen_from;     // levels >= degen_from hash (own label, degree) only (gk_selftest_wl_collision); INT_MAX = off
   FeatStats st;
   DevScalars* sc;
   long long* prof;  // optional [grid][L][16] globaltimer stamps (GRAKEL_B200_PROF), else NULL
@@ -342,7 +343,8 @@ wl_fused_kernel(WlFusedParams p) {
             wlf_seq_step(ha, hc, xs[j]);
           }
         }
-        key_s[i] = wlf_finish(ha, hc, lab_s[i], deg, p.seed);
+        const bool dg = lv >= p.degen_from;  // tests: neighbour terms left out, only the verification separates classes
+        key_s[i] = wlf_finish(dg ? 0x243F6A88u : ha, dg ? 0x85A308D3u : hc, lab_s[i], deg, p.seed);
       }
       if (p.prof) { __syncthreads(); WLF_STAMP(lv, 9); }
       // [A2] higher degrees: one warp per vertex.  <= 32: one label per lane, bitonic network on
@@ -407,7 +409,10 @@ wl_fused_kernel(WlFusedParams p) {
             ha += __shfl_xor_sync(0xffffffffu, ha, s);
             hc += __shfl_xor_sync(0xffffffffu, hc, s);
           }
-          if (lane == 0) key_s[i] = wlf_finish(ha, hc, lab_s[i], deg, p.seed);
+          if (lane == 0) {
+            const bool dg = lv >= p.degen_from;
+            key_s[i] = wlf_finish(dg ? 0u : ha, dg ? 0u : hc, lab_s[i], deg, p.seed);
+          }
         }
       }
       __syncthreads();

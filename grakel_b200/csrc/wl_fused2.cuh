@@ -56,6 +56,7 @@ struct WlFused2Params {
   unsigned* coo_cnt;
   unsigned* barrier;  // zeroed by the host before the launch
   unsigned long long seed;
+  int degen_from;     // levels >= degen_from hash (own label, degree) only (gk_selftest_wl_collision); INT_MAX = off
   FeatStats st;
   unsigned long long* diag_frozen;  // [N] zeroed by the host: the frozen vertices' share of st.diag (WL-OA re-adds it)
   DevScalars* sc;     // level_dims[1..] zeroed by the host, level_base[0], [1] set
@@ -426,7 +427,8 @@ wl_fused2_kernel(WlFused2Params p) {
             wlf_seq_step(ha, hc, xs[j]);
           }
         }
-        key_s[i] = wlf_finish(ha, hc, lab_s[i], deg, p.seed);
+        const bool dg = lv >= p.degen_from;  // tests: neighbour terms left out, only the verification separates classes
+        key_s[i] = wlf_finish(dg ? 0x243F6A88u : ha, dg ? 0x85A308D3u : hc, lab_s[i], deg, p.seed);
       }
       // [A2] higher degrees: one warp per vertex (shuffle bitonic <= 32, in-segment bitonic above)
       for (int i0 = wid * 32; i0 < nv; i0 += WLF_THREADS) {
@@ -487,7 +489,10 @@ wl_fused2_kernel(WlFused2Params p) {
             ha += __shfl_xor_sync(0xffffffffu, ha, s);
             hc += __shfl_xor_sync(0xffffffffu, hc, s);
           }
-          if (lane == 0) key_s[i] = wlf_finish(ha, hc, lab_s[i], deg, p.seed);
+          if (lane == 0) {
+            const bool dg = lv >= p.degen_from;
+            key_s[i] = wlf_finish(dg ? 0u : ha, dg ? 0u : hc, lab_s[i], deg, p.seed);
+          }
         }
       }
       __syncthreads();

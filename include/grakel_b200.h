@@ -325,11 +325,17 @@ int gk_pm_cells(gk_handle* h, int32_t set, int32_t level, int64_t* out);
  * gk_hc_vectors recomputes the vectors of one level of the last gk_hc_features call on the packed block:
  * out[V * W], vertex v's vector at v * W (zeros for a skipped vertex at levels >= 1).
  * gk_selftest_hc_collision (tests only): the next gk_hc_features starts with a degenerate hash (every z_c = 0), so its
- * verification must see collisions and its retry must give the right classes. */
+ * verification must see collisions and its retry must give the right classes.
+ * gk_selftest_wl_collision (tests only): the next `attempts` WL relabel attempts on the handle -- each iteration of
+ * gk_wl_features' retry loop, and the asynchronous pass of gk_wl_gram, counts as one -- hash every vertex of the levels
+ * >= from_level by its own label and degree only, on every relabel route, so vertices with equal (label, degree) and
+ * different neighbour labels share a hash slot and only the signature verification can tell their classes apart.
+ * attempts > 8 exhausts gk_wl_features' retries. */
 #define GK_HC_SP 8
 int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* skip, int32_t flags, gk_stats* stats);
 int gk_hc_vectors(gk_handle* h, int32_t level, int64_t* out);
 int gk_selftest_hc_collision(gk_handle* h);
+int gk_selftest_wl_collision(gk_handle* h, int32_t attempts, int32_t from_level);
 
 /* Gram matrix of the current feature block.
  *   n_fit == n_graphs : K is [n_graphs x n_graphs]                      (fit_transform)
