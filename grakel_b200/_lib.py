@@ -28,6 +28,7 @@ GK_RW_LABELED = 1
 GK_PK_ATTR, GK_PK_SQRT, GK_PK_STORE_F32, GK_PK_STORE_INT, GK_PK_NEW_LABELS = 1, 2, 4, 8, 16
 GK_PM_LABELS, GK_PM_WL_LABELS = 1, 2
 GK_HC_SP = 8
+GK_SM_KV_NONE, GK_SM_KV_DIRAC, GK_SM_KE_NONE, GK_SM_KE_DIRAC = 1, 2, 4, 8
 
 
 class GkStats(C.Structure):
@@ -80,6 +81,8 @@ _SYMBOLS = {
     "gk_rw_features": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_double, _P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_rw_iterations": (C.c_int, [_P, _P]),
+    "gk_sm_features": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_sm_counts": (C.c_int, [_P, C.c_int64, C.c_int64, _P]),
     "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
@@ -354,6 +357,29 @@ class Engine:
                                                 0 if cf is None else len(cf), _ptr(vals), _ptr(trp), _ptr(tci), _ptr(tv),
                                                 _ptr(qq), _ptr(ww), GK_RW_LABELED if labeled else 0, C.byref(st)))
         return st
+
+    def sm_features(self, k, lambdas, vtable=None, etable=None, edge_label=None, flags=0):
+        """SubgraphMatching records, weight tables and lambdas of the packed block (gk_sm_features); the next gram()
+        runs it pair by pair.  vtable / etable: square fp64 tables over the label ids, or None with the matching
+        GK_SM_* flag; edge_label[E]: the edge label ids of the packed edges."""
+        lam = np.ascontiguousarray(lambdas, dtype=np.float64).ravel()
+        vt = None if vtable is None else np.ascontiguousarray(vtable, dtype=np.float64)
+        et = None if etable is None else np.ascontiguousarray(etable, dtype=np.float64)
+        el = None if edge_label is None else _i32(edge_label)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_sm_features(self.h, int(k), _ptr(lam), _ptr(vt), 0 if vt is None else vt.shape[0],
+                                                _ptr(et), 0 if et is None else et.shape[0], _ptr(el), int(flags),
+                                                C.byref(st)))
+        self.sm_k = int(k)
+        return st
+
+    def sm_counts(self, n_fit, row):
+        """tv [n_fit, k + 1] of the pairs of row `row` of the gram() request with this n_fit."""
+        out = np.empty((int(n_fit), self.sm_k + 1), dtype=np.float64)
+        with self._lock:
+            self._check(self.lib.gk_sm_counts(self.h, int(n_fit), int(row), _ptr(out)))
+        return out
 
     def pk_features(self, t_max, w, u, b, dim, dim_orig, n_fit, t_values, p0=None, flags=0):
         """Propagation bins of t_max levels and their (graph, column) counts (gk_pk_features).  u: [t_max, dim],

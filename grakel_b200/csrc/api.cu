@@ -33,6 +33,7 @@
 #include "pyramid_match.cuh"
 #include "hadamard_code.cuh"
 #include "nspd.cuh"
+#include "subgraph_matching.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -341,7 +342,8 @@ int gk_destroy(gk_handle* h) {
                         &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt,
                         &h->pm_U, &h->pm_ncols, &h->pm_skip, &h->hc_S, &h->hc_z, &h->hc_skip,
                         &h->nspd_lvl, &h->nspd_q, &h->nspd_H, &h->nspd_aux, &h->nspd_ws, &h->nspd_pairs, &h->nspd_blk,
-                        &h->nspd_tab, &h->nspd_keys, &h->nspd_C};
+                        &h->nspd_tab, &h->nspd_keys, &h->nspd_C,
+                        &h->sm_rec, &h->sm_off, &h->sm_el, &h->sm_vtab, &h->sm_etab, &h->sm_lam, &h->sm_stack, &h->sm_ctl};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1729,6 +1731,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_PK     */ {"Propagation", true, true, false, false},
     /* FK_PM     */ {"PyramidMatch", false, true, false, false},
     /* FK_NSPD   */ {"NeighborhoodSubgraphPairwiseDistance", false, true, false, false},
+    /* FK_SM     */ {"SubgraphMatching", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -3098,6 +3101,219 @@ static int gram_rw(gk_handle* h, const GramReq& q, gk_stats* stats) {
 }
 
 // ---------------------------------------------------------------------------
+// SubgraphMatching (subgraph_matching.cuh).  gk_sm_features builds every graph's record and uploads the weight
+// tables and lambdas; gk_gram (gram_sm) runs one warp per graph pair.
+static bool sm_integral(const double* t, int64_t n) {
+  for (int64_t i = 0; i < n; ++i)
+    if (t[i] != std::floor(t[i])) return false;
+  return true;
+}
+
+int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double* vtable, int32_t n_vlabels,
+                   const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sm_features: no graphs packed");
+  if (flags & ~(GK_SM_KV_NONE | GK_SM_KV_DIRAC | GK_SM_KE_NONE | GK_SM_KE_DIRAC))
+    return fail(GK_ERR_ARG, "gk_sm_features: unknown flags");
+  if ((flags & GK_SM_KV_NONE) && (flags & GK_SM_KV_DIRAC)) return fail(GK_ERR_ARG, "gk_sm_features: two vertex kernels");
+  if ((flags & GK_SM_KE_NONE) && (flags & GK_SM_KE_DIRAC)) return fail(GK_ERR_ARG, "gk_sm_features: two edge kernels");
+  if (k < 0 || !lambdas) return fail(GK_ERR_ARG, "gk_sm_features: k < 0 or no lambdas");
+  const int kv = (flags & GK_SM_KV_NONE) ? SM_W_NONE : (flags & GK_SM_KV_DIRAC) ? SM_W_DIRAC : SM_W_TABLE;
+  const int ke = (flags & GK_SM_KE_NONE) ? SM_W_NONE : (flags & GK_SM_KE_DIRAC) ? SM_W_DIRAC : SM_W_TABLE;
+  if (kv != SM_W_NONE && !h->has_labels) return fail(GK_ERR_ARG, "gk_sm_features: the vertex kernel needs packed labels");
+  if (ke != SM_W_NONE && h->E > 0 && !edge_label) return fail(GK_ERR_ARG, "gk_sm_features: the edge kernel needs edge labels");
+  const int64_t nvt = (int64_t)n_vlabels * n_vlabels, net = (int64_t)n_elabels * n_elabels;
+  if (kv == SM_W_TABLE && (!vtable || n_vlabels < 1)) return fail(GK_ERR_ARG, "gk_sm_features: no vertex table");
+  if (ke == SM_W_TABLE && (!etable || n_elabels < 1)) return fail(GK_ERR_ARG, "gk_sm_features: no edge table");
+  if ((kv == SM_W_TABLE && nvt > SM_TAB_MAX) || (ke == SM_W_TABLE && net > SM_TAB_MAX))
+    return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: a weight table has more than 4096 entries (64 labels)");
+  for (int64_t i = 0; kv == SM_W_TABLE && i < nvt; ++i)
+    if (!std::isfinite(vtable[i])) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: non-finite vertex weight");
+  for (int64_t i = 0; ke == SM_W_TABLE && i < net; ++i)
+    if (!std::isfinite(etable[i])) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: non-finite edge weight");
+  const int n_tv = k + 1;
+  for (int i = 0; i < n_tv; ++i)
+    if (!std::isfinite(lambdas[i])) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: non-finite lambda");
+  if (n_tv > 15 && !sm_integral(lambdas, n_tv))
+    return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: real lambdas are folded in the reference's order for k + 1 <= 15 only");
+  // cliques of the product graph have at most min(n_x, n_y) vertices
+  const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
+  if (kk > SM_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: subgraphs of more than 32 vertices");
+  GK_CUDA(cudaSetDevice(h->dev));
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N;
+  const bool elab = ke != SM_W_NONE;
+  std::vector<long long> off(N + 1, 0);
+  for (int64_t g = 0; g < N; ++g) off[g + 1] = off[g] + sm_record_words(ex->graph_ptr[g + 1] - ex->graph_ptr[g], elab);
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  GK_TRY(h->sm_off.ensure((N + 1) * 8));
+  GK_TRY(h->sm_rec.ensure(std::max<long long>(off[N], 1) * 4));
+  GK_CUDA(cudaMemcpyAsync(h->sm_off.p, off.data(), (N + 1) * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_TRY(h->sm_el.ensure(std::max<int64_t>(h->E, 1) * 4));
+  GK_TRY(h->sm_ctl.ensure(16));
+  GK_CUDA(cudaMemsetAsync(h->sm_ctl.p, 0, 16, h->stream));
+  int* d_max_und = reinterpret_cast<int*>(h->sm_ctl.as<unsigned char>() + 12);
+  if (elab && h->E > 0) GK_CUDA(cudaMemcpyAsync(h->sm_el.p, edge_label, h->E * 4, cudaMemcpyHostToDevice, h->stream));
+  sm_build_records<<<(int)std::min<int64_t>(N, h->sm_count * 16), 256, 0, h->stream>>>(
+      h->graph_ptr.as<int>(), h->row_ptr.as<int>(), h->col_idx.as<int>(), kv != SM_W_NONE ? h->labels0.as<int>() : nullptr,
+      elab ? h->sm_el.as<int>() : nullptr, h->sm_off.as<long long>(), h->sm_rec.as<unsigned>(), (int)N, d_max_und);
+  LAUNCH_CHECK(h);
+  GK_TRY(h->sm_vtab.ensure(std::max<int64_t>(nvt, 1) * 8));
+  GK_TRY(h->sm_etab.ensure(std::max<int64_t>(net, 1) * 8));
+  GK_TRY(h->sm_lam.ensure((size_t)n_tv * 8));
+  if (kv == SM_W_TABLE) GK_CUDA(cudaMemcpyAsync(h->sm_vtab.p, vtable, nvt * 8, cudaMemcpyHostToDevice, h->stream));
+  if (ke == SM_W_TABLE) GK_CUDA(cudaMemcpyAsync(h->sm_etab.p, etable, net * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->sm_lam.p, lambdas, (size_t)n_tv * 8, cudaMemcpyHostToDevice, h->stream));
+  int max_und = 0;
+  GK_CUDA(cudaMemcpyAsync(&max_und, d_max_und, 4, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffers may be reused once we return
+  h->sm_max_und = max_und;
+  h->sm_k = k; h->sm_kk = kk; h->sm_kv = kv; h->sm_ke = ke;
+  h->sm_n_vl = kv == SM_W_TABLE ? n_vlabels : 0;
+  h->sm_n_el = ke == SM_W_TABLE ? n_elabels : 0;
+  h->sm_exact = (kv != SM_W_TABLE || sm_integral(vtable, nvt)) && (ke != SM_W_TABLE || sm_integral(etable, net));
+  h->feature_kind = FK_SM;
+  h->features_ready = true; h->feat_serial++;
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->ms_h2d = ev_ms(h->tev[0], h->tev[1]);
+  }
+  return GK_OK;
+}
+
+// Launch sm_pairs over p.n_pairs pairs: a persistent grid, each warp with a stack slice sized for the deepest
+// extension sets of the block and, when the two records of the largest pair fit, a shared-memory staging area.
+static int sm_launch(gk_handle* h, SmParams p) {
+  if (p.n_pairs <= 0) return GK_OK;
+  const int nmax = std::max(h->max_graph_size, 1);
+  const long long nv = (long long)nmax * nmax;
+  // the extension set of S (|S| = d) lies in the c-neighbourhood of S: at most d D^2 vertices, D the largest number
+  // of distinct out- or in-neighbours of a vertex (counted by sm_build_records)
+  const long long D = h->sm_max_und;
+  long long cap = 1;
+  for (int d = 1; d < p.kk; ++d) cap += std::min(nv, d * D * D);
+  p.stack_cap = cap;
+  const size_t tab_bytes = ((p.kv == SM_W_TABLE ? (size_t)p.n_vl * p.n_vl : 0) +
+                            (p.ke == SM_W_TABLE ? (size_t)p.n_el * p.n_el : 0)) * 8;
+  const long long pair_words = 2 * sm_record_words(nmax, p.ke != SM_W_NONE);
+  // GRAKEL_B200_SM_GLOBAL=1 reads every record from global memory (the route of pairs too large to stage)
+  const char* e_glob = getenv("GRAKEL_B200_SM_GLOBAL");
+  const bool staged = !(e_glob && atoi(e_glob) != 0) && tab_bytes + SM_WARPS * pair_words * 4 <= 96 * 1024;
+  p.stage_words = staged ? (int)pair_words : 0;
+  const size_t smem = tab_bytes + (size_t)SM_WARPS * p.stage_words * 4;
+  GK_CUDA(cudaFuncSetAttribute(sm_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
+  int per_sm = 0;
+  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sm_pairs, SM_THREADS, smem));
+  long long grid = (long long)h->sm_count * std::max(per_sm, 1);
+  // at most 1 GiB of stacks: fewer CTAs (down to one) when a lane's stack is large
+  const long long per_cta = (long long)SM_WARPS * 32 * cap * 4;
+  grid = std::min(grid, std::max<long long>(1, (1LL << 30) / per_cta));
+  grid = std::min<long long>(grid, (p.n_pairs + SM_WARPS - 1) / SM_WARPS);
+  GK_TRY(h->sm_stack.ensure((size_t)grid * per_cta));
+  p.stack = h->sm_stack.as<unsigned>();
+  GK_CUDA(cudaMemsetAsync(h->sm_ctl.p, 0, 8, h->stream));
+  p.next = h->sm_ctl.as<unsigned long long>();
+  sm_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
+  LAUNCH_CHECK(h);
+  return GK_OK;
+}
+
+static SmParams sm_params(gk_handle* h) {
+  SmParams p;
+  memset(&p, 0, sizeof(p));
+  p.graph_ptr = h->graph_ptr.as<int>();
+  p.rec_off = h->sm_off.as<long long>(); p.rec = h->sm_rec.as<unsigned>();
+  p.vtab = h->sm_vtab.as<double>(); p.n_vl = h->sm_n_vl;
+  p.etab = h->sm_etab.as<double>(); p.n_el = h->sm_n_el;
+  p.kv = h->sm_kv; p.ke = h->sm_ke;
+  p.kk = h->sm_kk; p.n_tv = h->sm_k + 1;
+  p.lam = h->sm_lam.as<double>();
+  p.exact = h->sm_exact ? 1 : 0;
+  p.err = reinterpret_cast<unsigned*>(h->sm_ctl.as<unsigned char>() + 8);
+  return p;
+}
+
+static int sm_check_err(gk_handle* h) {
+  unsigned err = 0;
+  GK_CUDA(cudaMemcpyAsync(&err, h->sm_ctl.as<unsigned char>() + 8, 4, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  if (err & 1u) return fail(GK_ERR_RANGE, "SubgraphMatching: a clique count reached 2^53, past exact fp64");
+  if (err & 2u) return fail(GK_ERR_RANGE, "SubgraphMatching: an extension set overflowed its stack");
+  return GK_OK;
+}
+
+// Gram of SubgraphMatching (gram_path 13): fp64, host or GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges.
+// The self similarities come from the same pair kernel, so a square K's diagonal equals them bit for bit; the full
+// square case computes the upper triangle and mirrors it.
+static int gram_sm(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const int64_t N = h->N, k_rows = q.k_rows, k_cols = q.k_cols;
+  const int64_t launches0 = h->launches;
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  GK_TRY(h->diag_f64.ensure((size_t)N * 8));
+  GK_CUDA(cudaMemsetAsync(h->sm_ctl.as<unsigned char>() + 8, 0, 8, h->stream));
+  const SmParams p = sm_params(h);
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  {
+    SmParams d = p;
+    d.pairs = RW_PAIRS_DIAG;
+    d.n_pairs = N;
+    d.out = h->diag_f64.as<double>();
+    GK_TRY(sm_launch(h, d));
+  }
+  const bool mirror = q.full_square && !(q.flags & GK_FULL_TILES);
+  if (k_rows > 0) {
+    SmParams k = p;
+    k.pairs = mirror ? RW_PAIRS_TRIANGLE : RW_PAIRS_RECT;
+    k.ordered = q.square ? 1 : 0;
+    k.n_pairs = mirror ? N * (N + 1) / 2 : k_rows * k_cols;
+    k.row_g0 = q.a0;
+    k.rows = (int)k_rows; k.cols = (int)k_cols;
+    k.out = out.p; k.ld = out.ld;
+    GK_TRY(sm_launch(h, k));
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_TRY(sm_check_err(h));
+  GK_TRY(f64_deliver(h, q, out, true, h->tev[3], h->tev[4]));
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->gram_path = 13;
+    stats->gemm_tiles = mirror ? N * (N + 1) / 2 : k_rows * k_cols;
+    stats->gemm_launches = h->launches - launches0;
+    stats->ms_rw = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_gemm = stats->ms_rw;
+    stats->ms_d2h = ev_ms(h->tev[3], h->tev[4]);
+    stats->ms_total = stats->ms_rw + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
+int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_counts: null argument");
+  if (h->feature_kind != FK_SM || !h->features_ready) return fail(GK_ERR_STATE, "gk_sm_counts: call gk_sm_features first");
+  if (n_fit <= 0 || n_fit > h->N) return fail(GK_ERR_ARG, "gk_sm_counts: n_fit out of range");
+  const bool square = n_fit == h->N;
+  if (row < 0 || row >= (square ? h->N : h->N - n_fit)) return fail(GK_ERR_ARG, "gk_sm_counts: row out of range");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t bytes = (size_t)n_fit * (h->sm_k + 1) * 8;
+  GK_TRY(h->K_stage.ensure(bytes));
+  GK_CUDA(cudaMemsetAsync(h->sm_ctl.as<unsigned char>() + 8, 0, 8, h->stream));
+  SmParams p = sm_params(h);
+  p.pairs = RW_PAIRS_RECT;
+  p.ordered = square ? 1 : 0;
+  p.n_pairs = n_fit;
+  p.row_g0 = (int)((square ? 0 : n_fit) + row);
+  p.rows = 1; p.cols = (int)n_fit;
+  p.tv_out = h->K_stage.as<double>();
+  GK_TRY(sm_launch(h, p));
+  GK_TRY(sm_check_err(h));
+  GK_CUDA(cudaMemcpyAsync(out, h->K_stage.p, bytes, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+// ---------------------------------------------------------------------------
 }  // extern "C"
 
 // ---------------------------------------------------------------------------
@@ -4009,6 +4225,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_PM: return gram_pm(h, q, stats);
     case FK_NSPD: return gram_nspd(h, q, stats);
     case FK_RW: return gram_rw(h, q, stats);
+    case FK_SM: return gram_sm(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }
 }

@@ -124,6 +124,7 @@ enum FeatureKind : int {
   FK_PK = 7,      // Propagation counts in the SP layout: the integer Gram
   FK_PM = 8,      // PyramidMatch per-level expanded blocks (the NeighborhoodHash layout)
   FK_NSPD = 9,    // NeighborhoodSubgraphPairwiseDistance per-(radius, distance) count tables
+  FK_SM = 10,     // SubgraphMatching per-graph bitset records
 };
 
 }  // namespace gk
@@ -254,6 +255,13 @@ struct gk_handle {
   double rw_lamda = 0.0;
   bool rw_labeled = false;
   int64_t rw_iter_rows = 0, rw_iter_cols = 0;  // shape of the iteration counts of the last gk_gram
+
+  // ---- SubgraphMatching (FK_SM): per-graph records and their offsets, edge label ids, weight tables, lambdas, the
+  // extension-set stacks, [pair counter u64 | error bits u32 | largest neighbour count u32]
+  gk::DevBuf sm_rec, sm_off, sm_el, sm_vtab, sm_etab, sm_lam, sm_stack, sm_ctl;
+  int sm_k = 0, sm_kk = 1, sm_kv = 0, sm_ke = 0, sm_n_vl = 0, sm_n_el = 0;
+  int sm_max_und = 0;  // largest number of distinct out- or in-neighbours of a packed vertex
+  bool sm_exact = true;
 
   // ---- Propagation (FK_PK): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
   // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]

@@ -259,32 +259,40 @@ __device__ double rw_pair_spectral(const RwParams& P, int gi, int gj, double* re
   return acc[0];
 }
 
-// One CTA per pair (grid-stride).  RECT: entry (r, c) of the request; TRIANGLE: the upper triangle of the square case,
-// written to (r, c) and mirrored to (c, r); DIAG: graph g against itself.
+// Entry (r, c) of pair number pi and the graphs (gi, gj) it is evaluated on.  RECT: entry (r, c) of the request;
+// TRIANGLE: the upper triangle of the square case (the caller mirrors it to (c, r)); DIAG: graph r against itself.
+// `ordered`: rows and columns index the same graphs and the pair is evaluated as op(min, max).
+__device__ __forceinline__ void rw_pair_of(int pairs, int cols, int row_g0, int ordered, long long pi, int& r, int& c,
+                                           int& gi, int& gj) {
+  if (pairs == RW_PAIRS_TRIANGLE) {
+    // row r holds cols - r entries starting at r cols - r (r - 1) / 2
+    const double n = (double)cols;
+    r = (int)floor(((2.0 * n + 1.0) - sqrt((2.0 * n + 1.0) * (2.0 * n + 1.0) - 8.0 * (double)pi)) * 0.5);
+    r = max(0, min(r, cols - 1));
+    auto start = [&](long long rr) { return rr * (long long)cols - rr * (rr - 1) / 2; };
+    while (r > 0 && start(r) > pi) --r;
+    while (r + 1 < cols && start(r + 1) <= pi) ++r;
+    c = r + (int)(pi - start(r));
+  } else if (pairs == RW_PAIRS_DIAG) {
+    r = c = (int)pi;
+  } else {
+    r = (int)(pi / cols);
+    c = (int)(pi - (long long)r * cols);
+  }
+  gi = pairs == RW_PAIRS_DIAG ? r : row_g0 + r;
+  gj = c;
+  if (ordered && gi > gj) { const int x = gi; gi = gj; gj = x; }
+}
+
+// One CTA per pair (grid-stride), written to (r, c) of the request and, for TRIANGLE, mirrored to (c, r).
 __global__ void __launch_bounds__(RW_THREADS) rw_pairs(RwParams P) {
   extern __shared__ double rw_smem[];
   __shared__ double red[2 * 2 * RW_WARPS];
   double* buf = P.ws ? P.ws + (size_t)blockIdx.x * P.ws_stride : rw_smem;
   int parity = 0;
   for (long long pi = blockIdx.x; pi < P.n_pairs; pi += gridDim.x) {
-    int r, c;
-    if (P.pairs == RW_PAIRS_TRIANGLE) {
-      // row r holds cols - r entries starting at r cols - r (r - 1) / 2
-      const double n = (double)P.cols;
-      r = (int)floor(((2.0 * n + 1.0) - sqrt((2.0 * n + 1.0) * (2.0 * n + 1.0) - 8.0 * (double)pi)) * 0.5);
-      r = max(0, min(r, P.cols - 1));
-      auto start = [&](long long rr) { return rr * (long long)P.cols - rr * (rr - 1) / 2; };
-      while (r > 0 && start(r) > pi) --r;
-      while (r + 1 < P.cols && start(r + 1) <= pi) ++r;
-      c = r + (int)(pi - start(r));
-    } else if (P.pairs == RW_PAIRS_DIAG) {
-      r = c = (int)pi;
-    } else {
-      r = (int)(pi / P.cols);
-      c = (int)(pi - (long long)r * P.cols);
-    }
-    int gi = P.pairs == RW_PAIRS_DIAG ? r : P.row_g0 + r, gj = c;
-    if (P.ordered && gi > gj) { const int x = gi; gi = gj; gj = x; }
+    int r, c, gi, gj;
+    rw_pair_of(P.pairs, P.cols, P.row_g0, P.ordered, pi, r, c, gi, gj);
     int it = 0;
     double v;
     if (P.route == RW_ROUTE_CG) v = rw_pair_cg(P, gi, gj, buf, red, parity, &it);

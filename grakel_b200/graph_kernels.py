@@ -11,6 +11,7 @@ the kernels of the device hot path:
     "graph_hopper" / "GH"
     "neighborhood_hash" / "NH"
     "neighborhood_subgraph_pairwise_distance" / "NSPD"  (+ r, d)
+    "subgraph_matching" / "SM"  (+ k, kv, ke, lw)
     "propagation" / "PR"        (+ with_attributes: PropagationAttr)
     "pyramid_match" / "PM"      (+ with_labels, L, d)
 
@@ -35,13 +36,13 @@ from sklearn.utils.validation import check_is_fitted
 from .core_framework import CoreFramework
 from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, NeighborhoodSubgraphPairwiseDistance,
                       Propagation, PropagationAttr, PyramidMatch,
-                      ShortestPath, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
+                      ShortestPath, SubgraphMatching, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
 
 # reference names outside the hot path (graph_kernels.py:38-64)
 _OUTSIDE = frozenset((
-    "random_walk", "RW", "graphlet_sampling", "GR", "subgraph_matching", "SM", "multiscale_laplacian", "ML",
+    "random_walk", "RW", "graphlet_sampling", "GR", "multiscale_laplacian", "ML",
     "lovasz_theta", "LOVT", "svm_theta", "SVMT", "odd_sth", "ODD"))
 
 
@@ -64,6 +65,7 @@ for _names, _framework, _build in (
         (("neighborhood_hash", "NH"), False, lambda p: (NeighborhoodHash, p)),
         (("neighborhood_subgraph_pairwise_distance", "NSPD"), False,
          lambda p: (NeighborhoodSubgraphPairwiseDistance, p)),
+        (("subgraph_matching", "SM"), False, lambda p: (SubgraphMatching, p)),
         (("propagation", "PR"), False, _propagation),
         (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),

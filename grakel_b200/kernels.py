@@ -2937,3 +2937,257 @@ class NeighborhoodSubgraphPairwiseDistance(Kernel):
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
+
+
+# ------------------------------------------------------------------------------
+def _dirac(a, b):
+    """The reference's default vertex and edge kernel, int(a == b).  SubgraphMatching recognises this function by
+    identity and compares label ids on the device."""
+    return int(a == b)
+
+
+_SM_ELEMENT_MSG = ("each element of X must be either a graph object or a list with at least a graph like object and "
+                   "node, edge labels dict \n")
+_SM_TABLE_MAX = 4096
+_MISSING = object()
+
+
+class SubgraphMatching(Kernel):
+    """Subgraph matching kernel (subgraph_matching.py; Kriege & Mutzel 2012).  k(x, y) = sum_s lambda_s tv_s, where
+    tv[s - 1] sums prod cv * prod |ce| over the vertex sets of size s <= k of the weighted product graph that are
+    cliques (every pair has ce != 0) connected by its c-edges (ce > 0).  The clique enumeration of every pair runs on
+    the device, one warp per pair, without building the product graph; integer-valued weights (the default `_dirac`,
+    None, integer tables) are counted exactly, and the lambdas are folded in np.dot's order, so K equals the
+    reference's bit for bit for them.
+
+    Vertices are the indices of an adjacency matrix or the sorted symbols of an edge dictionary, and an edge is an
+    adjacency entry > 0, as after the reference's change_format("adjacency").  Deviations: a `kv` / `ke` other than
+    `_dirac` or None is called once per pair of distinct labels (the reference calls it once per vertex or edge pair),
+    and more than 64 distinct labels on either side raise NotImplementedError; an edge without a label raises the
+    reference's TypeError at parse time even when no pair would read it; real lambdas with k + 1 > 15, k < 0 and
+    cliques of more than 32 vertices raise NotImplementedError; a count of 2^53 or more raises an error."""
+
+    _graph_format = "all"
+
+    def __init__(self, n_jobs=None, verbose=False, normalize=False, k=5, kv=_dirac, ke=_dirac, lw="uniform"):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.k = k
+        self.kv = kv
+        self.ke = ke
+        self.lw = lw
+        self._initialized.update({"k": False, "kv": False, "ke": False, "lw": False})
+
+    def initialize(self):
+        """subgraph_matching.py:70-120, in its order and with its checks (`k` is validated with `and`)."""
+        super().initialize()
+        if not self._initialized["k"]:
+            if type(self.k) is not int and self.k < 1:
+                raise TypeError("k must be an integer greater-equal than 1")
+            self._initialized["k"] = True
+        if not self._initialized["kv"]:
+            if not callable(self.kv) and self.kv is not None:
+                raise TypeError("kv must be callable or None")
+            self._initialized["kv"] = True
+        if not self._initialized["ke"]:
+            if not callable(self.ke) and self.ke is not None:
+                raise TypeError("ke must be callable or None")
+            self._initialized["ke"] = True
+        if not self._initialized["lw"]:
+            k = self.k + 1
+            not_str_iter = type(self.lw) is not str and isinstance(self.lw, Iterable)
+            if not_str_iter:
+                lw = list(self.lw)
+            if not_str_iter and len(lw) == self.k and all(isinstance(x, Real) for x in lw):
+                self.lambdas_ = np.array(lw).reshape((1, k))
+            elif self.lw == "uniform":
+                self.lambdas_ = np.full((1, k), 1.0)
+            elif self.lw == "increasing":
+                self.lambdas_ = np.arange(1.0, float(k) + 1.0).reshape(1, k)
+            elif self.lw == "decreasing":
+                self.lambdas_ = np.full((1, k), 1.0) / np.arange(1.0, float(k) + 1.0).reshape(1, k)
+            elif self.lw == "strong_decreasing":
+                self.lambdas_ = np.full((1, k), 1.0) / np.square(np.arange(1.0, float(k) + 1.0)).reshape(1, k)
+            elif callable(self.lw):
+                try:
+                    self.lambdas_ = np.array([self.lw(i) for i in range(k)]).reshape((1, k))
+                except Exception as e:
+                    raise TypeError("Incorrect Callable: " + str(e))
+            else:
+                raise TypeError('lw can either be str with values "uniform", "increasing", "decreasing", '
+                                '"strong_decreasing" or an iterable of k+1 elements or a callable of one integer '
+                                "argument.")
+            self._initialized["lw"] = True
+        if int(self.k) < 0:
+            raise NotImplementedError("SubgraphMatching: k < 0 has no defined result")
+
+    # ---- input
+    def _graph(self, g, node_labels, edge_labels):
+        """(n, sorted (i, j) edges without self-loops, vertex labels or None, edge labels or None)."""
+        need_v, need_e = self.kv is not None, self.ke is not None
+        if need_v and not node_labels:
+            raise ValueError("Graph does not have any labels for vertices.")
+        if need_e and not edge_labels:
+            raise ValueError("Graph does not have any labels for edges.")
+        A, order = adjacency_and_order(g)
+        order = list(order)
+        ii, jj = np.nonzero(A > 0)
+        edges = [(i, j) for i, j in zip(ii.tolist(), jj.tolist()) if i != j]
+        vl = [node_labels[s] for s in order] if need_v else None
+        el = None
+        if need_e:
+            el = []
+            for i, j in edges:
+                lab = edge_labels.get((order[i], order[j]), _MISSING)
+                if lab is _MISSING:
+                    # the reference adds a str to the KeyError it catches, which raises a TypeError
+                    raise TypeError("unsupported operand type(s) for +: 'KeyError' and 'str'")
+                el.append(lab)
+        return len(order), edges, vl, el
+
+    def _block(self, X, edge_labels):
+        """The graphs of a datasets.read_tu block (the nodes that occur in an edge, as in its edge dictionaries),
+        with the block's per-edge label ids `edge_labels` (read_tu's `edge_labels`) when ke is not None."""
+        X.require("sp", labels=self.kv is not None)
+        if self.ke is not None and edge_labels is None:
+            raise ValueError("Graph does not have any labels for edges.")
+        gp, rp, ci = X.graph_ptr, X.row_ptr, X.col_idx
+        out = []
+        for g in range(X.n_graphs):
+            a, b = int(gp[g]), int(gp[g + 1])
+            ed = {}
+            for u in range(a, b):
+                for e in range(int(rp[u]), int(rp[u + 1])):
+                    v = int(ci[e])
+                    if v != u and (X.weights is None or X.weights[e] > 0):
+                        ed[(u - a, v - a)] = None if edge_labels is None else int(edge_labels[e])
+            edges = sorted(ed)
+            out.append((b - a, edges, list(X.labels[a:b]) if self.kv is not None else None,
+                        [ed[e] for e in edges] if self.ke is not None else None))
+        return out
+
+    def parse_input(self, X):
+        """subgraph_matching.py:142-207: Graph objects or 3-element iterables; empty elements are skipped with a
+        warning.  Also the result of datasets.read_tu(kernel="SP") (its block and edge labels), or its block alone
+        with ke=None."""
+        if isinstance(X, dict) and isinstance(X.get("data"), Block):
+            return self._block(X["data"], X.get("edge_labels"))
+        if isinstance(X, Block):
+            if self.ke is not None:
+                raise NotImplementedError("a packed block carries no edge labels: pass ke=None or the whole result of "
+                                          "datasets.read_tu")
+            return self._block(X, None)
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            elif isinstance(x, Iterable):
+                x = list(x)
+                if len(x) not in (0, 3):
+                    raise TypeError(_SM_ELEMENT_MSG)
+                if len(x) == 0:
+                    warnings.warn("Ignoring empty element on index: " + str(idx))
+                    continue
+            else:
+                raise TypeError(_SM_ELEMENT_MSG)
+            out.append(self._graph(x[0], x[1], x[2]))
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    # ---- estimator protocol
+    def fit(self, X, y=None):
+        self._method_calling = 1
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        self.X = self.parse_input(X)
+        self.__dict__.pop("_X_diag", None)
+        return self
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        K, xd, _ = self._sm_run(self.X, len(self.X))
+        self._X_diag = xd
+        if self.normalize:
+            self._warn_unnormalizable(xd)
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        Y = self.parse_input(X)
+        K, xd, yd = self._sm_run(self.X + Y, len(self.X))
+        self._X_diag, self._Y_diag = xd, yd
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xd, yd)
+        return K
+
+    def diagonal(self):
+        check_is_fitted(self, ["X"])
+        try:
+            check_is_fitted(self, ["_X_diag"])
+        except NotFittedError:
+            _, self._X_diag, _ = self._sm_run(self.X, len(self.X), want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
+
+    @staticmethod
+    def _table(fn, labels, what):
+        if len(labels) ** 2 > _SM_TABLE_MAX:
+            raise NotImplementedError("SubgraphMatching: a custom " + what + " kernel is tabulated over the distinct "
+                                      "labels, at most 64 of them (got " + str(len(labels)) + ")")
+        return np.array([[float(fn(a, b)) for b in labels] for a in labels], dtype=np.float64).reshape(
+            len(labels), len(labels))
+
+    def _pack(self, graphs):
+        """(graph_ptr, row_ptr, col_idx, vertex label ids, edge label ids, kv table, ke table, flags)."""
+        gp, rp, ci, lab, el = [0], [0], [], [], []
+        lid, eid = {}, {}
+        for n, edges, vl, elab in graphs:
+            v0 = gp[-1]
+            deg = np.zeros(n, dtype=np.int64)
+            for i, j in edges:
+                deg[i] += 1
+                ci.append(v0 + j)
+            if elab is not None:
+                el.extend(eid.setdefault(s, len(eid)) for s in elab)
+            rp.extend((rp[-1] + np.cumsum(deg)).tolist())
+            if vl is not None:
+                lab.extend(lid.setdefault(s, len(lid)) for s in vl)
+            gp.append(v0 + n)
+        flags, vt, et = 0, None, None
+        if self.kv is None:
+            flags |= _lib.GK_SM_KV_NONE
+        elif self.kv is _dirac:
+            flags |= _lib.GK_SM_KV_DIRAC
+        else:
+            vt = self._table(self.kv, list(lid), "vertex")
+        if self.ke is None:
+            flags |= _lib.GK_SM_KE_NONE
+        elif self.ke is _dirac:
+            flags |= _lib.GK_SM_KE_DIRAC
+        else:
+            et = self._table(self.ke, list(eid), "edge")
+        ids = np.array(lab, dtype=np.int64) if self.kv is not None else None
+        elids = np.array(el, dtype=np.int64) if self.ke is not None else None
+        return (np.array(gp), np.array(rp), np.array(ci, dtype=np.int64), ids, elids, vt, et, flags)
+
+    def _sm_run(self, graphs, n_fit, want_matrix=True, device_ptr=None, row_range=None):
+        gp, rp, ci, ids, elids, vt, et, flags = self._pack(graphs)
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(gp, rp, ci, ids, None, None)
+            self.stats_ = eng.sm_features(int(self.k), self.lambdas_, vt, et, elids, flags)
+            K, xd, yd = eng.gram(len(graphs), n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 out=None if want_matrix else False, device_ptr=device_ptr, row_range=row_range,
+                                 stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd

@@ -254,6 +254,25 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
                    const double* q, const double* w, int32_t flags, gk_stats* stats);
 int gk_rw_iterations(gk_handle* h, uint8_t* out);
 
+/* SubgraphMatching (subgraph_matching.py), one graph pair per warp.  The packed CSR gives each graph's edges
+ * (self-loops are ignored), the packed labels its vertex label ids, edge_label[E] the edge label ids of the packed
+ * edges (with an edge kernel).  Vertex weights cv(a, b) are 1 (GK_SM_KV_NONE), [La == Lb] (GK_SM_KV_DIRAC) or
+ * vtable[La * n_vlabels + Lb]; c-edge weights 1 (GK_SM_KE_NONE), [Lea == Leb] (GK_SM_KE_DIRAC) or
+ * etable[Lea * n_elabels + Leb]; each table at most 4096 finite entries.  tv[s - 1] (s = 1 .. k; tv[k] = 0, and
+ * k = 0 gives tv[0] = sum cv) sums the connected cliques of the weighted product graph; gk_gram (gram_path 13) returns
+ * K = fma chain over lambdas[0 .. k] * tv from 0.  Integer-valued tables are summed exactly (a sum of 2^53 or more
+ * is GK_ERR_RANGE), real ones in fp64.  Real lambdas with k + 1 > 15, and cliques past 32 vertices, are
+ * GK_ERR_UNSUPPORTED.  gk_gram: fp64 only, host or GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges; GK_DIST
+ * and row maps are GK_ERR_UNSUPPORTED.  gk_sm_counts writes tv of the n_fit pairs of row `row` of the gk_gram
+ * request with the same n_fit: out[n_fit * (k + 1)]. */
+#define GK_SM_KV_NONE 1
+#define GK_SM_KV_DIRAC 2
+#define GK_SM_KE_NONE 4
+#define GK_SM_KE_DIRAC 8
+int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double* vtable, int32_t n_vlabels,
+                   const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags, gk_stats* stats);
+int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out);
+
 /* Propagation / PropagationAttr (propagation.py:27-689).  The packed CSR (gk_pack_csr without weights; with the
  * label ids for the labelled kernel) is the sparsity pattern of every graph's row-normalised transition matrix T,
  * t_values[E] its entries.  P (V x dim, fp64) starts one-hot from the packed label ids or as p0[V * dim] (GK_PK_ATTR).
