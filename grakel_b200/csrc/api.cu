@@ -773,6 +773,9 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
         std::vector<long long> pr((size_t)G * L * 16);
         GK_CUDA(cudaMemcpyAsync(pr.data(), h->K_stage.p, pr.size() * 8, cudaMemcpyDeviceToHost, h->stream));
         GK_CUDA(cudaStreamSynchronize(h->stream));
+        if (const char* out = getenv("GRAKEL_B200_PROF_OUT")) {  // raw int64 stamps [G][L][16] (tools/prof_wl_phases.py)
+          if (FILE* f = fopen(out, "wb")) { fwrite(pr.data(), 8, pr.size(), f); fclose(f); }
+        }
         long long t0 = pr[0];
         for (int b = 0; b < G; ++b) t0 = std::min(t0, pr[(size_t)b * L * 16]);
         fprintf(stderr, "[wl_fused2 prof] us; per level: avg over CTAs of the phase duration (max)\n");

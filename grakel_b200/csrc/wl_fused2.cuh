@@ -92,21 +92,19 @@ __device__ __forceinline__ void wlf2_count(const WlFused2Params& p, int nv, cons
   if (4 * n_act > nv) {
     for (int s2 = tid; s2 < WLF2_CT; s2 += WLF_THREADS) ct[s2] = 0xFFFFFFFFu;
     __syncthreads();
-    unsigned slot[WLF_VPT];
-    bool inst[WLF_VPT];
+    // the installing vertex keeps its slot in cf_s (emitter bit | slot) until every vertex has counted
 #pragma unroll
     for (int k = 0; k < WLF_VPT; ++k) {
       const int i = tid + k * WLF_THREADS;
-      inst[k] = false;
-      slot[k] = 0;
       if (i < nv && !frz_s[i]) {
+        cf_s[i] = 0;
         const int l = lab_s[i], g = gid_s[i];
         unsigned h = (((unsigned)l * 0x9E3779B1u) ^ ((unsigned)g * 0x85EBCA77u)) >> 15 & (WLF2_CT - 1);
         while (true) {
           unsigned w = ct[h];
           if (w == 0xFFFFFFFFu) {
             w = atomicCAS(&ct[h], 0xFFFFFFFFu, (1u << 16) | (unsigned)i);
-            if (w == 0xFFFFFFFFu) { inst[k] = true; slot[k] = h; break; }
+            if (w == 0xFFFFFFFFu) { cf_s[i] = (unsigned short)(0x8000u | h); break; }
           }
           const unsigned o = w & 0xFFFFu;
           if (lab_s[o] == l && gid_s[o] == g) { atomicAdd(&ct[h], 1u << 16); break; }
@@ -118,7 +116,7 @@ __device__ __forceinline__ void wlf2_count(const WlFused2Params& p, int nv, cons
 #pragma unroll
     for (int k = 0; k < WLF_VPT; ++k) {
       const int i = tid + k * WLF_THREADS;
-      if (i < nv && !frz_s[i]) cf_s[i] = inst[k] ? (unsigned short)((ct[slot[k]] >> 16) | 0x8000u) : (unsigned short)0;
+      if (i < nv && !frz_s[i] && (cf_s[i] & 0x8000u)) cf_s[i] = (unsigned short)((ct[cf_s[i] & 0x7FFFu] >> 16) | 0x8000u);
     }
   } else {
     int ex = ex0;
@@ -152,22 +150,13 @@ __device__ __forceinline__ void wlf2_emit(const WlFused2Params& p, int v0, int n
   const int tid = threadIdx.x, lane = tid & 31;
   wlf2_count(p, nv, lab_s, frz_s, gid_s, gbeg_s, gend_s, cf_s, ct, list_s, s_warp);
   __syncthreads();
-  int g[WLF_VPT], l[WLF_VPT];
-  unsigned cnt[WLF_VPT];
-  bool emit[WLF_VPT];
+  // a vertex emits iff it is not frozen and carries the emitter bit; read again from shared memory below rather than
+  // kept in registers across the scan
   int n_emit = 0;
 #pragma unroll
   for (int k = 0; k < WLF_VPT; ++k) {
     const int i = tid + k * WLF_THREADS;
-    g[k] = i < nv ? gid_s[i] : -1;  // every vertex of the tile, frozen or not: graphs stay contiguous lane runs
-    l[k] = 0; cnt[k] = 0; emit[k] = false;
-    if (i < nv && !frz_s[i]) {
-      const unsigned cf = cf_s[i];
-      l[k] = lab_s[i];
-      cnt[k] = cf & 0x7FFFu;
-      emit[k] = (cf & 0x8000u) != 0;
-      n_emit += emit[k] ? 1 : 0;
-    }
+    n_emit += (i < nv && !frz_s[i] && (cf_s[i] & 0x8000u)) ? 1 : 0;
   }
   int total;
   int ex = wlf_block_scan(n_emit, &total, s_warp);
@@ -181,12 +170,17 @@ __device__ __forceinline__ void wlf2_emit(const WlFused2Params& p, int v0, int n
   for (int i = total + tid; i < nv; i += WLF_THREADS) p.coo_keys[coo_off + i] = EMPTY64;  // unused rest of the fixed region
 #pragma unroll
   for (int k = 0; k < WLF_VPT; ++k) {
-    if (emit[k]) {
-      const unsigned col = (unsigned)(base + l[k]);
-      p.coo_keys[coo_off + ex] = ((unsigned long long)(unsigned)g[k] << 32) | col;
-      p.coo_cnt[coo_off + ex] = cnt[k];
+    const int i = tid + k * WLF_THREADS;
+    const int gg = i < nv ? gid_s[i] : -1;  // every vertex of the tile, frozen or not: graphs stay contiguous lane runs
+    const unsigned cf = (i < nv && !frz_s[i]) ? cf_s[i] : 0u;
+    const bool emit = (cf & 0x8000u) != 0;
+    const unsigned cnt = cf & 0x7FFFu;
+    if (emit) {
+      const unsigned col = (unsigned)(base + lab_s[i]);
+      p.coo_keys[coo_off + ex] = ((unsigned long long)(unsigned)gg << 32) | col;
+      p.coo_cnt[coo_off + ex] = cnt;
       ++ex;
-      mx = max(mx, cnt[k]);
+      mx = max(mx, cnt);
       n_new += 1u;
       if (use_agg) {
         unsigned slot = (col * 0x9E3779B1u >> 12) & (WLF_AGG - 1);
@@ -201,8 +195,7 @@ __device__ __forceinline__ void wlf2_emit(const WlFused2Params& p, int v0, int n
       }
     }
     // exact self similarity: sum of squared counts per graph (runs of equal g inside the warp)
-    unsigned long long val = emit[k] ? (unsigned long long)cnt[k] * cnt[k] : 0ULL;
-    const int gg = g[k];
+    unsigned long long val = emit ? (unsigned long long)cnt * cnt : 0ULL;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
       const unsigned long long y = __shfl_down_sync(0xffffffffu, val, d);
@@ -220,6 +213,23 @@ __device__ __forceinline__ void wlf2_emit(const WlFused2Params& p, int v0, int n
     }
   }
   __syncthreads();  // agg is reused by the next tile / overwritten by the next level's signatures
+}
+
+// The tile's non-frozen vertices in ascending order, act_s[0, n_act).  [A], [B] and the label write-back of a level
+// run over this list, so the deep levels (a few per cent of the vertices still active) cost their live vertices, not
+// the tile.  Ascending, so the vertices of one graph stay contiguous lane runs ([B]'s per-graph sums).
+__device__ __forceinline__ int wlf2_compact(int nv, const unsigned char* frz_s, unsigned short* act_s, int* s_warp) {
+  const int i0 = threadIdx.x * WLF_VPT;
+  int mine = 0;
+#pragma unroll
+  for (int k = 0; k < WLF_VPT; ++k) mine += (i0 + k < nv && !frz_s[i0 + k]) ? 1 : 0;
+  int n_act;
+  int ex = wlf_block_scan(mine, &n_act, s_warp);
+#pragma unroll
+  for (int k = 0; k < WLF_VPT; ++k)
+    if (i0 + k < nv && !frz_s[i0 + k]) act_s[ex++] = (unsigned short)(i0 + k);
+  __syncthreads();
+  return n_act;
 }
 
 constexpr int WLF2_SMEM = WLF_SMEM + WLF_TILE_V /*frz_s*/ + WLF_TILE_V * 4 /*gid_s*/ + WLF_TILE_V * 4 /*gbeg_s, gend_s*/ +
@@ -271,8 +281,9 @@ __device__ __forceinline__ void wlf2_stage_labels(const WlFused2Params& p, const
 
 // PAY: slot payloads (see [A3]) instead of the representative's CSR row as the verification reference.  A template
 // parameter, not a runtime switch: with both schemes live in one instance the kernel spilled 368 bytes per thread
-// at its 64-register budget.  Compiled for sm_90a, each instance alone still spills (PAY = true: 212 bytes of spill
-// stores per thread, PAY = false: 46); the register budget of this kernel on H100 is an open item (DESIGN.md §7).
+// at its 64-register budget.  Compiled for sm_90a, each instance alone fits the 64 registers with no spill (ptxas
+// -v: 0 bytes of spill stores and loads) because no phase holds more than a pair of items in registers ([A3], [B]),
+// the feature phase re-reads its per-vertex state from shared memory, and one warp reduces the per-CTA partials.
 template <bool PAY>
 __global__ void __launch_bounds__(WLF_THREADS, 1)
 wl_fused2_kernel(WlFused2Params p) {
@@ -292,6 +303,7 @@ wl_fused2_kernel(WlFused2Params p) {
   unsigned* slot_s = reinterpret_cast<unsigned*>(gend_s + WLF_TILE_V);
   unsigned short* list_s = reinterpret_cast<unsigned short*>(slot_s);
   unsigned short* cf_s = reinterpret_cast<unsigned short*>(slot_s + WLF_TILE_V);  // emit phase: in-graph count | emitter bit
+  unsigned short* act_s = cf_s;  // [A] to the label write-back: the tile's non-frozen vertices (wlf2_compact)
   unsigned* ct = reinterpret_cast<unsigned*>(key_s);  // emit phase: the (graph, label) table (key_s is free after [A])
   __shared__ int s_warp[32];
   __shared__ unsigned s_red[128];
@@ -316,13 +328,21 @@ wl_fused2_kernel(WlFused2Params p) {
     }
     if (lane == 0) { s_red[wid] = mx; s_red[32 + wid] = n_new; s_red[64 + wid] = n_rep; s_red[96 + wid] = n_fz; }
     __syncthreads();
-    if (tid == 0) {
-      unsigned m = 0, n = 0, r = 0, z = 0;
-      for (int w = 0; w < 32; ++w) { m = max(m, s_red[w]); n += s_red[32 + w]; r += s_red[64 + w]; z += s_red[96 + w]; }
-      if (z) atomicAdd(&p.sc->sp_coo, (unsigned long long)z);  // total of diag_frozen (WL-OA's entry count)
-      p.st.part_max[(size_t)level * G + b] = m;
-      p.st.part_new[(size_t)level * G + b] = n;
-      if (level > 0 && r) atomicAdd((unsigned long long*)&p.sc->level_dims[level], (unsigned long long)r);
+    if (wid == 0) {  // one warp reduces the 32 warp partials (one thread unrolling it was the kernel's register peak)
+      unsigned m = s_red[lane], n = s_red[32 + lane], r = s_red[64 + lane], z = s_red[96 + lane];
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) {
+        m = max(m, __shfl_xor_sync(0xffffffffu, m, d));
+        n += __shfl_xor_sync(0xffffffffu, n, d);
+        r += __shfl_xor_sync(0xffffffffu, r, d);
+        z += __shfl_xor_sync(0xffffffffu, z, d);
+      }
+      if (lane == 0) {
+        if (z) atomicAdd(&p.sc->sp_coo, (unsigned long long)z);  // total of diag_frozen (WL-OA's entry count)
+        p.st.part_max[(size_t)level * G + b] = m;
+        p.st.part_new[(size_t)level * G + b] = n;
+        if (level > 0 && r) atomicAdd((unsigned long long*)&p.sc->level_dims[level], (unsigned long long)r);
+      }
     }
     mx = 0; n_new = 0; n_rep = 0; n_fz = 0;
     __syncthreads();
@@ -387,6 +407,7 @@ wl_fused2_kernel(WlFused2Params p) {
 
     // ---------------- [A] signatures + insert (non-frozen vertices)
     WLF_STAMP(lv, 0);
+    int n_act = 0;  // resident tile: the list built in [A] serves [B] of the same level
     for (int t = t_beg; t < t_end; ++t) {
       const int v0 = p.tile_vbeg[t], nv = p.tile_vbeg[t + 1] - v0;
       const int e0 = p.row_ptr[v0], ne = p.row_ptr[v0 + nv] - e0;
@@ -396,12 +417,14 @@ wl_fused2_kernel(WlFused2Params p) {
         wlf2_stage_labels(p, lab_in, v0, nv, lab_s, frz_s, tid);
         __syncthreads();
       }
+      n_act = wlf2_compact(nv, frz_s, act_s, s_warp);
       WLF_STAMP(lv, 8);
       // [A1] one thread per vertex of degree <= 8: 19-comparator network in registers
-      for (int i = tid; i < nv; i += WLF_THREADS) {
+      for (int a = tid; a < n_act; a += WLF_THREADS) {
+        const int i = act_s[a];
         const int beg = rp_s[i];
         const int deg = rp_s[i + 1] - beg;
-        if (deg > 8 || frz_s[i]) continue;
+        if (deg > 8) continue;
         int x0, x1, x2, x3, x4, x5, x6, x7;
         x0 = 0 < deg ? lab_s[col_s[beg + 0]] : 0x7fffffff;
         x1 = 1 < deg ? lab_s[col_s[beg + 1]] : 0x7fffffff;
@@ -431,12 +454,12 @@ wl_fused2_kernel(WlFused2Params p) {
         key_s[i] = wlf_finish(dg ? 0x243F6A88u : ha, dg ? 0x85A308D3u : hc, lab_s[i], deg, p.seed);
       }
       // [A2] higher degrees: one warp per vertex (shuffle bitonic <= 32, in-segment bitonic above)
-      for (int i0 = wid * 32; i0 < nv; i0 += WLF_THREADS) {
-        const int iv = i0 + lane;
-        const bool big = iv < nv && (rp_s[iv + 1] - rp_s[iv]) > 8 && !frz_s[iv];
+      for (int a0 = wid * 32; a0 < n_act; a0 += WLF_THREADS) {
+        const int iv = a0 + lane < n_act ? act_s[a0 + lane] : 0;
+        const bool big = a0 + lane < n_act && (rp_s[iv + 1] - rp_s[iv]) > 8;
         unsigned m = __ballot_sync(0xffffffffu, big);
         while (m) {
-          const int i = i0 + __ffs(m) - 1;
+          const int i = __shfl_sync(0xffffffffu, iv, __ffs(m) - 1);
           m &= m - 1;
           const int beg = rp_s[i], deg = rp_s[i + 1] - beg;
           int* seg = sig_s + beg;
@@ -497,48 +520,48 @@ wl_fused2_kernel(WlFused2Params p) {
       }
       __syncthreads();
       WLF_STAMP(lv, 10);
-      // [A3] insert every non-frozen vertex of the tile; the (<= 4) probes of a thread are issued together
-      {
-        unsigned long long key[WLF_VPT], w[WLF_VPT];
-        unsigned slot[WLF_VPT];
-        bool act[WLF_VPT], ins[WLF_VPT], won[WLF_VPT];
+      // [A3] insert every non-frozen vertex of the tile.  Items in pairs, like [B]: the probes of two items are issued
+      // together; item u of pair k0 is act_s[tid + (k0 + u) * WLF_THREADS], its tile index re-read from shared memory.
+#pragma unroll 1
+      for (int k0 = 0; k0 < WLF_VPT; k0 += 2) {
+        if (tid + k0 * WLF_THREADS >= n_act) break;
+        unsigned long long key[2], w[2];
+        unsigned slot[2];
+        bool act[2], won[2];
 #pragma unroll
-        for (int k = 0; k < WLF_VPT; ++k) {
-          const int i = tid + k * WLF_THREADS;
-          act[k] = i < nv && !frz_s[i];
-          key[k] = act[k] ? key_s[i] : 0ULL;
-          won[k] = false;
-        }
-#pragma unroll
-        for (int k = 0; k < WLF_VPT; ++k) {
-          ins[k] = act[k];
-          slot[k] = (unsigned)((key[k] & 0xFFFFFFFFULL) * 0x9E3779B1ULL >> 8) & p.ht_mask;
+        for (int u = 0; u < 2; ++u) {
+          const int a = tid + (k0 + u) * WLF_THREADS;
+          act[u] = a < n_act;
+          key[u] = act[u] ? key_s[act_s[a]] : 0ULL;
+          won[u] = false;
+          slot[u] = (unsigned)((key[u] & 0xFFFFFFFFULL) * 0x9E3779B1ULL >> 8) & p.ht_mask;
         }
         bool any = true;
         while (any) {
           // CAS first (no read-before-CAS): a new signature costs ONE L2 round trip; an existing one gets the
           // slot's word back from the failed CAS
 #pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            const unsigned long long mine = (key[k] & 0xFFFFFFFE00000000ULL) | (1ULL << 32) |
-                                            (unsigned)(v0 + tid + k * WLF_THREADS);
-            w[k] = act[k] ? atomicCAS(&tab[slot[k]], EMPTY64, mine) : 0ULL;
+          for (int u = 0; u < 2; ++u) {
+            if (!act[u]) { w[u] = 0ULL; continue; }
+            const unsigned long long mine = (key[u] & 0xFFFFFFFE00000000ULL) | (1ULL << 32) |
+                                            (unsigned)(v0 + act_s[tid + (k0 + u) * WLF_THREADS]);
+            w[u] = atomicCAS(&tab[slot[u]], EMPTY64, mine);
           }
           any = false;
 #pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            if (!act[k]) continue;
-            const int v = v0 + tid + k * WLF_THREADS;
-            if (w[k] == EMPTY64) { act[k] = false; won[k] = true; continue; }  // the CAS installed our word (single bit set)
-            if ((w[k] >> 33) == (key[k] >> 33)) {
-              const unsigned rep = (unsigned)w[k];
+          for (int u = 0; u < 2; ++u) {
+            if (!act[u]) continue;
+            if (w[u] == EMPTY64) { act[u] = false; won[u] = true; continue; }  // the CAS installed our word (single bit set)
+            if ((w[u] >> 33) == (key[u] >> 33)) {
+              const unsigned rep = (unsigned)w[u];
+              const unsigned v = (unsigned)(v0 + act_s[tid + (k0 + u) * WLF_THREADS]);
               // a second member: clear the single bit and keep the smaller representative in one atomicMin
-              if (((w[k] >> 32) & 1ULL) || rep > (unsigned)v)
-                atomicMin(&tab[slot[k]], (key[k] & 0xFFFFFFFE00000000ULL) | (unsigned)min(rep, (unsigned)v));
-              act[k] = false;
+              if (((w[u] >> 32) & 1ULL) || rep > v)
+                atomicMin(&tab[slot[u]], (key[u] & 0xFFFFFFFE00000000ULL) | min(rep, v));
+              act[u] = false;
               continue;
             }
-            slot[k] = (slot[k] + 1) & p.ht_mask;
+            slot[u] = (slot[u] + 1) & p.ht_mask;
             any = true;
           }
         }
@@ -551,18 +574,19 @@ wl_fused2_kernel(WlFused2Params p) {
           // collision flag.  Degrees above 6: the payload holds five labels and the installer's row offset, the rest of
           // the row is compared through sig_nbr (only installers of such degrees write their rows there).
 #pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            const int i = tid + k * WLF_THREADS;
-            if (!ins[k]) continue;
-            const unsigned sw = slot[k] | (won[k] ? 0x80000000u : 0u);
+          for (int u = 0; u < 2; ++u) {
+            const int a = tid + (k0 + u) * WLF_THREADS;
+            if (a >= n_act) continue;
+            const int i = act_s[a];
+            const unsigned sw = slot[u] | (won[u] ? 0x80000000u : 0u);
             if (resident) slot_s[i] = sw; else p.slot_of[v0 + i] = (int)sw;
-            if (won[k]) {
+            if (won[u]) {
               const int beg = rp_s[i], deg = rp_s[i + 1] - beg;
               int nb[6];
 #pragma unroll
               for (int j = 0; j < 6; ++j) nb[j] = j < deg ? sig_s[beg + j] : 0x7fffffff;
               if (deg > 6) nb[5] = e0 + beg;
-              uint4* dst = reinterpret_cast<uint4*>(pay + (size_t)slot[k] * 8);
+              uint4* dst = reinterpret_cast<uint4*>(pay + (size_t)slot[u] * 8);
               dst[0] = make_uint4((unsigned)lab_s[i], (unsigned)deg, (unsigned)nb[0], (unsigned)nb[1]);
               dst[1] = make_uint4((unsigned)nb[2], (unsigned)nb[3], (unsigned)nb[4], (unsigned)nb[5]);
               if (resident && deg > 6)
@@ -571,31 +595,23 @@ wl_fused2_kernel(WlFused2Params p) {
           }
         } else {
 #pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            const int i = tid + k * WLF_THREADS;
-            if (ins[k]) p.slot_of[v0 + i] = (int)slot[k];
+          for (int u = 0; u < 2; ++u) {
+            const int a = tid + (k0 + u) * WLF_THREADS;
+            if (a < n_act) p.slot_of[v0 + act_s[a]] = (int)slot[u];
           }
         }
-        // sorted neighbour labels of the inserted vertices to global memory: other CTAs verify against them.  Most of
-        // the tile inserting: one coalesced copy of the whole segment array (stale rows are never read); few: row by row
-        // (payload scheme on a resident tile: nothing -- own rows stay in shared memory, see above)
-        int n_ins = 0;
-        if (!(PAY && resident)) {
-#pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) n_ins += __syncthreads_count(ins[k] ? 1 : 0);
-        }
-        if (PAY && resident) {
-        } else if (2 * n_ins >= nv) {
-          for (int j = tid; j < ne; j += WLF_THREADS) sig_g[e0 + j] = sig_s[j];
-        } else {
-#pragma unroll
-          for (int k = 0; k < WLF_VPT; ++k) {
-            const int i = tid + k * WLF_THREADS;
-            if (ins[k]) {
-              const int beg = rp_s[i], end = rp_s[i + 1];
-              for (int j = beg; j < end; ++j) sig_g[e0 + j] = sig_s[j];
-            }
-          }
+      }
+      // sorted neighbour labels of the inserted vertices to global memory: other CTAs verify against them.  Most of
+      // the tile inserting: one coalesced copy of the whole segment array (stale rows are never read); few: row by row
+      // (payload scheme on a resident tile: nothing -- own rows stay in shared memory, see above)
+      if (PAY && resident) {
+      } else if (2 * n_act >= nv) {
+        for (int j = tid; j < ne; j += WLF_THREADS) sig_g[e0 + j] = sig_s[j];
+      } else {
+        for (int a = tid; a < n_act; a += WLF_THREADS) {
+          const int i = act_s[a];
+          const int beg = rp_s[i], end = rp_s[i + 1];
+          for (int j = beg; j < end; ++j) sig_g[e0 + j] = sig_s[j];
         }
       }
     }
@@ -612,135 +628,131 @@ wl_fused2_kernel(WlFused2Params p) {
         wlf2_stage_labels(p, lab_in, v0, nv, lab_s, frz_s, tid);
         stage_graphs(v0, nv);
         __syncthreads();
+        n_act = wlf2_compact(nv, frz_s, act_s, s_warp);
       }
-      int r[WLF_VPT];
-      bool act[WLF_VPT], sgl[WLF_VPT];
+      if (tid == 0) n_rep += (unsigned)(nv - n_act);  // a frozen vertex is a class of its own at every level
+      int* res_s = reinterpret_cast<int*>(key_s);  // per list position: new label | 0x80000000 if it freezes now
+      // Items in pairs: the table words and payloads of two items are in flight together, and nothing of a pair stays
+      // live in registers past it (under the 64-register budget of 1024 threads the whole batch of four spilled).
+#pragma unroll 1
+      for (int k0 = 0; k0 < WLF_VPT; k0 += 2) {
+        if ((tid & ~31) + k0 * WLF_THREADS >= n_act) break;  // warp-uniform: no item of this warp from here on
+        unsigned long long word[2];
+        uint4 pl0[2], pl1[2];  // payload scheme: the installer's signature (vertices that did not install)
+        bool chk[2];
 #pragma unroll
-      for (int k = 0; k < WLF_VPT; ++k) {
-        const int i = tid + k * WLF_THREADS;
-        act[k] = i < nv && !frz_s[i];
-        r[k] = act[k] ? ((PAY && resident) ? (int)slot_s[i] : p.slot_of[v0 + i]) : 0;
-      }
-      uint4 pl0[WLF_VPT], pl1[WLF_VPT];  // payload scheme: the installer's signature (vertices that did not install)
-      bool chk[WLF_VPT];
-#pragma unroll
-      for (int k = 0; k < WLF_VPT; ++k) {
-        const int i = tid + k * WLF_THREADS;
-        sgl[k] = false;
-        chk[k] = false;
-        pl0[k] = pl1[k] = make_uint4(0u, 0u, 0u, 0u);
-        if (act[k]) {
-          const unsigned sl = (unsigned)r[k] & 0x7fffffffu;
-          if (PAY && !((unsigned)r[k] >> 31)) {
-            chk[k] = true;
-            const uint4* src = reinterpret_cast<const uint4*>(pay + (size_t)sl * 8);
-            pl0[k] = __ldcg(src);
-            pl1[k] = __ldcg(src + 1);
-          }
-          const unsigned long long word = __ldcg(&tab[PAY ? sl : (unsigned)r[k]]);
-          r[k] = (int)(unsigned)word;
-          sgl[k] = ((word >> 32) & 1ULL) && r[k] == v0 + i;
-        }
-      }
-      // verification against the representative: CSR row and label of both sides first, then the sorted labels
-      int bv[WLF_VPT], dv[WLF_VPT], br[WLF_VPT], dr[WLF_VPT], lo[WLF_VPT], lr[WLF_VPT];
-#pragma unroll
-      for (int k = 0; k < WLF_VPT; ++k) {
-        const int i = tid + k * WLF_THREADS;
-        bv[k] = dv[k] = br[k] = dr[k] = lo[k] = lr[k] = 0;
-        if (PAY) {
-          if (chk[k]) {
-            if (resident) { bv[k] = rp_s[i]; dv[k] = rp_s[i + 1] - bv[k]; }
-            else { bv[k] = p.row_ptr[v0 + i]; dv[k] = p.row_ptr[v0 + i + 1] - bv[k]; }
-            lo[k] = lab_s[i];
-          }
-        } else if (act[k] && r[k] != v0 + i) {
-          if (resident) { bv[k] = rp_s[i]; dv[k] = rp_s[i + 1] - bv[k]; }  // own side from shared memory (sig_s)
-          else { bv[k] = p.row_ptr[v0 + i]; dv[k] = p.row_ptr[v0 + i + 1] - bv[k]; }
-          br[k] = p.row_ptr[r[k]]; dr[k] = p.row_ptr[r[k] + 1] - br[k];
-          lo[k] = lab_s[i]; lr[k] = __ldcg(&lab_in[r[k]]);
-        }
-      }
-#pragma unroll
-      for (int k = 0; k < WLF_VPT; ++k) {
-        const int i = tid + k * WLF_THREADS;
-        const int v = v0 + i;
-        unsigned long long fz = 0ULL;  // self-similarity contribution of a vertex that freezes now
-        const int gg = i < nv ? gid_s[i] : -1;  // every vertex: graphs stay contiguous lane runs
-        if (PAY && chk[k]) {  // compare with the installer's signature in the slot payload
-          const int pn[6] = {(int)pl0[k].z, (int)pl0[k].w, (int)pl1[k].x, (int)pl1[k].y, (int)pl1[k].z, (int)pl1[k].w};
-          const int d = dv[k];
-          bool same = ((int)pl0[k].x == lo[k]) && ((int)pl0[k].y == d);
-          if (same) {
-            const int nd = d > 6 ? 5 : d;
-#pragma unroll
-            for (int j = 0; j < 6; ++j)
-              if (j < nd) same = same && ((resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) == pn[j]);
-            if (d > 6) {
-              const int off = pn[5];  // installer's row offset in sig_nbr
-              for (int j = 5; same && j < d; ++j)
-                same = (resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) == __ldcg(&sig_g[off + j]);
+        for (int u = 0; u < 2; ++u) {
+          const int a = tid + (k0 + u) * WLF_THREADS;
+          word[u] = 0ULL;
+          chk[u] = false;
+          pl0[u] = pl1[u] = make_uint4(0u, 0u, 0u, 0u);
+          if (a < n_act) {
+            const int i = act_s[a];
+            const unsigned sw = (PAY && resident) ? slot_s[i] : (unsigned)p.slot_of[v0 + i];
+            const unsigned sl = PAY ? sw & 0x7fffffffu : sw;
+            if (PAY && !(sw >> 31)) {
+              chk[u] = true;
+              const uint4* src = reinterpret_cast<const uint4*>(pay + (size_t)sl * 8);
+              pl0[u] = __ldcg(src);
+              pl1[u] = __ldcg(src + 1);
             }
+            word[u] = __ldcg(&tab[sl]);
           }
-          if (!same) atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
         }
-        if (act[k]) {
-          if (PAY) {
-            if (r[k] == v) n_rep += 1u;
-          } else if (r[k] != v) {
-            bool same = (dv[k] == dr[k]) && (lo[k] == lr[k]);
-            if (same && dv[k] <= 8) {
-              int a[8], c[8];
 #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                a[j] = j < dv[k] ? (resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) : 0;
-                c[j] = j < dv[k] ? __ldcg(&sig_g[br[k] + j]) : 0;
+        for (int u = 0; u < 2; ++u) {
+          const int a = tid + (k0 + u) * WLF_THREADS;
+          const bool act = a < n_act;
+          const int i = act ? act_s[a] : 0;
+          const int v = v0 + i;
+          const int r = (int)(unsigned)word[u];
+          const bool sgl = act && ((word[u] >> 32) & 1ULL) && r == v;
+          unsigned long long fz = 0ULL;  // self-similarity contribution of a vertex that freezes now
+          const int gg = act ? gid_s[i] : -1;
+          if (act) {
+            // verification against the representative: CSR row and label of both sides, then the sorted labels
+            if (PAY) {
+              if (chk[u]) {  // compare with the installer's signature in the slot payload
+                int bv, d;
+                if (resident) { bv = rp_s[i]; d = rp_s[i + 1] - bv; }
+                else { bv = p.row_ptr[v]; d = p.row_ptr[v + 1] - bv; }
+                const int pn[6] = {(int)pl0[u].z, (int)pl0[u].w, (int)pl1[u].x, (int)pl1[u].y, (int)pl1[u].z, (int)pl1[u].w};
+                bool same = ((int)pl0[u].x == lab_s[i]) && ((int)pl0[u].y == d);
+                if (same) {
+                  const int nd = d > 6 ? 5 : d;
+#pragma unroll
+                  for (int j = 0; j < 6; ++j)
+                    if (j < nd) same = same && ((resident ? sig_s[bv + j] : sig_g[bv + j]) == pn[j]);
+                  if (d > 6) {
+                    const int off = pn[5];  // installer's row offset in sig_nbr
+                    for (int j = 5; same && j < d; ++j)
+                      same = (resident ? sig_s[bv + j] : sig_g[bv + j]) == __ldcg(&sig_g[off + j]);
+                  }
+                }
+                if (!same) atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
               }
+              if (r == v) n_rep += 1u;
+            } else if (r != v) {
+              int bv, dv;
+              if (resident) { bv = rp_s[i]; dv = rp_s[i + 1] - bv; }  // own side from shared memory (sig_s)
+              else { bv = p.row_ptr[v]; dv = p.row_ptr[v + 1] - bv; }
+              const int br = p.row_ptr[r], dr = p.row_ptr[r + 1] - br;
+              bool same = (dv == dr) && (lab_s[i] == __ldcg(&lab_in[r]));
+              if (same && dv <= 8) {
+                int x[8], c[8];
 #pragma unroll
-              for (int j = 0; j < 8; ++j) same = same && (a[j] == c[j]);
+                for (int j = 0; j < 8; ++j) {
+                  x[j] = j < dv ? (resident ? sig_s[bv + j] : sig_g[bv + j]) : 0;
+                  c[j] = j < dv ? __ldcg(&sig_g[br + j]) : 0;
+                }
+#pragma unroll
+                for (int j = 0; j < 8; ++j) same = same && (x[j] == c[j]);
+              } else {
+                for (int j = 0; same && j < dv; ++j)
+                  same = (resident ? sig_s[bv + j] : sig_g[bv + j]) == __ldcg(&sig_g[br + j]);
+              }
+              if (!same) atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
             } else {
-              for (int j = 0; same && j < dv[k]; ++j)
-                same = (resident ? sig_s[bv[k] + j] : sig_g[bv[k] + j]) == __ldcg(&sig_g[br[k] + j]);
+              n_rep += 1u;
             }
-            if (!same) atomicOr(&p.sc->collision, 1u << min(lv, 30));  // bit = level (error message / retry)
-          } else {
-            n_rep += 1u;
+            if (sgl) {  // a class of one vertex: frozen from this level on, one diagonal unit per remaining level
+              fz = (unsigned long long)(p.L - lv);
+              n_new += (unsigned)(p.L - lv);
+              n_fz += (unsigned)(p.L - lv);
+              mx = max(mx, 1u);
+            }
+            res_s[a] = r | (sgl ? (int)0x80000000u : 0);
           }
-          if (sgl[k]) {  // a class of one vertex: frozen from this level on, one diagonal unit per remaining level
-            fz = (unsigned long long)(p.L - lv);
-            n_new += (unsigned)(p.L - lv);
-            n_fz += (unsigned)(p.L - lv);
-            mx = max(mx, 1u);
-          }
-        } else if (i < nv) {
-          n_rep += 1u;  // a frozen vertex is a class of its own at every level
-        }
-        // per-graph aggregation of the frozen contributions (runs of equal graph inside the warp)
-        unsigned long long val = fz;
+          // per-graph aggregation of the frozen contributions (runs of equal graph inside the warp: the list ascends)
+          unsigned long long val = fz;
 #pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const unsigned long long y = __shfl_down_sync(0xffffffffu, val, d);
-          const int gy = __shfl_down_sync(0xffffffffu, gg, d);
-          if (lane + d < 32 && gy == gg) val += y;
-        }
-        const int gprev = __shfl_up_sync(0xffffffffu, gg, 1);
-        if (gg >= 0 && (lane == 0 || gprev != gg) && val) {
-          atomicAdd(&p.st.diag[gg], val);
-          atomicAdd(&p.diag_frozen[gg], val);
+          for (int d = 1; d < 32; d <<= 1) {
+            const unsigned long long y = __shfl_down_sync(0xffffffffu, val, d);
+            const int gy = __shfl_down_sync(0xffffffffu, gg, d);
+            if (lane + d < 32 && gy == gg) val += y;
+          }
+          const int gprev = __shfl_up_sync(0xffffffffu, gg, 1);
+          if (gg >= 0 && (lane == 0 || gprev != gg) && val) {
+            atomicAdd(&p.st.diag[gg], val);
+            atomicAdd(&p.diag_frozen[gg], val);
+          }
         }
       }
       WLF_STAMP(lv, 4);
-      __syncthreads();  // every thread has read the old labels / flags of the tile it needs
-#pragma unroll
-      for (int k = 0; k < WLF_VPT; ++k) {
-        const int i = tid + k * WLF_THREADS;
-        if (act[k]) {
-          lab_s[i] = r[k];
-          if (sgl[k]) { frz_s[i] = 1; p.frozen[v0 + i] = 1; }
+      __syncthreads();  // every thread has read the old labels of the tile it needs
+      // new labels of the live vertices; a vertex that freezes writes its own id for every deeper level now, so a
+      // frozen vertex is never visited again
+      for (int a = tid; a < n_act; a += WLF_THREADS) {
+        const int i = act_s[a], v = v0 + i, x = res_s[a], r = x & 0x7fffffff;
+        lab_s[i] = r;
+        lab_out[v] = r;
+        if (x < 0) {
+          frz_s[i] = 1;
+          p.frozen[v] = 1;
+          for (int l2 = lv + 1; l2 < p.L; ++l2) p.labels_all[(size_t)l2 * V + v] = v;
         }
       }
       __syncthreads();
-      for (int i = tid; i < nv; i += WLF_THREADS) lab_out[v0 + i] = lab_s[i];
       WLF_STAMP(lv, 5);
       wlf2_emit(p, v0, nv, lab_s, frz_s, gid_s, gbeg_s, gend_s, cf_s, ct, list_s, agg, level_base, (size_t)lv * V + v0, s_warp, mx, n_new);
     }
