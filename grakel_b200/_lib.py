@@ -83,6 +83,10 @@ _SYMBOLS = {
     "gk_rw_iterations": (C.c_int, [_P, _P]),
     "gk_sm_features": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_sm_counts": (C.c_int, [_P, C.c_int64, C.c_int64, _P]),
+    "gk_odd_features": (C.c_int, [_P, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_odd_info": (C.c_int, [_P, _P]),
+    "gk_odd_signatures": (C.c_int, [_P, _P, _P, _P, _P]),
+    "gk_selftest_odd_collision": (C.c_int, [_P, C.c_int32]),
     "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
@@ -451,6 +455,33 @@ class Engine:
         classes and every such attempt must detect a collision and be repeated."""
         with self._lock:
             self._check(self.lib.gk_selftest_wl_collision(self.h, int(attempts), int(from_level)))
+
+    def odd_features(self, h, rank):
+        """OddSth DAGs, identities and per-bit-plane count tables (gk_odd_features); h < 0: no depth limit."""
+        rk = _i32(rank)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_odd_features(self.h, int(h), _ptr(rk), 0, C.byref(st)))
+        return st
+
+    def odd_signatures(self):
+        """(label id, child offsets, child identity ids, C) of every identity after odd_features."""
+        info = np.zeros(3, dtype=np.int64)
+        with self._lock:
+            self._check(self.lib.gk_odd_info(self.h, _ptr(info)))
+            F, nch = int(info[0]), int(info[1])
+            label = np.empty(F, dtype=np.int32)
+            off = np.empty(F + 1, dtype=np.int64)
+            child = np.empty(max(nch, 1), dtype=np.int32)
+            Cf = np.empty(F, dtype=np.int32)
+            self._check(self.lib.gk_odd_signatures(self.h, _ptr(label), _ptr(off), _ptr(child), _ptr(Cf)))
+        return label, off, child[:nch], Cf
+
+    def selftest_odd_collision(self, attempts):
+        """Tests only: the next `attempts` identity passes of odd_features hash (label, child count) alone, so each
+        must detect a collision and be repeated."""
+        with self._lock:
+            self._check(self.lib.gk_selftest_odd_collision(self.h, int(attempts)))
 
     def nspd_features(self, r, d, sym_hash, edge_label, tokens):
         """NeighborhoodSubgraphPairwiseDistance hashes and per-level count tables (gk_nspd_features).  `tokens` is

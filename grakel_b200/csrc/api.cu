@@ -34,6 +34,7 @@
 #include "hadamard_code.cuh"
 #include "nspd.cuh"
 #include "subgraph_matching.cuh"
+#include "odd_sth.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -176,6 +177,10 @@ struct HandleExtra {
   // and columns; per graph, the mask of the distances it has pairs at
   std::vector<long long> nspd_off, nspd_cap, nspd_M, nspd_cols;
   std::vector<unsigned long long> nspd_mask;
+  // OddSth: node slots, child slots, identities; per bit plane of C, its table's byte offset in odd_blk, slots,
+  // entries and columns
+  long long odd_S = 0, odd_T = 0, odd_F = 0, odd_maxC = 0;
+  std::vector<long long> odd_off, odd_cap, odd_M, odd_cols;
 };
 static std::vector<std::pair<gk_handle*, HandleExtra*>> g_extra;
 static HandleExtra* extra_of(gk_handle* h) {
@@ -343,7 +348,9 @@ int gk_destroy(gk_handle* h) {
                         &h->pm_U, &h->pm_ncols, &h->pm_skip, &h->hc_S, &h->hc_z, &h->hc_skip,
                         &h->nspd_lvl, &h->nspd_q, &h->nspd_H, &h->nspd_aux, &h->nspd_ws, &h->nspd_pairs, &h->nspd_blk,
                         &h->nspd_tab, &h->nspd_keys, &h->nspd_C,
-                        &h->sm_rec, &h->sm_off, &h->sm_el, &h->sm_vtab, &h->sm_etab, &h->sm_lam, &h->sm_stack, &h->sm_ctl};
+                        &h->sm_rec, &h->sm_off, &h->sm_el, &h->sm_vtab, &h->sm_etab, &h->sm_lam, &h->sm_stack, &h->sm_ctl,
+                        &h->odd_aux, &h->odd_nodes, &h->odd_ch, &h->odd_tab, &h->odd_feat, &h->odd_phi, &h->odd_blk,
+                        &h->odd_ctl, &h->odd_diag};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1735,6 +1742,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_PM     */ {"PyramidMatch", false, true, false, false},
     /* FK_NSPD   */ {"NeighborhoodSubgraphPairwiseDistance", false, true, false, false},
     /* FK_SM     */ {"SubgraphMatching", false, true, false, false},
+    /* FK_ODD    */ {"OddSth", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -4212,6 +4220,361 @@ static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
   return GK_OK;
 }
 
+// ---------------------------------------------------------------------------
+// OddSth (odd_sth.cuh).  gk_odd_features builds every root's DAG and the identities of its nodes, repeating the
+// identity pass with another seed while a collision is detected, then counts phi per (graph, identity), C per
+// identity, the self similarities, and splits the counts into one NeighborhoodSubgraphPairwiseDistance-layout table per
+// bit of C.  odd_ctl: [collision | identities | entries of plane b (32) | columns of plane b (32)] u64.
+static NspdLevel odd_plane(gk_handle* h, int b) {
+  HandleExtra* ex = extra_of(h);
+  char* p = h->odd_blk.as<char>() + ex->odd_off[b];
+  const long long cap = ex->odd_cap[b], M = ex->odd_M[b];
+  NspdLevel L;
+  L.keys = reinterpret_cast<unsigned long long*>(p);
+  L.cnt = reinterpret_cast<unsigned*>(p + cap * 8);
+  L.colcnt = reinterpret_cast<unsigned*>(p + cap * 12);
+  L.diag = reinterpret_cast<unsigned long long*>(p + cap * 12 + ((M + 1) * 4 + 7) / 8 * 8);
+  L.part = reinterpret_cast<unsigned*>(L.diag + std::max<long long>(h->N, 1));
+  return L;
+}
+
+constexpr int ODD_CTL_WORDS = 2 + 32 + 32;
+constexpr int ODD_MAX_ATTEMPTS = 8;
+
+// Device views of the node records (S slots) and the per-identity arrays.
+struct OddNodes {
+  unsigned long long* key;
+  int *lab, *gr, *cb, *nc, *slot, *fid;
+  int *rep_of, *Cf, *colb;
+};
+
+static OddNodes odd_nodes(gk_handle* h) {
+  HandleExtra* ex = extra_of(h);
+  const size_t S1 = (size_t)std::max<long long>(ex->odd_S, 1);
+  OddNodes o;
+  o.key = h->odd_nodes.as<unsigned long long>();
+  o.lab = reinterpret_cast<int*>(o.key + S1);
+  o.gr = o.lab + S1; o.cb = o.gr + S1; o.nc = o.cb + S1; o.slot = o.nc + S1; o.fid = o.slot + S1;
+  o.rep_of = h->odd_feat.as<int>();
+  o.Cf = o.rep_of + S1; o.colb = o.Cf + S1;
+  return o;
+}
+
+extern "C" {
+
+int gk_selftest_odd_collision(gk_handle* h, int32_t attempts) {
+  if (!h || attempts < 0) return fail(GK_ERR_ARG, "gk_selftest_odd_collision: bad argument");
+  h->odd_degen = attempts;
+  return GK_OK;
+}
+
+int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_odd_features: no graphs packed");
+  if (!h->has_labels) return fail(GK_ERR_ARG, "gk_odd_features: vertex labels are required");
+  if (depth == 0) return fail(GK_ERR_ARG, "gk_odd_features: h must be > 0 (or < 0 for no limit)");
+  if (flags != 0) return fail(GK_ERR_ARG, "gk_odd_features: no flags are defined");
+  if (!rank && h->V) return fail(GK_ERR_ARG, "gk_odd_features: null rank table");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t N = h->N, V = h->V, E = h->E;
+  const int64_t launches0 = h->launches;
+  HandleExtra* ex = extra_of(h);
+  h->features_ready = false; h->feat_serial++;
+  const std::vector<int>& gp = ex->graph_ptr;
+  std::vector<long long> base(2 * (N + 1), 0);
+  long long* nbase = base.data();
+  long long* ebase = nbase + N + 1;
+  int max_n = 1;
+  for (int64_t g = 0; g < N; ++g) {
+    const long long n = gp[g + 1] - gp[g], m = ex->graph_eptr[g + 1] - ex->graph_eptr[g];
+    max_n = std::max<int>(max_n, (int)n);
+    nbase[g + 1] = nbase[g] + n * n;
+    ebase[g + 1] = ebase[g] + n * m;
+  }
+  if (max_n > ODD_MAX_N) return fail(GK_ERR_UNSUPPORTED, "gk_odd_features: a graph has more than 4096 vertices");
+  const long long S = nbase[N], T = ebase[N];
+  if (S >= (1LL << 30) || T >= (1LL << 30))
+    return fail(GK_ERR_UNSUPPORTED, "gk_odd_features: 2^30 or more (root, vertex) or (root, edge) pairs");
+  ex->odd_S = S; ex->odd_T = T; ex->odd_maxC = 0;
+  const size_t S1 = (size_t)std::max<long long>(S, 1), T1 = (size_t)std::max<long long>(T, 1);
+  const size_t cap = std::max<size_t>(next_pow2(S1 * 2), 1024);
+  GK_TRY(h->odd_aux.ensure(base.size() * 8 + (size_t)std::max<int64_t>(V, 1) * 4));
+  GK_TRY(h->odd_nodes.ensure(S1 * 32));
+  GK_TRY(h->odd_ch.ensure(T1 * 4));
+  GK_TRY(h->odd_tab.ensure(cap * 16));  // keys | representative | identity of the slot
+  GK_TRY(h->odd_feat.ensure(S1 * 12));
+  GK_TRY(h->odd_phi.ensure(cap * 12));
+  GK_TRY(h->odd_ctl.ensure(ODD_CTL_WORDS * 8));
+  GK_TRY(h->odd_diag.ensure((size_t)N * 8));
+  GK_CUDA(cudaMemcpyAsync(h->odd_aux.p, base.data(), base.size() * 8, cudaMemcpyHostToDevice, h->stream));
+  int* d_rank = reinterpret_cast<int*>(h->odd_aux.as<long long>() + base.size());
+  if (V) GK_CUDA(cudaMemcpyAsync(d_rank, rank, (size_t)V * 4, cudaMemcpyHostToDevice, h->stream));
+  const OddNodes o = odd_nodes(h);
+  unsigned long long* tab = h->odd_tab.as<unsigned long long>();
+  int* rep = reinterpret_cast<int*>(tab + cap);
+  int* colid = rep + cap;
+  unsigned long long* ctl = h->odd_ctl.as<unsigned long long>();
+  unsigned long long* phi_keys = h->odd_phi.as<unsigned long long>();
+  unsigned* phi_cnt = reinterpret_cast<unsigned*>(phi_keys + cap);
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+
+  // ---- DAGs and identities; repeated with another seed while a collision is detected
+  OddParams p;
+  p.N = (int)N; p.V = V;
+  p.graph_ptr = h->graph_ptr.as<int>(); p.row_ptr = h->row_ptr.as<int>(); p.col_idx = h->col_idx.as<int>();
+  p.vgraph = h->vgraph.as<int>(); p.labels = h->labels0.as<int>(); p.rank = d_rank;
+  p.node_base = h->odd_aux.as<long long>(); p.edge_base = p.node_base + N + 1;
+  p.depth = depth < 0 ? -1 : depth;
+  p.n_pad = (max_n + 3) / 4 * 4;
+  p.key = o.key; p.lab = o.lab; p.gr = o.gr; p.cb = o.cb; p.nc = o.nc; p.ch = h->odd_ch.as<int>();
+  const size_t warp_smem = (size_t)p.n_pad * ODD_SMEM_PER_V;
+  const int wpc = (int)std::max<size_t>(1, std::min<size_t>(ODD_MAX_WARPS, ((size_t)200 << 10) / warp_smem));
+  const size_t smem = warp_smem * wpc;
+  if (smem > (48 << 10))
+    GK_CUDA(cudaFuncSetAttribute(odd_dags, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv(std::max<int64_t>(V, 1), wpc), (int64_t)h->sm_count * 16));
+  int64_t retries = 0;
+  for (int attempt = 0;; ++attempt) {
+    if (attempt == ODD_MAX_ATTEMPTS)
+      return fail(GK_ERR_STATE, "gk_odd_features: identity hashes collided on every attempt");
+    p.seed = mix64(0x6f6464ULL + (unsigned long long)attempt * 0x9e3779b97f4a7c15ULL);
+    p.degenerate = h->odd_degen > 0 ? 1 : 0;
+    if (h->odd_degen > 0) h->odd_degen--;
+    GK_CUDA(cudaMemsetAsync(ctl, 0, 8, h->stream));
+    if (V) {
+      odd_dags<<<grid, wpc * 32, smem, h->stream>>>(p);
+      LAUNCH_CHECK(h);
+    }
+    GK_CUDA(cudaMemsetAsync(tab, 0xFF, cap * 8, h->stream));
+    GK_CUDA(cudaMemsetAsync(rep, 0x7F, cap * 4, h->stream));
+    if (S) {
+      odd_insert<<<cdiv(S, 256), 256, 0, h->stream>>>(S, o.key, o.lab, tab, rep, cap - 1, o.slot);
+      LAUNCH_CHECK(h);
+      odd_verify<<<cdiv(S, 256), 256, 0, h->stream>>>(S, o.lab, o.nc, o.cb, h->odd_ch.as<int>(), o.slot, rep,
+                                                       reinterpret_cast<unsigned*>(ctl));
+      LAUNCH_CHECK(h);
+    }
+    unsigned long long coll = 0;
+    GK_CUDA(cudaMemcpyAsync(&coll, ctl, 8, cudaMemcpyDeviceToHost, h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));
+    if (!coll) break;
+    ++retries;
+  }
+  GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
+
+  // ---- identities numbered, C, phi, self similarities, entries per bit plane
+  GK_CUDA(cudaMemsetAsync(ctl, 0, ODD_CTL_WORDS * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(o.Cf, 0, S1 * 4, h->stream));
+  GK_CUDA(cudaMemsetAsync(phi_keys, 0xFF, cap * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(phi_cnt, 0, cap * 4, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->odd_diag.p, 0, (size_t)N * 8, h->stream));
+  if (S) {
+    odd_number<<<cdiv(S, 256), 256, 0, h->stream>>>(S, o.lab, o.slot, rep, colid, o.rep_of, ctl + 1);
+    LAUNCH_CHECK(h);
+    odd_count<<<cdiv(S, 256), 256, 0, h->stream>>>(S, o.lab, o.gr, o.slot, colid, o.rep_of, o.fid,
+                                                   reinterpret_cast<unsigned*>(o.Cf), phi_keys, phi_cnt, cap - 1);
+    LAUNCH_CHECK(h);
+    odd_phi_stats<<<cdiv((long long)cap, 256), 256, 0, h->stream>>>(cap, phi_keys, phi_cnt,
+                                                                    reinterpret_cast<unsigned*>(o.Cf),
+                                                                    h->odd_diag.as<unsigned long long>(), ctl + 2);
+    LAUNCH_CHECK(h);
+  }
+  std::vector<unsigned long long> hc(ODD_CTL_WORDS);
+  GK_CUDA(cudaMemcpyAsync(hc.data(), ctl, ODD_CTL_WORDS * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  const long long F = (long long)hc[1];
+  ex->odd_F = F;
+  int B = 0;
+  for (int b = 0; b < 32; ++b)
+    if (hc[2 + b]) B = b + 1;
+  ex->odd_off.assign(B, 0); ex->odd_cap.assign(B, 0); ex->odd_M.assign(B, 0); ex->odd_cols.assign(B, 0);
+  size_t blk = 0;
+  for (int b = 0; b < B; ++b) {
+    const long long M = (long long)hc[2 + b];
+    ex->odd_M[b] = M;
+    ex->odd_cap[b] = (long long)std::max<size_t>(next_pow2((size_t)std::max<long long>(M, 1) * 2), 1024);
+    ex->odd_off[b] = (long long)blk;
+    blk += nspd_level_bytes(ex->odd_cap[b], M, N);
+  }
+  GK_TRY(h->odd_blk.ensure(std::max<size_t>(blk, 256)));
+  if (blk) GK_CUDA(cudaMemsetAsync(h->odd_blk.p, 0, blk, h->stream));
+  for (int b = 0; b < B; ++b) {
+    const NspdLevel L = odd_plane(h, b);
+    const size_t pcap = (size_t)ex->odd_cap[b];
+    GK_CUDA(cudaMemsetAsync(L.keys, 0xFF, pcap * 8, h->stream));
+    if (!ex->odd_M[b]) continue;
+    odd_plane_cols<<<cdiv(F, 256), 256, 0, h->stream>>>((int)F, reinterpret_cast<unsigned*>(o.Cf), b, o.colb, ctl + 34 + b);
+    LAUNCH_CHECK(h);
+    odd_plane_fill<<<cdiv((long long)cap, 256), 256, 0, h->stream>>>(cap, phi_keys, phi_cnt, reinterpret_cast<unsigned*>(o.Cf),
+                                                                     b, o.colb, L.keys, L.cnt, pcap - 1);
+    LAUNCH_CHECK(h);
+    nspd_level_stats<<<cdiv((long long)pcap, 256), 256, 0, h->stream>>>(pcap, L.keys, L.cnt, L.colcnt, L.diag, L.part);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_CUDA(cudaMemcpyAsync(hc.data() + 34, ctl + 34, 32 * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  for (int b = 0; b < B; ++b) ex->odd_cols[b] = (long long)hc[34 + b];
+  h->n_columns = F;
+  h->features_ready = true; h->feat_serial++;
+  h->feature_kind = FK_ODD;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
+    stats->n_levels = B;
+    for (int b = 0; b < B; ++b) stats->level_dims[b] = ex->odd_cols[b];
+    stats->n_columns = F;
+    stats->n_entries = S;
+    stats->hash_retries = retries;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_features = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_hash = ev_ms(h->tev[2], h->tev[6]);
+    stats->ms_columns = ev_ms(h->tev[6], h->tev[3]);
+  }
+  return GK_OK;
+}
+
+// The signature of every identity, from its representative node: label id, children's identities in order, C.
+static int odd_host_signatures(gk_handle* h, std::vector<int>* label, std::vector<int64_t>* off, std::vector<int>* child,
+                               std::vector<int>* C) {
+  if (h->feature_kind != FK_ODD || !h->features_ready) return fail(GK_ERR_STATE, "gk_odd_signatures: run gk_odd_features first");
+  GK_CUDA(cudaSetDevice(h->dev));
+  HandleExtra* ex = extra_of(h);
+  const long long S = ex->odd_S, T = ex->odd_T, F = ex->odd_F;
+  const OddNodes o = odd_nodes(h);
+  std::vector<int> lab(S), cb(S), nc(S), fid(S), ch(T), rep_of(F);
+  C->resize(F);
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  if (S) {
+    GK_CUDA(cudaMemcpy(lab.data(), o.lab, S * 4, cudaMemcpyDeviceToHost));
+    GK_CUDA(cudaMemcpy(cb.data(), o.cb, S * 4, cudaMemcpyDeviceToHost));
+    GK_CUDA(cudaMemcpy(nc.data(), o.nc, S * 4, cudaMemcpyDeviceToHost));
+    GK_CUDA(cudaMemcpy(fid.data(), o.fid, S * 4, cudaMemcpyDeviceToHost));
+  }
+  if (T) GK_CUDA(cudaMemcpy(ch.data(), h->odd_ch.p, T * 4, cudaMemcpyDeviceToHost));
+  if (F) {
+    GK_CUDA(cudaMemcpy(rep_of.data(), o.rep_of, F * 4, cudaMemcpyDeviceToHost));
+    GK_CUDA(cudaMemcpy(C->data(), o.Cf, F * 4, cudaMemcpyDeviceToHost));
+  }
+  label->resize(F);
+  off->assign(F + 1, 0);
+  child->clear();
+  for (long long f = 0; f < F; ++f) {
+    const int r = rep_of[f];
+    (*label)[f] = lab[r];
+    for (int k = 0; k < nc[r]; ++k) child->push_back(fid[ch[cb[r] + k]]);
+    (*off)[f + 1] = (int64_t)child->size();
+  }
+  return GK_OK;
+}
+
+int gk_odd_info(gk_handle* h, int64_t* info3) {
+  if (!h || !info3) return fail(GK_ERR_ARG, "gk_odd_info: null argument");
+  std::vector<int> label, child, C;
+  std::vector<int64_t> off;
+  GK_TRY(odd_host_signatures(h, &label, &off, &child, &C));
+  info3[0] = (int64_t)label.size();
+  info3[1] = (int64_t)child.size();
+  info3[2] = C.empty() ? 0 : *std::max_element(C.begin(), C.end());
+  return GK_OK;
+}
+
+int gk_odd_signatures(gk_handle* h, int32_t* label, int64_t* child_off, int32_t* child, int32_t* C) {
+  if (!h || !label || !child_off || !C) return fail(GK_ERR_ARG, "gk_odd_signatures: null argument");
+  std::vector<int> lb, ch, c;
+  std::vector<int64_t> off;
+  GK_TRY(odd_host_signatures(h, &lb, &off, &ch, &c));
+  if (!lb.empty()) {
+    memcpy(label, lb.data(), lb.size() * 4);
+    memcpy(C, c.data(), c.size() * 4);
+  }
+  memcpy(child_off, off.data(), off.size() * 8);
+  if (!ch.empty()) {
+    if (!child) return fail(GK_ERR_ARG, "gk_odd_signatures: null child array");
+    memcpy(child, ch.data(), ch.size() * 4);
+  }
+  return GK_OK;
+}
+
+}  // extern "C"
+
+// Gram of OddSth (gram_path 14): per bit plane b of C, the exact integer Gram G_b of its count table as fp64 counts,
+// folded into K as 2^b G_b (one count matrix live), so K = sum_f C[f] phi_i[f] phi_j[f] exactly below 2^53.  The self
+// similarities d (sum_f C[f] phi[f]^2, u64 from the feature pass) give GK_NORMALIZE's K / sqrt(d_i d_j) and xdiag /
+// ydiag.  Rows go in chunks when one plane's count matrix of the whole request would exceed 8 GiB
+// (GRAKEL_B200_ODD_C_BUDGET=<bytes> lowers it).
+static int gram_odd(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
+  const int B = (int)ex->odd_M.size();
+  const int64_t launches0 = h->launches;
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  const int64_t ldc = (k_cols + 7) / 8 * 8;
+  size_t c_budget = (size_t)8 << 30;
+  if (const char* e = getenv("GRAKEL_B200_ODD_C_BUDGET")) c_budget = std::max<size_t>(1, strtoull(e, nullptr, 10));
+  const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(std::max<int64_t>(k_rows, 1), (int64_t)(c_budget / ((size_t)ldc * 8))));
+  GK_TRY(h->nh_C.ensure((size_t)chunk * ldc * 8));
+  double* C = h->nh_C.as<double>();
+  const int32_t gflags = (q.flags & (GK_GRAM_SIMT | GK_DENSE_ALL)) | GK_FULL_TILES | GK_OUT_DEVICE;
+  std::vector<float> ms_plane(64, 0.f);
+  float ms_fold = 0.f;
+  int64_t max_T = 0, gram_launches = 0, elem_bytes = 0, max_count = 0;
+  for (int64_t cb = q.row_begin; cb < q.row_end; cb += chunk) {
+    const int64_t ce = std::min<int64_t>(q.row_end, cb + chunk), rows = ce - cb;
+    double* o = out.p + (size_t)(cb - q.row_begin) * out.ld;
+    GK_CUDA(cudaMemset2DAsync(o, (size_t)out.ld * 8, 0, (size_t)k_cols * 8, (size_t)rows, h->stream));
+    for (int b = 0; b < B; ++b) {
+      if (!ex->odd_M[b]) continue;
+      const NspdLevel L = odd_plane(h, b);
+      IntBlock fb;
+      fb.keys = L.keys; fb.cnt = L.cnt; fb.cap = (size_t)ex->odd_cap[b];
+      fb.colcnt = L.colcnt; fb.col_cap = ex->odd_M[b] + 1; fb.n_columns = ex->odd_cols[b];
+      fb.diag = L.diag; fb.part_max = L.part; fb.part_new = L.part + 1; fb.n_part = 1;
+      fb.prologue_on_host = false;
+      GramReq lq;
+      GK_TRY(gram_request(h, FK_WL, n_fit, gflags, cb, ce, C, GK_F64, ldc, nullptr, nullptr, &lq));
+      gk_stats st;
+      memset(&st, 0, sizeof(st));
+      GK_TRY(gram_int(h, lq, fb, &st));
+      ms_plane[b] += st.ms_total;
+      max_T = std::max<int64_t>(max_T, st.threshold);
+      max_count = std::max<int64_t>(max_count, st.max_count);
+      gram_launches += st.gemm_launches;
+      elem_bytes = std::max<int64_t>(elem_bytes, st.gemm_elem_bytes);
+      if (rows > 0) {
+        GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+        odd_fold<<<cdiv(rows * k_cols, 256), 256, 0, h->stream>>>((int)rows, (int)k_cols, C, ldc, b, o, out.ld);
+        LAUNCH_CHECK(h);
+        GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+        GK_CUDA(cudaEventSynchronize(h->tev[1]));
+        ms_fold += ev_ms(h->tev[0], h->tev[1]);
+      }
+    }
+  }
+  // gram_int left its planes' self similarities in diag_f64: replace them with d
+  GK_TRY(h->diag_f64.ensure((size_t)N * 8));
+  odd_diag_f64<<<cdiv(N, 256), 256, 0, h->stream>>>((int)N, h->odd_diag.as<unsigned long long>(), h->diag_f64.as<double>());
+  LAUNCH_CHECK(h);
+  GK_TRY(f64_deliver(h, q, out, true, h->ev[14], h->ev[15]));
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->n_levels = B;
+    stats->gram_path = 14;
+    stats->threshold = max_T;
+    stats->max_count = max_count;
+    stats->gemm_launches = gram_launches + (h->launches - launches0);
+    stats->gemm_elem_bytes = elem_bytes;
+    float tot = ms_fold;
+    for (int b = 0; b < B && b < 64; ++b) { stats->ms_level_gram[b] = ms_plane[b]; tot += ms_plane[b]; }
+    stats->ms_gemm = tot - ms_fold;
+    stats->ms_combine = ms_fold;
+    stats->ms_d2h = ev_ms(h->ev[14], h->ev[15]);
+    stats->ms_total = tot + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
 extern "C" {
 
 int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
@@ -4229,6 +4592,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_NSPD: return gram_nspd(h, q, stats);
     case FK_RW: return gram_rw(h, q, stats);
     case FK_SM: return gram_sm(h, q, stats);
+    case FK_ODD: return gram_odd(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }
 }

@@ -125,6 +125,7 @@ enum FeatureKind : int {
   FK_PM = 8,      // PyramidMatch per-level expanded blocks (the NeighborhoodHash layout)
   FK_NSPD = 9,    // NeighborhoodSubgraphPairwiseDistance per-(radius, distance) count tables
   FK_SM = 10,     // SubgraphMatching per-graph bitset records
+  FK_ODD = 11,    // OddSth per-bit-plane (graph, identity) count tables
 };
 
 }  // namespace gk
@@ -262,6 +263,12 @@ struct gk_handle {
   int sm_k = 0, sm_kk = 1, sm_kv = 0, sm_ke = 0, sm_n_vl = 0, sm_n_el = 0;
   int sm_max_und = 0;  // largest number of distinct out- or in-neighbours of a packed vertex
   bool sm_exact = true;
+
+  // ---- OddSth (FK_ODD): graph offsets and label ranks, node records [S] (hash | label | graph | first child | child
+  // count | slot | identity), children [T], the interning table, per-identity arrays (representative | C | plane
+  // column), the (graph, identity) counts, the bit-plane tables, counters, self similarities
+  gk::DevBuf odd_aux, odd_nodes, odd_ch, odd_tab, odd_feat, odd_phi, odd_blk, odd_ctl, odd_diag;
+  int odd_degen = 0;  // gk_selftest_odd_collision: degenerate identity passes still to come
 
   // ---- Propagation (FK_PK): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
   // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]

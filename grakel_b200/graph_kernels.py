@@ -35,7 +35,7 @@ from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
 from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, NeighborhoodSubgraphPairwiseDistance,
-                      Propagation, PropagationAttr, PyramidMatch,
+                      OddSth, Propagation, PropagationAttr, PyramidMatch,
                       ShortestPath, SubgraphMatching, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
@@ -43,7 +43,7 @@ default_n_components = 100
 # reference names outside the hot path (graph_kernels.py:38-64)
 _OUTSIDE = frozenset((
     "random_walk", "RW", "graphlet_sampling", "GR", "multiscale_laplacian", "ML",
-    "lovasz_theta", "LOVT", "svm_theta", "SVMT", "odd_sth", "ODD"))
+    "lovasz_theta", "LOVT", "svm_theta", "SVMT"))
 
 
 def _propagation(params):
@@ -66,6 +66,7 @@ for _names, _framework, _build in (
         (("neighborhood_subgraph_pairwise_distance", "NSPD"), False,
          lambda p: (NeighborhoodSubgraphPairwiseDistance, p)),
         (("subgraph_matching", "SM"), False, lambda p: (SubgraphMatching, p)),
+        (("odd_sth", "ODD"), False, lambda p: (OddSth, p)),
         (("propagation", "PR"), False, _propagation),
         (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),

@@ -3191,3 +3191,163 @@ class SubgraphMatching(Kernel):
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
+
+
+# ------------------------------------------------------------------------------
+_ODD_ELEMENT_MSG = ("each element of X must have either a graph with labels for node and edge or 3 elements consisting "
+                    "of a graph type object, labels for vertices and labels for edges.")
+
+
+def _value_ranks(values):
+    """Dense ranks of `values` by Python's `<` (equal values share a rank): the order the reference's stable
+    `q.sort(key=label)` puts them in."""
+    uniq = sorted(set(values))
+    at = {}
+    r = -1
+    for i, v in enumerate(uniq):
+        if i == 0 or uniq[i - 1] < v:
+            r += 1
+        at[v] = r
+    return [at[v] for v in values]
+
+
+def odd_label_tables(labels, graph_ptr):
+    """(label id of every vertex: one per distinct str(label), in first-seen order; rank of its value within its
+    graph; the distinct strings).  A label whose str has '(', ',' or ')' raises NotImplementedError: the reference's
+    identity strings could then be equal for different trees.  Labels of one graph that cannot be compared raise
+    TypeError."""
+    strs = [str(l) for l in labels]
+    ids_of = {}
+    ids = np.fromiter((ids_of.setdefault(s, len(ids_of)) for s in strs), dtype=np.int32, count=len(strs))
+    for s in ids_of:
+        if "(" in s or "," in s or ")" in s:
+            raise NotImplementedError("OddSth: the label %r contains '(', ',' or ')', so the reference's subtree "
+                                      "strings are ambiguous for it" % s)
+    try:
+        rank = _value_ranks(labels)  # one order for all graphs: only the order within a graph matters
+    except TypeError:
+        rank = []
+        gp = np.asarray(graph_ptr, dtype=np.int64)
+        for g in range(len(gp) - 1):
+            rank.extend(_value_ranks(labels[gp[g]:gp[g + 1]]))
+    return ids, np.asarray(rank, dtype=np.int32), list(ids_of)
+
+
+class OddSth(Kernel):
+    """ODD-ST_h kernel (odd_sth.py; Da San Martino et al. 2012).  Every vertex v of a graph roots a DAG: the BFS from
+    v over the out-neighbours, cut at depth h, ordered by Kahn's algorithm that pops the least (label value,
+    insertion sequence).  A DAG node's identity is str(label) + "(" + its children's identities in ascending
+    ordering + ")"; phi[f, g] counts the (root, node) pairs of graph g with identity f, and
+    K[i, j] = sum_f C[f] phi[f, i] phi[f, j] with C[f] = phi[f, g0] for the first graph g0 that has f (the reference's
+    `big_dag_append(..., merge_features=False)` keeps that graph's frequency).  The DAGs, the identities (hashed,
+    verified and interned without building a string) and the exact integer Gram run on the device; K equals the
+    reference's with ==.
+
+    Vertices are the indices of an adjacency matrix or the symbols that occur in an edge of an edge dictionary; a
+    vertex's neighbours come in ascending column order or in the order the edges were first listed, as in the
+    reference's edge dictionary, and that order is part of the result.  Edge labels are ignored.  Labels are compared
+    by value for the order and by str for the identity (1 and 1.0 tie in the order but are different features).  As
+    in the reference, `transform` with normalize=True after `fit` (not `fit_transform`) raises AttributeError, and
+    `diagonal()` is only defined after `transform`.  Deviations: a label whose str contains '(', ',' or ')', a graph
+    of more than 4096 vertices, 2^30 or more (root, vertex) or (root, edge) pairs and a datasets.read_tu block (its
+    edge sets carry no neighbour order) raise NotImplementedError; labels of one graph that cannot be compared raise
+    TypeError."""
+
+    _graph_format = "dictionary"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, h=None):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.h = h
+        self._initialized.update({"h": False})
+
+    def initialize(self):
+        """odd_sth.py:60-72."""
+        if not self._initialized["n_jobs"]:
+            if self.n_jobs is not None:
+                warnings.warn("no implemented parallelization for OddSth")
+            self._initialized["n_jobs"] = True
+        if not self._initialized["h"]:
+            if self.h is not None and (type(self.h) is not int or self.h <= 0):
+                raise ValueError("h must be an integer bigger than zero")
+            self.h_ = -1 if self.h is None else self.h
+            self._initialized["h"] = True
+
+    def parse_input(self, X):
+        """odd_sth.py:74-127: the element checks, then the graphs packed with the edge dictionary's neighbour order."""
+        if isinstance(X, Block):
+            raise NotImplementedError("OddSth: a datasets.read_tu block does not carry the neighbour order of the "
+                                      "reference's edge sets, which the result depends on; pass the list of graphs")
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        els = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            if is_iter and len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            if not (is_iter and len(x) >= 2):
+                raise TypeError(_ODD_ELEMENT_MSG)
+            if type(x[0]) is dict and x[0] and all(type(d) is list for d in x[0].values()) and not all(x[0].values()):
+                # {u: []}: u is a vertex without an edge-dictionary entry (graph.py:849-855)
+                raise ValueError("vertex not inside edge dictionary")
+            els.append([x[0], x[1]])
+        if not els:
+            raise ValueError("parsed input is empty")
+        block = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
+                     keep_edge_order=True)
+        ids, rank, strings = odd_label_tables(block.labels, block.graph_ptr)
+        out = Fitted(block, ids, strings)
+        out.rank = rank
+        return out
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self.fit(X)
+        K, xd, _ = self._odd_run(self.X.block, self.X.ids, self.X.rank, self.X.block.n_graphs)
+        self._X_diag = xd
+        return K
+
+    def transform(self, X):
+        """odd_sth.py:176-225: the fitted and the new graphs' identities in one dictionary, C from the first graph
+        that has each identity (a fitted one for every identity that reaches K)."""
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("transform input cannot be None")
+        Y = self.parse_input(X)
+        if self.normalize and getattr(self, "_X_diag", None) is None:
+            # diagonal() of the reference reads self._phi_X, which it never sets
+            raise AttributeError("'OddSth' object has no attribute '_phi_X'")
+        # one label id per distinct str over both sides; ranks only order labels within a graph
+        at = {s: i for i, s in enumerate(self.X.dictionary)}
+        y_ids = np.array([at.setdefault(s, len(at)) for s in Y.dictionary], dtype=np.int32)[Y.ids]
+        K, _, yd = self._odd_run(Block.concat(self.X.block, Y.block), np.concatenate([self.X.ids, y_ids]),
+                                 np.concatenate([self.X.rank, Y.rank]), self.X.block.n_graphs)
+        self._Y_diag = yd.reshape(-1, 1)
+        self._is_transformed = True
+        return K
+
+    def diagonal(self):
+        """odd_sth.py:227-255: (X diagonal, Y diagonal as a column) after `transform`."""
+        check_is_fitted(self, ["_Y_diag"])
+        if getattr(self, "_X_diag", None) is None:
+            raise AttributeError("'OddSth' object has no attribute '_phi_X'")
+        return self._X_diag, self._Y_diag
+
+    def _odd_run(self, block, ids, rank, n_fit, want_matrix=True, device_ptr=None, row_range=None):
+        """pack -> gk_odd_features (DAGs, identities, bit-plane tables) -> gk_gram (gram_path 14)."""
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
+            self.stats_ = eng.odd_features(self.h_, rank)
+            K, xd, yd = eng.gram(block.n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 out=None if want_matrix else False, device_ptr=device_ptr, row_range=row_range,
+                                 stats=self.stats_)
+            if getattr(self, "_keep_signatures", False):  # tests: the identities' signatures
+                self.signatures_ = eng.odd_signatures()
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd

@@ -108,7 +108,9 @@ typedef struct gk_stats {
                                 NeighborhoodHash: 7 = one exact integer Gram per level + the fp64 combine,
                                 random walk: 8 = conjugate gradients, 9 = spectral pair sum, 10 = power series,
                                 PyramidMatch: 11 = one exact integer Gram per level + the fp64 combine,
-                                NeighborhoodSubgraphPairwiseDistance: 12 = one exact integer Gram per level + the fp64 fold */
+                                NeighborhoodSubgraphPairwiseDistance: 12 = one exact integer Gram per level + the fp64 fold,
+                                SubgraphMatching: 13 = per-pair clique counts + the lambda fold,
+                                OddSth: 14 = one exact integer Gram per bit of C + the fp64 sum of 2^b G_b */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -272,6 +274,30 @@ int gk_rw_iterations(gk_handle* h, uint8_t* out);
 int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double* vtable, int32_t n_vlabels,
                    const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags, gk_stats* stats);
 int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out);
+
+/* OddSth (odd_sth.py), one warp per root vertex.  The packed CSR lists every vertex's out-neighbours in the reference's
+ * edge-dictionary order (every packed vertex is a root), the packed labels are one id per distinct str(label), and
+ * rank[V] orders the label values within each graph (equal values share a rank).  Root v's DAG is the BFS from v cut
+ * at depth h (h < 0: no limit), ordered by Kahn's algorithm with the (rank, insertion sequence) priority; every DAG
+ * node's subtree identity is interned exactly (hash, verification of (label id, child identities), and a repeat with
+ * another seed on a detected collision: stats->hash_retries).  phi[f, g] counts the (root, node) pairs of graph g with
+ * identity f, and C[f] = phi[f, g0] for the first graph g0 that has f.  gk_gram (gram_path 14) returns
+ * K[i, j] = sum_f C[f] phi[f, i] phi[f, j] exactly in fp64 (one exact integer Gram per bit of C, summed as
+ * sum_b 2^b G_b), with K / sqrt(d_i d_j) under GK_NORMALIZE and xdiag / ydiag = d.  In a transform (n_fit < N) the
+ * transformed graphs' identities take part in numbering and in d, as in the reference.  gk_gram: fp64 only, host or
+ * GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges; GK_DIST and row maps are GK_ERR_UNSUPPORTED.
+ * GK_ERR_UNSUPPORTED also for a graph of more than 4096 vertices and for 2^30 or more (root, vertex) or (root, edge)
+ * pairs (sum of n^2, sum of n m).  h == 0 is GK_ERR_ARG.  flags must be 0.  stats: n_columns = identities,
+ * n_levels = bit planes of C, level_dims = columns per plane, n_entries = node slots (sum of n^2), hash_retries,
+ * ms_hash (DAGs and identities), ms_columns.
+ * gk_odd_info writes [identities, child ids of all signatures, largest C]; gk_odd_signatures the signature of every
+ * identity (label[F], child_off[F + 1], child[child_off[F]] identity ids in order, C[F]). */
+int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t flags, gk_stats* stats);
+int gk_odd_info(gk_handle* h, int64_t* info3);
+int gk_odd_signatures(gk_handle* h, int32_t* label, int64_t* child_off, int32_t* child, int32_t* C);
+/* Tests only: the next `attempts` identity passes of gk_odd_features hash (label id, number of children) alone, so
+ * only the verification separates identities and every such pass must detect a collision and be repeated. */
+int gk_selftest_odd_collision(gk_handle* h, int32_t attempts);
 
 /* Propagation / PropagationAttr (propagation.py:27-689).  The packed CSR (gk_pack_csr without weights; with the
  * label ids for the labelled kernel) is the sparsity pattern of every graph's row-normalised transition matrix T,
