@@ -87,6 +87,10 @@ _SYMBOLS = {
     "gk_odd_info": (C.c_int, [_P, _P]),
     "gk_odd_signatures": (C.c_int, [_P, _P, _P, _P, _P]),
     "gk_selftest_odd_collision": (C.c_int, [_P, C.c_int32]),
+    "gk_ml_begin": (C.c_int, [_P, C.c_int32, C.c_double, C.c_double, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_ml_project": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.POINTER(GkStats)]),
+    "gk_ml_level": (C.c_int, [_P, C.c_int32, _P, C.c_int32, _P, _P, _P, C.POINTER(GkStats)]),
+    "gk_ml_finish": (C.c_int, [_P, _P, C.c_int64, _P, C.POINTER(GkStats)]),
     "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
@@ -384,6 +388,54 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_sm_counts(self.h, int(n_fit), int(row), _ptr(out)))
         return out
+
+    def ml_begin(self, L, gamma, heta, phi):
+        """MultiscaleLaplacian: adjacency, balls and level-0 features phi [V, dim] of the packed block (gk_ml_begin)."""
+        ph = np.ascontiguousarray(phi, dtype=np.float64)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_ml_begin(self.h, int(L), float(gamma), float(heta), _ptr(ph), ph.shape[1],
+                                             C.byref(st)))
+        return st
+
+    def ml_project(self, Q):
+        """features <- features Q (gk_ml_project)."""
+        q = np.ascontiguousarray(Q, dtype=np.float64)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_ml_project(self.h, _ptr(q), q.shape[0], q.shape[1], C.byref(st)))
+        return st
+
+    def ml_level(self, level, width, samples=None, samp_rec=None):
+        """Vertex records of `level` and the projection against its sample records (gk_ml_level).  Fit: `samples`
+        (packed vertex ids) -> (sample records, ns x ns block, stats); transform: `samp_rec` -> (None, None, stats).
+        `width` is the current feature width P'."""
+        st = GkStats()
+        stride = width * width + 1
+        if samples is not None:
+            ids = _i32(samples)
+            ns = len(ids)
+            rec = np.empty((ns, stride), dtype=np.float64)
+            kss = np.empty((ns, ns), dtype=np.float64)
+            with self._lock:
+                self._check(self.lib.gk_ml_level(self.h, int(level), _ptr(ids), ns, None, _ptr(rec), _ptr(kss),
+                                                 C.byref(st)))
+            return rec, kss, st
+        sr = np.ascontiguousarray(samp_rec, dtype=np.float64)
+        assert sr.shape[1] == stride
+        with self._lock:
+            self._check(self.lib.gk_ml_level(self.h, int(level), None, sr.shape[0], _ptr(sr), None, None, C.byref(st)))
+        return None, None, st
+
+    def ml_finish(self, width, fit_rec=None, want_records=True):
+        """Final records of the packed graphs after the fitted ones `fit_rec` (gk_ml_finish): (records or None, stats)."""
+        fr = None if fit_rec is None else np.ascontiguousarray(fit_rec, dtype=np.float64)
+        out = np.empty((self.n_graphs, width * width + 1), dtype=np.float64) if want_records else None
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_ml_finish(self.h, _ptr(fr), 0 if fr is None else fr.shape[0], _ptr(out),
+                                              C.byref(st)))
+        return out, st
 
     def pk_features(self, t_max, w, u, b, dim, dim_orig, n_fit, t_values, p0=None, flags=0):
         """Propagation bins of t_max levels and their (graph, column) counts (gk_pk_features).  u: [t_max, dim],

@@ -35,6 +35,7 @@
 #include "nspd.cuh"
 #include "subgraph_matching.cuh"
 #include "odd_sth.cuh"
+#include "multiscale_laplacian.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -350,7 +351,9 @@ int gk_destroy(gk_handle* h) {
                         &h->nspd_tab, &h->nspd_keys, &h->nspd_C,
                         &h->sm_rec, &h->sm_off, &h->sm_el, &h->sm_vtab, &h->sm_etab, &h->sm_lam, &h->sm_stack, &h->sm_ctl,
                         &h->odd_aux, &h->odd_nodes, &h->odd_ch, &h->odd_tab, &h->odd_feat, &h->odd_phi, &h->odd_blk,
-                        &h->odd_ctl, &h->odd_diag};
+                        &h->odd_ctl, &h->odd_diag,
+                        &h->ml_adj, &h->ml_adj_off, &h->ml_ball, &h->ml_U, &h->ml_U2, &h->ml_vrec, &h->ml_samp, &h->ml_rec,
+                        &h->ml_aux, &h->ml_ctl};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -426,6 +429,7 @@ int gk_pack_csr(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const 
   h->feature_kind = FK_NONE;
   h->n_rows = 0;  // a new block starts without a row map
   h->hc_W = 0;    // ... and without HadamardCode vectors
+  h->ml_w = 0;    // ... and without MultiscaleLaplacian features
   HandleExtra* ex = extra_of(h);
   ex->wl_tiles_valid = false;
   ex->graph_ptr.assign(graph_ptr, graph_ptr + N + 1);
@@ -1743,6 +1747,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_NSPD   */ {"NeighborhoodSubgraphPairwiseDistance", false, true, false, false},
     /* FK_SM     */ {"SubgraphMatching", false, true, false, false},
     /* FK_ODD    */ {"OddSth", false, true, false, false},
+    /* FK_ML     */ {"MultiscaleLaplacian", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -1750,7 +1755,8 @@ static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t f
                         GramReq* q) {
   const GramRules& r = GRAM_RULES[kind];
   if (out_dtype != GK_F32 && out_dtype != GK_F64) return fail(GK_ERR_ARG, "gk_gram: bad out_dtype");
-  const int64_t N = h->n_rows > 0 ? h->n_rows : h->N;
+  // MultiscaleLaplacian's rows are its records: the fitted graphs' (kept from the fit) and then the packed ones
+  const int64_t N = h->n_rows > 0 ? h->n_rows : kind == FK_ML ? h->ml_nrec : h->N;
   if (n_fit <= 0 || n_fit > N) return fail(GK_ERR_ARG, "gk_gram: n_fit out of range");
   const bool dist = (flags & (GK_DIST | GK_DIST_GATHER)) != 0;
   if (h->n_rows > 0 && !r.row_map) return fail(GK_ERR_UNSUPPORTED, std::string("gk_gram: row map with ") + r.name + " features");
@@ -4575,6 +4581,302 @@ static int gram_odd(gk_handle* h, const GramReq& q, gk_stats* stats) {
   return GK_OK;
 }
 
+// ---------------------------------------------------------------------------
+// MultiscaleLaplacian (multiscale_laplacian.cuh).  A staged pipeline, because the reference's eigen-decompositions
+// of the sampled blocks run on the host between the levels:
+//   gk_ml_begin    dense adjacency, radius-l balls and the attributes of the packed block (the level-0 features)
+//   gk_ml_project  U <- U Q (phi ksi at level 0, K_proj Q after each level)
+//   gk_ml_level    every vertex's record at level l, the projection block against the level's sample records
+//   gk_ml_finish   every graph's final record, appended to the fitted graphs' records for gk_gram (gram_path 15)
+static int ml_check_err(gk_handle* h) {
+  unsigned err = 0;
+  GK_CUDA(cudaMemcpyAsync(&err, h->ml_ctl.p, 4, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  if (err & 2u) return fail(GK_ERR_UNSUPPORTED, "MultiscaleLaplacian: a non-symmetric adjacency matrix");
+  if (err & 1u) return fail(GK_ERR_RANGE, "MultiscaleLaplacian: a Cholesky factorisation met a non-positive pivot");
+  return GK_OK;
+}
+
+static size_t ml_unit_smem(int mcap, int P) {
+  return ((size_t)std::max(mcap * mcap, P * P) + (size_t)mcap * P + (size_t)P * P) * 8;
+}
+
+// Records of n_units units (vertices with `ball`, else graphs) from the current features, into `rec`.
+static int ml_records(gk_handle* h, const unsigned long long* ball, int dup_loops, int mcap, int n_units, double* rec) {
+  if (n_units <= 0) return GK_OK;
+  MlUnits p;
+  p.graph_ptr = h->graph_ptr.as<int>(); p.vgraph = h->vgraph.as<int>();
+  p.adj_off = h->ml_adj_off.as<long long>(); p.adj = h->ml_adj.as<double>();
+  p.ball = ball; p.dup_loops = dup_loops;
+  p.U = h->ml_U.as<double>(); p.P = h->ml_w;
+  p.gamma = h->ml_gamma; p.heta = h->ml_heta;
+  p.n_units = n_units; p.rec = rec;
+  p.err = h->ml_ctl.as<unsigned>();
+  const size_t smem = ml_unit_smem(mcap, h->ml_w);
+  GK_CUDA(cudaFuncSetAttribute(ml_vertex_C, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 0;
+  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ml_vertex_C, ML_THREADS, smem));
+  const int grid = (int)std::min<long long>(n_units, (long long)h->sm_count * std::max(per_sm, 1));
+  ml_vertex_C<<<grid, ML_THREADS, smem, h->stream>>>(p, mcap);
+  LAUNCH_CHECK(h);
+  return GK_OK;
+}
+
+static int ml_flg_grid(gk_handle* h, const void* fn, int P, long long n_pairs, size_t* smem, int* grid) {
+  *smem = (size_t)ML_FLG_WARPS * P * P * 8;
+  GK_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(*smem, 1)));
+  int per_sm = 0;
+  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 32 * ML_FLG_WARPS, *smem));
+  *grid = (int)std::max<long long>(1, std::min<long long>((n_pairs + ML_FLG_WARPS - 1) / ML_FLG_WARPS,
+                                                           (long long)h->sm_count * std::max(per_sm, 1)));
+  return GK_OK;
+}
+
+static int ml_ready(gk_handle* h, const char* who) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->ml_L < 0 || !h->ml_U.p || h->ml_w <= 0) return fail(GK_ERR_STATE, std::string(who) + ": call gk_ml_begin first");
+  return GK_OK;
+}
+
+extern "C" {
+
+int gk_ml_begin(gk_handle* h, int32_t L, double gamma, double heta, const double* phi, int32_t dim, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_ml_begin: no graphs packed");
+  if (L < 0 || L > 64) return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: L outside [0, 64]");
+  if (!(gamma > 0.0) || !(heta > 0.0) || !std::isfinite(gamma) || !std::isfinite(heta))
+    return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: gamma and heta must be positive and finite (the Cholesky route)");
+  if (dim < 1 || !phi) return fail(GK_ERR_ARG, "gk_ml_begin: no attributes");
+  if (h->max_graph_size > ML_NMAX)
+    return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: a graph of more than 128 vertices (the neighbourhood matrix lives in "
+                                    "shared memory)");
+  GK_CUDA(cudaSetDevice(h->dev));
+  HandleExtra* ex = extra_of(h);
+  const int64_t N = h->N, V = h->V;
+  std::vector<long long> off(N + 1, 0);
+  for (int64_t g = 0; g < N; ++g) {
+    const long long n = ex->graph_ptr[g + 1] - ex->graph_ptr[g];
+    off[g + 1] = off[g] + n * n;
+  }
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  GK_TRY(h->ml_adj_off.ensure((N + 1) * 8));
+  GK_TRY(h->ml_adj.ensure(std::max<long long>(off[N], 1) * 8));
+  GK_TRY(h->ml_ball.ensure(std::max<long long>((long long)L * V * 2, 1) * 8));
+  GK_TRY(h->ml_U.ensure(std::max<long long>(V * dim, 1) * 8));
+  GK_TRY(h->ml_ctl.ensure(16));
+  GK_CUDA(cudaMemcpyAsync(h->ml_adj_off.p, off.data(), (N + 1) * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->ml_U.p, phi, (size_t)V * dim * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->ml_adj.p, 0, std::max<long long>(off[N], 1) * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->ml_ctl.p, 0, 16, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  unsigned long long* ball = h->ml_ball.as<unsigned long long>();
+  std::vector<int> mcap(L + 1, 1);
+  if (V > 0) {
+    const int grid = cdiv(V, 256);
+    ml_dense_adj<<<grid, 256, 0, h->stream>>>((int)V, h->graph_ptr.as<int>(), h->vgraph.as<int>(), h->row_ptr.as<int>(),
+                                             h->col_idx.as<int>(), h->has_weights ? h->weights.as<double>() : nullptr,
+                                             h->ml_adj_off.as<long long>(), h->ml_adj.as<double>());
+    LAUNCH_CHECK(h);
+    if (L >= 1) {
+      ml_ball1<<<grid, 256, 0, h->stream>>>((int)V, h->graph_ptr.as<int>(), h->vgraph.as<int>(),
+                                            h->ml_adj_off.as<long long>(), h->ml_adj.as<double>(), ball,
+                                            h->ml_ctl.as<unsigned>());
+      LAUNCH_CHECK(h);
+    }
+    for (int l = 2; l <= L; ++l) {
+      ml_ball_next<<<grid, 256, 0, h->stream>>>((int)V, h->graph_ptr.as<int>(), h->vgraph.as<int>(),
+                                                ball + (size_t)(l - 2) * V * 2, ball + (size_t)(l - 1) * V * 2);
+      LAUNCH_CHECK(h);
+    }
+  }
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  // the symmetry check, and the largest neighbourhood of every level (it sizes the record kernel's shared memory)
+  if (L >= 1 && V > 0) {
+    std::vector<unsigned long long> hb((size_t)L * V * 2);
+    GK_CUDA(cudaMemcpyAsync(hb.data(), ball, hb.size() * 8, cudaMemcpyDeviceToHost, h->stream));
+    GK_TRY(ml_check_err(h));
+    for (int l = 1; l <= L; ++l) {
+      int mx = 1;
+      for (int64_t u = 0; u < V; ++u) {
+        const unsigned long long* b = &hb[((size_t)(l - 1) * V + u) * 2];
+        mx = std::max(mx, __builtin_popcountll(b[0]) + __builtin_popcountll(b[1]));
+      }
+      mcap[l] = std::min(ML_MMAX, mx + (l == 1 ? 1 : 0));  // + a self-loop's second listing
+    }
+  } else {
+    GK_TRY(ml_check_err(h));
+  }
+  h->ml_L = L; h->ml_w = dim;
+  for (int l = 0; l <= L; ++l) h->ml_mcap[l] = mcap[l];
+  h->ml_gamma = gamma; h->ml_heta = heta;
+  h->ml_nrec = 0;
+  h->features_ready = false; h->feat_serial++;
+  h->feature_kind = FK_NONE;
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->n_levels = L;
+    stats->ms_h2d = ev_ms(h->tev[0], h->tev[1]);
+    stats->ms_features = ev_ms(h->tev[1], h->tev[2]);
+  }
+  return GK_OK;
+}
+
+int gk_ml_project(gk_handle* h, const double* Q, int32_t rows, int32_t cols, gk_stats* stats) {
+  GK_TRY(ml_ready(h, "gk_ml_project"));
+  if (!Q || rows != h->ml_w) return fail(GK_ERR_ARG, "gk_ml_project: Q must have as many rows as the features have columns");
+  if (cols < 1 || cols > ML_PMAX)
+    return fail(GK_ERR_UNSUPPORTED, "gk_ml_project: the feature width must lie in [1, 32] (got " + std::to_string(cols) + ")");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const long long V = h->V;
+  GK_TRY(h->ml_aux.ensure((size_t)rows * cols * 8));
+  GK_TRY(h->ml_U2.ensure(std::max<long long>(V * cols, 1) * 8));
+  GK_CUDA(cudaMemcpyAsync(h->ml_aux.p, Q, (size_t)rows * cols * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  if (V > 0) {
+    ml_matmul<<<(int)std::min<long long>(cdiv(V * cols, 256), (long long)h->sm_count * 16), 256, 0, h->stream>>>(
+        V, rows, cols, h->ml_U.as<double>(), h->ml_aux.as<double>(), h->ml_U2.as<double>());
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  std::swap(h->ml_U, h->ml_U2);
+  h->ml_w = cols;
+  if (stats) stats->ms_combine = ev_ms(h->tev[0], h->tev[1]);
+  return GK_OK;
+}
+
+int gk_ml_level(gk_handle* h, int32_t level, const int32_t* samples, int32_t ns, const double* samp_rec,
+                double* samp_rec_out, double* K_samples, gk_stats* stats) {
+  GK_TRY(ml_ready(h, "gk_ml_level"));
+  if (level < 1 || level > h->ml_L) return fail(GK_ERR_ARG, "gk_ml_level: level outside [1, L]");
+  if (ns < 1) return fail(GK_ERR_ARG, "gk_ml_level: no samples");
+  if (ns > ML_NSMAX) return fail(GK_ERR_UNSUPPORTED, "gk_ml_level: more than 1024 samples");
+  if (!samples == !samp_rec) return fail(GK_ERR_ARG, "gk_ml_level: give either sample ids or sample records");
+  if (h->ml_w > ML_PMAX) return fail(GK_ERR_UNSUPPORTED, "gk_ml_level: records of more than 32 features");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const long long V = h->V, P = h->ml_w, stride = P * P + 1;
+  GK_TRY(h->ml_vrec.ensure(std::max<long long>(V * stride, 1) * 8));
+  GK_TRY(h->ml_samp.ensure((size_t)ns * stride * 8));
+  GK_TRY(h->ml_U2.ensure(std::max<long long>(V * ns, 1) * 8));
+  GK_TRY(h->ml_aux.ensure((size_t)ns * 4 + (size_t)ns * ns * 8 + 64));
+  int* d_ids = h->ml_aux.as<int>();
+  double* d_kss = reinterpret_cast<double*>(h->ml_aux.as<char>() + ((size_t)ns * 4 + 63) / 64 * 64);
+  if (samples) {
+    for (int i = 0; i < ns; ++i)
+      if (samples[i] < 0 || samples[i] >= V) return fail(GK_ERR_ARG, "gk_ml_level: sample id out of range");
+    GK_CUDA(cudaMemcpyAsync(d_ids, samples, (size_t)ns * 4, cudaMemcpyHostToDevice, h->stream));
+  } else {
+    GK_CUDA(cudaMemcpyAsync(h->ml_samp.p, samp_rec, (size_t)ns * stride * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  GK_CUDA(cudaMemsetAsync(h->ml_ctl.p, 0, 4, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  GK_TRY(ml_records(h, h->ml_ball.as<unsigned long long>() + (size_t)(level - 1) * V * 2, level == 1 ? 1 : 0,
+                    h->ml_mcap[level], (int)V, h->ml_vrec.as<double>()));
+  if (samples && ns > 0) {
+    ml_gather_rows<<<cdiv((long long)ns * stride, 256), 256, 0, h->stream>>>(ns, d_ids, h->ml_vrec.as<double>(), stride,
+                                                                           h->ml_samp.as<double>());
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  if (V > 0) {
+    size_t smem;
+    int grid;
+    GK_TRY(ml_flg_grid(h, (const void*)ml_flg_project, (int)P, V * ns, &smem, &grid));
+    ml_flg_project<<<grid, 32 * ML_FLG_WARPS, smem, h->stream>>>(h->ml_samp.as<double>(), h->ml_vrec.as<double>(), (int)P,
+                                                                 V, ns, h->ml_U2.as<double>(), h->ml_ctl.as<unsigned>());
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  if (samples && K_samples) {
+    ml_gather_rows<<<cdiv((long long)ns * ns, 256), 256, 0, h->stream>>>(ns, d_ids, h->ml_U2.as<double>(), ns, d_kss);
+    LAUNCH_CHECK(h);
+    GK_CUDA(cudaMemcpyAsync(K_samples, d_kss, (size_t)ns * ns * 8, cudaMemcpyDeviceToHost, h->stream));
+  }
+  if (samples && samp_rec_out)
+    GK_CUDA(cudaMemcpyAsync(samp_rec_out, h->ml_samp.p, (size_t)ns * stride * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_TRY(ml_check_err(h));
+  std::swap(h->ml_U, h->ml_U2);
+  h->ml_w = ns;
+  if (stats) {
+    stats->n_graphs = h->N; stats->n_vertices = V;
+    stats->ms_features = ev_ms(h->tev[0], h->tev[1]);
+    stats->ms_rw = ev_ms(h->tev[1], h->tev[2]);
+    stats->ms_d2h = ev_ms(h->tev[2], h->tev[3]);
+  }
+  return GK_OK;
+}
+
+int gk_ml_finish(gk_handle* h, const double* fit_rec, int64_t n_fit, double* rec_out, gk_stats* stats) {
+  GK_TRY(ml_ready(h, "gk_ml_finish"));
+  if (n_fit < 0 || (n_fit > 0 && !fit_rec)) return fail(GK_ERR_ARG, "gk_ml_finish: bad fitted records");
+  if (h->ml_w > ML_PMAX) return fail(GK_ERR_UNSUPPORTED, "gk_ml_finish: records of more than 32 features");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const long long N = h->N, P = h->ml_w, stride = P * P + 1;
+  GK_TRY(h->ml_rec.ensure((size_t)(n_fit + N) * stride * 8));
+  double* rec = h->ml_rec.as<double>();
+  if (n_fit > 0) GK_CUDA(cudaMemcpyAsync(rec, fit_rec, (size_t)n_fit * stride * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->ml_ctl.p, 0, 4, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  GK_TRY(ml_records(h, nullptr, 0, std::max(h->max_graph_size, 1), (int)N, rec + (size_t)n_fit * stride));
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  if (rec_out)
+    GK_CUDA(cudaMemcpyAsync(rec_out, rec + (size_t)n_fit * stride, (size_t)N * stride * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_TRY(ml_check_err(h));
+  h->ml_nrec = n_fit + N;
+  h->feature_kind = FK_ML;
+  h->features_ready = true; h->feat_serial++;
+  if (stats) stats->ms_features = ev_ms(h->tev[0], h->tev[1]);
+  return GK_OK;
+}
+
+}  // extern "C"
+
+// Gram of MultiscaleLaplacian (gram_path 15): K[r][c] = flg(record a0 + r, record c), one warp per pair; fp64, host
+// or GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges.  The self similarities come from the same pair
+// function, so a square K's diagonal equals them bit for bit; the full square case computes the upper triangle and
+// mirrors it.
+static int gram_ml(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const int64_t N = q.N, k_rows = q.k_rows, k_cols = q.k_cols;
+  const int P = h->ml_w;
+  const int64_t launches0 = h->launches;
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  GK_TRY(h->diag_f64.ensure((size_t)N * 8));
+  GK_CUDA(cudaMemsetAsync(h->ml_ctl.p, 0, 4, h->stream));
+  const double* rec = h->ml_rec.as<double>();
+  unsigned* err = h->ml_ctl.as<unsigned>();
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  size_t smem;
+  int grid;
+  GK_TRY(ml_flg_grid(h, (const void*)ml_flg_gram, P, N, &smem, &grid));
+  ml_flg_gram<<<grid, 32 * ML_FLG_WARPS, smem, h->stream>>>(rec, P, RW_PAIRS_DIAG, N, (int)N, (int)N, 0,
+                                                            h->diag_f64.as<double>(), 1, err);
+  LAUNCH_CHECK(h);
+  const bool mirror = q.full_square && !(q.flags & GK_FULL_TILES);
+  const long long n_pairs = mirror ? N * (N + 1) / 2 : k_rows * k_cols;
+  if (n_pairs > 0) {
+    GK_TRY(ml_flg_grid(h, (const void*)ml_flg_gram, P, n_pairs, &smem, &grid));
+    ml_flg_gram<<<grid, 32 * ML_FLG_WARPS, smem, h->stream>>>(rec, P, mirror ? RW_PAIRS_TRIANGLE : RW_PAIRS_RECT, n_pairs,
+                                                              (int)k_rows, (int)k_cols, q.a0, out.p, out.ld, err);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_TRY(ml_check_err(h));
+  GK_TRY(f64_deliver(h, q, out, true, h->tev[3], h->tev[4]));
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->gram_path = 15;
+    stats->gemm_tiles = n_pairs;
+    stats->gemm_launches = h->launches - launches0;
+    stats->ms_rw = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_gemm = stats->ms_rw;
+    stats->ms_d2h = ev_ms(h->tev[3], h->tev[4]);
+    stats->ms_total = stats->ms_rw + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
 extern "C" {
 
 int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
@@ -4593,6 +4895,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_RW: return gram_rw(h, q, stats);
     case FK_SM: return gram_sm(h, q, stats);
     case FK_ODD: return gram_odd(h, q, stats);
+    case FK_ML: return gram_ml(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }
 }

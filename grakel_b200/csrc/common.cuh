@@ -126,6 +126,7 @@ enum FeatureKind : int {
   FK_NSPD = 9,    // NeighborhoodSubgraphPairwiseDistance per-(radius, distance) count tables
   FK_SM = 10,     // SubgraphMatching per-graph bitset records
   FK_ODD = 11,    // OddSth per-bit-plane (graph, identity) count tables
+  FK_ML = 12,     // MultiscaleLaplacian per-graph (S^-1, log det S) records
 };
 
 }  // namespace gk
@@ -269,6 +270,14 @@ struct gk_handle {
   // column), the (graph, identity) counts, the bit-plane tables, counters, self similarities
   gk::DevBuf odd_aux, odd_nodes, odd_ch, odd_tab, odd_feat, odd_phi, odd_blk, odd_ctl, odd_diag;
   int odd_degen = 0;  // gk_selftest_odd_collision: degenerate identity passes still to come
+
+  // ---- MultiscaleLaplacian (FK_ML): dense per-graph adjacency and its offsets, radius-l ball masks [L][V][2], the
+  // features of the current level and their successor, vertex records [V][P' P' + 1], the sample records of the current
+  // level, sample ids / Q scratch, error bits; after gk_ml_finish ml_rec holds the Gram's records (fitted ones first)
+  gk::DevBuf ml_adj, ml_adj_off, ml_ball, ml_U, ml_U2, ml_vrec, ml_samp, ml_rec, ml_aux, ml_ctl;
+  int ml_L = 0, ml_w = 0, ml_mcap[65] = {};
+  double ml_gamma = 0.0, ml_heta = 0.0;
+  int64_t ml_nrec = 0;
 
   // ---- Propagation (FK_PK): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
   // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]

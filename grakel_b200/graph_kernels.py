@@ -14,6 +14,7 @@ the kernels of the device hot path:
     "subgraph_matching" / "SM"  (+ k, kv, ke, lw)
     "propagation" / "PR"        (+ with_attributes: PropagationAttr)
     "pyramid_match" / "PM"      (+ with_labels, L, d)
+    "multiscale_laplacian" / "ML"  (+ L, P, gamma, heta, n_samples; random_state forwarded)
 
 Any other reference kernel name raises NotImplementedError (not ValueError, which the reference reserves for
 unknown names).  The public surface (constructor parameters, `fit` / `transform` / `fit_transform`, the fitted
@@ -35,14 +36,14 @@ from sklearn.utils.validation import check_is_fitted
 
 from .core_framework import CoreFramework
 from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, NeighborhoodSubgraphPairwiseDistance,
-                      OddSth, Propagation, PropagationAttr, PyramidMatch,
+                      MultiscaleLaplacian, OddSth, Propagation, PropagationAttr, PyramidMatch,
                       ShortestPath, SubgraphMatching, ShortestPathAttr, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
 
 default_n_components = 100
 
 # reference names outside the hot path (graph_kernels.py:38-64)
 _OUTSIDE = frozenset((
-    "random_walk", "RW", "graphlet_sampling", "GR", "multiscale_laplacian", "ML",
+    "random_walk", "RW", "graphlet_sampling", "GR",
     "lovasz_theta", "LOVT", "svm_theta", "SVMT"))
 
 
@@ -69,6 +70,7 @@ for _names, _framework, _build in (
         (("odd_sth", "ODD"), False, lambda p: (OddSth, p)),
         (("propagation", "PR"), False, _propagation),
         (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
+        (("multiscale_laplacian", "ML"), False, lambda p: (MultiscaleLaplacian, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),
         (("hadamard_code", "HC"), True, lambda p: (HadamardCode, p)),
         (("core_framework", "CORE"), True, lambda p: (CoreFramework, p))):
@@ -202,7 +204,7 @@ class GraphKernel(BaseEstimator, TransformerMixin):
                 raise NotImplementedError("kernel '" + str(name) + "' is outside the device hot path of grakel_b200")
             raise ValueError("Unsupported kernel: " + str(name))
         framework, build = entry
-        if name in ("propagation", "PR"):  # graph_kernels.py:486-489, 530-535
+        if name in ("propagation", "PR", "multiscale_laplacian", "ML"):  # graph_kernels.py:486-489, 515-517, 530-535
             params["random_state"] = params.pop("random_state",
                                                 self.random_state_ if self.random_state is not None else None)
         if framework:

@@ -3351,3 +3351,261 @@ class OddSth(Kernel):
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
+
+
+# ------------------------------------------------------------------------------
+# The eigen-decomposition of MultiscaleLaplacian's sampled blocks, by module-level name (the reference's numpy call):
+# tests hand recorded eigenpairs back through it where a truncation boundary is nearly tied.
+ml_eig = np.linalg.eig
+_ML_POSITIVE = float("+1e-6")
+_ML_NMAX = 128
+_ML_ELEMENT_MSG = ("each element of X must be either a graph or an iterable with at least 1 and at most 3 elements\n")
+
+
+def ml_truncate(K, P):
+    """(v, w) of the reference's eig of the sample block K, its `argpartition(v, -P)[-P:]` cut and the 1e-6 filter:
+    (eigenvalues kept, their eigenvectors as rows)."""
+    v, w = ml_eig(K)
+    v, w = np.real(v), np.real(w.T)
+    vpos = np.argpartition(v, -P)[-P:]
+    vpos = vpos[np.where(v[vpos] > _ML_POSITIVE)]
+    return v[vpos], w[vpos]
+
+
+class MultiscaleLaplacian(Kernel):
+    """Multiscale Laplacian graph kernel (multiscale_laplacian.py; Kondor & Pan 2016), the fast FLG variant of the
+    reference.  Per level l = 1 .. L every vertex's neighbourhood of radius l gives S = U^T (L_nb + heta I)^-1 U +
+    gamma I over the previous level's features U, and the features of the next level are the FLG kernel values of the
+    vertex against n_samples sampled vertices, projected on the top-P eigenvectors of the sampled block.  K is the FLG
+    kernel of every graph's final S over its whole Laplacian.
+
+    The samples are the reference's: the same list of (graph, vertex) pairs shuffled by `random_state_`, so a second
+    `fit` draws new ones as the reference does.  The eigen-decompositions of the sampled blocks run on the host through
+    `ml_eig` (numpy's eig, with the reference's argpartition and 1e-6 cut); every neighbourhood, record, projection and
+    the Gram run on the device in fp64.  The device factors each matrix by Cholesky where the reference calls inv and
+    eigvals, so K agrees with the reference to about 1e-11 relative rather than bit for bit; K is exactly symmetric and
+    its diagonal is what `diagonal()` returns.
+
+    Deviations (NotImplementedError): a non-symmetric adjacency matrix, a negative edge weight, gamma == 0 or heta == 0
+    (the reference warns that it may crash; the warning is kept), a graph of more than 128 vertices, a feature width
+    P' (eigenvalues kept) of 0 or above 32, more than 1024 samples.  A non-positive pivot met on the device raises an
+    error rather than returning NaN."""
+
+    _graph_format = "adjacency"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, random_state=None, L=3, P=10, gamma=0.01,
+                 heta=0.01, n_samples=50):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.random_state = random_state
+        self.gamma = gamma
+        self.heta = heta
+        self.L = L
+        self.P = P
+        self.n_samples = n_samples
+        self._initialized.update({"random_state": False, "gamma": False, "heta": False, "L": False,
+                                  "n_samples": False, "P": False})
+
+    def initialize(self):
+        """multiscale_laplacian.py:86-131, in its order and with its errors."""
+        super().initialize()
+        if not self._initialized["random_state"]:
+            self.random_state_ = check_random_state(self.random_state)
+            self._initialized["random_state"] = True
+        for name in ("gamma", "heta"):
+            if not self._initialized[name]:
+                val = getattr(self, name)
+                if not isinstance(val, Real):
+                    raise TypeError(name + " must be a real number")
+                elif val == .0:
+                    warnings.warn("with zero " + name + " the calculation may crash")
+                elif val < 0:
+                    raise TypeError(name + " must be positive")
+                self._initialized[name] = True
+        if not self._initialized["L"]:
+            if type(self.L) is not int:
+                raise TypeError("L must be an integer")
+            elif self.L < 0:
+                raise TypeError("L must be positive")
+            self._initialized["L"] = True
+        if not self._initialized["n_samples"]:
+            if type(self.n_samples) is not int or self.n_samples <= 0:
+                raise TypeError("n_samples must be a positive integer")
+            self._initialized["n_samples"] = True
+        if not self._initialized["P"]:
+            if type(self.P) is not int or self.P <= 0:
+                raise TypeError("P must be a positive integer")
+            self._initialized["P"] = True
+
+    # ---- input
+    @staticmethod
+    def _features(A, labels):
+        try:
+            phi = np.array([list(labels[i]) for i in range(A.shape[0])])
+        except TypeError:
+            raise TypeError("Features must be iterable and castable in total to a numpy array.")
+        return A, phi
+
+    def _elements(self, X):
+        """(adjacency matrix, attribute matrix) of every element (multiscale_laplacian.py:154-186)."""
+        from .packing import adjacency_and_labels
+        if isinstance(X, Block):  # datasets.read_tu: the vertices that occur in an edge, with their attribute rows
+            out = []
+            gp = X.graph_ptr
+            for g, (A, _) in enumerate(_block_adjacency(X, False)):
+                rows = None if X.attrs is None else X.attrs[int(gp[g]):int(gp[g + 1])]
+                out.append(self._features(A, rows if rows is not None else [0] * A.shape[0]))
+            if not out:
+                raise ValueError("parsed input is empty")
+            return out
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            if not (is_iter and len(x) in (0, 2, 3)):
+                raise TypeError(_ML_ELEMENT_MSG)
+            if len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            A, labels = adjacency_and_labels(x[0], x[1])
+            out.append(self._features(A, labels))
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    def _check_scope(self, els):
+        if self.gamma == 0 or self.heta == 0:
+            raise NotImplementedError("MultiscaleLaplacian: gamma == 0 or heta == 0 has no Cholesky route")
+        for A, _ in els:
+            if A.shape[0] > _ML_NMAX:
+                raise NotImplementedError("MultiscaleLaplacian: a graph of more than 128 vertices")
+            if np.any(A < 0):
+                raise NotImplementedError("MultiscaleLaplacian: a negative edge weight")
+            if not np.array_equal(A, A.T):
+                raise NotImplementedError("MultiscaleLaplacian: a non-symmetric adjacency matrix")
+
+    def _ml_pipeline(self, eng, els, fit_rec=None):
+        """multiscale_laplacian.py:188-310 on the device `eng`: fit (`_method_calling` 1) samples and keeps every
+        level's basis, transform (3) applies them.  Leaves the Gram's records on `eng` (the fitted ones `fit_rec`
+        first) and returns the packed graphs' final records."""
+        sizes = [A.shape[0] for A, _ in els]
+        gp = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        # CSR of every graph's non-zero entries (diagonal included: it marks level-1 self-loops) with their weights
+        rows, cols, vals = [], [], []
+        for g, (A, _) in enumerate(els):
+            ii, jj = np.nonzero(A)
+            rows.append(ii + gp[g]); cols.append(jj + gp[g]); vals.append(A[ii, jj])
+        rows = np.concatenate(rows) if rows else np.zeros(0, np.int64)
+        cols = np.concatenate(cols) if cols else np.zeros(0, np.int64)
+        vals = np.concatenate(vals) if vals else np.zeros(0)
+        rp = np.concatenate([[0], np.cumsum(np.bincount(rows, minlength=int(gp[-1])))])
+        phi = np.concatenate([np.asarray(p, dtype=np.float64).reshape(len(p), -1) for _, p in els])
+        stats = {"host_eig_ms": 0.0}
+        import time
+        eng.pack(gp, rp, cols, None, vals, None)
+        stats["begin"] = eng.ml_begin(self.L, self.gamma, self.heta, phi).as_dict()
+        fit = self._method_calling == 1
+        if fit:
+            V = [(k, j) for k in range(len(els)) for j in range(sizes[k])]
+            ns = min(len(V), self.n_samples)
+            self.random_state_.shuffle(V)
+            vs = V[:ns]
+            phi_k = np.array([els[k][1][j, :] for (k, j) in vs])
+            t0 = time.perf_counter()
+            v, w = ml_truncate(phi_k.dot(phi_k.T), self.P)
+            stats["host_eig_ms"] += (time.perf_counter() - t0) * 1e3
+            ksi = w.dot(phi_k).T / np.sqrt(v)
+            self._data_level = {0: ksi}
+            self.samples_ = [vs]
+        else:
+            ksi = self._data_level[0]
+        stats["project"] = [eng.ml_project(self._width_check(ksi)).as_dict()]
+        width = ksi.shape[1]
+        stats["levels"] = []
+        for l in range(1, self.L + 1):
+            if fit:
+                self.random_state_.shuffle(V)
+                vs = V[:ns]
+                ids = np.array([gp[k] + j for k, j in vs], dtype=np.int32)
+                rec, kss, s = eng.ml_level(l, width, samples=ids)
+                t0 = time.perf_counter()
+                v, w = ml_truncate(kss, self.P)
+                stats["host_eig_ms"] += (time.perf_counter() - t0) * 1e3
+                Q = w.T / np.sqrt(v)
+                self._data_level[l] = (rec, Q)
+                self.samples_.append(vs)
+            else:
+                rec, Q = self._data_level[l]
+                _, _, s = eng.ml_level(l, width, samp_rec=rec)
+            stats["levels"].append(s.as_dict())
+            stats["project"].append(eng.ml_project(self._width_check(Q)).as_dict())
+            width = Q.shape[1]
+        recs, s = eng.ml_finish(width, fit_rec=fit_rec)
+        stats["finish"] = s.as_dict()
+        self.ml_stats_ = stats
+        return recs
+
+    @staticmethod
+    def _width_check(Q):
+        if Q.shape[1] == 0:
+            raise NotImplementedError("MultiscaleLaplacian: no eigenvalue of the sampled block above 1e-6")
+        return Q
+
+    # ---- estimator protocol
+    def fit(self, X, y=None):
+        self._method_calling = 1
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        self.__dict__.pop("_X_diag", None)
+        self._ml_fit(X, want_matrix=False)
+        return self
+
+    def _ml_fit(self, X, want_matrix):
+        els = self._elements(X)
+        self._check_scope(els)
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            self.X = self._ml_pipeline(eng, els)
+            K, xd, _ = eng.gram(len(self.X), normalize=bool(self.normalize) and want_matrix,
+                                out=None if want_matrix else False)
+        self._X_diag = xd
+        return K
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 1  # fit_transform sets 2, and fit resets it to 1: the sampling route
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        K = self._ml_fit(X, want_matrix=True)
+        if self.normalize:
+            self._warn_unnormalizable(self._X_diag)
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        els = self._elements(X)
+        self._check_scope(els)
+        nx = len(self.X)
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            Y = self._ml_pipeline(eng, els, fit_rec=self.X)
+            K, xd, yd = eng.gram(nx + len(Y), n_fit=nx, normalize=bool(self.normalize))
+        self._X_diag, self._Y_diag = xd, yd
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xd, yd)
+        return K
+
+    def diagonal(self):
+        check_is_fitted(self, ["X"])
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag

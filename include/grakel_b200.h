@@ -299,6 +299,36 @@ int gk_odd_signatures(gk_handle* h, int32_t* label, int64_t* child_off, int32_t*
  * only the verification separates identities and every such pass must detect a collision and be repeated. */
 int gk_selftest_odd_collision(gk_handle* h, int32_t attempts);
 
+/* MultiscaleLaplacian (multiscale_laplacian.py), fp64 throughout, in stages because the reference's eigen-decompositions
+ * of the sampled blocks run on the host between them.  The packed CSR (with weights) must be a symmetric adjacency
+ * with non-negative weights and graphs of at most 128 vertices; gamma > 0 and heta > 0.  Every matrix is then SPD and
+ * is factored by Cholesky; a non-positive pivot met anyway is GK_ERR_RANGE, never a NaN in K.
+ *   gk_ml_begin    dense adjacency, the radius-l balls for l = 1 .. L (level 1 lists a vertex with a self-loop twice,
+ *                  as the reference's [v] + neighbours(v)), and phi[V * dim] as the current features.  A non-symmetric
+ *                  adjacency, L > 64, gamma or heta <= 0 and a graph of more than 128 vertices are GK_ERR_UNSUPPORTED.
+ *                  stats: ms_h2d, ms_features (adjacency and balls).
+ *   gk_ml_project  features <- features Q, Q[rows * cols] row-major with rows = the current width; the new width must
+ *                  lie in [1, 32] (else GK_ERR_UNSUPPORTED).  stats: ms_combine.
+ *   gk_ml_level    every vertex's record at `level` (1 .. L): S = U^T (L_nb + heta I)^-1 U + gamma I over its
+ *                  neighbourhood nb, record = (S^-1 row-major, log det S), P' * P' + 1 doubles.  The level's sample
+ *                  records are those of the vertices samples[ns] (fit: also written to samp_rec_out if given, and the
+ *                  ns x ns block of the new features at those rows to K_samples if given) or samp_rec[ns] (transform).
+ *                  The new features are K_proj[v, m] = flg(sample m, vertex v), V x ns, ns <= 1024 (else
+ *                  GK_ERR_UNSUPPORTED).  stats: ms_features (records), ms_rw (projection), ms_d2h.
+ *   gk_ml_finish   every packed graph's final record over its whole Laplacian, written to rec_out[N] if given; the
+ *                  Gram's records are fit_rec[n_fit] (the fitted graphs' final records, 0 in a fit) followed by them.
+ *                  stats: ms_features.
+ * flg(a, b) = exp((-log det(S_a^-1 + S_b^-1) - (ld_a + ld_b) / 2) / 2), 0 when the exponent is below -30.
+ * gk_gram (gram_path 15) returns K[r, c] = flg(record row_g0 + r, record c) over the records, one warp per pair: fp64
+ * only, host or GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges (n_fit counts records); the full square case
+ * computes the upper triangle and mirrors it, and xdiag / ydiag come from the same pair function.  GK_DIST and row
+ * maps are GK_ERR_UNSUPPORTED. */
+int gk_ml_begin(gk_handle* h, int32_t L, double gamma, double heta, const double* phi, int32_t dim, gk_stats* stats);
+int gk_ml_project(gk_handle* h, const double* Q, int32_t rows, int32_t cols, gk_stats* stats);
+int gk_ml_level(gk_handle* h, int32_t level, const int32_t* samples, int32_t ns, const double* samp_rec,
+                double* samp_rec_out, double* K_samples, gk_stats* stats);
+int gk_ml_finish(gk_handle* h, const double* fit_rec, int64_t n_fit, double* rec_out, gk_stats* stats);
+
 /* Propagation / PropagationAttr (propagation.py:27-689).  The packed CSR (gk_pack_csr without weights; with the
  * label ids for the labelled kernel) is the sparsity pattern of every graph's row-normalised transition matrix T,
  * t_values[E] its entries.  P (V x dim, fp64) starts one-hot from the packed label ids or as p0[V * dim] (GK_PK_ATTR).
