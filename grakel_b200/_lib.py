@@ -91,6 +91,10 @@ _SYMBOLS = {
     "gk_ml_project": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.POINTER(GkStats)]),
     "gk_ml_level": (C.c_int, [_P, C.c_int32, _P, C.c_int32, _P, _P, _P, C.POINTER(GkStats)]),
     "gk_ml_finish": (C.c_int, [_P, _P, C.c_int64, _P, C.POINTER(GkStats)]),
+    "gk_svmt_solve": (C.c_int, [_P, C.c_int64, _P, _P, C.POINTER(GkStats)]),
+    "gk_svmt_draw": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int32, C.c_int32, _P, _P, C.c_int64]),
+    "gk_svmt_phi": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, C.c_int64, _P, C.c_int64, _P, _P, _P, _P,
+                              C.POINTER(GkStats)]),
     "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
@@ -184,6 +188,26 @@ def nspd_set_order(h0, h1):
     if lib.gk_selftest_nspd_set_order(len(a), _ptr(a), _ptr(b), _ptr(out)) != 0:
         raise GrakelB200Error(lib.gk_last_error().decode())
     return out
+
+
+def svmt_draw(rs, sizes, lo, counts):
+    """Host only: the index arrays SvmTheta draws with `rs.choice(n, level, replace=False)` for every graph, level
+    (lo + column of `counts`, ascending) and sample, concatenated (gk_svmt_draw); `rs` continues after them, its
+    gaussian cache untouched."""
+    name, key, pos, has_gauss, gauss = rs.get_state()
+    key = np.array(key, dtype=np.uint32)
+    p = C.c_int32(int(pos))
+    sz = _i32(sizes)
+    cnt = _i32(counts)
+    L = cnt.shape[1]
+    levels = lo + np.arange(L)
+    n_idx = int(np.sum(cnt * levels * (levels[None, :] <= sz[:, None])))
+    idx = np.empty(n_idx, dtype=np.uint8)
+    lib = load_library()
+    if lib.gk_svmt_draw(_ptr(key), C.byref(p), len(sz), _ptr(sz), int(lo), L, _ptr(cnt), _ptr(idx), n_idx) != 0:
+        raise GrakelB200Error(lib.gk_last_error().decode())
+    rs.set_state((name, key, p.value, has_gauss, gauss))
+    return idx
 
 
 class _HostBlock:
@@ -436,6 +460,35 @@ class Engine:
             self._check(self.lib.gk_ml_finish(self.h, _ptr(fr), 0 if fr is None else fr.shape[0], _ptr(out),
                                               C.byref(st)))
         return out, st
+
+    def svmt_solve(self, sizes, adj):
+        """SvmTheta: launch the smallest eigenvalues and the one-class SMO of graphs of `sizes` vertices with out-edge
+        masks adj [V, 4] u32 (gk_svmt_solve); returns without waiting for them."""
+        sz = _i32(sizes)
+        a = np.ascontiguousarray(adj, dtype=np.uint32)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_svmt_solve(self.h, len(sz), _ptr(sz), _ptr(a), C.byref(st)))
+        self._svmt_keep = (sz, a)
+        return st
+
+    def svmt_phi(self, lo, counts, idx, fit_phi0=None, details=False):
+        """phi [N, L] of the solved graphs from the drawn indexes (gk_svmt_phi), their first level placed after
+        `fit_phi0` for gram(); with `details` also (m, alphas, iteration counts).  Returns (phi, details or None, stats)."""
+        cnt = _i32(counts)
+        ix = np.ascontiguousarray(idx, dtype=np.uint8)
+        fp = None if fit_phi0 is None else np.ascontiguousarray(fit_phi0, dtype=np.float64)
+        N, L = cnt.shape
+        phi = np.empty((N, L), dtype=np.float64)
+        det = None
+        if details:
+            det = (np.empty(N), np.empty(int(np.sum(self._svmt_keep[0]))), np.empty(N, dtype=np.int32))
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_svmt_phi(self.h, int(lo), L, _ptr(cnt), _ptr(ix), len(ix), _ptr(fp),
+                                             0 if fp is None else len(fp), _ptr(phi),
+                                             *(_ptr(a) for a in (det or (None, None, None))), C.byref(st)))
+        return phi, det, st
 
     def pk_features(self, t_max, w, u, b, dim, dim_orig, n_fit, t_values, p0=None, flags=0):
         """Propagation bins of t_max levels and their (graph, column) counts (gk_pk_features).  u: [t_max, dim],

@@ -36,6 +36,7 @@
 #include "subgraph_matching.cuh"
 #include "odd_sth.cuh"
 #include "multiscale_laplacian.cuh"
+#include "svm_theta.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -353,7 +354,9 @@ int gk_destroy(gk_handle* h) {
                         &h->odd_aux, &h->odd_nodes, &h->odd_ch, &h->odd_tab, &h->odd_feat, &h->odd_phi, &h->odd_blk,
                         &h->odd_ctl, &h->odd_diag,
                         &h->ml_adj, &h->ml_adj_off, &h->ml_ball, &h->ml_U, &h->ml_U2, &h->ml_vrec, &h->ml_samp, &h->ml_rec,
-                        &h->ml_aux, &h->ml_ctl};
+                        &h->ml_aux, &h->ml_ctl,
+                        &h->svmt_vptr, &h->svmt_adj, &h->svmt_m, &h->svmt_alpha, &h->svmt_iters, &h->svmt_cnt,
+                        &h->svmt_off, &h->svmt_idx, &h->svmt_sums, &h->svmt_phi, &h->svmt_rec, &h->svmt_ctl};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1748,6 +1751,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_SM     */ {"SubgraphMatching", false, true, false, false},
     /* FK_ODD    */ {"OddSth", false, true, false, false},
     /* FK_ML     */ {"MultiscaleLaplacian", false, true, false, false},
+    /* FK_SVMT   */ {"SvmTheta", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -1755,8 +1759,8 @@ static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t f
                         GramReq* q) {
   const GramRules& r = GRAM_RULES[kind];
   if (out_dtype != GK_F32 && out_dtype != GK_F64) return fail(GK_ERR_ARG, "gk_gram: bad out_dtype");
-  // MultiscaleLaplacian's rows are its records: the fitted graphs' (kept from the fit) and then the packed ones
-  const int64_t N = h->n_rows > 0 ? h->n_rows : kind == FK_ML ? h->ml_nrec : h->N;
+  // MultiscaleLaplacian's and SvmTheta's rows are their records: the fitted graphs' (kept from the fit), then the new ones
+  const int64_t N = h->n_rows > 0 ? h->n_rows : kind == FK_ML ? h->ml_nrec : kind == FK_SVMT ? h->svmt_nrec : h->N;
   if (n_fit <= 0 || n_fit > N) return fail(GK_ERR_ARG, "gk_gram: n_fit out of range");
   const bool dist = (flags & (GK_DIST | GK_DIST_GATHER)) != 0;
   if (h->n_rows > 0 && !r.row_map) return fail(GK_ERR_UNSUPPORTED, std::string("gk_gram: row map with ") + r.name + " features");
@@ -4877,6 +4881,211 @@ static int gram_ml(gk_handle* h, const GramReq& q, gk_stats* stats) {
   return GK_OK;
 }
 
+// ---------------------------------------------------------------------------
+// SvmTheta (svm_theta.cuh).  gk_svmt_solve launches the eigenvalue and SMO kernels and returns; the caller draws the
+// samples on the host (gk_svmt_draw, which needs no alphas) while they run; gk_svmt_phi then forms phi and leaves the
+// first level of every graph, after the fitted graphs' (n_fit), for gk_gram (gram_path 16).
+// Gram of SvmTheta (gram_path 16): K[r][c] = phi0[a0 + r] phi0[c] (the reference's default metric np.inner(x, y)[0, 0])
+// by the fp64 CUDA-core Gram over a one-column feature matrix, a single rounded product per entry; the self
+// similarities are the same products, so GK_NORMALIZE divides by sqrt(d_r d_c) as numpy's K / sqrt(outer(d, d)).
+static int gram_svmt(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const int64_t N = q.N, k_rows = q.k_rows, k_cols = q.k_cols;
+  const int64_t launches0 = h->launches;
+  F64Out out;
+  GK_TRY(f64_target(h, q, &out));
+  GK_TRY(h->diag_f64.ensure((size_t)N * 8));
+  const double* rec = h->svmt_rec.as<double>();
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  svmt_diag<<<(int)std::max<int64_t>(1, std::min<int64_t>(cdiv(N, 256), (int64_t)h->sm_count * 8)), 256, 0, h->stream>>>(
+      rec, N, h->diag_f64.as<double>());
+  LAUNCH_CHECK(h);
+  if (k_rows > 0) {
+    dim3 grid((unsigned)cdiv(k_cols, 64), (unsigned)cdiv(k_rows, 64));
+    gram_f64_kernel<<<grid, 256, 0, h->stream>>>(rec, 1, q.a0, q.a1, 0, (int)q.n_fit, out.p, out.ld);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  GK_TRY(f64_deliver(h, q, out, true, h->tev[3], h->tev[4]));
+  if (stats) {
+    stats->n_graphs = N;
+    stats->gram_path = 16;
+    stats->gemm_launches = h->launches - launches0;
+    stats->ms_gemm = ev_ms(h->tev[2], h->tev[3]);
+    stats->ms_d2h = ev_ms(h->tev[3], h->tev[4]);
+    stats->ms_total = stats->ms_gemm + stats->ms_d2h;
+  }
+  return GK_OK;
+}
+
+extern "C" {
+
+int gk_svmt_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int32_t* sizes, int32_t lo,
+                 int32_t n_levels, const int32_t* counts, uint8_t* idx, int64_t n_idx) {
+  if (!mt_key || !mt_pos || n_graphs < 0 || (n_graphs > 0 && (!sizes || !counts)) || n_levels < 1 || lo < 1)
+    return fail(GK_ERR_ARG, "gk_svmt_draw: bad arguments");
+  if (*mt_pos < 0 || *mt_pos > 624) return fail(GK_ERR_ARG, "gk_svmt_draw: MT19937 position outside [0, 624]");
+  int64_t need = 0;
+  for (int64_t g = 0; g < n_graphs; ++g) {
+    if (sizes[g] < 1 || sizes[g] > SVMT_NMAX) return fail(GK_ERR_UNSUPPORTED, "gk_svmt_draw: a graph outside 1 .. 128 vertices");
+    for (int li = 0; li < n_levels; ++li) {
+      const int32_t v = counts[g * n_levels + li];
+      if (v < 0) return fail(GK_ERR_ARG, "gk_svmt_draw: negative sample count");
+      if (lo + li <= sizes[g]) need += (int64_t)v * (lo + li);
+    }
+  }
+  if (need != n_idx || (need > 0 && !idx)) return fail(GK_ERR_ARG, "gk_svmt_draw: index buffer does not match the schedule");
+  SvmtMT mt{mt_key, *mt_pos};
+  uint8_t perm[SVMT_NMAX];
+  int64_t o = 0;
+  for (int64_t g = 0; g < n_graphs; ++g) {
+    const int n = sizes[g];
+    for (int li = 0; li < n_levels; ++li) {
+      const int level = lo + li;
+      if (level > n) continue;  // the reference sums all n alphas without drawing
+      for (int32_t s = 0; s < counts[g * n_levels + li]; ++s) {
+        // choice(n, level, replace=False): the first `level` entries of a Fisher-Yates shuffle of arange(n)
+        for (int i = 0; i < n; ++i) perm[i] = (uint8_t)i;
+        for (int i = n - 1; i >= 1; --i) {
+          const uint32_t j = mt.interval((uint32_t)i);
+          const uint8_t t = perm[i]; perm[i] = perm[j]; perm[j] = t;
+        }
+        memcpy(idx + o, perm, level);
+        o += level;
+      }
+    }
+  }
+  *mt_pos = mt.pos;
+  return GK_OK;
+}
+
+int gk_svmt_solve(gk_handle* h, int64_t n_graphs, const int32_t* sizes, const uint32_t* adj, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (n_graphs < 1 || n_graphs > INT_MAX || !sizes || !adj) return fail(GK_ERR_ARG, "gk_svmt_solve: no graphs");
+  std::vector<int> vptr(n_graphs + 1, 0);
+  int nmax = 0;
+  for (int64_t g = 0; g < n_graphs; ++g) {
+    if (sizes[g] < 1) return fail(GK_ERR_ARG, "gk_svmt_solve: a graph without vertices");
+    if (sizes[g] > SVMT_NMAX)
+      return fail(GK_ERR_UNSUPPORTED, "gk_svmt_solve: a graph of more than 128 vertices (the eigenvalue workspace is "
+                                      "n^2 doubles of shared memory)");
+    if ((int64_t)vptr[g] + sizes[g] > INT_MAX) return fail(GK_ERR_UNSUPPORTED, "gk_svmt_solve: 2^31 or more vertices");
+    vptr[g + 1] = vptr[g] + sizes[g];
+    nmax = std::max(nmax, (int)sizes[g]);
+  }
+  const int64_t N = n_graphs, V = vptr[N];
+  GK_CUDA(cudaSetDevice(h->dev));
+  GK_TRY(h->svmt_vptr.ensure((size_t)(N + 1) * 4));
+  GK_TRY(h->svmt_adj.ensure((size_t)V * 16));
+  GK_TRY(h->svmt_m.ensure((size_t)N * 8));
+  GK_TRY(h->svmt_alpha.ensure((size_t)V * 8));
+  GK_TRY(h->svmt_iters.ensure((size_t)N * 4));
+  GK_TRY(h->svmt_ctl.ensure(16));
+  GK_CUDA(cudaEventRecord(h->tev[5], h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->svmt_vptr.p, vptr.data(), (size_t)(N + 1) * 4, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->svmt_adj.p, adj, (size_t)V * 16, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->svmt_ctl.p, 0, 16, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  const size_t smem = ((size_t)nmax * nmax + 4 * (size_t)nmax) * 8;
+  GK_CUDA(cudaFuncSetAttribute(svmt_eig, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 0;
+  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, svmt_eig, SVMT_EIG_THREADS, smem));
+  int grid = (int)std::min<int64_t>(N, (int64_t)h->sm_count * std::max(per_sm, 1));
+  svmt_eig<<<grid, SVMT_EIG_THREADS, smem, h->stream>>>(h->svmt_vptr.as<int>(), h->svmt_adj.as<unsigned>(), (int)N,
+                                                        h->svmt_m.as<double>());
+  LAUNCH_CHECK(h);
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, svmt_smo, 32 * SVMT_SMO_WARPS, 0));
+  grid = (int)std::min<int64_t>(cdiv(N, SVMT_SMO_WARPS), (int64_t)h->sm_count * std::max(per_sm, 1));
+  svmt_smo<<<grid, 32 * SVMT_SMO_WARPS, 0, h->stream>>>(h->svmt_vptr.as<int>(), h->svmt_adj.as<unsigned>(), (int)N,
+                                                        h->svmt_m.as<double>(), h->svmt_alpha.as<double>(),
+                                                        h->svmt_iters.as<int>(), h->svmt_ctl.as<unsigned>());
+  LAUNCH_CHECK(h);
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  h->svmt_sizes.assign(sizes, sizes + N);
+  h->features_ready = false;
+  h->n_rows = 0;  // a new block starts without a row map
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = V;
+  }
+  return GK_OK;
+}
+
+int gk_svmt_phi(gk_handle* h, int32_t lo, int32_t n_levels, const int32_t* counts, const uint8_t* idx, int64_t n_idx,
+                const double* fit_phi0, int64_t n_fit, double* phi, double* m_out, double* alpha_out, int32_t* iters_out,
+                gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  const int64_t N = (int64_t)h->svmt_sizes.size();
+  if (N == 0) return fail(GK_ERR_STATE, "gk_svmt_phi: call gk_svmt_solve first");
+  if (lo < 1 || n_levels < 1 || !counts || n_fit < 0 || (n_fit > 0 && !fit_phi0))
+    return fail(GK_ERR_ARG, "gk_svmt_phi: bad arguments");
+  std::vector<long long> off(2 * N);
+  long long draws = 0, samples = 0;
+  for (int64_t g = 0; g < N; ++g) {
+    off[g] = draws; off[N + g] = samples;
+    for (int li = 0; li < n_levels; ++li) {
+      const int32_t v = counts[g * n_levels + li];
+      if (v < 0) return fail(GK_ERR_ARG, "gk_svmt_phi: negative sample count");
+      samples += v;
+      if (lo + li <= h->svmt_sizes[g]) draws += (long long)v * (lo + li);
+    }
+  }
+  if (draws != n_idx || (draws > 0 && !idx)) return fail(GK_ERR_ARG, "gk_svmt_phi: index buffer does not match the schedule");
+  GK_CUDA(cudaSetDevice(h->dev));
+  GK_TRY(h->svmt_cnt.ensure((size_t)N * n_levels * 4));
+  GK_TRY(h->svmt_off.ensure((size_t)N * 16));
+  GK_TRY(h->svmt_idx.ensure((size_t)std::max<long long>(draws, 1)));
+  GK_TRY(h->svmt_sums.ensure((size_t)std::max<long long>(samples, 1) * 8));
+  GK_TRY(h->svmt_phi.ensure((size_t)N * n_levels * 8));
+  GK_TRY(h->svmt_rec.ensure((size_t)(n_fit + N) * 8));
+  double* rec = h->svmt_rec.as<double>();
+  GK_CUDA(cudaEventRecord(h->tev[7], h->stream));
+  // word 0: the solve's SMO bit, word 1: this call's index bit
+  GK_CUDA(cudaMemsetAsync(h->svmt_ctl.as<unsigned>() + 1, 0, 4, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->svmt_cnt.p, counts, (size_t)N * n_levels * 4, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->svmt_off.p, off.data(), (size_t)N * 16, cudaMemcpyHostToDevice, h->stream));
+  if (draws > 0) GK_CUDA(cudaMemcpyAsync(h->svmt_idx.p, idx, (size_t)draws, cudaMemcpyHostToDevice, h->stream));
+  if (n_fit > 0) GK_CUDA(cudaMemcpyAsync(rec, fit_phi0, (size_t)n_fit * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  const long long* d_off = h->svmt_off.as<long long>();
+  const int grid = (int)std::min<int64_t>(cdiv(N, SVMT_PHI_WARPS), (int64_t)h->sm_count * 16);
+  svmt_phi<<<grid, 32 * SVMT_PHI_WARPS, 0, h->stream>>>(h->svmt_vptr.as<int>(), (int)N, h->svmt_alpha.as<double>(), lo,
+                                                        n_levels, h->svmt_cnt.as<int>(), d_off, h->svmt_idx.as<unsigned char>(),
+                                                        d_off + N, h->svmt_sums.as<double>(), h->svmt_phi.as<double>(),
+                                                        rec + n_fit, h->svmt_ctl.as<unsigned>() + 1);
+  LAUNCH_CHECK(h);
+  GK_CUDA(cudaEventRecord(h->tev[4], h->stream));
+  unsigned ctl[2] = {0, 0};
+  GK_CUDA(cudaMemcpyAsync(ctl, h->svmt_ctl.p, 8, cudaMemcpyDeviceToHost, h->stream));
+  if (phi) GK_CUDA(cudaMemcpyAsync(phi, h->svmt_phi.p, (size_t)N * n_levels * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (m_out) GK_CUDA(cudaMemcpyAsync(m_out, h->svmt_m.p, (size_t)N * 8, cudaMemcpyDeviceToHost, h->stream));
+  int64_t nv = 0;
+  for (int s : h->svmt_sizes) nv += s;
+  if (alpha_out) GK_CUDA(cudaMemcpyAsync(alpha_out, h->svmt_alpha.p, (size_t)nv * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (iters_out) GK_CUDA(cudaMemcpyAsync(iters_out, h->svmt_iters.p, (size_t)N * 4, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaEventRecord(h->tev[6], h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  const unsigned err = ctl[0] | ctl[1];
+  if (err & SVMT_ERR_INDEX) return fail(GK_ERR_ARG, "gk_svmt_phi: a drawn index is not a vertex of its graph");
+  if (err & SVMT_ERR_ITER)
+    return fail(GK_ERR_RANGE, "SvmTheta: the one-class SMO did not converge within 10 000 000 iterations on a graph (libsvm "
+                              "need not converge on a non-symmetric matrix)");
+  h->svmt_nrec = n_fit + N;
+  h->feature_kind = FK_SVMT;
+  h->features_ready = true; h->feat_serial++;
+  if (stats) {
+    stats->n_graphs = N; stats->n_vertices = nv;
+    stats->ms_h2d = ev_ms(h->tev[5], h->tev[0]) + ev_ms(h->tev[7], h->tev[3]);
+    stats->ms_features = ev_ms(h->tev[0], h->tev[1]);  // smallest eigenvalues
+    stats->ms_rw = ev_ms(h->tev[1], h->tev[2]);        // SMO
+    stats->ms_combine = ev_ms(h->tev[3], h->tev[4]);   // subset sums and phi
+    stats->ms_d2h = ev_ms(h->tev[4], h->tev[6]);
+  }
+  return GK_OK;
+}
+
+}  // extern "C"
+
 extern "C" {
 
 int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
@@ -4896,6 +5105,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_SM: return gram_sm(h, q, stats);
     case FK_ODD: return gram_odd(h, q, stats);
     case FK_ML: return gram_ml(h, q, stats);
+    case FK_SVMT: return gram_svmt(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }
 }

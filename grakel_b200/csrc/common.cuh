@@ -127,6 +127,7 @@ enum FeatureKind : int {
   FK_SM = 10,     // SubgraphMatching per-graph bitset records
   FK_ODD = 11,    // OddSth per-bit-plane (graph, identity) count tables
   FK_ML = 12,     // MultiscaleLaplacian per-graph (S^-1, log det S) records
+  FK_SVMT = 13,   // SvmTheta per-graph first-level phi
 };
 
 }  // namespace gk
@@ -278,6 +279,14 @@ struct gk_handle {
   int ml_L = 0, ml_w = 0, ml_mcap[65] = {};
   double ml_gamma = 0.0, ml_heta = 0.0;
   int64_t ml_nrec = 0;
+
+  // ---- SvmTheta (FK_SVMT): vertex offsets, out-edge bitmask rows [V][4], smallest eigenvalues, alphas [V], iteration
+  // counts, schedule / draw / sum offsets, drawn indexes, sample sums, phi [N][L], error bits; svmt_rec holds the Gram's
+  // first-level phi (fitted graphs first)
+  gk::DevBuf svmt_vptr, svmt_adj, svmt_m, svmt_alpha, svmt_iters, svmt_cnt, svmt_off, svmt_idx, svmt_sums, svmt_phi,
+      svmt_rec, svmt_ctl;
+  std::vector<int> svmt_sizes;  // vertices of the graphs of the last gk_svmt_solve
+  int64_t svmt_nrec = 0;
 
   // ---- Propagation (FK_PK): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
   // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]

@@ -19,8 +19,10 @@ from collections.abc import Iterable
 from collections import Counter
 from itertools import chain, filterfalse
 from numbers import Real
+import time
 
 import numpy as np
+from scipy.special import binom
 from sklearn.base import BaseEstimator, TransformerMixin
 from sklearn.exceptions import NotFittedError
 from sklearn.utils import check_random_state
@@ -3609,3 +3611,211 @@ class MultiscaleLaplacian(Kernel):
         if getattr(self, "_is_transformed", False):
             return self._X_diag, self._Y_diag
         return self._X_diag
+
+
+# ------------------------------------------------------------------------------
+_SVMT_NMAX = 128
+
+
+def svm_theta_inner(x, y):
+    """SvmTheta's default metric, the reference's `_inner`: np.inner(x, y)[0, 0], the product of the first levels."""
+    return np.inner(x, y)[0, 0]
+
+
+def svmt_distribute(n, subsets_size_range, n_samples):
+    """{subset size: samples} for a graph of n vertices, as the reference's schedule: every size k from the smallest to
+    min(largest, n) gets floor(n_samples * C(n, k) / sum of the C(n, k)) samples; what is left over is handed out one
+    sample at a time from the largest size downwards, wrapping round, so each size gets rem // m more and the last
+    rem % m sizes one beyond that.  Sizes left without a sample are omitted.  A graph below the smallest size raises
+    ZeroDivisionError, as the reference does."""
+    lo, hi = subsets_size_range
+    sizes = np.arange(lo, min(hi, n) + 1)
+    m = len(sizes)
+    if m == 0:
+        raise ZeroDivisionError("integer modulo by zero")
+    share = np.array([binom(n, int(k)) for k in sizes], dtype=float)
+    share = share / np.sum(share)
+    count = np.floor(share * n_samples).astype(int)
+    rem = max(int(n_samples - np.sum(count)), 0)
+    count += rem // m
+    if rem % m:
+        count[m - rem % m:] += 1
+    return {int(k): int(c) for k, c in zip(sizes, count) if c > 0}
+
+
+class SvmTheta(Kernel):
+    """SVM-theta kernel (svm_theta.py; Johansson et al. 2014).  Per graph: the smallest eigenvalue m of the 0/1
+    adjacency (upper triangle mirrored), a one-class SVM fit on the adjacency scaled by 1 / -m with a unit diagonal,
+    then phi[level] = the mean over sampled vertex subsets of that size of the sum of their alphas.  K[i, j] =
+    metric(phi_i, phi_j); the default metric is the product of the first levels.
+
+    The eigenvalue, libsvm's one-class SMO (restated with its rounding, so the alphas and iteration counts are the
+    reference's), the subset sums and means (in numpy's summation order) and the Gram run on the device in fp64.  The
+    subsets are the reference's: `RandomState.choice(n, level, replace=False)` restated in the library's host code on
+    `random_state_`'s MT19937 stream, which then continues as the reference's does (a second fit, or a transform, draws
+    after the earlier ones).  Any metric other than the default goes through the host pairwise driver.
+
+    With the default subsets_size_range (2, 8) the first level gets no samples once a graph has 12 vertices or more,
+    so the default kernel is 0 for such graphs; this is the reference's behaviour and is kept.
+
+    Deviations (NotImplementedError): a graph of more than 128 vertices.  libsvm need not converge on the non-symmetric
+    matrix of a directed graph, where the reference never returns; the device stops after 10^7 iterations with an
+    error.
+
+    `svmt_stats_` holds the stage times of the last run (ms): `h2d_ms` (masks, schedule and indexes), `eigenvalue_ms`,
+    `smo_ms`, `host_draw_ms` (overlapping the two before it), `phi_ms`, `d2h_ms`."""
+
+    _graph_format = "adjacency"
+    # Not a parameter: set on an instance to keep, in `details_`, the last run's per-graph smallest eigenvalues (m),
+    # alphas, SMO iteration counts (iters) and drawn indexes (drawn), for tests and diagnostics.
+    _keep_details = False
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, random_state=None, n_samples=50,
+                 subsets_size_range=(2, 8), metric=svm_theta_inner):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.n_samples = n_samples
+        self.subsets_size_range = subsets_size_range
+        self.metric = metric
+        self.random_state = random_state
+        self._initialized.update({"n_samples": False, "subsets_size_range": False, "metric": False,
+                                  "random_state": False})
+
+    def initialize(self):
+        """svm_theta.py:70-99, in its order and with its errors."""
+        super().initialize()
+        if not self._initialized["n_samples"]:
+            if self.n_samples <= 0 or type(self.n_samples) is not int:
+                raise TypeError("n_samples must an integer be bigger than zero")
+            self._initialized["n_samples"] = True
+        if not self._initialized["subsets_size_range"]:
+            r = self.subsets_size_range
+            if (type(r) is not tuple or len(r) != 2 or any(type(i) is not int for i in r) or r[0] > r[1]
+                    or r[0] <= 0):
+                raise TypeError("subsets_size_range subset size rangemust be a tuple of two integers in increasing "
+                                "order, bigger than 1")
+            self._initialized["subsets_size_range"] = True
+        if not self._initialized["metric"]:
+            if not callable(self.metric):
+                raise TypeError("metric between argumentsmust be a function")
+            self._initialized["metric"] = True
+        if not self._initialized["random_state"]:
+            self.random_state_ = check_random_state(self.random_state)
+            self._initialized["random_state"] = True
+
+    def _elements(self, X):
+        """Adjacency matrices of every element (svm_theta.py:121-151)."""
+        from .packing import adjacency_and_labels
+        if isinstance(X, Block):
+            return [A for A, _ in _block_adjacency(X, False)]
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            if not (is_iter and len(x) in (0, 1, 2, 3)):
+                raise TypeError(_RW_ELEMENT_MSG)
+            if len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            out.append(adjacency_and_labels(x[0])[0])
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    def _schedule(self, sizes):
+        """Samples per (graph, level); a graph below the smallest level raises ZeroDivisionError after the draws of the
+        graphs before it, as in the reference."""
+        lo, hi = self.subsets_size_range
+        counts = np.zeros((len(sizes), hi - lo + 1), dtype=np.int32)
+        memo = {}
+        for g, n in enumerate(sizes):
+            if n not in memo:
+                try:
+                    memo[n] = svmt_distribute(n, self.subsets_size_range, self.n_samples)
+                except ZeroDivisionError:
+                    _lib.svmt_draw(self.random_state_, sizes[:g], lo, counts[:g])
+                    raise
+            for level, v in memo[n].items():
+                counts[g, level - lo] = v
+        return counts
+
+    def _svmt_run(self, eng, X, fit_phi0=None):
+        """phi of every graph of X on the device `eng`, drawing from random_state_; leaves the first levels after
+        `fit_phi0` on `eng` for its Gram.  Returns the list of (L, 1) phi arrays."""
+        els = self._elements(X)
+        sizes = np.array([A.shape[0] for A in els], dtype=np.int32)
+        if np.any(sizes > _SVMT_NMAX):
+            raise NotImplementedError("SvmTheta: a graph of more than 128 vertices")
+        counts = self._schedule(sizes)
+        adj = np.zeros((int(sizes.sum()), 128), dtype=bool)
+        o = 0
+        for A in els:
+            n = A.shape[0]
+            M = A > 1e-10
+            np.fill_diagonal(M, False)
+            adj[o:o + n, :n] = M
+            o += n
+        masks = np.packbits(adj, axis=1, bitorder="little").view("<u4")
+        eng.svmt_solve(sizes, masks)
+        t0 = time.perf_counter()
+        idx = _lib.svmt_draw(self.random_state_, sizes, self.subsets_size_range[0], counts)
+        draw_ms = (time.perf_counter() - t0) * 1e3
+        phi, det, s = eng.svmt_phi(self.subsets_size_range[0], counts, idx, fit_phi0=fit_phi0,
+                                   details=self._keep_details)
+        self.svmt_stats_ = {"n_graphs": len(sizes), "n_vertices": int(sizes.sum()), "h2d_ms": s.ms_h2d,
+                            "eigenvalue_ms": s.ms_features, "smo_ms": s.ms_rw, "host_draw_ms": draw_ms,
+                            "phi_ms": s.ms_combine, "d2h_ms": s.ms_d2h}
+        if det is not None:
+            self.details_ = dict(m=det[0], alpha=det[1], iters=det[2], drawn=idx, sizes=sizes)
+        return [row.reshape(-1, 1) for row in phi]
+
+    def parse_input(self, X):
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            return self._svmt_run(eng, X)
+
+    def pairwise_operation(self, x, y):
+        return self.metric(x, y)
+
+    def _device_gram(self):
+        return self.metric is svm_theta_inner
+
+    def fit_transform(self, X, y=None):
+        if not self._device_gram():
+            return self._pairwise_fit_transform(X)
+        self._method_calling = 2
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            self.X = self._svmt_run(eng, X)
+            K, xd, _ = eng.gram(len(self.X), normalize=bool(self.normalize))
+        self._X_diag = xd
+        if self.normalize:
+            self._warn_unnormalizable(xd)
+        return K
+
+    def transform(self, X):
+        if not self._device_gram():
+            return self._pairwise_transform(X)
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("`transform` input cannot be None")
+        nx = len(self.X)
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            Y = self._svmt_run(eng, X, fit_phi0=np.array([x[0, 0] for x in self.X]))
+            K, xd, yd = eng.gram(nx + len(Y), n_fit=nx, normalize=bool(self.normalize))
+        self._Y = Y
+        self._X_diag, self._Y_diag = xd, yd
+        self._is_transformed = True
+        if self.normalize:
+            self._warn_unnormalizable(xd, yd)
+        return K
+
+    def diagonal(self):
+        return self._pairwise_diagonal()

@@ -110,7 +110,8 @@ typedef struct gk_stats {
                                 PyramidMatch: 11 = one exact integer Gram per level + the fp64 combine,
                                 NeighborhoodSubgraphPairwiseDistance: 12 = one exact integer Gram per level + the fp64 fold,
                                 SubgraphMatching: 13 = per-pair clique counts + the lambda fold,
-                                OddSth: 14 = one exact integer Gram per bit of C + the fp64 sum of 2^b G_b */
+                                OddSth: 14 = one exact integer Gram per bit of C + the fp64 sum of 2^b G_b,
+                                MultiscaleLaplacian: 15 = per-pair FLG values, SvmTheta: 16 = fp64 product of first-level phi */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -328,6 +329,35 @@ int gk_ml_project(gk_handle* h, const double* Q, int32_t rows, int32_t cols, gk_
 int gk_ml_level(gk_handle* h, int32_t level, const int32_t* samples, int32_t ns, const double* samp_rec,
                 double* samp_rec_out, double* K_samples, gk_stats* stats);
 int gk_ml_finish(gk_handle* h, const double* fit_rec, int64_t n_fit, double* rec_out, gk_stats* stats);
+
+/* SvmTheta (svm_theta.py), fp64 throughout, per graph of 1 .. 128 vertices (more is GK_ERR_UNSUPPORTED).
+ *   gk_svmt_solve  sizes[N] vertices per graph, adj[V * 4] the row-major 128-bit out-edge masks of every vertex
+ *                  (bit j of row i: A[i][j] > 1e-10, diagonal cleared).  Launches, and returns without waiting for:
+ *                  the smallest eigenvalue m of the mask with its upper triangle mirrored (scipy's eigvalsh with
+ *                  lower=False), then libsvm's one-class SMO (nu = 0.5, tol = 1e-3, shrinking) on K = mask / -m with a
+ *                  unit diagonal when m < -1e-6, else on the mask itself, with libsvm's float Q entries and its rounding
+ *                  of every operation.  A solve that does not converge within 10^7 iterations is GK_ERR_RANGE in
+ *                  gk_svmt_phi.  stats: n_graphs, n_vertices.
+ *   gk_svmt_draw   host only: numpy's legacy `RandomState.choice(n, level, replace=False)` for every graph in order,
+ *                  every level lo + li (li < n_levels) not above n in ascending order, counts[g * n_levels + li] times
+ *                  each; appends the drawn indexes to idx[n_idx] (n_idx must be the schedule's total).  mt_key[624] /
+ *                  mt_pos are the MT19937 state of `get_state()`, advanced in place.
+ *   gk_svmt_phi    phi[g][li] = mean over the level's samples of the sum of the alphas at the drawn indexes (all n alphas
+ *                  for a level above n), 0 without samples, both in numpy's summation order; idx / counts as given to
+ *                  gk_svmt_draw.  A total index count other than the schedule's, or a drawn index not below its graph's
+ *                  vertex count, is GK_ERR_ARG.  Optional outputs: phi[N * n_levels], m_out[N], alpha_out[V], iters_out[N].  The
+ *                  first level of each graph follows fit_phi0[n_fit] (the fitted graphs', 0 in a fit) as the rows of
+ *                  gk_gram.  stats: ms_h2d (both calls' uploads), ms_features (eigenvalues), ms_rw (SMO), ms_combine
+ *                  (phi), ms_d2h.
+ * gk_gram (gram_path 16) returns K[r][c] = phi0[row_g0 + r] * phi0[c], fp64 only, host or GK_OUT_DEVICE output,
+ * GK_NORMALIZE (by sqrt(d_r d_c), d = phi0^2), n_fit and row ranges (n_fit counts rows).  GK_DIST and row maps are
+ * GK_ERR_UNSUPPORTED. */
+int gk_svmt_solve(gk_handle* h, int64_t n_graphs, const int32_t* sizes, const uint32_t* adj, gk_stats* stats);
+int gk_svmt_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int32_t* sizes, int32_t lo,
+                 int32_t n_levels, const int32_t* counts, uint8_t* idx, int64_t n_idx);
+int gk_svmt_phi(gk_handle* h, int32_t lo, int32_t n_levels, const int32_t* counts, const uint8_t* idx, int64_t n_idx,
+                const double* fit_phi0, int64_t n_fit, double* phi, double* m_out, double* alpha_out, int32_t* iters_out,
+                gk_stats* stats);
 
 /* Propagation / PropagationAttr (propagation.py:27-689).  The packed CSR (gk_pack_csr without weights; with the
  * label ids for the labelled kernel) is the sparsity pattern of every graph's row-normalised transition matrix T,
