@@ -24,7 +24,6 @@
 #include "spattr.cuh"
 #include "graph_hopper.cuh"
 #include "wl.cuh"
-#include "wl_fused.cuh"
 #include "wl_fused2.cuh"
 #include "wl_oa.cuh"
 #include "neighborhood_hash.cuh"
@@ -247,7 +246,6 @@ int gk_create(int device_ordinal, gk_handle** out) {
   GK_CUDA(cudaFuncSetAttribute(gram_tc2_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
-  GK_CUDA(cudaFuncSetAttribute(wl_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
   *out = h;
@@ -589,7 +587,7 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
   GK_TRY(h->ht_keys.ensure(h->ht_cap * 8 * 3));  // three tables: the fused kernel rotates them over the levels
   GK_TRY(h->ht_rep.ensure(h->ht_cap * 4 * 2));
   const size_t ft_level_cap = std::max<size_t>(next_pow2((size_t)V * 2), 1024);  // one L2-sized sub-table per level
-  // Fused persistent kernel (wl_fused.cuh) whenever the graphs can be cut into shared-memory tiles of
+  // Fused persistent kernel (wl_fused2.cuh) whenever the graphs can be cut into shared-memory tiles of
   // whole graphs; otherwise (a graph above the tile capacity) the multi-kernel path below.
   bool fused = true;
   if (const char* e = getenv("GRAKEL_B200_WL_FUSED")) fused = atoi(e) != 0;
@@ -632,14 +630,14 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
         for (int c = 0; c <= G; ++c) ct[c] = c * per;
         long long max_cta = 0;
         for (int c = 0; c < G; ++c) max_cta = std::max<long long>(max_cta, tv[ct[c + 1]] - tv[ct[c]]);
-        if (max_cta >= (1 << WLF_RANK_BITS)) ok = false;
+        if (max_cta >= WLF_CTA_V_LIMIT) ok = false;
       }
       if (h->max_graph_size > WLF_TILE_V) break;
     }
     fused = ok;
     if (fused) {
-      // layout of wlf_buf (ints): [tile_vbeg (T+1) | cta_tile (G+1) | cta_count (G) | barrier]
-      const size_t n_int = (size_t)(n_tiles + 1) + (G + 1) + G + 1;
+      // layout of wlf_buf (ints): [tile_vbeg (T+1) | cta_tile (G+1) | barrier]
+      const size_t n_int = (size_t)(n_tiles + 1) + (G + 1) + 1;
       GK_TRY(h->wlf_buf.ensure(n_int * 4));
       GK_TRY(h->h_tiles.ensure(((size_t)n_tiles + G + 2) * 4));
       int* hp = h->h_tiles.as<int>();
@@ -670,7 +668,7 @@ static int wl_launch_v2(gk_handle* h, const WlPlan& pl, unsigned long long seed,
       // wl_fused2.cuh: labels = representative vertex ids (one grid barrier per level), frozen singleton classes
       int* wb = h->wlf_buf.as<int>();
       int* d_cta_tile = wb + n_tiles + 1;
-      unsigned* d_barrier = reinterpret_cast<unsigned*>(d_cta_tile + G + 1 + G);
+      unsigned* d_barrier = reinterpret_cast<unsigned*>(d_cta_tile + G + 1);
       GK_TRY(h->wl_single.ensure((size_t)V + 16));
       GK_TRY(h->diag_frozen.ensure((size_t)h->N * 8));
       {  // one launch clears everything the kernel expects cleared (no host upload, no synchronisation)
@@ -736,14 +734,13 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
   WlPlan pl;
   GK_TRY(wl_setup(h, n_iter, &pl));
   const bool fused = pl.fused;
-  const int G = pl.G, nb = pl.nb, n_tiles = pl.n_tiles;
+  const int G = pl.G, nb = pl.nb;
   const size_t ft_level_cap = pl.ft_level_cap;
-  (void)n_tiles;
 
   DevScalars* sc = h->scalars.as<DevScalars>();
   int* labels_all = h->labels_all.as<int>();
   int retries = 0;
-  bool pro_enqueued = false, used_v2 = false;
+  bool pro_enqueued = false;
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   for (;; ++retries) {
     pro_enqueued = false;
@@ -752,14 +749,11 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
                                     [&] { char b[16]; snprintf(b, sizeof(b), "%x", h->h_scalars.as<DevScalars>()->collision); return std::string(b); }() + ")");
     const unsigned long long seed = mix64(0x5851F42D4C957F2DULL + 0x9E3779B97F4A7C15ULL * (unsigned long long)retries);
     const int degen_from = wl_take_degen(h);
-    const char* e_v1 = getenv("GRAKEL_B200_WL_V1");
-    const bool wl_v2 = fused && !(e_v1 && atoi(e_v1) != 0);
     FeatStats fst;
-    if (!wl_v2) GK_TRY(init_scalars(h, h->n_labels0));
-    GK_TRY(reset_feature_stats(h, (int64_t)h->n_labels0 + V * (int64_t)(L - 1) + 1, (int64_t)std::max(nb, G) * L, &fst, !wl_v2));
+    if (!fused) GK_TRY(init_scalars(h, h->n_labels0));
+    GK_TRY(reset_feature_stats(h, (int64_t)h->n_labels0 + V * (int64_t)(L - 1) + 1, (int64_t)std::max(nb, G) * L, &fst, !fused));
     h->wl_sparse_ids = false;
-    used_v2 = wl_v2;
-    if (wl_v2) {
+    if (fused) {
       const bool prof = getenv("GRAKEL_B200_PROF") != nullptr;
       GK_TRY(wl_launch_v2(h, pl, seed, degen_from, fst, prof));
       h->wl_sparse_ids = L > 1;
@@ -783,105 +777,12 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
         GK_CUDA(cudaMemcpyAsync(h->h_colstats.p, h->colstats.p, sizeof(ColStats), cudaMemcpyDeviceToHost, h->stream));
         pro_enqueued = true;
       }
-      if (prof) {
+      if (prof) {  // raw int64 globaltimer stamps [G][L][16] (tools/prof_wl_phases.py)
         std::vector<long long> pr((size_t)G * L * 16);
         GK_CUDA(cudaMemcpyAsync(pr.data(), h->K_stage.p, pr.size() * 8, cudaMemcpyDeviceToHost, h->stream));
         GK_CUDA(cudaStreamSynchronize(h->stream));
-        if (const char* out = getenv("GRAKEL_B200_PROF_OUT")) {  // raw int64 stamps [G][L][16] (tools/prof_wl_phases.py)
+        if (const char* out = getenv("GRAKEL_B200_PROF_OUT")) {
           if (FILE* f = fopen(out, "wb")) { fwrite(pr.data(), 8, pr.size(), f); fclose(f); }
-        }
-        long long t0 = pr[0];
-        for (int b = 0; b < G; ++b) t0 = std::min(t0, pr[(size_t)b * L * 16]);
-        fprintf(stderr, "[wl_fused2 prof] us; per level: avg over CTAs of the phase duration (max)\n");
-        for (int lv = 0; lv < L; ++lv) {
-          double avg[4] = {0}, mxv[4] = {0}, sub[5] = {0};
-          long long end_max = 0;
-          for (int b = 0; b < G; ++b) {
-            const long long* q = &pr[((size_t)b * L + lv) * 16];
-            end_max = std::max(end_max, q[6] - t0);
-            if (lv == 0) {
-              avg[3] += (double)(q[6] - q[0]) / G; mxv[3] = std::max(mxv[3], (double)(q[6] - q[0]));
-              sub[0] += (double)(q[1] - q[0]) / G; sub[1] += (double)(q[2] - q[1]) / G; sub[2] += (double)(q[3] - q[2]) / G; sub[3] += (double)(q[6] - q[3]) / G;
-              continue;
-            }
-            const double d[4] = {(double)(q[1] - q[0]), (double)(q[2] - q[1]), (double)(q[3] - q[2]), (double)(q[6] - q[3])};
-            for (int k = 0; k < 4; ++k) { avg[k] += d[k] / G; mxv[k] = std::max(mxv[k], d[k]); }
-            sub[0] += (double)(q[10] - q[0]) / G; sub[1] += (double)(q[1] - q[10]) / G;   // A: signatures | insert + copy-out
-            sub[2] += (double)(q[4] - q[2]) / G; sub[3] += (double)(q[5] - q[4]) / G; sub[4] += (double)(q[3] - q[5]) / G;  // B: verify | labels | emit
-          }
-          if (lv == 0) {
-            fprintf(stderr, "  level 0: %.1f (%.1f) = stage %.1f + emit %.1f + table clear %.1f + flush %.1f | done at %.1f us\n", avg[3] / 1e3, mxv[3] / 1e3,
-                    sub[0] / 1e3, sub[1] / 1e3, sub[2] / 1e3, sub[3] / 1e3, end_max / 1e3);
-            continue;
-          }
-          fprintf(stderr, "  level %d: A %.1f (%.1f) wait %.1f (%.1f) B+emit %.1f (%.1f) clear+flush %.1f (%.1f) | A = sig %.1f + insert %.1f | B = verify %.1f + labels %.1f + emit %.1f | level done at %.1f us\n", lv,
-                  avg[0] / 1e3, mxv[0] / 1e3, avg[1] / 1e3, mxv[1] / 1e3, avg[2] / 1e3, mxv[2] / 1e3, avg[3] / 1e3, mxv[3] / 1e3,
-                  sub[0] / 1e3, sub[1] / 1e3, sub[2] / 1e3, sub[3] / 1e3, sub[4] / 1e3, end_max / 1e3);
-        }
-      }
-    } else if (fused) {
-      // one persistent cooperative kernel for all levels; it appends (graph, column, count) entries
-      // to ft_keys / ft_cnt used as a compact COO list
-      if (L > 1) GK_CUDA(cudaMemsetAsync(h->ht_keys.as<unsigned long long>() + h->ht_cap, 0xFF, h->ht_cap * 8, h->stream));
-      int* wb = h->wlf_buf.as<int>();
-      int* d_cta_tile = wb + n_tiles + 1;
-      int* d_cta_count = d_cta_tile + G + 1;
-      unsigned* d_barrier = reinterpret_cast<unsigned*>(d_cta_count + G);
-      GK_CUDA(cudaMemsetAsync(d_barrier, 0, 4, h->stream));
-      WlFusedParams fp;
-      memset(&fp, 0, sizeof(fp));
-      fp.V = (int)V; fp.L = L;
-      fp.graph_ptr = h->graph_ptr.as<int>();
-      fp.row_ptr = h->row_ptr.as<int>(); fp.col_idx = h->col_idx.as<int>(); fp.vgraph = h->vgraph.as<int>();
-      fp.labels0 = h->labels0.as<int>(); fp.tile_vbeg = wb; fp.cta_tile = d_cta_tile; fp.cta_count = d_cta_count;
-      fp.barrier = d_barrier;
-      fp.labels_all = labels_all; fp.sig_nbr = h->sig_nbr.as<int>(); fp.slot_of = h->slot_of.as<int>();
-      fp.rank_pack = h->flags.as<int>();
-      GK_TRY(h->wl_single.ensure((size_t)V));  // singleton flags (wl_fused.cuh)
-      GK_CUDA(cudaMemsetAsync(h->wl_single.p, 0, (size_t)V, h->stream));
-      fp.single = h->wl_single.as<unsigned char>();
-      fp.table = h->ht_keys.as<unsigned long long>();
-      fp.ht_mask = (unsigned)(h->ht_cap - 1);
-      fp.coo_keys = h->ft_keys.as<unsigned long long>(); fp.coo_cnt = h->ft_cnt.as<unsigned>();
-      fp.seed = seed; fp.degen_from = degen_from; fp.st = fst; fp.sc = sc;
-      const bool prof = getenv("GRAKEL_B200_PROF") != nullptr;
-      if (prof) {
-        GK_TRY(h->K_stage.ensure((size_t)G * L * 128));
-        GK_CUDA(cudaMemsetAsync(h->K_stage.p, 0, (size_t)G * L * 128, h->stream));
-        fp.prof = h->K_stage.as<long long>();
-      }
-      void* args[] = {&fp};
-      GK_CUDA(cudaLaunchCooperativeKernel((void*)wl_fused_kernel, dim3(G), dim3(WLF_THREADS), args, WLF_SMEM, h->stream));
-      LAUNCH_CHECK(h);
-      if (prof) {
-        std::vector<long long> pr((size_t)G * L * 16);
-        GK_CUDA(cudaMemcpyAsync(pr.data(), h->K_stage.p, pr.size() * 8, cudaMemcpyDeviceToHost, h->stream));
-        GK_CUDA(cudaStreamSynchronize(h->stream));
-        long long t0 = pr[0];
-        for (int b = 0; b < G; ++b) t0 = std::min(t0, pr[(size_t)b * L * 16]);
-        fprintf(stderr, "[wl_fused prof] ns since kernel start; per level: phase = avg over CTAs of its duration (max)\n");
-        for (int lv = 0; lv < L; ++lv) {
-          const char* names[6] = {"A", "wait1", "B", "clear", "wait2", "C"};
-          double avg[6] = {0}, mx[6] = {0};
-          long long end_max = 0;
-          for (int b = 0; b < G; ++b) {
-            const long long* q = &pr[((size_t)b * L + lv) * 16];
-            end_max = std::max(end_max, q[6] - t0);
-            if (lv == 0) { avg[5] += (double)(q[6] - q[0]) / G; mx[5] = std::max(mx[5], (double)(q[6] - q[0])); continue; }
-            for (int k = 0; k < 6; ++k) { const double d = (double)(q[k + 1] - q[k]); avg[k] += d / G; mx[k] = std::max(mx[k], d); }
-          }
-          fprintf(stderr, "  level %d:", lv);
-          for (int k = 0; k < 6; ++k) fprintf(stderr, " %s %.1f (%.1f)", names[k], avg[k] / 1e3, mx[k] / 1e3);
-          if (lv) {  // split of phase A (last tile of each CTA): stage | thread-per-vertex | warp-per-vertex | copy-out
-            double sa[4] = {0};
-            for (int b = 0; b < G; ++b) {
-              const long long* q = &pr[((size_t)b * L + lv) * 16];
-              sa[0] += (double)(q[8] - q[0]) / G; sa[1] += (double)(q[9] - q[8]) / G;
-              sa[2] += (double)(q[10] - q[9]) / G; sa[3] += (double)(q[1] - q[10]) / G;
-            }
-            fprintf(stderr, " | A = stage %.1f + thread %.1f + warp %.1f + out %.1f", sa[0] / 1e3, sa[1] / 1e3, sa[2] / 1e3, sa[3] / 1e3);
-          }
-          fprintf(stderr, " | level done at %.1f us\n", end_max / 1e3);
         }
       }
     } else {
@@ -932,7 +833,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
     if (hs->ft_overflow) return fail(GK_ERR_STATE, "gk_wl_features: feature table overflow");
     if (!hs->collision) break;
   }
-  if (!used_v2) {  // (wl_fused2 recorded the end of its stage right after the kernel; read_scalars synchronised)
+  if (!fused) {  // (wl_fused2 recorded the end of its stage right after the kernel; read_scalars synchronised)
     GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
     GK_CUDA(cudaEventSynchronize(h->tev[3]));
   }
@@ -5226,7 +5127,7 @@ int gk_tu_close(gk_tu* t) {
 static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_out, int32_t out_dtype, int64_t ld,
                          double* xdiag, gk_stats* stats, bool* done) {
   *done = false;
-  for (const char* name : {"GRAKEL_B200_NO_ASYNC", "GRAKEL_B200_PROF", "GRAKEL_B200_WL_V1", "GRAKEL_B200_WL_FUSED",
+  for (const char* name : {"GRAKEL_B200_NO_ASYNC", "GRAKEL_B200_PROF", "GRAKEL_B200_WL_FUSED",
                            "GRAKEL_B200_CTA2", "GRAKEL_B200_NO_TMA_STORE", "GRAKEL_B200_WIDEN", "GRAKEL_B200_NO_TRI",
                            "GRAKEL_B200_MIRROR_TMA", "GRAKEL_B200_DEBUG"})
     if (getenv(name)) return GK_OK;

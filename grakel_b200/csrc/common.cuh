@@ -164,10 +164,10 @@ struct gk_handle {
   gk::DevBuf ht_keys, ht_rep;
   size_t ht_cap = 0;
   gk::DevBuf flags, block_sums;
-  gk::DevBuf wlf_buf;  // fused WL kernel: [cta_vbeg (G+1) | cta_count (G) | barrier]
-  gk::DevBuf wl_payload;  // fused WL kernel v2: [2][ht_cap] 32-byte slot payloads (the installing vertex's signature)
-  gk::DevBuf wl_single;  // fused WL kernels: one byte per vertex (singleton class / frozen)
-  gk::DevBuf diag_frozen;  // fused WL kernel v2: frozen vertices' share of the self similarities (u64 per graph)
+  gk::DevBuf wlf_buf;  // fused WL kernel: [tile_vbeg (T+1) | cta_tile (G+1) | barrier]
+  gk::DevBuf wl_payload;  // fused WL kernel: [2][ht_cap] 32-byte slot payloads (the installing vertex's signature)
+  gk::DevBuf wl_single;  // fused WL kernel: one byte per vertex (frozen flag)
+  gk::DevBuf diag_frozen;  // fused WL kernel: frozen vertices' share of the self similarities (u64 per graph)
   bool wl_sparse_ids = false;  // labels of levels >= 1 are representative vertex ids (wl_fused2), not dense ranks
   gk::DevBuf scalars;  // gk::DevScalars
   gk::PinBuf h_scalars;

@@ -1,13 +1,24 @@
-// All WL levels in ONE persistent cooperative kernel, second generation (weisfeiler_lehman.py:199-258 +
-// vertex_histogram.py:107-122 for every level).  Same tile / shared-memory organisation and the same exact
-// hash-proposes / signature-verifies dedup as wl_fused.cuh; what changed is what a level has to do:
+// All WL levels in ONE persistent cooperative kernel (weisfeiler_lehman.py:199-258 + vertex_histogram.py:107-122 for
+// every level), staged through shared memory.
 //
+// Why: the multi-kernel pipeline of wl.cuh spends each level in five latency-bound launches, far above its HBM floor.
+// Micro-benchmarks (tools/mb/wl_mb.cu) show the limit is the number of SCATTERED L2 operations per vertex, so this
+// kernel is organised to minimise them:
+//
+//   * The graphs are cut into TILES of whole graphs (<= WLF_TILE_V vertices, <= WLF_TILE_E edges); each CTA owns a
+//     contiguous run of tiles.  A tile's CSR slice and labels are staged into shared memory with coalesced loads;
+//     neighbour gathers, sorting and the per-graph label counts never leave shared memory.
+//   * Signature dedup: the hash proposes, the signature verifies.  ONE packed 64-bit word per slot, {tag | single |
+//     representative vertex}: insert = one CAS, plus one atomicMin when a further member of the class has to clear
+//     the single bit or bring a smaller representative.
+//   * (graph, column) counts are produced inside the graph in shared memory (a graph never straddles a tile) and
+//     written to a compact COO list: no global feature hash table to fill and clear per level.
 //   * The compressed label of a class is the id of its REPRESENTATIVE vertex (the smallest vertex of the class),
 //     not a dense rank.  The reference's ids never leave the estimator (SURVEY 7: "bit-exact integer labels" =
-//     identical label partition), and K only needs distinct columns per class.  So the second half of a level
-//     -- CTA-local ranks, the scan of the CTA counts, the rank gather -- and with it the SECOND grid barrier
-//     disappear: a level is   [A] signatures + insert | grid barrier | [B] representative, verification,
-//     labels, feature entries.   Level l >= 1 owns the column range [n_labels0 + (l-1) V, n_labels0 + l V).
+//     identical label partition), and K only needs distinct columns per class.  So a level needs no CTA-local ranks,
+//     no scan of the CTA counts and no rank gather, and ONE grid barrier: a level is   [A] signatures + insert | grid
+//     barrier | [B] representative, verification, labels, feature entries.   Level l >= 1 owns the column range
+//     [n_labels0 + (l-1) V, n_labels0 + l V).
 //     Dense first-occurrence ids (gk_wl_labels, the WL-SP base kernel) are produced on demand by wl_densify.
 //   * A vertex whose class has a single member in the whole data set is FROZEN: its label (= its own id) never
 //     changes again, it needs no signature, insert or verification at deeper levels, and its feature column
@@ -22,14 +33,94 @@
 //   * A CTA that owns one tile keeps its CSR slice, labels and frozen flags resident in shared memory across
 //     levels.
 //
-// Exactness is unchanged: every non-frozen vertex's full signature (own label, degree, sorted neighbour labels)
+// Exactness: every non-frozen vertex's full signature (own label, degree, sorted neighbour labels)
 // is compared with its representative's; a mismatch raises the collision flag and the host retries with a new seed.
 #pragma once
 #include "common.cuh"
 #include "wl.cuh"
-#include "wl_fused.cuh"
 
 namespace gk {
+
+constexpr int WLF_THREADS = 1024;
+constexpr int WLF_TILE_V = 4096;    // vertices per tile (u16 local indices)
+constexpr int WLF_TILE_E = 16384;   // edges per tile
+constexpr int WLF_VPT = WLF_TILE_V / WLF_THREADS;  // vertices per thread and tile (register batches)
+constexpr int WLF_AGG = 8192;       // per-tile column -> graph-count aggregation table (shared memory)
+static_assert(WLF_AGG * 8 <= WLF_TILE_E * 4, "aggregation table must fit in the sig_s region");
+constexpr int WLF_CTA_V_LIMIT = 1 << 20;  // vertices per CTA: an input whose tiles give a CTA this many or more takes
+                                          // the per-level kernels (wl.cuh)
+
+__device__ __forceinline__ long long wlf_now() {
+  long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define WLF_STAMP(level, k) \
+  do { if (p.prof && tid == 0) p.prof[((size_t)b * p.L + (level)) * 16 + (k)] = wlf_now(); } while (0)
+
+__device__ __forceinline__ void wlf_grid_sync(unsigned* bar, unsigned target) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    atomicAdd(bar, 1u);
+    unsigned seen;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(bar) : "memory");
+    } while (seen < target);
+    __threadfence();
+  }
+  __syncthreads();
+}
+
+// block-wide exclusive scan for 1024 threads; returns the exclusive prefix, *total = block sum
+__device__ __forceinline__ int wlf_block_scan(int x, int* total, int* s_warp /*[32]*/) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int incl = x;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += y;
+  }
+  if (lane == 31) s_warp[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    int s = s_warp[lane];
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, s, d);
+      if (lane >= d) s += y;
+    }
+    s_warp[lane] = s;
+  }
+  __syncthreads();
+  const int off = wid ? s_warp[wid - 1] : 0;
+  *total = s_warp[31];
+  __syncthreads();
+  return off + incl - x;
+}
+
+// ---- signature hashes (32-bit arithmetic; two independent lanes -> {tag, home slot}).
+// Equal signatures have equal degree, hence always take the same code path, so the
+// thread-per-vertex path (sequential over the sorted labels) and the warp path (sum of
+// positional terms) may use different functions.  Exactness never depends on the hash:
+// every vertex is verified against its representative and a clash makes the host retry.
+__device__ __forceinline__ unsigned wlf_fmix(unsigned h) {
+  h ^= h >> 16; h *= 0x85EBCA6Bu; h ^= h >> 13; h *= 0xC2B2AE35u; h ^= h >> 16;
+  return h;
+}
+__device__ __forceinline__ unsigned long long wlf_finish(unsigned a, unsigned c, int own, int deg, unsigned long long seed) {
+  a = wlf_fmix(a ^ ((unsigned)own * 0x9E3779B1u) ^ (unsigned)seed);
+  c = wlf_fmix(c + (unsigned)own * 0x7FEB352Du + (unsigned)deg * 0x846CA68Bu + (unsigned)(seed >> 32));
+  return (((unsigned long long)a << 32) | c) >> 1;  // never EMPTY64
+}
+__device__ __forceinline__ void wlf_seq_step(unsigned& a, unsigned& c, int x) {
+  a = (a ^ (unsigned)x) * 0x9E3779B1u; a ^= a >> 15;
+  c = (c + (unsigned)x) * 0x85EBCA77u; c ^= c >> 13;
+}
+__device__ __forceinline__ void wlf_pos_term(unsigned& a, unsigned& c, int x, int pos, unsigned long long seed) {
+  a += wlf_fmix((unsigned)x * 0x9E3779B1u + (unsigned)pos * 0x85EBCA77u + (unsigned)seed);
+  c += wlf_fmix(((unsigned)x ^ 0x5bd1e995u) * 0xC2B2AE3Du + (unsigned)pos * 0x27D4EB2Fu + (unsigned)(seed >> 32));
+}
 
 struct WlFused2Params {
   int V, L;
@@ -232,8 +323,10 @@ __device__ __forceinline__ int wlf2_compact(int nv, const unsigned char* frz_s, 
   return n_act;
 }
 
-constexpr int WLF2_SMEM = WLF_SMEM + WLF_TILE_V /*frz_s*/ + WLF_TILE_V * 4 /*gid_s*/ + WLF_TILE_V * 4 /*gbeg_s, gend_s*/ +
-                          WLF_TILE_V * 4 /*slot_s | list_s*/ + WLF_TILE_V * 2 /*cf_s*/;
+constexpr int WLF2_SMEM = (WLF_TILE_V + 2) * 4 /*rp_s*/ + WLF_TILE_V * 8 /*key_s | ct*/ + WLF_TILE_V * 4 /*lab_s*/ +
+                          WLF_TILE_E * 4 /*sig_s | agg*/ + WLF_TILE_E * 2 /*col_s*/ + WLF_TILE_V /*frz_s*/ +
+                          WLF_TILE_V * 4 /*gid_s*/ + WLF_TILE_V * 4 /*gbeg_s, gend_s*/ + WLF_TILE_V * 4 /*slot_s | list_s*/ +
+                          WLF_TILE_V * 2 /*cf_s | act_s*/ + 16;
 static_assert(WLF2_SMEM <= 232448, "shared memory budget of one CTA");
 
 // Global -> shared staging of a tile with several loads in flight per thread.  A plain strided loop keeps ONE load

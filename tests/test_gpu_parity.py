@@ -296,9 +296,9 @@ def test_high_degree_and_empty_edge_graphs():
         _same(k.ShortestPath().fit_transform(X[:4]), SPOracle().fit_transform(X[:4]))
 
 
-@pytest.mark.parametrize("fused", ["0", "1", "1-multitile", "v1", "payload0", "payload0-multitile"])
+@pytest.mark.parametrize("fused", ["0", "1", "1-multitile", "payload0", "payload0-multitile"])
 def test_wl_fused_and_multikernel_paths_agree(fused, monkeypatch, eng):
-    """The persistent cooperative WL kernel (wl_fused.cuh) and the per-level kernels (wl.cuh)
+    """The persistent cooperative WL kernel (wl_fused2.cuh) and the per-level kernels (wl.cuh)
     must produce the same labels (first-occurrence ids), level sizes and Gram matrix -- on a
     sparse set (thread-per-vertex signatures), on a set with hubs of degree > 32 (warp path)
     and on a block smaller than the grid (empty CTA ranges)."""
@@ -307,9 +307,6 @@ def test_wl_fused_and_multikernel_paths_agree(fused, monkeypatch, eng):
         fused = fused.replace("payload0", "1")
     if fused == "1-multitile":  # several tiles per CTA: shared memory is re-staged per tile and level (large inputs)
         monkeypatch.setenv("GRAKEL_B200_WL_TILES_PER_CTA", "3")
-        fused = "1"
-    if fused == "v1":  # the first-generation fused kernel (dense ranks, two barriers per level)
-        monkeypatch.setenv("GRAKEL_B200_WL_V1", "1")
         fused = "1"
     monkeypatch.setenv("GRAKEL_B200_WL_FUSED", fused)
     k = _k()

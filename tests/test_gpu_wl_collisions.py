@@ -29,7 +29,6 @@ ROUTES = {
     "payload0": {"GRAKEL_B200_WL_PAYLOAD": "0"},  # wl_fused2, verification against the representative's row
     "multitile": {"GRAKEL_B200_WL_TILES_PER_CTA": "3"},  # wl_fused2, tiles re-staged per level (non-resident)
     "multitile-payload0": {"GRAKEL_B200_WL_TILES_PER_CTA": "3", "GRAKEL_B200_WL_PAYLOAD": "0"},
-    "v1": {"GRAKEL_B200_WL_V1": "1"},  # wl_fused.cuh
     "multikernel": {"GRAKEL_B200_WL_FUSED": "0"},  # wl_sig_* + wl_resolve
 }
 V2_ROUTES = ("default", "payload0", "multitile", "multitile-payload0")

@@ -2,7 +2,7 @@
 of its hash-table placement, for the natural-collision test.
 
 Key: wlf_seq_step over the sorted neighbour labels from (0x243F6A88, 0x85A308D3), then wlf_finish with the first-attempt
-seed mix64(0x5851F42D4C957F2D) (wl_fused.cuh).  Table: the start slot ((key & 0xFFFFFFFF) * 0x9E3779B1 >> 8) & mask and
+seed mix64(0x5851F42D4C957F2D) (wl_fused2.cuh).  Table: the start slot ((key & 0xFFFFFFFF) * 0x9E3779B1 >> 8) & mask and
 the tag key >> 33 ([A3]).  Two distinct signatures with equal tag and start slot meet in one slot and only the
 verification in [B] can tell them apart.  If the kernel's hash changes, this file must change with it (the GPU test
 then sees no collision)."""
