@@ -3866,6 +3866,16 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   const int64_t launches0 = h->launches;
   HandleExtra* ex = extra_of(h);
   h->features_ready = false; h->feat_serial++;
+  const std::vector<int>& gp = ex->graph_ptr;
+  long long max_n = 1, max_e = 1;
+  for (int64_t g = 0; g < N; ++g) {
+    max_n = std::max<long long>(max_n, gp[g + 1] - gp[g]);
+    max_e = std::max<long long>(max_e, ex->graph_eptr[g + 1] - ex->graph_eptr[g]);
+  }
+  // refused before any table is sized: the level matrices alone take 5 n^2 bytes per graph
+  const long long ball = r > 0 ? max_n + 1 : 1;
+  if (ball * ball >= (1LL << 32))  // label offsets are u32
+    return fail(GK_ERR_UNSUPPORTED, "gk_nspd_features: r > 0 with a graph of 65535 or more vertices");
   h->nspd_r = r; h->nspd_d = d;
   GK_TRY(init_scalars(h, 0));
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
@@ -3874,12 +3884,6 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   GK_TRY(nspd_build_params(h, sym_hash, edge_label, tok_rank, n_labels, rank_off, rank_bytes, rank_cp, n_ranks, el_off,
                            el_bytes, el_cp, n_elabels, &p, &loff));
   const long long P = loff[N];
-  const std::vector<int>& gp = ex->graph_ptr;
-  long long max_n = 1, max_e = 1;
-  for (int64_t g = 0; g < N; ++g) {
-    max_n = std::max<long long>(max_n, gp[g + 1] - gp[g]);
-    max_e = std::max<long long>(max_e, ex->graph_eptr[g + 1] - ex->graph_eptr[g]);
-  }
   // ---- BFS levels
   GK_TRY(h->nspd_lvl.ensure((size_t)std::max<long long>(P, 1)));
   GK_TRY(h->nspd_q.ensure((size_t)std::max<long long>(P, 1) * 4));
@@ -3894,9 +3898,7 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   p.set_cap = (long long)nspd_set_cap(max_e);
   p.max_e = max_e;
   p.max_n = max_n;
-  p.ball = r > 0 ? max_n + 1 : 1;
-  if (p.ball * p.ball >= (1LL << 32))  // label offsets are u32
-    return fail(GK_ERR_UNSUPPORTED, "gk_nspd_features: r > 0 with a graph of 65535 or more vertices");
+  p.ball = ball;
   p.slot_words = nspd_slot_words(p.set_cap, max_e, max_n, p.ball);
   size_t budget = (size_t)4 << 30;
   if (const char* e = getenv("GRAKEL_B200_NSPD_WS_BUDGET")) budget = std::max<size_t>(1, strtoull(e, nullptr, 10));

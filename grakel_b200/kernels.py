@@ -2928,6 +2928,9 @@ class NeighborhoodSubgraphPairwiseDistance(Kernel):
                 np.array(el, dtype=np.int64), np.array(sh, dtype=np.int64), tokens)
 
     def _nspd_run(self, graphs, n_fit, want_matrix=True, device_ptr=None, row_range=None, simt=False):
+        if self.r > 0 and max(g[0] for g in graphs) >= 65535:  # the device refuses it too; do not pack it first
+            raise NotImplementedError("NeighborhoodSubgraphPairwiseDistance: r > 0 with a graph of 65535 or more "
+                                      "vertices")
         gp, rp, ci, lab, el, sh, tokens = self._pack(graphs)
         with _lib.engine(getattr(self, "device_", None)) as eng:
             eng.pack(gp, rp, ci, lab, None, None)

@@ -58,8 +58,19 @@ def neighborhoods(n, edges, r, d):
     return N, D, dp
 
 
+_HASHES = {}
+
+
 def hashes(graph, r, d):
-    """H[(rho, v)] of one parsed graph (n, edges, vertex label strings, edge label strings)."""
+    """H[(rho, v)] of one parsed graph (n, edges, vertex label strings, edge label strings), memoised: a test that
+    compares fit_transform, transform and their normalised forms hashes every graph once."""
+    key = (graph[0], tuple(graph[1]), tuple(graph[2]), tuple(graph[3]), r, d)
+    if key not in _HASHES:
+        _HASHES[key] = _hashes(graph, r, d)
+    return _HASHES[key]
+
+
+def _hashes(graph, r, d):
     n, edges, vl, el = graph
     elab = dict(zip(edges, el))
     N, D, dp = neighborhoods(n, edges, r, d)

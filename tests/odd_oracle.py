@@ -77,11 +77,34 @@ def first_counts(phis):
 def kernel(X, Y=None, h=None, normalize=False):
     """fit_transform(X) or, with Y, transform(Y) after fit(X); exact integers in fp64."""
     px = features(X, h)
-    py = px if Y is None else features(Y, h)
-    C = first_counts(px + ([] if Y is None else py))
-    K = np.array([[sum(C[f] * c * q.get(f, 0) for f, c in a.items()) for q in px] for a in py], dtype=np.float64)
-    if normalize:
+    return gram(px, None if Y is None else features(Y, h), normalize)
+
+
+def gram(px, py=None, normalize=False):
+    """kernel() of the feature Counters of the fitted graphs (px) and of the transformed ones (py, None for
+    fit_transform).  The sums are exact: int64 sparse products when every self similarity, and so (Cauchy-Schwarz)
+    every entry, stays below 2^62 (thousands of graphs), Python integers otherwise."""
+    C = first_counts(px + ([] if py is None else py))
+    py_ = px if py is None else py
+    col = {f: i for i, f in enumerate(C)}
+    if max([sum(C[f] * c * c for f, c in p.items()) for p in px + py_] or [0]) < 2 ** 62:
+        from scipy.sparse import csr_matrix
+
+        def mat(ps):
+            rows = [i for i, p in enumerate(ps) for _ in p]
+            cols = [col[f] for p in ps for f in p]
+            vals = [c for p in ps for c in p.values()]
+            return csr_matrix((np.array(vals, dtype=np.int64), (rows, cols)), shape=(len(ps), len(col)))
+        cw = np.array(list(C.values()), dtype=np.int64)
+        ax, ay = mat(px), mat(py_)
+        K = np.asarray((ay.multiply(cw[None, :]).tocsr() @ ax.T).todense(), dtype=np.int64).astype(np.float64)
+        dx = np.asarray(ax.multiply(ax).multiply(cw[None, :]).sum(axis=1), dtype=np.int64).ravel().astype(np.float64)
+        dy = np.asarray(ay.multiply(ay).multiply(cw[None, :]).sum(axis=1), dtype=np.int64).ravel().astype(np.float64)
+    else:
+        K = np.array([[sum(C[f] * c * q.get(f, 0) for f, c in a.items()) for q in px] for a in py_], dtype=np.float64)
         dx = np.array([sum(C[f] * c * c for f, c in a.items()) for a in px], dtype=np.float64)
-        dy = dx if Y is None else np.array([sum(C[f] * c * c for f, c in a.items()) for a in py], dtype=np.float64)
+        dy = np.array([sum(C[f] * c * c for f, c in a.items()) for a in py_], dtype=np.float64)
+    K = K.reshape(len(py_), len(px))
+    if normalize:
         K = K / np.sqrt(np.outer(dy, dx))
     return K

@@ -46,6 +46,23 @@ def test_set_order_matches_interpreter(seed):
         _check_order(sub)
 
 
+@pytest.mark.parametrize("size", [19660, 19661, 78642, 78643, 78644, 157286, 320000])
+def test_set_order_past_the_doubling_resizes(size):
+    """Sizes around the table's growth steps: x4 up to 50 000 items (at insert 19 661 into 131 072 slots), x2 above
+    (at inserts 78 643, 157 286 and 314 573), each with a chained set built by iterating the first one."""
+    rng = random.Random(size)
+    pool = list(range(-700, 700))
+    items = set()
+    while len(items) < size:
+        items.add((rng.choice(pool), rng.choice(pool)))
+    seq = list(items)
+    rng.shuffle(seq)
+    _check_order(seq)
+    first = list({t for t in seq})
+    _check_order(first)
+    _check_order([t for t in first if rng.random() < 0.9])
+
+
 def test_errors_and_warnings():
     with pytest.raises(ValueError, match="r must be a positive integer"):
         NeighborhoodSubgraphPairwiseDistance(r=-1).fit([])
