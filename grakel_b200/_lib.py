@@ -95,6 +95,10 @@ _SYMBOLS = {
     "gk_svmt_draw": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int32, C.c_int32, _P, _P, C.c_int64]),
     "gk_svmt_phi": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, C.c_int64, _P, C.c_int64, _P, _P, _P, _P,
                               C.POINTER(GkStats)]),
+    "gk_gs_draw": (C.c_int, [_P, _P, C.c_int64, _P, C.c_int32, C.c_int64, _P, _P, C.c_int64, _P]),
+    "gk_gs_features": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P, C.c_int64, _P, C.c_int64,
+                                 C.POINTER(GkStats)]),
+    "gk_gs_counts": (C.c_int, [_P, C.c_int64, _P, _P]),
     "gk_pk_features": (C.c_int, [_P, C.c_int32, C.c_double, _P, _P, C.c_int32, C.c_int32, C.c_int64, _P, _P, C.c_int32,
                                  C.POINTER(GkStats)]),
     "gk_pk_hashes": (C.c_int, [_P, C.c_int32, _P, _P]),
@@ -208,6 +212,27 @@ def svmt_draw(rs, sizes, lo, counts):
         raise GrakelB200Error(lib.gk_last_error().decode())
     rs.set_state((name, key, p.value, has_gauss, gauss))
     return idx
+
+
+def gs_draw(rs, sizes, k, n_samples):
+    """Host only: GraphletSampling's draws for every graph of `sizes` in order, n_samples each (gk_gs_draw): the size
+    rs.randint(min(3, n), min(k, n) + 1) (none when the range is one size) and rs.choice(n, size, replace=False).
+    Returns (sizes of the samples u8, their indexes i32 concatenated); `rs` continues after them."""
+    name, key, pos, has_gauss, gauss = rs.get_state()
+    key = np.array(key, dtype=np.uint32)
+    p = C.c_int32(int(pos))
+    sz = _i32(sizes)
+    cap = int(n_samples) * int(np.minimum(sz, k).sum())
+    size = np.empty(len(sz) * int(n_samples), dtype=np.uint8)
+    idx = np.empty(max(cap, 1), dtype=np.int32)
+    n = C.c_int64()
+    lib = load_library()
+    if lib.gk_gs_draw(_ptr(key), C.byref(p), len(sz), _ptr(sz), int(k), int(n_samples), _ptr(size), _ptr(idx), cap,
+                      C.byref(n)) != 0:
+        msg = lib.gk_last_error().decode()
+        raise NotImplementedError(msg) if "more than 6" in msg else GrakelB200Error(msg)
+    rs.set_state((name, key, p.value, has_gauss, gauss))
+    return size, idx[:n.value]
 
 
 class _HostBlock:
@@ -489,6 +514,28 @@ class Engine:
                                              0 if fp is None else len(fp), _ptr(phi),
                                              *(_ptr(a) for a in (det or (None, None, None))), C.byref(st)))
         return phi, det, st
+
+    def gs_features(self, k, n_fit, g0, samp_off, samp_size, idx, prior=None):
+        """GraphletSampling classes and (graph, class) counts of the packed graphs (gk_gs_features): the samples of the
+        graphs g0 .. N-1, the counts `prior` [n, 3] (graph, class code, samples) of the graphs before g0."""
+        so = np.ascontiguousarray(samp_off, dtype=np.int64)
+        ss = np.ascontiguousarray(samp_size, dtype=np.uint8)
+        ix = _i32(idx)
+        pr = None if prior is None or len(prior) == 0 else np.ascontiguousarray(prior, dtype=np.int64)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_gs_features(self.h, int(k), int(n_fit), int(g0), _ptr(so), _ptr(ss), _ptr(ix),
+                                                len(ix), _ptr(pr), 0 if pr is None else len(pr), C.byref(st)))
+        return st
+
+    def gs_counts(self):
+        """[n, 4] int64 rows (graph, class code, samples, count) of the last gs_features, by graph and code."""
+        n = C.c_int64()
+        with self._lock:
+            self._check(self.lib.gk_gs_counts(self.h, 0, None, C.byref(n)))
+            out = np.empty((n.value, 4), dtype=np.int64)
+            self._check(self.lib.gk_gs_counts(self.h, n.value, _ptr(out), C.byref(n)))
+        return out
 
     def pk_features(self, t_max, w, u, b, dim, dim_orig, n_fit, t_values, p0=None, flags=0):
         """Propagation bins of t_max levels and their (graph, column) counts (gk_pk_features).  u: [t_max, dim],

@@ -1,6 +1,7 @@
 // C-ABI of the grakel_b200 engine (see include/grakel_b200.h for the contract and
 // the reference file:line each entry point replaces).  sm_90a (H100) only.
 #include <algorithm>
+#include <array>
 #include <climits>
 #include <cmath>
 #include <cstdlib>
@@ -36,6 +37,7 @@
 #include "odd_sth.cuh"
 #include "multiscale_laplacian.cuh"
 #include "svm_theta.cuh"
+#include "graphlet_sampling.cuh"
 #include "tu_reader.h"
 #include "comm.h"
 
@@ -354,7 +356,9 @@ int gk_destroy(gk_handle* h) {
                         &h->ml_adj, &h->ml_adj_off, &h->ml_ball, &h->ml_U, &h->ml_U2, &h->ml_vrec, &h->ml_samp, &h->ml_rec,
                         &h->ml_aux, &h->ml_ctl,
                         &h->svmt_vptr, &h->svmt_adj, &h->svmt_m, &h->svmt_alpha, &h->svmt_iters, &h->svmt_cnt,
-                        &h->svmt_off, &h->svmt_idx, &h->svmt_sums, &h->svmt_phi, &h->svmt_rec, &h->svmt_ctl};
+                        &h->svmt_off, &h->svmt_idx, &h->svmt_sums, &h->svmt_phi, &h->svmt_rec, &h->svmt_ctl,
+                        &h->gs_canon, &h->gs_first, &h->gs_colid, &h->gs_blk, &h->gs_colcnt, &h->gs_diag, &h->gs_ctl,
+                        &h->gs_samp};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -1653,6 +1657,7 @@ static const GramRules GRAM_RULES[] = {
     /* FK_ODD    */ {"OddSth", false, true, false, false},
     /* FK_ML     */ {"MultiscaleLaplacian", false, true, false, false},
     /* FK_SVMT   */ {"SvmTheta", false, true, false, false},
+    /* FK_GS     */ {"GraphletSampling", false, true, false, false},
 };
 
 static int gram_request(gk_handle* h, FeatureKind kind, int64_t n_fit, int32_t flags, int64_t row_begin,
@@ -4846,12 +4851,7 @@ int gk_svmt_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int3
       const int level = lo + li;
       if (level > n) continue;  // the reference sums all n alphas without drawing
       for (int32_t s = 0; s < counts[g * n_levels + li]; ++s) {
-        // choice(n, level, replace=False): the first `level` entries of a Fisher-Yates shuffle of arange(n)
-        for (int i = 0; i < n; ++i) perm[i] = (uint8_t)i;
-        for (int i = n - 1; i >= 1; --i) {
-          const uint32_t j = mt.interval((uint32_t)i);
-          const uint8_t t = perm[i]; perm[i] = perm[j]; perm[j] = t;
-        }
+        mt.permutation(perm, n);
         memcpy(idx + o, perm, level);
         o += level;
       }
@@ -4989,6 +4989,267 @@ int gk_svmt_phi(gk_handle* h, int32_t lo, int32_t n_levels, const int32_t* count
 
 }  // extern "C"
 
+// ---------------------------------------------------------------------------
+// GraphletSampling (graphlet_sampling.cuh), sampled route.  gk_gs_draw is host code on the estimator's MT19937 stream;
+// gk_gs_features classifies the drawn samples on the device into the (graph, class) table, after the counts of the
+// graphs before g0 handed back from an earlier run (a transform keeps the fit's samples without redrawing them).
+// Table block gs_blk: keys [cap] u64 | counts [cap] u32 | sample counts [cap] u32 | class codes [cap] u32.
+struct GsTable {
+  unsigned long long* keys;
+  unsigned *cnt, *raw, *code;
+};
+
+static GsTable gs_table(gk_handle* h) {
+  GsTable t;
+  char* b = h->gs_blk.as<char>();
+  const size_t cap = h->gs_cap;
+  t.keys = reinterpret_cast<unsigned long long*>(b);
+  t.cnt = reinterpret_cast<unsigned*>(b + cap * 8);
+  t.raw = t.cnt + cap;
+  t.code = t.raw + cap;
+  return t;
+}
+
+// gs_ctl: [error bits u32 | pad u32 | columns u64 | largest count u32 | entries u32]
+
+// Gram of GraphletSampling (gram_path 17): the exact integer Gram of the (graph, column) table (gram_int: tensor
+// cores, CUDA cores or no shared column), GK_NORMALIZE by the self similarities, which include the classes only the
+// new graphs have (the reference's diagonal() over phi_y with its Y-only bins).
+static int gram_gs(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  const GsTable t = gs_table(h);
+  IntBlock fb;
+  fb.keys = t.keys; fb.cnt = t.cnt; fb.cap = h->gs_cap;
+  fb.colcnt = h->gs_colcnt.as<unsigned>(); fb.col_cap = h->gs_cols + 1; fb.n_columns = h->gs_cols;
+  fb.diag = h->gs_diag.as<unsigned long long>();
+  fb.part_max = h->gs_ctl.as<unsigned>() + 4; fb.part_new = fb.part_max + 1; fb.n_part = 1;
+  fb.prologue_on_host = false;
+  GK_TRY(gram_int(h, q, fb, stats));
+  if (stats) stats->gram_path = 17;
+  return GK_OK;
+}
+
+extern "C" {
+
+int gk_gs_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int32_t* sizes, int32_t k, int64_t n_samples,
+               uint8_t* samp_size, int32_t* idx, int64_t idx_cap, int64_t* n_idx) {
+  if (!mt_key || !mt_pos || n_graphs < 0 || (n_graphs > 0 && !sizes) || n_samples < 0 || !n_idx || k < 3)
+    return fail(GK_ERR_ARG, "gk_gs_draw: bad arguments");
+  if (*mt_pos < 0 || *mt_pos > 624) return fail(GK_ERR_ARG, "gk_gs_draw: MT19937 position outside [0, 624]");
+  if (k > GS_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_gs_draw: graphlets of more than 6 vertices");
+  int64_t need = 0;
+  int nmax = 0;
+  for (int64_t g = 0; g < n_graphs; ++g) {
+    if (sizes[g] < 0) return fail(GK_ERR_ARG, "gk_gs_draw: a negative graph size");
+    need += n_samples * std::min<int64_t>(k, sizes[g]);
+    nmax = std::max(nmax, (int)sizes[g]);
+  }
+  if (need > idx_cap || (n_graphs * n_samples > 0 && !samp_size) || (need > 0 && !idx))
+    return fail(GK_ERR_ARG, "gk_gs_draw: output buffers too small");
+  SvmtMT mt{mt_key, *mt_pos};
+  std::vector<int32_t> perm(std::max(nmax, 1));
+  int64_t o = 0, s = 0;
+  for (int64_t g = 0; g < n_graphs; ++g) {
+    const int n = sizes[g], lo = std::min(3, n), hi = std::min<int>(k, n);
+    for (int64_t t = 0; t < n_samples; ++t, ++s) {
+      // rs.randint(min_r, max_r + 1) unless the range is one size, then rs.choice(n, r, replace=False)
+      const int r = lo == hi ? lo : lo + (int)mt.interval((uint32_t)(hi - lo));
+      mt.permutation(perm.data(), n);
+      memcpy(idx + o, perm.data(), (size_t)r * 4);
+      samp_size[s] = (uint8_t)r;
+      o += r;
+    }
+  }
+  *mt_pos = mt.pos;
+  *n_idx = o;
+  return GK_OK;
+}
+
+int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int64_t* samp_off,
+                   const uint8_t* samp_size, const int32_t* idx, int64_t n_idx, const int64_t* prior, int64_t n_prior,
+                   gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_gs_features: no graphs packed");
+  if (k < 1) return fail(GK_ERR_ARG, "gk_gs_features: k must be positive");
+  if (k > GS_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_gs_features: graphlets of more than 6 vertices");
+  const int64_t N = h->N;
+  if (n_fit < 1 || n_fit > N || g0 < 0 || g0 > N || !samp_off || n_prior < 0 || (n_prior && !prior))
+    return fail(GK_ERR_ARG, "gk_gs_features: bad arguments");
+  const int64_t n_new = N - g0, S = samp_off[n_new];
+  if (samp_off[0] != 0 || S < 0 || (S && !samp_size)) return fail(GK_ERR_ARG, "gk_gs_features: bad sample offsets");
+  // every check on the host arguments before the first launch (the drawn indexes are checked on the device)
+  const std::vector<int>& gp = extra_of(h)->graph_ptr;
+  std::vector<long long> ioff(n_new + 1, 0);
+  std::vector<long long> per_graph(n_new, 0);
+  for (int64_t w = 0; w < n_new; ++w) {
+    if (samp_off[w + 1] < samp_off[w]) return fail(GK_ERR_ARG, "gk_gs_features: bad sample offsets");
+    if (samp_off[w + 1] - samp_off[w] >= (1LL << 31) - 1)
+      return fail(GK_ERR_RANGE, "gk_gs_features: 2^31 or more samples of one graph (counts are u32)");
+    long long t = 0;
+    const int n = gp[g0 + w + 1] - gp[g0 + w];
+    for (int64_t s = samp_off[w]; s < samp_off[w + 1]; ++s) {
+      if (samp_size[s] > k || samp_size[s] > n) return fail(GK_ERR_ARG, "gk_gs_features: a sample larger than k or its graph");
+      t += samp_size[s];
+    }
+    ioff[w + 1] = ioff[w] + t;
+    per_graph[w] = samp_off[w + 1] - samp_off[w];
+  }
+  if (ioff[n_new] != n_idx || (n_idx && !idx)) return fail(GK_ERR_ARG, "gk_gs_features: index count does not match the sizes");
+  for (int64_t i = 0; i < n_prior; ++i)
+    if (prior[3 * i] < 0 || prior[3 * i] >= g0 || prior[3 * i + 1] < 0 || prior[3 * i + 1] >= gs_base(k + 1) ||
+        prior[3 * i + 2] < 1 || prior[3 * i + 2] >= (1LL << 31) - 1)
+      return fail(GK_ERR_ARG, "gk_gs_features: a bad prior count");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t launches0 = h->launches;
+  h->features_ready = false; h->feat_serial++;
+  GK_TRY(init_scalars(h, 0));
+  GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
+  // ---- class table of the code space (sizes 0 .. k), and the number of classes it has
+  const long long n_codes = gs_base(k + 1);
+  static std::mutex classes_mu;
+  static long long n_classes_of[GS_KMAX + 2] = {0};
+  if (h->gs_canon_k < k) {
+    GK_TRY(h->gs_canon.ensure((size_t)n_codes * 4));
+    gs_canon<<<cdiv(n_codes, 256), 256, 0, h->stream>>>(n_codes, h->gs_canon.as<unsigned>());
+    LAUNCH_CHECK(h);
+    h->gs_canon_k = k;
+    std::lock_guard<std::mutex> lk(classes_mu);
+    if (!n_classes_of[k]) {
+      std::vector<unsigned> c(n_codes);
+      GK_CUDA(cudaMemcpyAsync(c.data(), h->gs_canon.p, (size_t)n_codes * 4, cudaMemcpyDeviceToHost, h->stream));
+      GK_CUDA(cudaStreamSynchronize(h->stream));
+      long long m = 0;
+      for (long long x = 0; x < n_codes; ++x) m += c[x] == (unsigned)x;
+      n_classes_of[k] = m;
+    }
+  }
+  long long n_classes;
+  {
+    std::lock_guard<std::mutex> lk(classes_mu);
+    n_classes = n_classes_of[k] ? n_classes_of[k] : n_codes;
+  }
+  GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
+  // ---- (graph, class) table: at most one entry per prior count and per sample or class of a graph
+  long long bound = n_prior;
+  for (int64_t w = 0; w < n_new; ++w) bound += std::min<long long>(per_graph[w], n_classes);
+  const size_t cap = std::max<size_t>(next_pow2((size_t)std::max<long long>(bound, 1) * 2), 1024);
+  if (cap > (1ULL << 31)) return fail(GK_ERR_RANGE, "gk_gs_features: (graph, class) table of 2^31 or more slots");
+  h->gs_cap = cap;
+  GK_TRY(h->gs_blk.ensure(cap * 20));
+  GK_TRY(h->gs_first.ensure((size_t)n_codes * 8));
+  GK_TRY(h->gs_colid.ensure((size_t)n_codes * 4));
+  GK_TRY(h->gs_ctl.ensure(32));
+  GK_TRY(h->gs_diag.ensure((size_t)N * 8));
+  const size_t o_ioff = (size_t)(n_new + 1) * 8, o_size = o_ioff * 2, o_idx = (o_size + (size_t)S + 3) / 4 * 4;
+  GK_TRY(h->gs_samp.ensure(o_idx + (size_t)n_idx * 4 + (size_t)std::max<int64_t>(n_prior, 1) * 24 + 16));
+  const GsTable t = gs_table(h);
+  unsigned* first_fit = h->gs_first.as<unsigned>();
+  unsigned* first_new = first_fit + n_codes;
+  unsigned* ctl = h->gs_ctl.as<unsigned>();
+  char* sb = h->gs_samp.as<char>();
+  const size_t o_prior = (o_idx + (size_t)n_idx * 4 + 7) / 8 * 8;
+  GK_CUDA(cudaMemsetAsync(t.keys, 0xFF, cap * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(t.cnt, 0, cap * 4, h->stream));
+  GK_CUDA(cudaMemsetAsync(first_fit, 0xFF, (size_t)n_codes * 8, h->stream));
+  GK_CUDA(cudaMemsetAsync(ctl, 0, 32, h->stream));
+  GK_CUDA(cudaMemsetAsync(h->gs_diag.p, 0, (size_t)N * 8, h->stream));
+  GK_CUDA(cudaMemcpyAsync(sb, samp_off, o_ioff, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(sb + o_ioff, ioff.data(), o_ioff, cudaMemcpyHostToDevice, h->stream));
+  if (S) GK_CUDA(cudaMemcpyAsync(sb + o_size, samp_size, (size_t)S, cudaMemcpyHostToDevice, h->stream));
+  if (n_idx) GK_CUDA(cudaMemcpyAsync(sb + o_idx, idx, (size_t)n_idx * 4, cudaMemcpyHostToDevice, h->stream));
+  if (n_prior) {
+    GK_CUDA(cudaMemcpyAsync(sb + o_prior, prior, (size_t)n_prior * 24, cudaMemcpyHostToDevice, h->stream));
+    gs_prior<<<cdiv(n_prior, 256), 256, 0, h->stream>>>(n_prior, reinterpret_cast<const long long*>(sb + o_prior),
+                                                        (int)n_fit, t.keys, t.cnt, (unsigned)(cap - 1), first_fit,
+                                                        first_new);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
+  if (n_new > 0 && S > 0) {
+    GsSampleParams p;
+    p.g0 = (int)g0; p.g1 = (int)N;
+    p.samp_off = reinterpret_cast<const long long*>(sb);
+    p.idx_off = reinterpret_cast<const long long*>(sb + o_ioff);
+    p.size = reinterpret_cast<const unsigned char*>(sb + o_size);
+    p.idx = reinterpret_cast<const int*>(sb + o_idx);
+    p.graph_ptr = h->graph_ptr.as<int>(); p.row_ptr = h->row_ptr.as<int>(); p.col_idx = h->col_idx.as<int>();
+    p.canon = h->gs_canon.as<unsigned>();
+    p.n_fit = (int)n_fit;
+    p.keys = t.keys; p.cnt = t.cnt; p.mask = (unsigned)(cap - 1);
+    p.first_fit = first_fit; p.first_new = first_new;
+    p.err = ctl;
+    const int grid = (int)std::min<int64_t>(cdiv(n_new, 8), (int64_t)h->sm_count * 16);
+    gs_classify<<<grid, 256, 0, h->stream>>>(p);
+    LAUNCH_CHECK(h);
+  }
+  GK_CUDA(cudaEventRecord(h->tev[1], h->stream));
+  unsigned long long* n_cols = reinterpret_cast<unsigned long long*>(ctl + 2);
+  gs_number<<<cdiv(n_codes, 256), 256, 0, h->stream>>>(n_codes, first_fit, first_new, h->gs_colid.as<unsigned>(), n_cols);
+  LAUNCH_CHECK(h);
+  unsigned hc[4] = {0, 0, 0, 0};
+  GK_CUDA(cudaMemcpyAsync(hc, ctl, 16, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  if (hc[0] & 1u) return fail(GK_ERR_ARG, "gk_gs_features: a sample larger than 6 vertices");
+  if (hc[0] & 2u) return fail(GK_ERR_ARG, "gk_gs_features: a drawn index is not a vertex of its graph");
+  const int64_t M = (int64_t)(((unsigned long long)hc[3] << 32) | hc[2]);
+  GK_TRY(h->gs_colcnt.ensure((size_t)(M + 1) * 4));
+  GK_CUDA(cudaMemsetAsync(h->gs_colcnt.p, 0, (size_t)(M + 1) * 4, h->stream));
+  const int sgrid = (int)std::min<int64_t>(cdiv((int64_t)cap, 256), (int64_t)h->sm_count * 16);
+  gs_finish<<<sgrid, 256, 0, h->stream>>>(cap, (int)n_fit, first_fit, first_new, h->gs_colid.as<unsigned>(), t.keys,
+                                          t.cnt, t.raw, t.code);
+  LAUNCH_CHECK(h);
+  nspd_level_stats<<<sgrid, 256, 0, h->stream>>>(cap, t.keys, t.cnt, h->gs_colcnt.as<unsigned>(),
+                                                 h->gs_diag.as<unsigned long long>(), ctl + 4);
+  LAUNCH_CHECK(h);
+  GK_CUDA(cudaEventRecord(h->tev[4], h->stream));
+  std::vector<unsigned long long> d(N);
+  GK_CUDA(cudaMemcpyAsync(d.data(), h->gs_diag.p, (size_t)N * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaMemcpyAsync(hc, ctl, 16, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  // K[i][j] <= sqrt(d_i d_j) <= max d: below 2^53 every entry and partial sum of the fp64 result is exact
+  for (int64_t g = 0; g < N; ++g)
+    if (d[g] >= (1ULL << 53))
+      return fail(GK_ERR_RANGE, "GraphletSampling: a self similarity of 2^53 or more (K would not be exact in fp64)");
+  h->gs_cols = M;
+  h->n_columns = M;
+  h->feature_kind = FK_GS;
+  h->features_ready = true; h->feat_serial++;
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
+    stats->n_columns = M;
+    stats->n_entries = S;
+    stats->kernel_launches = h->launches - launches0;
+    stats->ms_hash = ev_ms(h->tev[2], h->tev[3]);      // class table
+    stats->ms_h2d = ev_ms(h->tev[3], h->tev[0]);       // samples to the device
+    stats->ms_features = ev_ms(h->tev[0], h->tev[1]);  // classification and counts
+    stats->ms_columns = ev_ms(h->tev[1], h->tev[4]);   // columns, "+1" rule, self similarities
+  }
+  return GK_OK;
+}
+
+int gk_gs_counts(gk_handle* h, int64_t cap, int64_t* out, int64_t* n_out) {
+  if (!h || !n_out || (cap > 0 && !out)) return fail(GK_ERR_ARG, "gk_gs_counts: null argument");
+  if (h->feature_kind != FK_GS || !h->features_ready) return fail(GK_ERR_STATE, "gk_gs_counts: run gk_gs_features first");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t tc = h->gs_cap;
+  std::vector<char> b(tc * 20);
+  GK_CUDA(cudaMemcpyAsync(b.data(), h->gs_blk.p, tc * 20, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  const unsigned long long* keys = reinterpret_cast<const unsigned long long*>(b.data());
+  const unsigned* cnt = reinterpret_cast<const unsigned*>(b.data() + tc * 8);
+  const unsigned *raw = cnt + tc, *code = raw + tc;
+  std::vector<std::array<int64_t, 4>> rows;
+  for (size_t i = 0; i < tc; ++i)
+    if (keys[i] != EMPTY64) rows.push_back({(int64_t)(keys[i] >> 32), (int64_t)code[i], (int64_t)raw[i], (int64_t)cnt[i]});
+  std::sort(rows.begin(), rows.end());
+  *n_out = (int64_t)rows.size();
+  if (cap >= (int64_t)rows.size())
+    for (size_t i = 0; i < rows.size(); ++i) memcpy(out + 4 * i, rows[i].data(), 32);
+  return GK_OK;
+}
+
+}  // extern "C"
+
 extern "C" {
 
 int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
@@ -5009,6 +5270,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
     case FK_ODD: return gram_odd(h, q, stats);
     case FK_ML: return gram_ml(h, q, stats);
     case FK_SVMT: return gram_svmt(h, q, stats);
+    case FK_GS: return gram_gs(h, q, stats);
     default: return gram_int(h, q, block_of(h), stats);
   }
 }

@@ -128,6 +128,7 @@ enum FeatureKind : int {
   FK_ODD = 11,    // OddSth per-bit-plane (graph, identity) count tables
   FK_ML = 12,     // MultiscaleLaplacian per-graph (S^-1, log det S) records
   FK_SVMT = 13,   // SvmTheta per-graph first-level phi
+  FK_GS = 14,     // GraphletSampling (graph, class) counts: the integer Gram
 };
 
 }  // namespace gk
@@ -287,6 +288,14 @@ struct gk_handle {
       svmt_rec, svmt_ctl;
   std::vector<int> svmt_sizes;  // vertices of the graphs of the last gk_svmt_solve
   int64_t svmt_nrec = 0;
+
+  // ---- GraphletSampling (FK_GS): the canonical class table of the code space (built once, for sizes up to gs_canon_k),
+  // the first graph of every class among the fitted / the new graphs, class -> column, the (graph, column) table with
+  // its sample counts and class codes, graphs per column, self similarities, [error bits | pad | columns u64 | max, entries]
+  gk::DevBuf gs_canon, gs_first, gs_colid, gs_blk, gs_colcnt, gs_diag, gs_ctl, gs_samp;
+  int gs_canon_k = 0;
+  size_t gs_cap = 0;
+  int64_t gs_cols = 0;
 
   // ---- Propagation (FK_PK): P double-buffered [2][V][D], every level's bins [t_max][V][K], the private
   // flags of every level [t_max][V], per-edge T values, draws, column scratch, counters [near u64 | nan u32 | pad]

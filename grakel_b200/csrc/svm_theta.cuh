@@ -532,6 +532,16 @@ struct SvmtMT {
     }
     return v;
   }
+  // legacy RandomState.permutation(n): arange(n) shuffled by Fisher-Yates from the top (choice(n, r, replace=False)
+  // is its first r entries)
+  template <class T>
+  void permutation(T* perm, int n) {
+    for (int i = 0; i < n; ++i) perm[i] = (T)i;
+    for (int i = n - 1; i >= 1; --i) {
+      const uint32_t j = interval((uint32_t)i);
+      const T t = perm[i]; perm[i] = perm[j]; perm[j] = t;
+    }
+  }
 };
 
 }  // namespace gk

@@ -16,6 +16,7 @@ the kernels of the device hot path:
     "pyramid_match" / "PM"      (+ with_labels, L, d)
     "multiscale_laplacian" / "ML"  (+ L, P, gamma, heta, n_samples; random_state forwarded)
     "svm_theta" / "SVMT"        (+ n_samples, subsets_size_range, metric; random_state forwarded)
+    "graphlet_sampling" / "GR"  (+ k, sampling; random_state forwarded; a sampling dictionary is required)
 
 Any other reference kernel name raises NotImplementedError (not ValueError, which the reference reserves for
 unknown names).  The public surface (constructor parameters, `fit` / `transform` / `fit_transform`, the fitted
@@ -38,14 +39,14 @@ from sklearn.utils.validation import check_is_fitted
 from .core_framework import CoreFramework
 from .kernels import (EdgeHistogram, GraphHopper, HadamardCode, NeighborhoodHash, NeighborhoodSubgraphPairwiseDistance,
                       MultiscaleLaplacian, OddSth, Propagation, PropagationAttr, PyramidMatch,
-                      ShortestPath, SubgraphMatching, ShortestPathAttr, SvmTheta, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
+                      ShortestPath, SubgraphMatching, ShortestPathAttr, SvmTheta, VertexHistogram, WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment,
+                      GraphletSampling)
 
 default_n_components = 100
 
 # reference names outside the hot path (graph_kernels.py:38-64)
 _OUTSIDE = frozenset((
-    "random_walk", "RW", "graphlet_sampling", "GR",
-    "lovasz_theta", "LOVT"))
+    "random_walk", "RW", "lovasz_theta", "LOVT"))
 
 
 def _propagation(params):
@@ -73,6 +74,7 @@ for _names, _framework, _build in (
         (("pyramid_match", "PM"), False, lambda p: (PyramidMatch, p)),
         (("multiscale_laplacian", "ML"), False, lambda p: (MultiscaleLaplacian, p)),
         (("svm_theta", "SVMT"), False, lambda p: (SvmTheta, p)),
+        (("graphlet_sampling", "GR"), False, lambda p: (GraphletSampling, p)),
         (("weisfeiler_lehman", "WL"), True, lambda p: (WeisfeilerLehman, p)),
         (("hadamard_code", "HC"), True, lambda p: (HadamardCode, p)),
         (("core_framework", "CORE"), True, lambda p: (CoreFramework, p))):
@@ -206,8 +208,8 @@ class GraphKernel(BaseEstimator, TransformerMixin):
                 raise NotImplementedError("kernel '" + str(name) + "' is outside the device hot path of grakel_b200")
             raise ValueError("Unsupported kernel: " + str(name))
         framework, build = entry
-        if name in ("propagation", "PR", "multiscale_laplacian", "ML", "svm_theta", "SVMT"):
-            # graph_kernels.py:486-489, 515-517, 521-523, 530-535
+        if name in ("propagation", "PR", "multiscale_laplacian", "ML", "svm_theta", "SVMT", "graphlet_sampling", "GR"):
+            # graph_kernels.py:486-489, 510-512, 515-517, 521-523, 530-535
             params["random_state"] = params.pop("random_state",
                                                 self.random_state_ if self.random_state is not None else None)
         if framework:

@@ -13,6 +13,7 @@ the level-0 label dictionary), so fitted estimators pickle like the reference's
 from __future__ import annotations
 
 import copy
+import math
 import functools
 import warnings
 from collections.abc import Iterable
@@ -3822,3 +3823,239 @@ class SvmTheta(Kernel):
 
     def diagonal(self):
         return self._pairwise_diagonal()
+
+
+_GS_KMAX = 6
+# graphlet_sampling.py:185-187: isomorphism classes of graphs of k vertices, used when `a` is -1
+_GS_CLASSES = {1: 1, 2: 2, 3: 4, 4: 8, 5: 19, 6: 53, 7: 209, 8: 1253, 9: 13599}
+
+
+class GraphletSampling(Kernel):
+    """Graphlet sampling kernel (graphlet_sampling.py; Shervashidze et al. 2009), the sampled route (`sampling` a
+    dict).  Every graph gets n_samples draws on `random_state_`'s legacy MT19937 stream, as the reference makes them:
+    a size r = randint(min(3, n), min(k, n) + 1) (no draw when that range is one size) and choice(n, r,
+    replace=False); the draws are host code and the stream continues as the reference's does (a second fit, or a
+    transform, draws after the earlier ones).  Each sample is the undirected graph induced on its vertices by A > 0 (a
+    pair is an edge when either direction is, a diagonal entry a self-loop); its class up to isomorphism, the
+    (graph, class) counts and the exact integer Gram run on the device.  A graph's count of a class is its number of
+    samples of that class, plus one unless it is the first graph in input order with the class (the reference's
+    bins); in a transform every class the fitted graphs have gets the plus one, and a class only the new graphs have
+    is counted from its first new graph.  Those classes add nothing to K but enter the diagonal, so normalize divides
+    by them too.  K equals the reference's with ==.
+
+    Deviations (NotImplementedError): sampling=None (every connected k-vertex subset, the reference's ConSubg) has no
+    device path; k > 6; a graph whose adjacency is not symmetric (the reference's `isomorphic` compares the directed
+    edges after bliss's canonical labeling of the undirected graph, so its classes of directed samples depend on
+    which labeling bliss picks).
+
+    `gs_stats_` holds the stage times of the last run (ms): `host_draw_ms`, `class_table_ms`, `h2d_ms`,
+    `classify_ms`, `columns_ms`, `gram_ms`."""
+
+    _graph_format = "adjacency"
+
+    def __init__(self, n_jobs=None, normalize=False, verbose=False, random_state=None, k=5, sampling=None):
+        super().__init__(n_jobs=n_jobs, normalize=normalize, verbose=verbose)
+        self.random_state = random_state
+        self.k = k
+        self.sampling = sampling
+        self._initialized.update({"random_state": False, "k": False, "sampling": False})
+
+    def initialize(self):
+        """graphlet_sampling.py:121-223, in its order and with its errors and warnings."""
+        if not self._initialized["n_jobs"]:
+            if self.n_jobs is not None:
+                warnings.warn("no implemented parallelization for GraphletSampling")
+            self._initialized["n_jobs"] = True
+        if not self._initialized["random_state"]:
+            self.random_state_ = check_random_state(self.random_state)
+            self._initialized["random_state"] = True
+        if not self._initialized["k"]:
+            if type(self.k) is not int:
+                raise TypeError("k must be an int")
+            if self.k > 10:
+                warnings.warn("graphlets are too big - computation may be slow")
+            elif self.k < 3:
+                raise TypeError("k must be bigger than 3")
+            self._initialized["k"] = True
+        if not self._initialized["sampling"]:
+            sampling, k = self.sampling, self.k
+            if sampling is None:
+                n_samples = None
+            elif type(sampling) is dict:
+                if "n_samples" in sampling:
+                    n_samples = sampling["n_samples"]
+                    args = [arg for arg in ["delta", "epsilon", "a"] if arg in sampling]
+                    if len(args):
+                        # the reference passes the names as the warning category, so this raises TypeError
+                        warnings.warn("Number of samples defined as input, ignoring arguments:", ", ".join(args))
+                elif "delta" in sampling or "epsilon" in sampling or "a" in sampling:
+                    delta = sampling.get("delta", 0.05)
+                    epsilon = sampling.get("epsilon", 0.05)
+                    a = sampling.get("a", -1)
+                    if delta > 1 or delta < 0:
+                        raise TypeError("delta must be in the range (0,1)")
+                    if epsilon > 1 or epsilon < 0:
+                        raise TypeError("epsilon must be in the range (0,1)")
+                    if type(a) is not int:
+                        raise TypeError("a must be an integer")
+                    elif a == 0:
+                        raise TypeError("a cannot be zero")
+                    elif a < -1:
+                        raise TypeError("negative a smaller than -1 have no meaning")
+                    if a == -1:
+                        if k > 9:
+                            warnings.warn("warning for such size number of isomorphisms is not known - "
+                                          "interpolation on know values will be used")
+                            from scipy.interpolate import interp1d
+                            a = interp1d(list(_GS_CLASSES.keys()), list(_GS_CLASSES.values()), kind="cubic")(k)
+                        else:
+                            a = _GS_CLASSES[k]
+                    n_samples = math.ceil(2 * (a * np.log10(2) + np.log10(1 / delta)) / (epsilon ** 2))
+                else:
+                    raise ValueError("sampling doesn't have a valid dictionary format")
+            else:
+                raise TypeError("sampling can either be a dictionary or None")
+            self.k_ = k
+            self.n_samples_ = n_samples
+            self._initialized["sampling"] = True
+
+    def _check_scope(self):
+        if self.n_samples_ is None:
+            raise NotImplementedError("GraphletSampling: sampling=None (every connected k-vertex subset) has no device "
+                                      "path; pass a sampling dictionary")
+        if self.k_ > _GS_KMAX:
+            raise NotImplementedError("GraphletSampling: graphlets of more than 6 vertices (k = %d)" % self.k_)
+        n = self.n_samples_
+        if type(n) is not int and not isinstance(n, np.integer):
+            raise TypeError("'%s' object cannot be interpreted as an integer" % type(n).__name__)
+        return max(int(n), 0)
+
+    def _elements(self, X):
+        """0/1 adjacency (A > 0) of every element, rows in sorted vertex order (graphlet_sampling.py:378-398)."""
+        from .packing import adjacency_and_labels
+        if isinstance(X, Block):
+            return [A > 0 for A, _ in _block_adjacency(X, False)]
+        if not isinstance(X, Iterable):
+            raise TypeError("input must be an iterable\n")
+        out = []
+        for idx, x in enumerate(iter(X)):
+            if isinstance(x, Graph):
+                x = x.as_element()
+            is_iter = isinstance(x, Iterable)
+            if is_iter:
+                x = list(x)
+            if not (is_iter and len(x) in (0, 1, 2, 3)):
+                raise TypeError("each element of X must be either a graph or an iterable with at least 1 and at most "
+                                "3 elements\n")
+            if len(x) == 0:
+                warnings.warn("Ignoring empty element on index: " + str(idx))
+                continue
+            out.append(adjacency_and_labels(x[0])[0] > 0)
+        if not out:
+            raise ValueError("parsed input is empty")
+        return out
+
+    @staticmethod
+    def _csr(mats):
+        sizes = np.array([A.shape[0] for A in mats], dtype=np.int64)
+        gp = np.zeros(len(mats) + 1, dtype=np.int64)
+        gp[1:] = np.cumsum(sizes)
+        rows, cols = [], []
+        for A, o in zip(mats, gp[:-1]):
+            r, c = np.nonzero(A)
+            rows.append(r + o)
+            cols.append(c + o)
+        r = np.concatenate(rows) if rows else np.zeros(0, dtype=np.int64)
+        c = np.concatenate(cols) if cols else np.zeros(0, dtype=np.int64)
+        rp = np.zeros(gp[-1] + 1, dtype=np.int64)
+        np.add.at(rp, r + 1, 1)
+        return sizes, gp, np.cumsum(rp), c
+
+    def _gs_run(self, new, fit_csr=None, fit_counts=None, want_matrix=True, device_ptr=None, row_range=None):
+        """Draw for the graphs `new`, classify and count them after the fitted graphs (fit_csr, their counts), and
+        return (K, xdiag, ydiag, counts of every graph)."""
+        n_samples = self._check_scope()
+        if any(not np.array_equal(A, A.T) for A in new):
+            raise NotImplementedError("GraphletSampling: a graph with a non-symmetric adjacency matrix (the reference's "
+                                      "classes of directed samples depend on bliss's canonical labeling)")
+        sizes, gp, rp, ci = self._csr(new)
+        t0 = time.perf_counter()
+        samp_size, idx = _lib.gs_draw(self.random_state_, sizes, self.k_, n_samples)
+        draw_ms = (time.perf_counter() - t0) * 1e3
+        samp_off = np.arange(len(new) + 1, dtype=np.int64) * n_samples
+        if fit_csr is not None:
+            fs, fgp, frp, fci = fit_csr
+            nx = len(fs)
+            gp = np.concatenate([fgp, fgp[-1] + gp[1:]])
+            rp = np.concatenate([frp, frp[-1] + rp[1:]])
+            ci = np.concatenate([fci, fgp[-1] + ci])
+        else:
+            nx = len(new)
+        N = len(gp) - 1
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(gp, rp, ci)
+            st = eng.gs_features(self.k_, nx, N - len(new), samp_off, samp_size, idx,
+                                 prior=None if fit_counts is None else fit_counts[:, :3])
+            counts = eng.gs_counts()
+            gst = _lib.GkStats()
+            K, xd, yd = eng.gram(N, n_fit=nx, normalize=bool(self.normalize) and want_matrix,
+                                 out=None if want_matrix else False, device_ptr=device_ptr, row_range=row_range,
+                                 stats=gst)
+        self.stats_ = st
+        self.gs_stats_ = {"n_graphs": N, "n_samples": int(len(samp_size)), "host_draw_ms": draw_ms,
+                          "class_table_ms": st.ms_hash, "h2d_ms": st.ms_h2d, "classify_ms": st.ms_features,
+                          "columns_ms": st.ms_columns, "gram_ms": gst.ms_total}
+        if self.verbose:
+            print(type(self).__name__, self.gs_stats_)
+        return K, xd, yd, counts
+
+    def fit(self, X, y=None):
+        self._is_transformed = False
+        self._method_calling = 1
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        self._fit(X, want_matrix=False)
+        return self
+
+    def _fit(self, X, want_matrix):
+        els = self._elements(X)
+        K, xd, _, counts = self._gs_run(els, want_matrix=want_matrix)
+        self._fit_csr = self._csr(els)
+        self._nx = len(els)
+        self.X = counts
+        for a in ("_X_diag", "_Y_diag", "_phi_X"):
+            self.__dict__.pop(a, None)
+        return K, xd
+
+    def fit_transform(self, X, y=None):
+        self._method_calling = 2
+        self._is_transformed = False
+        self.initialize()
+        if X is None:
+            raise ValueError("`fit` input cannot be None")
+        K, xd = self._fit(X, want_matrix=True)
+        self._X_diag = xd
+        self._phi_X = True
+        return K
+
+    def transform(self, X):
+        self._method_calling = 3
+        check_is_fitted(self, ["X"])
+        if X is None:
+            raise ValueError("transform input cannot be None")
+        els = self._elements(X)
+        K, xd, yd, counts = self._gs_run(els, fit_csr=self._fit_csr, fit_counts=self.X)
+        self._ny = len(els)
+        self.Y_ = counts[counts[:, 0] >= self._nx]
+        self._X_diag, self._Y_diag = xd, yd
+        self._phi_X = True
+        self._is_transformed = True
+        return K
+
+    def diagonal(self):
+        """graphlet_sampling.py:333-371: the X diagonal, and the Y diagonal after `transform`."""
+        check_is_fitted(self, ["_phi_X"])
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag

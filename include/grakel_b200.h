@@ -111,7 +111,8 @@ typedef struct gk_stats {
                                 NeighborhoodSubgraphPairwiseDistance: 12 = one exact integer Gram per level + the fp64 fold,
                                 SubgraphMatching: 13 = per-pair clique counts + the lambda fold,
                                 OddSth: 14 = one exact integer Gram per bit of C + the fp64 sum of 2^b G_b,
-                                MultiscaleLaplacian: 15 = per-pair FLG values, SvmTheta: 16 = fp64 product of first-level phi */
+                                MultiscaleLaplacian: 15 = per-pair FLG values, SvmTheta: 16 = fp64 product of first-level phi,
+                                GraphletSampling: 17 = the exact integer Gram of the (graph, class) counts */
   int64_t gemm_tiles;        /* output tiles computed */
   int64_t gemm_launches;     /* kernels launched by the last gk_gram */
   int64_t kernel_launches;   /* kernels launched by the last features call */
@@ -358,6 +359,36 @@ int gk_svmt_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int3
 int gk_svmt_phi(gk_handle* h, int32_t lo, int32_t n_levels, const int32_t* counts, const uint8_t* idx, int64_t n_idx,
                 const double* fit_phi0, int64_t n_fit, double* phi, double* m_out, double* alpha_out, int32_t* iters_out,
                 gk_stats* stats);
+
+/* GraphletSampling, sampled route (graphlet_sampling.py:290-463, `sampling` a dict).  The packed CSR is each graph's
+ * 0/1 adjacency (A > 0), rows ascending; labels are ignored.
+ *   gk_gs_draw      host only: for every graph of `sizes` in order, n_samples times, r = rs.randint(min(3, n),
+ *                   min(k, n) + 1) (no draw when the two are equal) and rs.choice(n, r, replace=False) on numpy's
+ *                   legacy MT19937 stream (mt_key[624] / mt_pos of `get_state()`, advanced in place): samp_size[g *
+ *                   n_samples + t] = r and the indexes appended to idx (n_idx of them, idx_cap >= n_samples * sum
+ *                   min(k, n)).  k > 6 is GK_ERR_UNSUPPORTED.
+ *   gk_gs_features  every sample of the graphs g0 .. N-1 (samp_off[N - g0 + 1] sample offsets, samp_size, idx as
+ *                   gk_gs_draw wrote them) classified on the device: the class is the undirected sample graph (a pair
+ *                   is an edge when either direction is, a diagonal entry a self-loop) up to isomorphism, exact for up
+ *                   to 6 vertices.  prior[n_prior][3] = (graph < g0, class code, samples) restores the counts of an
+ *                   earlier run (gk_gs_counts).  The first n_fit packed graphs are the fitted ones: a graph's count of
+ *                   a class is its samples + 1 unless it is the first fitted graph with that class, or, for a class no
+ *                   fitted graph has, the first new graph with it.  The arguments (offsets, sample sizes, index
+ *                   count, prior rows, counts below 2^31) are checked before the first launch; a drawn index outside
+ *                   its graph is found by the classification kernel, which skips that sample, and is GK_ERR_ARG with no
+ *                   feature block left behind.  A self similarity of 2^53 or more is GK_ERR_RANGE.  gk_gram (gram_path
+ *                   17, fp64 output only: a K entry above 2^24 would not be exact in fp32) then returns the exact
+ *                   integer Gram, GK_NORMALIZE by self similarities over all classes.
+ *                   stats: n_columns (classes), n_entries (samples), ms_hash (class table), ms_h2d, ms_features
+ *                   (classification), ms_columns.
+ *   gk_gs_counts    the table of the last gk_gs_features as rows (graph, class code, samples, count) sorted by graph
+ *                   and code; *n_out is the row count, the rows are written when cap >= it. */
+int gk_gs_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int32_t* sizes, int32_t k, int64_t n_samples,
+               uint8_t* samp_size, int32_t* idx, int64_t idx_cap, int64_t* n_idx);
+int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int64_t* samp_off,
+                   const uint8_t* samp_size, const int32_t* idx, int64_t n_idx, const int64_t* prior, int64_t n_prior,
+                   gk_stats* stats);
+int gk_gs_counts(gk_handle* h, int64_t cap, int64_t* out, int64_t* n_out);
 
 /* Propagation / PropagationAttr (propagation.py:27-689).  The packed CSR (gk_pack_csr without weights; with the
  * label ids for the labelled kernel) is the sparsity pattern of every graph's row-normalised transition matrix T,
