@@ -84,6 +84,9 @@ _SYMBOLS = {
     "gk_sm_features": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_sm_counts": (C.c_int, [_P, C.c_int64, C.c_int64, _P]),
     "gk_odd_features": (C.c_int, [_P, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_wl_odd_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.POINTER(GkStats)]),
+    "gk_wl_level_sum": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.POINTER(GkStats)]),
+    "gk_wl_level_sum_fetch": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P]),
     "gk_odd_info": (C.c_int, [_P, _P]),
     "gk_odd_signatures": (C.c_int, [_P, _P, _P, _P, _P]),
     "gk_selftest_odd_collision": (C.c_int, [_P, C.c_int32]),
@@ -615,6 +618,34 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_odd_features(self.h, int(h), _ptr(rk), 0, C.byref(st)))
         return st
+
+    def wl_odd_features(self, h, n_iter, ids, rank):
+        """OddSth over n_iter + 1 WL label sets at once (gk_wl_odd_features): `ids` / `rank` are [n_iter + 1, V], the
+        ids of every level above those of the level before."""
+        ids, rk = _i32(ids), _i32(rank)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_wl_odd_features(self.h, int(h), int(n_iter), _ptr(ids), _ptr(rk), 0, C.byref(st)))
+        return st
+
+    def wl_level_sum(self, level, n_fit, row_range=None):
+        """Add the K of WL level `level` (the NSPD features just computed) into the device-resident sum."""
+        rb, re_ = (0, -1) if row_range is None else row_range
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_wl_level_sum(self.h, int(level), int(n_fit), int(rb), int(re_), C.byref(st)))
+        return st
+
+    def wl_level_sum_fetch(self, rows, cols, normalize=False, xdiag=None, ydiag=None, want_kdiag=False):
+        """(K, diagonal of the sum before normalisation or None) of the level sum (gk_wl_level_sum_fetch)."""
+        K = host_matrix(rows, cols)
+        xd = None if xdiag is None else np.ascontiguousarray(xdiag, dtype=np.float64)
+        yd = None if ydiag is None else np.ascontiguousarray(ydiag, dtype=np.float64)
+        kd = np.empty(cols, dtype=np.float64) if want_kdiag else None
+        flags = (GK_NORMALIZE | GK_NAN_TO_NUM) if normalize else 0
+        with self._lock:
+            self._check(self.lib.gk_wl_level_sum_fetch(self.h, flags, _ptr(xd), _ptr(yd), _ptr(K), _ptr(kd)))
+        return K, kd
 
     def odd_signatures(self):
         """(label id, child offsets, child identity ids, C) of every identity after odd_features."""

@@ -358,7 +358,7 @@ int gk_destroy(gk_handle* h) {
                         &h->svmt_vptr, &h->svmt_adj, &h->svmt_m, &h->svmt_alpha, &h->svmt_iters, &h->svmt_cnt,
                         &h->svmt_off, &h->svmt_idx, &h->svmt_sums, &h->svmt_phi, &h->svmt_rec, &h->svmt_ctl,
                         &h->gs_canon, &h->gs_first, &h->gs_colid, &h->gs_blk, &h->gs_colcnt, &h->gs_diag, &h->gs_ctl,
-                        &h->gs_samp};
+                        &h->gs_samp, &h->wl_sum, &h->wl_lvl};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -4139,6 +4139,86 @@ static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
 }
 
 // ---------------------------------------------------------------------------
+// WL over NeighborhoodSubgraphPairwiseDistance.  Every WL level's K is itself a sum of cosine-normalised per-(radius,
+// distance) Grams, so the WL levels cannot share one feature block: the host packs each level's labels and runs
+// gk_nspd_features, gk_wl_level_sum folds that level's K (gram_nspd, un-normalised) and adds it into a running sum on
+// the device, in level order, and gk_wl_level_sum_fetch normalises the sum and copies it out.
+extern "C" {
+
+int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begin, int64_t row_end, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (!h->features_ready || h->feature_kind != FK_NSPD)
+    return fail(GK_ERR_STATE, "gk_wl_level_sum: run gk_nspd_features on the level's labels first");
+  if (level < 0 || (level > 0 && level != h->wl_sum_levels))
+    return fail(GK_ERR_ARG, "gk_wl_level_sum: levels must be added in order, starting at 0");
+  GramReq q;
+  GK_TRY(gram_request(h, FK_NSPD, n_fit, 0, row_begin, row_end, nullptr, GK_F64, 0, nullptr, nullptr, &q));
+  if (level > 0 && (q.k_rows != h->wl_sum_rows || q.k_cols != h->wl_sum_cols || q.square != h->wl_sum_square ||
+                    q.row_begin != h->wl_sum_row0))
+    return fail(GK_ERR_ARG, "gk_wl_level_sum: a level's K has another shape than the sum's");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t elems = (size_t)q.k_rows * q.k_cols;
+  gk::DevBuf& dst = level == 0 ? h->wl_sum : h->wl_lvl;
+  GK_TRY(dst.ensure(std::max<size_t>(elems, 1) * 8));
+  q.flags |= GK_OUT_DEVICE; q.dev_out = true; q.K_out = dst.p; q.ld = q.k_cols;
+  GK_TRY(gram_nspd(h, q, stats));
+  if (level > 0 && elems) {
+    add_f64<<<(int)std::min<size_t>((elems + 255) / 256, (size_t)h->sm_count * 16), 256, 0, h->stream>>>(
+        (long long)elems, h->wl_lvl.as<double>(), h->wl_sum.as<double>());
+    LAUNCH_CHECK(h);
+  }
+  h->wl_sum_rows = q.k_rows; h->wl_sum_cols = q.k_cols; h->wl_sum_row0 = q.row_begin; h->wl_sum_square = q.square;
+  h->wl_sum_levels = level + 1;
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+int gk_wl_level_sum_fetch(gk_handle* h, int32_t flags, const double* xdiag, const double* ydiag, double* K_out,
+                          double* kdiag) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->wl_sum_levels <= 0) return fail(GK_ERR_STATE, "gk_wl_level_sum_fetch: no level added (gk_wl_level_sum)");
+  if (flags & ~(GK_NORMALIZE | GK_NAN_TO_NUM)) return fail(GK_ERR_ARG, "gk_wl_level_sum_fetch: unknown flags");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const int64_t rows = h->wl_sum_rows, cols = h->wl_sum_cols;
+  const bool full_square = h->wl_sum_square && h->wl_sum_row0 == 0 && rows == cols;
+  double* K = h->wl_sum.as<double>();
+  GK_TRY(h->diag_f64.ensure((size_t)(rows + cols + 1) * 8));
+  double* dcol = h->diag_f64.as<double>();
+  double* drow = dcol + cols;
+  if (kdiag || ((flags & GK_NORMALIZE) && !xdiag)) {
+    if (!full_square) return fail(GK_ERR_ARG, "gk_wl_level_sum_fetch: the diagonal of K needs the full square sum");
+    if (cols) {
+      diag_of_f64<<<cdiv(cols, 256), 256, 0, h->stream>>>(cols, K, cols, dcol);
+      LAUNCH_CHECK(h);
+    }
+    if (kdiag) GK_CUDA(cudaMemcpyAsync(kdiag, dcol, (size_t)cols * 8, cudaMemcpyDeviceToHost, h->stream));
+  }
+  if ((flags & GK_NORMALIZE) && rows > 0) {
+    const double* dr = dcol;
+    if (xdiag) {  // the caller's self similarities: xdiag for the columns, ydiag (or xdiag's rows) for the rows
+      GK_CUDA(cudaMemcpyAsync(dcol, xdiag, (size_t)cols * 8, cudaMemcpyHostToDevice, h->stream));
+      if (h->wl_sum_square) {
+        dr = dcol + h->wl_sum_row0;
+      } else {
+        if (!ydiag) return fail(GK_ERR_ARG, "gk_wl_level_sum_fetch: a transform needs ydiag to normalise");
+        GK_CUDA(cudaMemcpyAsync(drow, ydiag + h->wl_sum_row0, (size_t)rows * 8, cudaMemcpyHostToDevice, h->stream));
+        dr = drow;
+      }
+    } else {
+      dr = dcol;
+    }
+    normalize_rows<double><<<h->sm_count * 8, 256, 0, h->stream>>>(rows, cols, K, cols, dr, dcol,
+                                                                    (flags & GK_NAN_TO_NUM) ? 1 : 0);
+    LAUNCH_CHECK(h);
+  }
+  if (K_out && rows > 0) GK_CUDA(cudaMemcpyAsync(K_out, K, (size_t)rows * cols * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------
 // OddSth (odd_sth.cuh).  gk_odd_features builds every root's DAG and the identities of its nodes, repeating the
 // identity pass with another seed while a collision is detected, then counts phi per (graph, identity), C per
 // identity, the self similarities, and splits the counts into one NeighborhoodSubgraphPairwiseDistance-layout table per
@@ -4186,13 +4266,13 @@ int gk_selftest_odd_collision(gk_handle* h, int32_t attempts) {
   return GK_OK;
 }
 
-int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_odd_features: no graphs packed");
-  if (!h->has_labels) return fail(GK_ERR_ARG, "gk_odd_features: vertex labels are required");
-  if (depth == 0) return fail(GK_ERR_ARG, "gk_odd_features: h must be > 0 (or < 0 for no limit)");
-  if (flags != 0) return fail(GK_ERR_ARG, "gk_odd_features: no flags are defined");
-  if (!rank && h->V) return fail(GK_ERR_ARG, "gk_odd_features: null rank table");
+}  // extern "C"
+
+// The feature pass of gk_odd_features (n_levels = 1, the packed labels) and gk_wl_odd_features (one label set per WL
+// level, `ids` [n_levels][V] disjoint across levels): every level's DAGs take their own node and child slots, so the
+// identities of different levels never meet and one table of (graph, identity) counts holds the sum over the levels.
+static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const int32_t* ids, const int32_t* rank,
+                             gk_stats* stats) {
   GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E;
   const int64_t launches0 = h->launches;
@@ -4209,14 +4289,19 @@ int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t fl
     nbase[g + 1] = nbase[g] + n * n;
     ebase[g + 1] = ebase[g] + n * m;
   }
-  if (max_n > ODD_MAX_N) return fail(GK_ERR_UNSUPPORTED, "gk_odd_features: a graph has more than 4096 vertices");
-  const long long S = nbase[N], T = ebase[N];
+  const char* who = n_levels > 1 ? "gk_wl_odd_features" : "gk_odd_features";
+  if (max_n > ODD_MAX_N) return fail(GK_ERR_UNSUPPORTED, std::string(who) + ": a graph has more than 4096 vertices");
+  // the slots of all levels together, checked before anything is sized
+  const long long S_lv = nbase[N], T_lv = ebase[N];
+  const long long S = S_lv * n_levels, T = T_lv * n_levels;
   if (S >= (1LL << 30) || T >= (1LL << 30))
-    return fail(GK_ERR_UNSUPPORTED, "gk_odd_features: 2^30 or more (root, vertex) or (root, edge) pairs");
+    return fail(GK_ERR_UNSUPPORTED, std::string(who) + ": 2^30 or more (root, vertex) or (root, edge) pairs" +
+                                         (n_levels > 1 ? " over all WL levels" : ""));
   ex->odd_S = S; ex->odd_T = T; ex->odd_maxC = 0;
   const size_t S1 = (size_t)std::max<long long>(S, 1), T1 = (size_t)std::max<long long>(T, 1);
   const size_t cap = std::max<size_t>(next_pow2(S1 * 2), 1024);
-  GK_TRY(h->odd_aux.ensure(base.size() * 8 + (size_t)std::max<int64_t>(V, 1) * 4));
+  const size_t LV = (size_t)n_levels * (size_t)V;
+  GK_TRY(h->odd_aux.ensure(base.size() * 8 + std::max<size_t>(LV, 1) * 4 * (ids ? 2 : 1)));
   GK_TRY(h->odd_nodes.ensure(S1 * 32));
   GK_TRY(h->odd_ch.ensure(T1 * 4));
   GK_TRY(h->odd_tab.ensure(cap * 16));  // keys | representative | identity of the slot
@@ -4226,7 +4311,9 @@ int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t fl
   GK_TRY(h->odd_diag.ensure((size_t)N * 8));
   GK_CUDA(cudaMemcpyAsync(h->odd_aux.p, base.data(), base.size() * 8, cudaMemcpyHostToDevice, h->stream));
   int* d_rank = reinterpret_cast<int*>(h->odd_aux.as<long long>() + base.size());
-  if (V) GK_CUDA(cudaMemcpyAsync(d_rank, rank, (size_t)V * 4, cudaMemcpyHostToDevice, h->stream));
+  int* d_ids = ids ? d_rank + std::max<size_t>(LV, 1) : h->labels0.as<int>();
+  if (LV) GK_CUDA(cudaMemcpyAsync(d_rank, rank, LV * 4, cudaMemcpyHostToDevice, h->stream));
+  if (LV && ids) GK_CUDA(cudaMemcpyAsync(d_ids, ids, LV * 4, cudaMemcpyHostToDevice, h->stream));
   const OddNodes o = odd_nodes(h);
   unsigned long long* tab = h->odd_tab.as<unsigned long long>();
   int* rep = reinterpret_cast<int*>(tab + cap);
@@ -4239,8 +4326,9 @@ int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t fl
   // ---- DAGs and identities; repeated with another seed while a collision is detected
   OddParams p;
   p.N = (int)N; p.V = V;
+  p.n_levels = n_levels; p.S = S_lv; p.T = T_lv;
   p.graph_ptr = h->graph_ptr.as<int>(); p.row_ptr = h->row_ptr.as<int>(); p.col_idx = h->col_idx.as<int>();
-  p.vgraph = h->vgraph.as<int>(); p.labels = h->labels0.as<int>(); p.rank = d_rank;
+  p.vgraph = h->vgraph.as<int>(); p.labels = d_ids; p.rank = d_rank;
   p.node_base = h->odd_aux.as<long long>(); p.edge_base = p.node_base + N + 1;
   p.depth = depth < 0 ? -1 : depth;
   p.n_pad = (max_n + 3) / 4 * 4;
@@ -4250,11 +4338,11 @@ int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t fl
   const size_t smem = warp_smem * wpc;
   if (smem > (48 << 10))
     GK_CUDA(cudaFuncSetAttribute(odd_dags, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv(std::max<int64_t>(V, 1), wpc), (int64_t)h->sm_count * 16));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(cdiv(std::max<int64_t>((int64_t)LV, 1), wpc), (int64_t)h->sm_count * 16));
   int64_t retries = 0;
   for (int attempt = 0;; ++attempt) {
     if (attempt == ODD_MAX_ATTEMPTS)
-      return fail(GK_ERR_STATE, "gk_odd_features: identity hashes collided on every attempt");
+      return fail(GK_ERR_STATE, std::string(who) + ": identity hashes collided on every attempt");
     p.seed = mix64(0x6f6464ULL + (unsigned long long)attempt * 0x9e3779b97f4a7c15ULL);
     p.degenerate = h->odd_degen > 0 ? 1 : 0;
     if (h->odd_degen > 0) h->odd_degen--;
@@ -4352,6 +4440,45 @@ int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t fl
   return GK_OK;
 }
 
+extern "C" {
+
+int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_odd_features: no graphs packed");
+  if (!h->has_labels) return fail(GK_ERR_ARG, "gk_odd_features: vertex labels are required");
+  if (depth == 0) return fail(GK_ERR_ARG, "gk_odd_features: h must be > 0 (or < 0 for no limit)");
+  if (flags != 0) return fail(GK_ERR_ARG, "gk_odd_features: no flags are defined");
+  if (!rank && h->V) return fail(GK_ERR_ARG, "gk_odd_features: null rank table");
+  return odd_features_impl(h, depth, 1, nullptr, rank, stats);
+}
+
+int gk_wl_odd_features(gk_handle* h, int32_t depth, int32_t n_iter, const int32_t* ids, const int32_t* rank,
+                       int32_t flags, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_wl_odd_features: no graphs packed");
+  if (depth == 0) return fail(GK_ERR_ARG, "gk_wl_odd_features: h must be > 0 (or < 0 for no limit)");
+  if (n_iter < 0 || n_iter >= MAX_LEVELS) return fail(GK_ERR_ARG, "gk_wl_odd_features: n_iter out of range");
+  if (flags != 0) return fail(GK_ERR_ARG, "gk_wl_odd_features: no flags are defined");
+  if ((!ids || !rank) && h->V) return fail(GK_ERR_ARG, "gk_wl_odd_features: null label or rank table");
+  // label ids are hashed and compared, ranks ordered as u32: both must be non-negative, and a level's ids must not
+  // reach into another level's (the host makes them disjoint by offsetting each level past the previous one)
+  const int64_t V = h->V;
+  int prev_hi = -1;
+  for (int lv = 0; lv <= n_iter; ++lv) {
+    int lo = INT_MAX, hi = -1;
+    for (int64_t v = 0; v < V; ++v) {
+      const int32_t a = ids[(size_t)lv * V + v];
+      if (a < 0 || rank[(size_t)lv * V + v] < 0) return fail(GK_ERR_ARG, "gk_wl_odd_features: negative label id or rank");
+      lo = std::min<int>(lo, a); hi = std::max<int>(hi, a);
+    }
+    if (V && lo <= prev_hi) return fail(GK_ERR_ARG, "gk_wl_odd_features: label ids of two levels overlap");
+    prev_hi = hi;
+  }
+  return odd_features_impl(h, depth, n_iter + 1, ids, rank, stats);
+}
+
+}  // extern "C"
+
 // The signature of every identity, from its representative node: label id, children's identities in order, C.
 static int odd_host_signatures(gk_handle* h, std::vector<int>* label, std::vector<int64_t>* off, std::vector<int>* child,
                                std::vector<int>* C) {
@@ -4385,6 +4512,8 @@ static int odd_host_signatures(gk_handle* h, std::vector<int>* label, std::vecto
   }
   return GK_OK;
 }
+
+extern "C" {
 
 int gk_odd_info(gk_handle* h, int64_t* info3) {
   if (!h || !info3) return fail(GK_ERR_ARG, "gk_odd_info: null argument");

@@ -253,6 +253,14 @@ struct gk_handle {
   gk::DevBuf nspd_lvl, nspd_q, nspd_H, nspd_aux, nspd_ws, nspd_pairs, nspd_blk, nspd_tab, nspd_keys, nspd_C;
   int nspd_r = 0, nspd_d = 0;
 
+  // ---- WL over a base kernel whose levels cannot share one feature block (gk_wl_level_sum): the running fp64 sum of
+  // the levels' K and the K of the current level; shape and square-ness of the sum, levels added so far.  No re-pack or
+  // feature pass touches them, so the sum survives the per-level gk_pack_csr / gk_nspd_features calls.
+  gk::DevBuf wl_sum, wl_lvl;
+  int64_t wl_sum_rows = 0, wl_sum_cols = 0, wl_sum_row0 = 0;
+  int32_t wl_sum_levels = 0;
+  bool wl_sum_square = false;
+
   // ---- random walk (FK_RW): edge values of the packed CSR, its transpose, eigen-data, coefficients
   gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;
   int rw_route = 0, rw_fn = 0, rw_ncoef = 0;

@@ -535,4 +535,19 @@ normalize_rows(long long rows, long long cols, OutT* __restrict__ out, long long
   }
 }
 
+// WL over a base kernel with per-level fp64 K: dst += src elementwise, one level at a time, so that the sum rounds as
+// numpy's np.sum(levels, axis=0) does: ((K_0 + K_1) + K_2) ...
+__global__ void __launch_bounds__(256)
+add_f64(long long n, const double* __restrict__ src, double* __restrict__ dst) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    dst[i] = dst[i] + src[i];
+}
+
+// out[i] = K[i ld + i]: the diagonal of a full square K
+__global__ void __launch_bounds__(256)
+diag_of_f64(long long n, const double* __restrict__ K, long long ld, double* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = K[i * ld + i];
+}
+
 }  // namespace gk

@@ -25,12 +25,14 @@ constexpr int ODD_MAX_WARPS = 4;     // odd_dags: up to four warps per CTA, each
 struct OddParams {
   int N;
   long long V;
+  int n_levels;                  // label sets: one DAG pass per (level, root); 1 for OddSth itself
+  long long S, T;                // node and child slots of one level (the last entries of node_base / edge_base)
   const int* graph_ptr;
   const int* row_ptr;
   const int* col_idx;
   const int* vgraph;
-  const int* labels;             // label id: one per distinct str(label)
-  const int* rank;               // rank of the label's value among the values of its graph (ties share a rank)
+  const int* labels;             // [n_levels][V] label id: one per distinct str(label), disjoint across levels
+  const int* rank;               // [n_levels][V] rank of the label's value among the values of its graph (ties share a rank)
   const long long* node_base;    // per graph: first node slot of its first root (sum of n^2 before it)
   const long long* edge_base;    // per graph: first child slot of its first root (sum of n m before it)
   int depth;                     // h, < 0 without a limit
@@ -79,13 +81,17 @@ odd_dags(OddParams p) {
   __shared__ int s_cnt[ODD_MAX_WARPS];
   const unsigned FULL = 0xffffffffu;
 
-  for (long long v = (long long)blockIdx.x * wpc + wib; v < p.V; v += (long long)gridDim.x * wpc) {
+  for (long long lvv = (long long)blockIdx.x * wpc + wib; lvv < p.V * p.n_levels; lvv += (long long)gridDim.x * wpc) {
+    // level-major: the nodes of level l take the slots [l S, (l + 1) S), their children [l T, (l + 1) T)
+    const long long level = lvv / p.V, v = lvv - level * p.V;
+    const int* labels = p.labels + level * p.V;
+    const int* rank = p.rank + level * p.V;
     const int g = p.vgraph[v];
     const int g0 = p.graph_ptr[g], n = p.graph_ptr[g + 1] - g0;
     const int m = p.row_ptr[g0 + n] - p.row_ptr[g0];
     const int lv = (int)(v - g0);
-    const long long nb = p.node_base[g] + (long long)lv * n;
-    const long long eb = p.edge_base[g] + (long long)lv * m;
+    const long long nb = level * p.S + p.node_base[g] + (long long)lv * n;
+    const long long eb = level * p.T + p.edge_base[g] + (long long)lv * m;
     const int* rp = p.row_ptr + g0;
     for (int i = lane; i < n; i += 32) { dep[i] = -1; indeg[i] = 0; }
     __syncwarp();
@@ -120,7 +126,7 @@ odd_dags(OddParams p) {
     }
     __syncwarp();
     // ---- Kahn: pop the least (rank, sequence); a child whose in-degree drops to 0 is queued in edge order
-    if (lane == 0) { qv[0] = lv; qk[0] = (unsigned long long)(unsigned)p.rank[g0 + lv] << 32; }
+    if (lane == 0) { qv[0] = lv; qk[0] = (unsigned long long)(unsigned)rank[g0 + lv] << 32; }
     int qn = 1, seq = 1;
     __syncwarp();
     for (int i = 0; i < cnt; ++i) {
@@ -157,7 +163,7 @@ odd_dags(OddParams p) {
           if (ready) {
             const int r = __popc(b & ((1u << lane) - 1u));
             qv[qn + r] = w;
-            qk[qn + r] = ((unsigned long long)(unsigned)p.rank[g0 + w] << 32) | (unsigned)(seq + r);
+            qk[qn + r] = ((unsigned long long)(unsigned)rank[g0 + w] << 32) | (unsigned)(seq + r);
           }
           qn += __popc(b);
           seq += __popc(b);
@@ -171,7 +177,7 @@ odd_dags(OddParams p) {
     int e_off = 0;
     for (int i = cnt - 1; i >= 0; --i) {
       const int u = at[i];
-      const int lab = p.labels[g0 + u];
+      const int lab = labels[g0 + u];
       unsigned long long acc = 0;
       int nch = 0;
       if (expanded(u)) {

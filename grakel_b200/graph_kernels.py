@@ -1,7 +1,8 @@
 """`GraphKernel`: the name -> kernel dispatcher of the reference (grakel/graph_kernels.py:77-571), restricted to
 the kernels of the device hot path:
 
-    "weisfeiler_lehman" / "WL"  (framework; base "vertex_histogram"/"subtree_wl"/"VH"/"ST-WL", "shortest_path", ...)
+    "weisfeiler_lehman" / "WL"  (framework; base "vertex_histogram"/"subtree_wl"/"VH"/"ST-WL", "shortest_path",
+                                 "edge_histogram", "pyramid_match", "NSPD", "ODD")
     "vertex_histogram" / "subtree_wl" / "VH" / "ST-WL"
     "shortest_path" / "SP"      (+ with_labels, algorithm_type, as_attributes)
     "edge_histogram" / "EH"

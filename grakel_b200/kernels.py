@@ -378,19 +378,26 @@ def _restore_level_dictionaries(content, owner):
     return d
 
 
-def wl_reference_dictionaries(row_ptr, col_idx, level0_ids, n_level0, classes):
+def wl_reference_dictionaries(row_ptr, col_idx, level0_ids, n_level0, classes, n_fit_vertices=None):
     """The reference's per-level label dictionaries from the device partition.
 
     `classes[i]` (i >= 1) holds one class id per vertex (any numbering; `gk_wl_labels`).  The reference names a
     class by the string  str(own label) + "," + str(sorted neighbour labels)  over the labels of level i-1, sorts the
     distinct strings and numbers them on from where the previous level stopped (weisfeiler_lehman.py:223-246).
     One string per CLASS is built here (from the class's first vertex), not one per vertex.
+
+    With `n_fit_vertices`, the block is the fitted graphs' vertices followed by a transform's (the joint partition of
+    both): the classes the fitted vertices have are numbered as in the fit, the others in sorted order after them, and
+    the next level again starts where the fit's did (weisfeiler_lehman.py:434-466).  Only the fitted classes enter the
+    dictionaries then.
     Returns ({level: {credential: label}}, [reference label of every vertex, per level])."""
     prev = np.asarray(level0_ids, dtype=np.int64)
     count = int(n_level0)
+    nfv = len(prev) if n_fit_vertices is None else int(n_fit_vertices)
     out, labels = {}, [prev]
     for i in range(1, len(classes)):
         uniq, first, inv = np.unique(np.asarray(classes[i]), return_index=True, return_inverse=True)
+        inv = inv.reshape(-1)
         creds = []
         for v in first.tolist():
             nb = prev[col_idx[row_ptr[v]:row_ptr[v + 1]]]
@@ -398,23 +405,35 @@ def wl_reference_dictionaries(row_ptr, col_idx, level0_ids, n_level0, classes):
         if len(set(creds)) != len(creds):
             raise RuntimeError("two classes of level %d share a signature: the device partition is not the "
                                "reference's" % i)
-        order = sorted(range(len(creds)), key=creds.__getitem__)
+        fitted = np.zeros(len(uniq), dtype=bool)
+        fitted[inv[:nfv]] = True
+        fit_k = [k for k in range(len(creds)) if fitted[k]]
+        new_k = [k for k in range(len(creds)) if not fitted[k]]
+        order = sorted(fit_k, key=creds.__getitem__) + sorted(new_k, key=creds.__getitem__)
         new_id = np.empty(len(uniq), dtype=np.int64)
         new_id[order] = count + np.arange(len(uniq), dtype=np.int64)
-        out[i] = {creds[k]: count + r for r, k in enumerate(order)}
-        prev = new_id[inv.reshape(-1)]
+        out[i] = {creds[k]: count + r for r, k in enumerate(order[:len(fit_k)])}
+        prev = new_id[inv]
         labels.append(prev)
-        count += len(uniq)
+        count += len(fit_k)
     return out, labels
 
 
 # ------------------------------------------------------------------------------
+_WL_GRAPH_BASES = ()  # set after the base classes: the bases whose WL route needs the list of graphs
+
+
 class WeisfeilerLehman(Kernel):
     """Weisfeiler-Lehman subtree kernel (weisfeiler_lehman.py:23-555).
 
-    K = sum over levels 0..n_iter of the vertex-histogram kernel on the level's
-    compressed labels.  Only the subtree base kernel (`VertexHistogram`, the
-    reference default) runs on the device."""
+    K = sum over levels 0..n_iter of the base kernel on the level's compressed
+    labels.  The base kernels that run on the device: VertexHistogram (the
+    subtree kernel, the reference default), EdgeHistogram, ShortestPath,
+    PyramidMatch, NeighborhoodSubgraphPairwiseDistance and OddSth.  Over the
+    last two every level's labels are numbered the reference's way on the host
+    (they read label numbers, not only the partition); OddSth's levels share
+    one DAG pass and one exact Gram, NSPD's levels are folded one by one into a
+    device-resident sum added in level order (DESIGN 4.21)."""
 
     _graph_format = "dictionary"
     _nan_to_num = True
@@ -445,10 +464,16 @@ class WeisfeilerLehman(Kernel):
                     raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
                                      "parameters names and values")
                 params.pop("normalize", None)
-            if base not in (VertexHistogram, EdgeHistogram, ShortestPath, PyramidMatch):
+            if base not in (VertexHistogram, EdgeHistogram, ShortestPath, PyramidMatch,
+                            NeighborhoodSubgraphPairwiseDistance, OddSth):
                 raise NotImplementedError("grakel_b200 runs WeisfeilerLehman over VertexHistogram (the subtree kernel), "
-                                          "EdgeHistogram, ShortestPath or PyramidMatch; other base kernels are outside "
-                                          "the device hot path")
+                                          "EdgeHistogram, ShortestPath, PyramidMatch, "
+                                          "NeighborhoodSubgraphPairwiseDistance or OddSth; other base kernels are "
+                                          "outside the device hot path")
+            if base is NeighborhoodSubgraphPairwiseDistance:  # the base kernel's own checks
+                NeighborhoodSubgraphPairwiseDistance(**{k: v for k, v in params.items() if k in ("r", "d")}).initialize()
+            if base is OddSth:
+                OddSth(h=params.get("h")).initialize()
             if base is PyramidMatch:  # the base kernel's own checks (pyramid_match.py:62-81)
                 PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
             if base is ShortestPath:
@@ -492,6 +517,9 @@ class WeisfeilerLehman(Kernel):
         if base is PyramidMatch and isinstance(X, Block):
             raise NotImplementedError("WeisfeilerLehman over PyramidMatch embeds every graph's adjacency matrix; pass "
                                       "the list of graphs")
+        if base in (NeighborhoodSubgraphPairwiseDistance, OddSth) and isinstance(X, Block):
+            raise NotImplementedError("WeisfeilerLehman over %s needs every graph's edge dictionary (edge labels, "
+                                      "neighbour order); pass the list of graphs" % base.__name__)
         if base is ShortestPath:
             # the base kernel receives the edge DICTIONARY of every graph (weisfeiler_lehman.py:188, 218):
             # Dijkstra semantics whatever the input spelling; labels are the WL vertex set
@@ -504,7 +532,7 @@ class WeisfeilerLehman(Kernel):
                 delattr(self, "_X_diag")
             if not isinstance(X, (Iterable, Block)):
                 raise TypeError("input must be an iterable\n")
-            if self._base_graph_kernel is PyramidMatch and not isinstance(X, Block):
+            if self._base_graph_kernel in _WL_GRAPH_BASES and not isinstance(X, Block):
                 X = list(X)
             block = self._pack_for_base(X, lambda n: n >= 2)  # weisfeiler_lehman.py:152
             self._nx = block.n_graphs
@@ -512,15 +540,18 @@ class WeisfeilerLehman(Kernel):
             self._inv_labels = _LevelDictionaries(dictionary, self)
             fitted = Fitted(block, ids, dictionary)
             fitted.pm = self._pm_embed(X, block)
+            fitted.base = self._base_data(X, block)
+            self._fit_transformed = self._method_calling == 2
             return fitted
         if self._method_calling != 3:
             raise ValueError("method call must be called either from fit or fit-transform")
-        if self._base_graph_kernel is PyramidMatch and not isinstance(X, Block):
+        if self._base_graph_kernel in _WL_GRAPH_BASES and not isinstance(X, Block):
             X = list(X)
         block = self._pack_for_base(X, lambda n: n in (2, 3))  # :367
         ids, _ = label_ids(block.labels, self._inv_labels[0], sort_new=True)  # :417-418
         fitted = Fitted(block, ids, self._inv_labels[0])
         fitted.pm = self._pm_embed(X, block)
+        fitted.base = self._base_data(X, block)
         return fitted
 
     def _pm_embed(self, X, block):
@@ -594,6 +625,10 @@ class WeisfeilerLehman(Kernel):
             raise ValueError("input must be an iterable\n")
         Y = self.parse_input(X)
         self._pm_y = Y.pm
+        self._base_y = Y.base
+        if self._base_graph_kernel is OddSth and self.normalize and not getattr(self, "_fit_transformed", False):
+            # the reference's diagonal() asks the fitted OddSth levels for self._phi_X, which they never set
+            raise AttributeError("'OddSth' object has no attribute '_phi_X'")
         K, xdiag, ydiag = self._run(Block.concat(self.X.block, Y.block), np.concatenate([self.X.ids, Y.ids]),
                                     n_fit=self._nx)
         self._X_diag = xdiag
@@ -615,9 +650,164 @@ class WeisfeilerLehman(Kernel):
                                    flags=_lib.GK_PM_WL_LABELS if with_labels else 0, skip=pm.skip)
         return eng.wl_features(self._n_iter - 1)
 
+    def diagonal(self):
+        if self._base_graph_kernel is OddSth:
+            check_is_fitted(self, ["X"])
+            if not getattr(self, "_fit_transformed", False):
+                if not getattr(self, "_is_transformed", False):
+                    raise NotFittedError("This OddSth instance is not fitted yet. Call 'fit' with appropriate arguments "
+                                         "before using this estimator.")
+                raise AttributeError("'OddSth' object has no attribute '_phi_X'")
+        return super().diagonal()
+
+    def _base_data(self, X, block):
+        """NeighborhoodSubgraphPairwiseDistance / OddSth base: every element's graph as that base kernel packs it, and
+        `src`, the WL vertex of every base vertex (the base kernel sees the WL labels through the element's labels
+        dictionary, whose key order is the WL block's)."""
+        base = self._base_graph_kernel
+        if base not in _WL_GRAPH_BASES or base is PyramidMatch:
+            return None
+        gp = np.asarray(block.graph_ptr, dtype=np.int64)
+        src, graphs, els = [], [], []
+        for x in X:
+            if isinstance(x, Graph):
+                x = x.as_element()
+            x = list(x)
+            if len(x) == 0:
+                continue
+            loc = {k: i for i, k in enumerate(x[1].keys())}
+            if base is NeighborhoodSubgraphPairwiseDistance:
+                if len(x) != 3:  # the element the reference hands on is (edges, labels) + edge labels
+                    raise TypeError(_NSPD_ELEMENT_MSG)
+                n, edges, _, el, order = _nspd_graph(x[0], x[1], x[2], with_order=True)
+                graphs.append((n, edges, None, el))
+            else:
+                if type(x[0]) is dict and x[0] and all(type(d) is list for d in x[0].values()) and not all(x[0].values()):
+                    raise ValueError("vertex not inside edge dictionary")
+                els.append([x[0], x[1]])
+                order = adjacency_and_order(x[0])[1]
+            src.append([loc.get(k, -1) for k in order])
+        out = _WlBaseData()
+        cols = []
+        for g, rows in enumerate(src):
+            rows = np.asarray(rows, dtype=np.int64)
+            if np.any(rows < 0):
+                raise NotImplementedError("WeisfeilerLehman over %s: a vertex of a graph's edges has no label"
+                                          % base.__name__)
+            cols.append(rows + gp[g])
+        out.src = np.concatenate(cols) if cols else np.zeros(0, dtype=np.int64)
+        out.wl_vertices = int(gp[-1])
+        if base is NeighborhoodSubgraphPairwiseDistance:
+            out.graphs = graphs
+        else:
+            b = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
+                     keep_edge_order=True)
+            if b.n_vertices != len(out.src):
+                raise NotImplementedError("WeisfeilerLehman over OddSth: a graph's vertices are not those of its edges")
+            out.block = b
+        return out
+
+    def _level_labels(self, block, ids, n_fit_vertices):
+        """The reference's label of every WL vertex at every level: the device partition, numbered on the host."""
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
+            eng.wl_features(self._n_iter - 1)
+            classes = [ids] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, self._n_iter)]
+        t0 = time.perf_counter()
+        _, labels = wl_reference_dictionaries(np.asarray(block.row_ptr), np.asarray(block.col_idx), ids,
+                                              len(self.X.dictionary), classes, n_fit_vertices=n_fit_vertices)
+        self.ms_host_numbering_ = (time.perf_counter() - t0) * 1e3
+        return labels
+
+    def _base_run(self, block, ids, n_fit, want_matrix=True, row_range=None):
+        """WL over NeighborhoodSubgraphPairwiseDistance or OddSth: K = sum over the levels of the base kernel on the
+        level's reference labels (weisfeiler_lehman.py:260-270)."""
+        if n_fit == block.n_graphs:
+            data = self.X.base
+        else:
+            data = _WlBaseData.concat(self.X.base, self._base_y)
+        n_fit_v = int(np.asarray(block.graph_ptr)[n_fit])
+        labels = self._level_labels(block, ids, n_fit_v)
+        if self._base_graph_kernel is OddSth:
+            return self._wl_odd_run(data, labels, n_fit, want_matrix, row_range)
+        return self._wl_nspd_run(data, labels, n_fit, want_matrix, row_range)
+
+    def _wl_odd_run(self, data, labels, n_fit, want_matrix, row_range):
+        b = data.block
+        ids, rank, off = [], [], 0
+        for lab in labels:
+            L = np.asarray(lab, dtype=np.int64)[data.src]
+            if len(L) and L.max() >= 2 ** 31:
+                raise NotImplementedError("WeisfeilerLehman over OddSth: a WL label of 2^31 or more")
+            uniq, inv = np.unique(L, return_inverse=True)
+            ids.append(inv.reshape(-1) + off)  # str(label) identities: one id per label, disjoint across levels
+            rank.append(L)                      # Kahn's order compares the label values themselves
+            off += len(uniq)
+        if off >= 2 ** 31:
+            raise NotImplementedError("WeisfeilerLehman over OddSth: 2^31 or more labels over all levels")
+        h = self._params.get("h")
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            eng.pack(b.graph_ptr, b.row_ptr, b.col_idx, ids[0], None, None)
+            self.stats_ = eng.wl_odd_features(-1 if h is None else h, self._n_iter - 1, np.stack(ids), np.stack(rank))
+            K, xd, yd = eng.gram(b.n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
+                                 stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd
+
+    def _wl_nspd_run(self, data, labels, n_fit, want_matrix, row_range):
+        p = self._params
+        r, d = p.get("r", 3), p.get("d", 4)
+        graphs = data.graphs
+        if r > 0 and max(g[0] for g in graphs) >= 65535:  # the device refuses it too; do not pack it first
+            raise NotImplementedError("NeighborhoodSubgraphPairwiseDistance: r > 0 with a graph of 65535 or more "
+                                      "vertices")
+        nsp = NeighborhoodSubgraphPairwiseDistance(r=r, d=d)
+        gp, rp, ci, _, el, sh, tok0 = nsp._pack([(n, e, ["0"] * n, l) for n, e, _, l in graphs])
+        elabels = [tok0.el_bytes[tok0.el_off[i]:tok0.el_off[i + 1]].tobytes().decode("utf-8")
+                   for i in range(tok0.n_elabels)]
+        N = len(gp) - 1
+        square = n_fit == N
+        rows_total = N if square else N - n_fit
+        rb, re_ = (0, rows_total) if row_range is None else row_range
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            for lv, lab in enumerate(labels):
+                L = np.asarray(lab, dtype=np.int64)[data.src]
+                uniq, inv = np.unique(L, return_inverse=True)
+                tokens = _NspdTokens(d, [str(int(u)) for u in uniq], elabels)
+                eng.pack(gp, rp, ci, inv.reshape(-1), None, None)
+                self.stats_, mask = eng.nspd_features(r, d, sh, el, tokens)
+                if want_matrix:
+                    eng.wl_level_sum(lv, n_fit, (rb, re_))
+            # diagonal() of every fitted level: its number of (radius, distance) levels (the reference's constant)
+            def levels(m):
+                top = max((int(x).bit_length() for x in m), default=0)
+                return (r + 1) * top
+            xd_lv = np.full(n_fit, float(levels(mask[:n_fit])))
+            yd_lv = None if square else np.full(N - n_fit, float(levels(mask[n_fit:])))
+            xd_sum = xd_lv.copy()
+            yd_sum = None if yd_lv is None else yd_lv.copy()
+            for _ in range(1, self._n_iter):
+                xd_sum += xd_lv
+                if yd_sum is not None:
+                    yd_sum += yd_lv
+            if not want_matrix:
+                return None, xd_sum, yd_sum
+            if square:
+                full = rb == 0 and re_ == N
+                K, kd = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(self.normalize), want_kdiag=full)
+                return K, kd, None
+            xd = getattr(self, "_X_diag", None)
+            xd = xd_sum if xd is None else np.asarray(xd, dtype=np.float64).reshape(-1)
+            K, _ = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(self.normalize), xdiag=xd, ydiag=yd_sum)
+            return K, xd, yd_sum
+
     def _run(self, block, ids, n_fit, want_matrix=True):
         """The plain subtree fit_transform (square, un-normalised) is ONE C call, gk_wl_gram: relabel, column statistics,
         head/tail decision on the device, GEMM, tail and delivery with a single host synchronisation."""
+        if self._base_graph_kernel in (NeighborhoodSubgraphPairwiseDistance, OddSth):
+            return self._base_run(block, ids, n_fit, want_matrix)
         if (want_matrix and not self.normalize and n_fit == block.n_graphs and self._base_graph_kernel is VertexHistogram
                 and type(self) is WeisfeilerLehman):
             with _lib.engine(getattr(self, "device_", None)) as eng:
@@ -640,6 +830,25 @@ class WeisfeilerLehman(Kernel):
             classes = [ids] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, self._n_iter)]
         out, self.wl_labels_ = wl_reference_dictionaries(np.asarray(block.row_ptr), np.asarray(block.col_idx), ids,
                                                          len(self.X.dictionary), classes)
+        return out
+
+
+class _WlBaseData:
+    """What WL over NeighborhoodSubgraphPairwiseDistance / OddSth keeps per call: the base kernel's graphs (NSPD: (n,
+    edges, -, edge label strings); OddSth: its packed block) and `src`, the WL vertex of every base vertex."""
+
+    graphs = None
+    block = None
+
+    @staticmethod
+    def concat(a, b):
+        out = _WlBaseData()
+        out.src = np.concatenate([a.src, b.src + a.wl_vertices])
+        out.wl_vertices = a.wl_vertices + b.wl_vertices
+        if a.graphs is not None:
+            out.graphs = a.graphs + b.graphs
+        else:
+            out.block = Block.concat(a.block, b.block)
         return out
 
 
@@ -2759,7 +2968,7 @@ _NSPD_ELEMENT_MSG = ("each element of X must have either a graph with labels for
                      "consisting of a graph type object, labels for vertices and labels for edges.")
 
 
-def _nspd_graph(g, node_labels, edge_labels):
+def _nspd_graph(g, node_labels, edge_labels, with_order=False):
     """One graph as the reference sees it after change_format("adjacency") then ("dictionary") (graph.py:912-1053):
     the spelling is read by packing.classify (graph.py's is_adjacency / is_edge_dictionary), the vertices are the
     indices 0 .. n-1 of an adjacency matrix or of the sorted symbols of an edge dictionary, and an edge survives when
@@ -2775,6 +2984,8 @@ def _nspd_graph(g, node_labels, edge_labels):
     edges = sorted(zip(ii.tolist(), jj.tolist()))
     vl = [str(node_labels[s]) for s in order]
     el = [str(edge_labels[(order[i], order[j])]) for i, j in edges]
+    if with_order:
+        return len(order), edges, vl, el, order
     return len(order), edges, vl, el
 
 
@@ -4059,3 +4270,6 @@ class GraphletSampling(Kernel):
         if getattr(self, "_is_transformed", False):
             return self._X_diag, self._Y_diag
         return self._X_diag
+
+
+_WL_GRAPH_BASES = (PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth)

@@ -231,6 +231,18 @@ int gk_nspd_hashes(gk_handle* h, int32_t radius, uint32_t* out);
  * hashes) in order k = 0 .. n-1 */
 int gk_selftest_nspd_set_order(int64_t n, const int64_t* h0, const int64_t* h1, int64_t* order);
 
+/* WeisfeilerLehman over NeighborhoodSubgraphPairwiseDistance: every WL level's K is a sum of cosine-normalised level
+ * Grams, so the levels are added as matrices.  For level = 0, 1, ... in order: pack the level's labels, run
+ * gk_nspd_features, then gk_wl_level_sum folds the level's K (gram_path 12, un-normalised; n_fit and the row range as in
+ * gk_gram) into a device-resident fp64 sum, sum = sum + K_level, which rounds as numpy's np.sum(axis=0).  No re-pack or
+ * feature pass touches the sum.  gk_wl_level_sum_fetch then applies GK_NORMALIZE (and GK_NAN_TO_NUM) with the self
+ * similarities xdiag (the columns) and ydiag (a transform's rows; a square sum takes its rows' from xdiag), or with the
+ * sum's own diagonal when xdiag is NULL (full square sum only), and copies K (rows x cols, row-major) to the host
+ * array K_out; kdiag (may be NULL) receives the sum's diagonal before normalisation (full square sum only). */
+int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begin, int64_t row_end, gk_stats* stats);
+int gk_wl_level_sum_fetch(gk_handle* h, int32_t flags, const double* xdiag, const double* ydiag, double* K_out,
+                          double* kdiag);
+
 /* RandomWalk / RandomWalkLabeled (random_walk.py:28-541), one graph pair per CTA in fp64.  The packed CSR gives the
  * structure (gk_pack_csr without weights; with labels for GK_RW_LABELED), `values[E]` the adjacency entries of its
  * edges (any sign, self-loops included), `t_row_ptr[V+1]` / `t_col_idx[E]` / `t_values[E]` the same block transposed
@@ -295,6 +307,14 @@ int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out);
  * gk_odd_info writes [identities, child ids of all signatures, largest C]; gk_odd_signatures the signature of every
  * identity (label[F], child_off[F + 1], child[child_off[F]] identity ids in order, C[F]). */
 int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t flags, gk_stats* stats);
+/* WeisfeilerLehman over OddSth: the pass of gk_odd_features over n_iter + 1 label sets at once.  ids and rank are
+ * [n_iter + 1][V]: level l's label ids (non-negative, every id of level l above every id of level l - 1, so the
+ * identities of different levels are disjoint) and rank values (non-negative).  Each level's DAGs take their own node
+ * and child slots; one (graph, identity) table then holds the sum over the levels, and gk_gram (gram_path 14) returns
+ * sum_levels K_level exactly.  The 4096-vertex and 2^30-pair limits apply to the (n_iter + 1)-fold totals and are
+ * checked before anything is sized. */
+int gk_wl_odd_features(gk_handle* h, int32_t depth, int32_t n_iter, const int32_t* ids, const int32_t* rank,
+                       int32_t flags, gk_stats* stats);
 int gk_odd_info(gk_handle* h, int64_t* info3);
 int gk_odd_signatures(gk_handle* h, int32_t* label, int64_t* child_off, int32_t* child, int32_t* C);
 /* Tests only: the next `attempts` identity passes of gk_odd_features hash (label id, number of children) alone, so

@@ -49,3 +49,12 @@ print("gk_wl_gram", Kg.shape, float(Kg.sum()), "asynchronous pass" if st.gemm_la
 Km = ShortestPathAttr(metric=lambda a, c: float(np.exp(-np.sum((np.asarray(a) - np.asarray(c)) ** 2)))).fit_transform(At[:8])
 print("SP-attr metric", Km.shape, float(Km.sum()))
 print("sanitize_small ok")
+# WeisfeilerLehman over NeighborhoodSubgraphPairwiseDistance (per-level fold, device-resident level sum) and over OddSth
+# (one DAG pass over all levels), fit_transform and a normalised transform
+from grakel_b200 import NeighborhoodSubgraphPairwiseDistance, OddSth  # noqa: E402
+Xe = [[g, L, {(u, v): (L[u] + L[v]) % 3 for (u, v) in g}] for g, L in gen_list(40, 10, 6)]
+for base in ((NeighborhoodSubgraphPairwiseDistance, {"r": 1, "d": 2}), (OddSth, {"h": 2})):
+    wlb = WeisfeilerLehman(n_iter=2, normalize=True, base_graph_kernel=base)
+    Kb = wlb.fit_transform(Xe[:30])
+    Kt = wlb.transform(Xe[30:])
+    print("WL over", base[0].__name__, Kb.shape, float(Kb.sum()), Kt.shape)
