@@ -87,6 +87,8 @@ _SYMBOLS = {
     "gk_wl_odd_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_wl_level_sum": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.POINTER(GkStats)]),
     "gk_wl_level_sum_fetch": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P]),
+    "gk_core_sum_begin": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int32]),
+    "gk_core_level_add": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, _P, _P, _P, _P, C.POINTER(GkStats)]),
     "gk_odd_info": (C.c_int, [_P, _P]),
     "gk_odd_signatures": (C.c_int, [_P, _P, _P, _P, _P]),
     "gk_selftest_odd_collision": (C.c_int, [_P, C.c_int32]),
@@ -646,6 +648,24 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_wl_level_sum_fetch(self.h, flags, _ptr(xd), _ptr(yd), _ptr(K), _ptr(kd)))
         return K, kd
+
+    def core_sum_begin(self, n_rows, n_cols, square):
+        """Zero the device-resident sum of a CoreFramework fold (gk_core_sum_begin)."""
+        with self._lock:
+            self._check(self.lib.gk_core_sum_begin(self.h, int(n_rows), int(n_cols), int(bool(square))))
+
+    def core_level_add(self, level, n_fit, rows, cols, n_graphs, want_diag=True, stats=None):
+        """Add the K of core level `level` (the base kernel's features just computed; `n_graphs` packed, the first
+        `n_fit` its columns) into the sum at rows[j], cols[c] (gk_core_level_add).  Returns (xdiag, ydiag)."""
+        rows, cols = _i32(rows), _i32(cols)
+        square = n_fit == n_graphs
+        xd = np.empty(n_fit, dtype=np.float64) if want_diag else None
+        yd = np.empty(n_graphs - n_fit, dtype=np.float64) if (want_diag and not square) else None
+        st = stats if stats is not None else GkStats()
+        with self._lock:
+            self._check(self.lib.gk_core_level_add(self.h, int(level), int(n_fit), len(rows), _ptr(rows), _ptr(cols),
+                                                   _ptr(xd), _ptr(yd), C.byref(st)))
+        return xd, yd
 
     def odd_signatures(self):
         """(label id, child offsets, child identity ids, C) of every identity after odd_features."""

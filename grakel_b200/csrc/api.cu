@@ -358,7 +358,7 @@ int gk_destroy(gk_handle* h) {
                         &h->svmt_vptr, &h->svmt_adj, &h->svmt_m, &h->svmt_alpha, &h->svmt_iters, &h->svmt_cnt,
                         &h->svmt_off, &h->svmt_idx, &h->svmt_sums, &h->svmt_phi, &h->svmt_rec, &h->svmt_ctl,
                         &h->gs_canon, &h->gs_first, &h->gs_colid, &h->gs_blk, &h->gs_colcnt, &h->gs_diag, &h->gs_ctl,
-                        &h->gs_samp, &h->wl_sum, &h->wl_lvl};
+                        &h->gs_samp, &h->wl_sum, &h->wl_lvl, &h->core_map};
   for (auto* b : bufs) b->release();
   h->h_scalars.release();
   h->h_colstats.release();
@@ -4138,6 +4138,29 @@ static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
   return GK_OK;
 }
 
+static int gram_odd(gk_handle* h, const GramReq& q, gk_stats* stats);
+static int gram_ml(gk_handle* h, const GramReq& q, gk_stats* stats);
+static int gram_svmt(gk_handle* h, const GramReq& q, gk_stats* stats);
+static int gram_gs(gk_handle* h, const GramReq& q, gk_stats* stats);
+
+// The route of the packed feature kind: gk_gram and gk_core_level_add.
+static int gram_route(gk_handle* h, const GramReq& q, gk_stats* stats) {
+  switch (h->feature_kind) {
+    case FK_SPATTR: return gram_spattr(h, q, stats);
+    case FK_GH: return h->gh_node_kernel == GK_GH_LINEAR ? gram_spattr(h, q, stats) : gram_gh_nodepair(h, q, stats);
+    case FK_NH: return gram_nh(h, q, stats);
+    case FK_PM: return gram_pm(h, q, stats);
+    case FK_NSPD: return gram_nspd(h, q, stats);
+    case FK_RW: return gram_rw(h, q, stats);
+    case FK_SM: return gram_sm(h, q, stats);
+    case FK_ODD: return gram_odd(h, q, stats);
+    case FK_ML: return gram_ml(h, q, stats);
+    case FK_SVMT: return gram_svmt(h, q, stats);
+    case FK_GS: return gram_gs(h, q, stats);
+    default: return gram_int(h, q, block_of(h), stats);
+  }
+}
+
 // ---------------------------------------------------------------------------
 // WL over NeighborhoodSubgraphPairwiseDistance.  Every WL level's K is itself a sum of cosine-normalised per-(radius,
 // distance) Grams, so the WL levels cannot share one feature block: the host packs each level's labels and runs
@@ -4149,7 +4172,7 @@ int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begi
   if (!h) return fail(GK_ERR_ARG, "null handle");
   if (!h->features_ready || h->feature_kind != FK_NSPD)
     return fail(GK_ERR_STATE, "gk_wl_level_sum: run gk_nspd_features on the level's labels first");
-  if (level < 0 || (level > 0 && level != h->wl_sum_levels))
+  if (level < 0 || (level > 0 && (level != h->wl_sum_levels || h->core_sum)))
     return fail(GK_ERR_ARG, "gk_wl_level_sum: levels must be added in order, starting at 0");
   GramReq q;
   GK_TRY(gram_request(h, FK_NSPD, n_fit, 0, row_begin, row_end, nullptr, GK_F64, 0, nullptr, nullptr, &q));
@@ -4169,6 +4192,7 @@ int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begi
   }
   h->wl_sum_rows = q.k_rows; h->wl_sum_cols = q.k_cols; h->wl_sum_row0 = q.row_begin; h->wl_sum_square = q.square;
   h->wl_sum_levels = level + 1;
+  h->core_sum = false;
   GK_CUDA(cudaStreamSynchronize(h->stream));
   return GK_OK;
 }
@@ -4176,7 +4200,8 @@ int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begi
 int gk_wl_level_sum_fetch(gk_handle* h, int32_t flags, const double* xdiag, const double* ydiag, double* K_out,
                           double* kdiag) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->wl_sum_levels <= 0) return fail(GK_ERR_STATE, "gk_wl_level_sum_fetch: no level added (gk_wl_level_sum)");
+  if (h->wl_sum_levels <= 0 && !h->core_sum)
+    return fail(GK_ERR_STATE, "gk_wl_level_sum_fetch: no level added (gk_wl_level_sum) and no gk_core_sum_begin");
   if (flags & ~(GK_NORMALIZE | GK_NAN_TO_NUM)) return fail(GK_ERR_ARG, "gk_wl_level_sum_fetch: unknown flags");
   GK_CUDA(cudaSetDevice(h->dev));
   const int64_t rows = h->wl_sum_rows, cols = h->wl_sum_cols;
@@ -4212,6 +4237,80 @@ int gk_wl_level_sum_fetch(gk_handle* h, int32_t flags, const double* xdiag, cons
     LAUNCH_CHECK(h);
   }
   if (K_out && rows > 0) GK_CUDA(cudaMemcpyAsync(K_out, K, (size_t)rows * cols * 8, cudaMemcpyDeviceToHost, h->stream));
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------
+// CoreFramework over a base kernel whose core levels cannot share one feature block (NeighborhoodHash, OddSth,
+// WeisfeilerLehmanOptimalAssignment, SubgraphMatching).  The reference fits one base kernel per core level and adds
+// its K into the rows and columns of the graphs that have that level's subgraph, K[idx_j, idx] += K_i[j, :], from the
+// largest core down (core_framework.py:177-223).  gk_core_sum_begin zeroes the sum (the wl_sum buffer of
+// gk_wl_level_sum), gk_core_level_add computes one level's un-normalised K on the device (wl_lvl) and scatters it into
+// the sum, and gk_wl_level_sum_fetch normalises and copies the sum out once.
+extern "C" {
+
+int gk_core_sum_begin(gk_handle* h, int64_t n_rows, int64_t n_cols, int32_t square) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (n_rows < 0 || n_cols <= 0 || n_rows > INT32_MAX || n_cols > INT32_MAX)
+    return fail(GK_ERR_ARG, "gk_core_sum_begin: bad shape");
+  if (square && n_rows != n_cols) return fail(GK_ERR_ARG, "gk_core_sum_begin: a square sum needs n_rows == n_cols");
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t elems = (size_t)n_rows * (size_t)n_cols;
+  GK_TRY(h->wl_sum.ensure(std::max<size_t>(elems, 1) * 8));
+  if (elems) GK_CUDA(cudaMemsetAsync(h->wl_sum.p, 0, elems * 8, h->stream));
+  h->wl_sum_rows = n_rows; h->wl_sum_cols = n_cols; h->wl_sum_row0 = 0; h->wl_sum_square = square != 0;
+  h->wl_sum_levels = 0;
+  h->core_sum = true;
+  h->core_level = INT32_MAX;
+  GK_CUDA(cudaStreamSynchronize(h->stream));
+  return GK_OK;
+}
+
+int gk_core_level_add(gk_handle* h, int32_t level, int64_t n_fit, int64_t n_level_rows, const int32_t* rows,
+                      const int32_t* cols, double* xdiag, double* ydiag, gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (!h->core_sum) return fail(GK_ERR_STATE, "gk_core_level_add: no sum begun (gk_core_sum_begin)");
+  if (!h->features_ready) return fail(GK_ERR_STATE, "gk_core_level_add: run the base kernel's feature pass first");
+  if (level < 0 || level >= h->core_level)
+    return fail(GK_ERR_ARG, "gk_core_level_add: core levels must be added in strictly descending order");
+  if (!GRAM_RULES[h->feature_kind].dev_out)
+    return fail(GK_ERR_UNSUPPORTED, std::string("gk_core_level_add: ") + GRAM_RULES[h->feature_kind].name +
+                                        " Gram has no device output");
+  GramReq q;
+  GK_TRY(gram_request(h, h->feature_kind, n_fit, 0, 0, -1, nullptr, GK_F64, 0, xdiag, ydiag, &q));
+  if (q.k_rows != n_level_rows) return fail(GK_ERR_ARG, "gk_core_level_add: the level's K has another number of rows");
+  if ((q.k_rows && !rows) || !cols) return fail(GK_ERR_ARG, "gk_core_level_add: null index map");
+  // every index in range and none twice: the scatter adds without atomics, one thread per element of the sum
+  std::vector<uint8_t> seen((size_t)std::max(h->wl_sum_rows, h->wl_sum_cols), 0);
+  for (int64_t j = 0; j < q.k_rows; ++j) {
+    if (rows[j] < 0 || rows[j] >= h->wl_sum_rows || seen[rows[j]]++)
+      return fail(GK_ERR_ARG, "gk_core_level_add: row map out of range or repeated");
+  }
+  std::fill(seen.begin(), seen.end(), 0);
+  for (int64_t c = 0; c < q.k_cols; ++c) {
+    if (cols[c] < 0 || cols[c] >= h->wl_sum_cols || seen[cols[c]]++)
+      return fail(GK_ERR_ARG, "gk_core_level_add: column map out of range or repeated");
+  }
+  GK_CUDA(cudaSetDevice(h->dev));
+  const size_t elems = (size_t)q.k_rows * q.k_cols;
+  GK_TRY(h->wl_lvl.ensure(std::max<size_t>(elems, 1) * 8));
+  GK_TRY(h->core_map.ensure((size_t)(q.k_rows + q.k_cols) * 4));
+  int* d_rows = h->core_map.as<int>();
+  int* d_cols = d_rows + q.k_rows;
+  if (q.k_rows) GK_CUDA(cudaMemcpyAsync(d_rows, rows, (size_t)q.k_rows * 4, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(d_cols, cols, (size_t)q.k_cols * 4, cudaMemcpyHostToDevice, h->stream));
+  q.flags |= GK_OUT_DEVICE; q.dev_out = true; q.K_out = h->wl_lvl.p; q.ld = q.k_cols;
+  GK_TRY(gram_route(h, q, stats));
+  if (elems) {
+    core_scatter_add_f64<<<(int)std::min<size_t>((elems + 255) / 256, (size_t)h->sm_count * 16), 256, 0, h->stream>>>(
+        q.k_rows, q.k_cols, h->wl_lvl.as<double>(), d_rows, d_cols, h->wl_sum.as<double>(), h->wl_sum_cols);
+    LAUNCH_CHECK(h);
+  }
+  h->core_level = level;
+  h->wl_sum_levels += 1;
   GK_CUDA(cudaStreamSynchronize(h->stream));
   return GK_OK;
 }
@@ -5388,20 +5487,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
   GramReq q;
   GK_TRY(gram_request(h, h->feature_kind, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, &q));
   GK_CUDA(cudaSetDevice(h->dev));
-  switch (h->feature_kind) {
-    case FK_SPATTR: return gram_spattr(h, q, stats);
-    case FK_GH: return h->gh_node_kernel == GK_GH_LINEAR ? gram_spattr(h, q, stats) : gram_gh_nodepair(h, q, stats);
-    case FK_NH: return gram_nh(h, q, stats);
-    case FK_PM: return gram_pm(h, q, stats);
-    case FK_NSPD: return gram_nspd(h, q, stats);
-    case FK_RW: return gram_rw(h, q, stats);
-    case FK_SM: return gram_sm(h, q, stats);
-    case FK_ODD: return gram_odd(h, q, stats);
-    case FK_ML: return gram_ml(h, q, stats);
-    case FK_SVMT: return gram_svmt(h, q, stats);
-    case FK_GS: return gram_gs(h, q, stats);
-    default: return gram_int(h, q, block_of(h), stats);
-  }
+  return gram_route(h, q, stats);
 }
 
 int gk_set_row_map(gk_handle* h, int64_t n_rows, const int32_t* row_of_graph) {

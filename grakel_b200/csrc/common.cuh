@@ -260,6 +260,11 @@ struct gk_handle {
   int64_t wl_sum_rows = 0, wl_sum_cols = 0, wl_sum_row0 = 0;
   int32_t wl_sum_levels = 0;
   bool wl_sum_square = false;
+  // CoreFramework reuses the sum (gk_core_sum_begin / gk_core_level_add): the sum is a core fold, the last core level
+  // added (levels go strictly downwards), the level's row and column maps
+  bool core_sum = false;
+  int32_t core_level = 0;
+  gk::DevBuf core_map;
 
   // ---- random walk (FK_RW): edge values of the packed CSR, its transpose, eigen-data, coefficients
   gk::DevBuf rw_val, rw_trp, rw_tci, rw_tval, rw_q, rw_w, rw_coef, rw_ws, rw_iters, rw_cap;

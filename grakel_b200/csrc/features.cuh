@@ -543,6 +543,19 @@ add_f64(long long n, const double* __restrict__ src, double* __restrict__ dst) {
     dst[i] = dst[i] + src[i];
 }
 
+// CoreFramework: sum[rows[j], cols[c]] += K[j, c] for one core level, the reference's K[idx_j, idx] += K_i[j, :].
+// The maps hold no index twice, so every element of the sum has one writer.
+__global__ void __launch_bounds__(256)
+core_scatter_add_f64(long long k_rows, long long k_cols, const double* __restrict__ K, const int* __restrict__ rows,
+                     const int* __restrict__ cols, double* __restrict__ sum, long long sum_ld) {
+  const long long n = k_rows * k_cols;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long j = i / k_cols, c = i - j * k_cols;
+    double* d = sum + (long long)rows[j] * sum_ld + cols[c];
+    *d = *d + K[i];
+  }
+}
+
 // out[i] = K[i ld + i]: the diagonal of a full square K
 __global__ void __launch_bounds__(256)
 diag_of_f64(long long n, const double* __restrict__ K, long long ld, double* __restrict__ out) {

@@ -6,7 +6,8 @@ the kernels of the device hot path:
     "vertex_histogram" / "subtree_wl" / "VH" / "ST-WL"
     "shortest_path" / "SP"      (+ with_labels, algorithm_type, as_attributes)
     "edge_histogram" / "EH"
-    "core_framework" / "CORE"   (framework; base "shortest_path" or "weisfeiler_lehman" ...)
+    "core_framework" / "CORE"   (framework; base "shortest_path", "weisfeiler_lehman", "vertex_histogram", "NH",
+                                 "ODD", "WL-OA", "SM" with ke=None)
     "hadamard_code" / "HC"      (framework; base "vertex_histogram", "shortest_path" or "edge_histogram")
     "weisfeiler_lehman_optimal_assignment" / "WL-OA"
     "graph_hopper" / "GH"

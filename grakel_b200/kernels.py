@@ -12,6 +12,7 @@ the level-0 label dictionary), so fitted estimators pickle like the reference's
 """
 from __future__ import annotations
 
+import contextlib
 import copy
 import math
 import functools
@@ -43,6 +44,32 @@ class Fitted:
 
     def __len__(self):
         return self.block.n_graphs
+
+
+class CoreLevel:
+    """One core level of a CoreFramework fold (core_framework.py): while it is set as a base kernel's `_core_level`,
+    the kernel's runs use the fold's engine, and a run that produces K adds it into the device-resident sum at `rows`
+    (its rows) and `cols` (its fitted columns) instead of returning it; the fold's seconds add up in times["fold"]."""
+
+    def __init__(self, eng, level, rows, cols, times):
+        self.eng, self.level, self.rows, self.cols, self.times = eng, level, rows, cols, times
+
+
+def _run_engine(est):
+    lvl = getattr(est, "_core_level", None)
+    return _lib.engine(getattr(est, "device_", None)) if lvl is None else contextlib.nullcontext(lvl.eng)
+
+
+def _gram_or_fold(est, eng, n_graphs, n_fit, want_matrix=True, want_diag=True, stats=None, **kw):
+    """eng.gram, or for a CoreFramework level the fold of its K (the base kernels run un-normalised there)."""
+    lvl = getattr(est, "_core_level", None)
+    if lvl is None or not want_matrix:
+        return eng.gram(n_graphs, n_fit=n_fit, out=None if want_matrix else False, want_diag=want_diag, stats=stats,
+                        **kw)
+    t = time.perf_counter()
+    xd, yd = eng.core_level_add(lvl.level, n_fit, lvl.rows, lvl.cols, n_graphs, want_diag=want_diag, stats=stats)
+    lvl.times["fold"] += time.perf_counter() - t
+    return None, xd, yd
 
 
 class Kernel(BaseEstimator, TransformerMixin):
@@ -212,12 +239,12 @@ class Kernel(BaseEstimator, TransformerMixin):
 
     def _run(self, block, ids, n_fit, want_matrix=True):
         """pack -> feature kernels -> Gram, all on the device.  Returns (K, xdiag, ydiag)."""
-        with _lib.engine(getattr(self, "device_", None)) as eng:
+        with _run_engine(self) as eng:
             eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, block.weights, block.attrs)
             self.stats_ = self._device_features(eng)
-            K, xd, yd = eng.gram(block.n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
-                                 nan_to_num=self._nan_to_num, out=None if want_matrix else False,
-                                 stats=self.stats_)
+            K, xd, yd = _gram_or_fold(self, eng, block.n_graphs, n_fit, want_matrix,
+                                      normalize=bool(self.normalize) and want_matrix, nan_to_num=self._nan_to_num,
+                                      stats=self.stats_)
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
@@ -888,7 +915,7 @@ class WeisfeilerLehmanOptimalAssignment(Kernel):
             if hasattr(self, "_X_diag"):
                 delattr(self, "_X_diag")
             if isinstance(X, Block):  # packed input (datasets.read_tu)
-                block = X.require("sp", "wloa")
+                block = X.require("sp", "wloa", "core")
             elif not isinstance(X, Iterable):
                 raise TypeError("input must be an iterable\n")
             else:
@@ -901,7 +928,7 @@ class WeisfeilerLehmanOptimalAssignment(Kernel):
         if self._method_calling != 3:
             raise ValueError("method call must be called either from fit or fit-transform")
         if isinstance(X, Block):
-            block = X.require("sp", "wloa")
+            block = X.require("sp", "wloa", "core")
         else:
             try:
                 block = pack(X, "wloa", len_ok=lambda n: n in (2, 3), type_error_msg=msg)  # :323
@@ -1446,7 +1473,10 @@ class NeighborhoodHash(Kernel):
 
     def parse_input(self, X):
         fit = self._method_calling in (1, 2)
-        if isinstance(X, Block):
+        if isinstance(X, Block) and X.mode == "core":  # a CoreFramework level: every vertex, neighbours in order
+            block, gp = X, X.graph_ptr
+            values = [X.labels[gp[g]:gp[g + 1]] for g in range(X.n_graphs)]
+        elif isinstance(X, Block):
             block, values = self._from_packed(X)
         else:
             els = self._elements(X)
@@ -1474,7 +1504,7 @@ class NeighborhoodHash(Kernel):
         ids, dictionary = label_ids(block.labels, None, sort_new=False)
         hd = self._labels_hash_dict
         fitted = Fitted(block, ids, dictionary)
-        fitted.order_known = not isinstance(X, Block)
+        fitted.order_known = not isinstance(X, Block) or X.mode == "core"
         fitted.codes = np.array([hd.get(l, 0) for l in dictionary], dtype=np.uint64)
         fitted.valid = np.array([l in hd for l in dictionary], dtype=np.uint8)
         return fitted
@@ -1521,7 +1551,7 @@ class NeighborhoodHash(Kernel):
     def _nh_run(self, block, ids, codes, valid, n_fit, order_known=True):
         """pack -> gk_nh_features (R hash levels, per-level columns) -> gk_gram (per-level Grams, fp64 combine).
         `order_known`: the block's rows list every vertex's neighbours in the reference's edge-dictionary order."""
-        with _lib.engine(getattr(self, "device_", None)) as eng:
+        with _run_engine(self) as eng:
             eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
             self.stats_ = eng.nh_features(self.R, self._nh_code, self.bits, codes, valid)
             if self.stats_.nh_order_dependent and not order_known:
@@ -1529,7 +1559,7 @@ class NeighborhoodHash(Kernel):
                     "NeighborhoodHash(nh_type='count_sensitive'): a vertex has two different neighbour codes with equal "
                     "low bits, so its code depends on the neighbour order of the reference's edge sets, which a packed "
                     "block does not carry; pass the list of graphs instead")
-            K, _, _ = eng.gram(block.n_graphs, n_fit=n_fit, stats=self.stats_, want_diag=False)
+            K, _, _ = _gram_or_fold(self, eng, block.n_graphs, n_fit, stats=self.stats_, want_diag=False)
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K
@@ -3264,7 +3294,7 @@ class SubgraphMatching(Kernel):
     def _block(self, X, edge_labels):
         """The graphs of a datasets.read_tu block (the nodes that occur in an edge, as in its edge dictionaries),
         with the block's per-edge label ids `edge_labels` (read_tu's `edge_labels`) when ke is not None."""
-        X.require("sp", labels=self.kv is not None)
+        X.require("sp", "core", labels=self.kv is not None)
         if self.ke is not None and edge_labels is None:
             raise ValueError("Graph does not have any labels for edges.")
         gp, rp, ci = X.graph_ptr, X.row_ptr, X.col_idx
@@ -3399,12 +3429,12 @@ class SubgraphMatching(Kernel):
 
     def _sm_run(self, graphs, n_fit, want_matrix=True, device_ptr=None, row_range=None):
         gp, rp, ci, ids, elids, vt, et, flags = self._pack(graphs)
-        with _lib.engine(getattr(self, "device_", None)) as eng:
+        with _run_engine(self) as eng:
             eng.pack(gp, rp, ci, ids, None, None)
             self.stats_ = eng.sm_features(int(self.k), self.lambdas_, vt, et, elids, flags)
-            K, xd, yd = eng.gram(len(graphs), n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
-                                 out=None if want_matrix else False, device_ptr=device_ptr, row_range=row_range,
-                                 stats=self.stats_)
+            K, xd, yd = _gram_or_fold(self, eng, len(graphs), n_fit, want_matrix,
+                                      normalize=bool(self.normalize) and want_matrix, device_ptr=device_ptr,
+                                      row_range=row_range, stats=self.stats_)
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
@@ -3491,6 +3521,8 @@ class OddSth(Kernel):
 
     def parse_input(self, X):
         """odd_sth.py:74-127: the element checks, then the graphs packed with the edge dictionary's neighbour order."""
+        if isinstance(X, Block) and X.mode == "core":  # a CoreFramework level: neighbours in the edge dictionary's order
+            return self._fitted(X)
         if isinstance(X, Block):
             raise NotImplementedError("OddSth: a datasets.read_tu block does not carry the neighbour order of the "
                                       "reference's edge sets, which the result depends on; pass the list of graphs")
@@ -3514,8 +3546,11 @@ class OddSth(Kernel):
             els.append([x[0], x[1]])
         if not els:
             raise ValueError("parsed input is empty")
-        block = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
-                     keep_edge_order=True)
+        return self._fitted(pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
+                                 keep_edge_order=True))
+
+    @staticmethod
+    def _fitted(block):
         ids, rank, strings = odd_label_tables(block.labels, block.graph_ptr)
         out = Fitted(block, ids, strings)
         out.rank = rank
@@ -3557,12 +3592,12 @@ class OddSth(Kernel):
 
     def _odd_run(self, block, ids, rank, n_fit, want_matrix=True, device_ptr=None, row_range=None):
         """pack -> gk_odd_features (DAGs, identities, bit-plane tables) -> gk_gram (gram_path 14)."""
-        with _lib.engine(getattr(self, "device_", None)) as eng:
+        with _run_engine(self) as eng:
             eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
             self.stats_ = eng.odd_features(self.h_, rank)
-            K, xd, yd = eng.gram(block.n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
-                                 out=None if want_matrix else False, device_ptr=device_ptr, row_range=row_range,
-                                 stats=self.stats_)
+            K, xd, yd = _gram_or_fold(self, eng, block.n_graphs, n_fit, want_matrix,
+                                      normalize=bool(self.normalize) and want_matrix, device_ptr=device_ptr,
+                                      row_range=row_range, stats=self.stats_)
             if getattr(self, "_keep_signatures", False):  # tests: the identities' signatures
                 self.signatures_ = eng.odd_signatures()
         if self.verbose:

@@ -243,6 +243,20 @@ int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begi
 int gk_wl_level_sum_fetch(gk_handle* h, int32_t flags, const double* xdiag, const double* ydiag, double* K_out,
                           double* kdiag);
 
+/* CoreFramework over a base kernel whose core levels cannot share one feature block: the reference's
+ * K[idx_j, idx] += K_i[j, :] for every core level i from the largest down (core_framework.py:177-223), on the device.
+ * gk_core_sum_begin sizes the sum of gk_wl_level_sum (n_rows x n_cols fp64, row-major) and sets it to zero; `square`
+ * marks a fit_transform sum, whose own diagonal gk_wl_level_sum_fetch may then read.  For each level: pack the level's
+ * graphs, run the base kernel's feature pass, then gk_core_level_add computes the level's un-normalised K (the packed
+ * feature kind's gram path, n_fit as in gk_gram, all rows; xdiag / ydiag as in gk_gram, may be NULL) into a
+ * handle-owned buffer and adds it into the sum, sum[rows[j], cols[c]] += K_level[j, c], rows[n_level_rows] and
+ * cols[n_fit] being distinct indices of the sum.  Levels must come in strictly descending order.  Every argument is
+ * checked before the first launch.  No re-pack or feature pass touches the sum; gk_wl_level_sum_fetch then normalises
+ * and copies it out once. */
+int gk_core_sum_begin(gk_handle* h, int64_t n_rows, int64_t n_cols, int32_t square);
+int gk_core_level_add(gk_handle* h, int32_t level, int64_t n_fit, int64_t n_level_rows, const int32_t* rows,
+                      const int32_t* cols, double* xdiag, double* ydiag, gk_stats* stats);
+
 /* RandomWalk / RandomWalkLabeled (random_walk.py:28-541), one graph pair per CTA in fp64.  The packed CSR gives the
  * structure (gk_pack_csr without weights; with labels for GK_RW_LABELED), `values[E]` the adjacency entries of its
  * edges (any sign, self-loops included), `t_row_ptr[V+1]` / `t_col_idx[E]` / `t_values[E]` the same block transposed

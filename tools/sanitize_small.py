@@ -58,3 +58,13 @@ for base in ((NeighborhoodSubgraphPairwiseDistance, {"r": 1, "d": 2}), (OddSth, 
     Kb = wlb.fit_transform(Xe[:30])
     Kt = wlb.transform(Xe[30:])
     print("WL over", base[0].__name__, Kb.shape, float(Kb.sum()), Kt.shape)
+# CoreFramework over the fold bases (per-level Grams scattered into a device-resident sum), fit_transform and a
+# normalised transform
+from grakel_b200 import (CoreFramework, NeighborhoodHash, SubgraphMatching,  # noqa: E402
+                         WeisfeilerLehmanOptimalAssignment)
+for base in ((NeighborhoodHash, {"random_state": 0}), (OddSth, {}), (WeisfeilerLehmanOptimalAssignment, {}),
+             (SubgraphMatching, {"k": 3, "ke": None})):
+    cf = CoreFramework(normalize=base[0] is not OddSth, base_graph_kernel=base)
+    Kc = cf.fit_transform(Xe[:30])
+    Kt = cf.transform(Xe[30:])
+    print("CORE over", base[0].__name__, Kc.shape, float(Kc.sum()), Kt.shape)
