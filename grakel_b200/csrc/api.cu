@@ -3067,6 +3067,7 @@ int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double*
   const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
   if (kk > SM_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: subgraphs of more than 32 vertices");
   GK_CUDA(cudaSetDevice(h->dev));
+  h->sm_n_lv = 0;
   HandleExtra* ex = extra_of(h);
   const int64_t N = h->N;
   const bool elab = ke != SM_W_NONE;
@@ -3123,15 +3124,19 @@ static int sm_launch(gk_handle* h, SmParams p) {
   p.stack_cap = cap;
   const size_t tab_bytes = ((p.kv == SM_W_TABLE ? (size_t)p.n_vl * p.n_vl : 0) +
                             (p.ke == SM_W_TABLE ? (size_t)p.n_el * p.n_el : 0)) * 8;
+  // sm_wl_pairs' (depth, size) bins: per warp when exact, per lane when real
+  const size_t bin_bytes = p.n_lv == 0 ? 0 : (size_t)p.n_lv * p.kk * 8 * (p.exact ? 2 * SM_WARPS : SM_THREADS);
   const long long pair_words = 2 * sm_record_words(nmax, p.ke != SM_W_NONE);
   // GRAKEL_B200_SM_GLOBAL=1 reads every record from global memory (the route of pairs too large to stage)
   const char* e_glob = getenv("GRAKEL_B200_SM_GLOBAL");
-  const bool staged = !(e_glob && atoi(e_glob) != 0) && tab_bytes + SM_WARPS * pair_words * 4 <= 96 * 1024;
+  const bool staged =
+      !(e_glob && atoi(e_glob) != 0) && tab_bytes + bin_bytes + SM_WARPS * pair_words * 4 <= 96 * 1024;
   p.stage_words = staged ? (int)pair_words : 0;
-  const size_t smem = tab_bytes + (size_t)SM_WARPS * p.stage_words * 4;
-  GK_CUDA(cudaFuncSetAttribute(sm_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
+  const size_t smem = tab_bytes + bin_bytes + (size_t)SM_WARPS * p.stage_words * 4;
+  const void* kern = p.n_lv > 0 ? (const void*)sm_wl_pairs : (const void*)sm_pairs;
+  GK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
   int per_sm = 0;
-  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sm_pairs, SM_THREADS, smem));
+  GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SM_THREADS, smem));
   long long grid = (long long)h->sm_count * std::max(per_sm, 1);
   // at most 1 GiB of stacks: fewer CTAs (down to one) when a lane's stack is large
   const long long per_cta = (long long)SM_WARPS * 32 * cap * 4;
@@ -3141,7 +3146,10 @@ static int sm_launch(gk_handle* h, SmParams p) {
   p.stack = h->sm_stack.as<unsigned>();
   GK_CUDA(cudaMemsetAsync(h->sm_ctl.p, 0, 8, h->stream));
   p.next = h->sm_ctl.as<unsigned long long>();
-  sm_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
+  if (p.n_lv > 0)
+    sm_wl_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
+  else
+    sm_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
   LAUNCH_CHECK(h);
   return GK_OK;
 }
@@ -3158,6 +3166,7 @@ static SmParams sm_params(gk_handle* h) {
   p.lam = h->sm_lam.as<double>();
   p.exact = h->sm_exact ? 1 : 0;
   p.err = reinterpret_cast<unsigned*>(h->sm_ctl.as<unsigned char>() + 8);
+  p.wl_cls = h->sm_wl_cls.as<int>(); p.n_lv = h->sm_n_lv;
   return p;
 }
 
@@ -3216,14 +3225,14 @@ static int gram_sm(gk_handle* h, const GramReq& q, gk_stats* stats) {
   return GK_OK;
 }
 
-int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
-  if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_counts: null argument");
-  if (h->feature_kind != FK_SM || !h->features_ready) return fail(GK_ERR_STATE, "gk_sm_counts: call gk_sm_features first");
-  if (n_fit <= 0 || n_fit > h->N) return fail(GK_ERR_ARG, "gk_sm_counts: n_fit out of range");
+// tv of every level of the n_fit pairs of row `row`: out[n_fit][n_lv][k + 1] (gk_sm_wl_features' levels) or
+// out[n_fit][k + 1]
+static int sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out, const char* what) {
+  if (n_fit <= 0 || n_fit > h->N) return fail(GK_ERR_ARG, std::string(what) + ": n_fit out of range");
   const bool square = n_fit == h->N;
-  if (row < 0 || row >= (square ? h->N : h->N - n_fit)) return fail(GK_ERR_ARG, "gk_sm_counts: row out of range");
+  if (row < 0 || row >= (square ? h->N : h->N - n_fit)) return fail(GK_ERR_ARG, std::string(what) + ": row out of range");
   GK_CUDA(cudaSetDevice(h->dev));
-  const size_t bytes = (size_t)n_fit * (h->sm_k + 1) * 8;
+  const size_t bytes = (size_t)n_fit * std::max(h->sm_n_lv, 1) * (h->sm_k + 1) * 8;
   GK_TRY(h->K_stage.ensure(bytes));
   GK_CUDA(cudaMemsetAsync(h->sm_ctl.as<unsigned char>() + 8, 0, 8, h->stream));
   SmParams p = sm_params(h);
@@ -3238,6 +3247,48 @@ int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
   GK_CUDA(cudaMemcpyAsync(out, h->K_stage.p, bytes, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
   return GK_OK;
+}
+
+int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_counts: null argument");
+  if (h->feature_kind != FK_SM || !h->features_ready || h->sm_n_lv != 0)
+    return fail(GK_ERR_STATE, "gk_sm_counts: call gk_sm_features first");
+  return sm_counts(h, n_fit, row, out, "gk_sm_counts");
+}
+
+
+// WeisfeilerLehman over SubgraphMatching (sm_wl_pairs): gk_sm_features' records, tables and lambdas, and the WL class
+// of every packed vertex at every level; gk_gram then returns the level sum of the per-level SubgraphMatching Grams
+int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
+                      const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                      gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sm_wl_features: no graphs packed");
+  if (n_iter < 1) return fail(GK_ERR_ARG, "gk_sm_wl_features: n_iter < 1");
+  if (!(flags & (GK_SM_KV_NONE | GK_SM_KV_DIRAC)))
+    return fail(GK_ERR_UNSUPPORTED, "gk_sm_wl_features: the vertex kernel must be GK_SM_KV_DIRAC or GK_SM_KV_NONE");
+  const bool all_levels = (flags & GK_SM_KV_NONE) != 0;
+  if (!all_levels && !level_ids) return fail(GK_ERR_ARG, "gk_sm_wl_features: no level ids");
+  const int n_lv = n_iter + 1;
+  const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
+  if ((int64_t)n_lv * kk > SM_WL_BINS)
+    return fail(GK_ERR_UNSUPPORTED, "gk_sm_wl_features: (n_iter + 1) * min(k, largest graph) is more than 64");
+  GK_TRY(gk_sm_features(h, k, lambdas, nullptr, 0, etable, n_elabels, edge_label, flags, stats));
+  const size_t bytes = (size_t)h->V * n_lv * 4;
+  GK_TRY(h->sm_wl_cls.ensure(std::max<size_t>(bytes, 4)));
+  if (!all_levels && bytes > 0) {
+    GK_CUDA(cudaMemcpyAsync(h->sm_wl_cls.p, level_ids, bytes, cudaMemcpyHostToDevice, h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffer may be reused once we return
+  }
+  h->sm_n_lv = n_lv;
+  return GK_OK;
+}
+
+int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
+  if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_wl_counts: null argument");
+  if (h->feature_kind != FK_SM || !h->features_ready || h->sm_n_lv == 0)
+    return fail(GK_ERR_STATE, "gk_sm_wl_counts: call gk_sm_wl_features first");
+  return sm_counts(h, n_fit, row, out, "gk_sm_wl_counts");
 }
 
 // ---------------------------------------------------------------------------

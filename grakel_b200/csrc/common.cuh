@@ -278,6 +278,8 @@ struct gk_handle {
   gk::DevBuf sm_rec, sm_off, sm_el, sm_vtab, sm_etab, sm_lam, sm_stack, sm_ctl;
   int sm_k = 0, sm_kk = 1, sm_kv = 0, sm_ke = 0, sm_n_vl = 0, sm_n_el = 0;
   int sm_max_und = 0;  // largest number of distinct out- or in-neighbours of a packed vertex
+  gk::DevBuf sm_wl_cls;  // gk_sm_wl_features: sm_n_lv WL class ids per packed vertex (0 levels: plain SubgraphMatching)
+  int sm_n_lv = 0;
   bool sm_exact = true;
 
   // ---- OddSth (FK_ODD): graph offsets and label ranks, node records [S] (hash | label | graph | first child | child

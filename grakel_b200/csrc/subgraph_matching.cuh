@@ -30,6 +30,7 @@ constexpr int SM_THREADS = 256;
 constexpr int SM_WARPS = SM_THREADS / 32;
 constexpr int SM_KMAX = 32;            // largest clique size enumerated
 constexpr int SM_TAB_MAX = 4096;       // entries of one weight table (64 x 64 labels)
+constexpr int SM_WL_BINS = 64;         // sm_wl_pairs: (n_iter + 1) x sizes enumerated, at most
 enum { SM_W_TABLE = 0, SM_W_NONE = 1, SM_W_DIRAC = 2 };
 
 // Per-graph record (32-bit words) of n vertices, W = ceil(n / 32):
@@ -60,6 +61,9 @@ struct SmParams {
   int stage_words;            // shared-memory words per warp for the two records (0: read them from global memory)
   unsigned long long* next;   // pair counter
   unsigned* err;              // bit 1: exact sum reached 2^53, bit 2: stack overflow
+  // sm_wl_pairs only: n_lv (WL levels 0 .. n_iter) class ids per packed vertex, vertex-major; tv_out then holds
+  // n_lv x n_tv values per pair
+  const int* wl_cls; int n_lv;
 };
 
 struct SmGraph {
@@ -103,18 +107,13 @@ __device__ __forceinline__ double sm_ce(const SmParams& P, const SmGraph& X, con
   return etab[la * P.n_el + lb];
 }
 
-// tv of the pair (x, y) for this lane's roots: exact sums in cnt / cabs, real sums in sum
-__device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph& Y, const double* vtab,
-                             const double* etab, unsigned* stk, long long* cnt, unsigned long long* cabs,
-                             double* sum) {
-  const int lane = threadIdx.x & 31;
-  const int ny = Y.n, nv = X.n * Y.n, kk = P.kk;
-  const long long cap = P.stack_cap;
-  int Sa[SM_KMAX], Sb[SM_KMAX];
-  double term[SM_KMAX];
-  long long f_start[SM_KMAX + 1];
-  int f_len[SM_KMAX + 1], f_pos[SM_KMAX + 1];
-  auto add = [&](int s, double t) {
+// One lane's per-size sums of sm_pairs: exact sums in cnt / cabs, real sums in sum
+struct SmLaneAcc {
+  static constexpr bool wl = false;
+  long long* cnt;
+  unsigned long long* cabs;
+  double* sum;
+  __device__ __forceinline__ void add(const SmParams& P, int s, double t) const {
     if (P.exact) {
       const double at = fabs(t);
       if (at >= 0x1p53) atomicOr(P.err, 1u);
@@ -123,7 +122,54 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
     } else {
       sum[s] += t;
     }
-  };
+  }
+};
+
+// The (depth, size) bins of sm_wl_pairs.  A product vertex (a, b) has depth D(a, b), the largest WL level h with
+// c_h(a) == c_h(b) (WL refines its partition, so the levels 0 .. D all agree); a clique counts at the levels 0 .. the
+// least depth of its vertices.  Exact sums go to the warp's bins in shared memory ([depth][size] signed sums, then
+// [depth][size] absolute sums, 64-bit shared atomics: integer addition, so the order does not matter); real sums go to
+// the lane's own bins ([level][size], stride SM_THREADS), added at every level 0 .. depth in the enumeration order, so
+// each level's lane sum is the one the per-level enumeration forms.
+struct SmWlAcc {
+  static constexpr bool wl = true;
+  const int *cx, *cy;         // n_lv class ids per vertex of x and of y
+  int n_lv, kk;
+  bool all_levels;            // kv = None: every product vertex exists at every level
+  unsigned long long* wbin;   // exact: this warp's bins
+  double* lbin;               // real: this lane's bins
+  __device__ __forceinline__ int depth(int a, int b) const {
+    if (all_levels) return n_lv - 1;
+    const int* p = cx + (size_t)a * n_lv;
+    const int* q = cy + (size_t)b * n_lv;
+    int d = 0;
+    while (d + 1 < n_lv && p[d + 1] == q[d + 1]) ++d;
+    return d;
+  }
+  __device__ __forceinline__ void add(const SmParams& P, int s, double t, int d) const {
+    if (P.exact) {
+      const double at = fabs(t);
+      if (at >= 0x1p53) atomicOr(P.err, 1u);
+      atomicAdd(&wbin[d * kk + s], (unsigned long long)(long long)t);
+      atomicAdd(&wbin[(n_lv + d) * kk + s], (unsigned long long)at);
+    } else {
+      for (int h = 0; h <= d; ++h) lbin[(size_t)(h * kk + s) * SM_THREADS] += t;
+    }
+  }
+};
+
+// tv of the pair (x, y) for this lane's roots, into `acc`
+template <class Acc>
+__device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph& Y, const double* vtab,
+                             const double* etab, unsigned* stk, const Acc& acc) {
+  const int lane = threadIdx.x & 31;
+  const int ny = Y.n, nv = X.n * Y.n, kk = P.kk;
+  const long long cap = P.stack_cap;
+  int Sa[SM_KMAX], Sb[SM_KMAX];
+  double term[SM_KMAX];
+  long long f_start[SM_KMAX + 1];
+  int f_len[SM_KMAX + 1], f_pos[SM_KMAX + 1];
+  unsigned char md[Acc::wl ? SM_KMAX : 1];  // least depth of S's first i + 1 vertices (sm_wl_pairs)
   auto push = [&](long long& top, unsigned u) {
     if (top >= cap) { atomicOr(P.err, 2u); return; }
     stk[(size_t)top * 32] = u;
@@ -133,7 +179,12 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
     const int va = v / ny, vb = v - va * ny;
     const double c0 = sm_cv(P, X, Y, vtab, va, vb);
     if (c0 == 0.0) continue;
-    add(0, c0);
+    if constexpr (Acc::wl) {
+      md[0] = (unsigned char)acc.depth(va, vb);
+      acc.add(P, 0, c0, md[0]);
+    } else {
+      acc.add(P, 0, c0);
+    }
     if (kk < 2) continue;
     Sa[0] = va; Sb[0] = vb; term[0] = c0;
     // extension set of {v}: its c-neighbours with a larger id
@@ -165,7 +216,13 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
       const int wa = (int)(w / (unsigned)ny), wb = (int)(w - (unsigned)wa * ny);
       double t = term[depth - 1] * sm_cv(P, X, Y, vtab, wa, wb);
       for (int i = 0; i < depth; ++i) t *= fabs(sm_ce(P, X, Y, etab, wa, wb, Sa[i], Sb[i]));
-      add(depth, t);
+      if constexpr (Acc::wl) {
+        const int dw = min((int)md[depth - 1], acc.depth(wa, wb));
+        acc.add(P, depth, t, dw);
+        md[depth] = (unsigned char)dw;
+      } else {
+        acc.add(P, depth, t);
+      }
       if (depth + 1 >= kk) continue;
       // the child's extension set, above this frame
       top = fs + fl;
@@ -238,7 +295,7 @@ __global__ void __launch_bounds__(SM_THREADS, 1) sm_pairs(SmParams P) {
     }
     const SmGraph X = sm_graph(ax, nx, elab), Y = sm_graph(ay, ny, elab);
     for (int s = 0; s < P.kk; ++s) { cnt[s] = 0; cabs[s] = 0; sum[s] = 0.0; }
-    sm_lane_pair(P, X, Y, vtab, etab, stk, cnt, cabs, sum);
+    sm_lane_pair(P, X, Y, vtab, etab, stk, SmLaneAcc{cnt, cabs, sum});
     // tv over the warp (fixed shuffle order), then the lambda fold on lane 0
     double acc = 0.0;
     for (int s = 0; s < P.n_tv; ++s) {
@@ -270,6 +327,99 @@ __global__ void __launch_bounds__(SM_THREADS, 1) sm_pairs(SmParams P) {
       }
     }
     __syncwarp();  // the next pair overwrites the staged records
+  }
+}
+
+// WeisfeilerLehman over SubgraphMatching in one enumeration (DESIGN 4.23).  With kv = _dirac the level-h product graph
+// is the level-0 one induced on the vertices of depth >= h, and ESU's extension sets at level h are the level-0 ones
+// restricted to them, in the same order; so a clique's term is the same at every level that has it, and every
+// level's lane sums see the terms in the order the per-level enumeration does.  Per pair: the (depth, size) bins,
+// then in the epilogue each level's tv (suffix sums over the depths), its fma lambda fold, and the level sum
+// ((K_0 + K_1) + K_2) ... -- no per-level matrix exists.  Dynamic shared memory: the weight tables, the bins
+// (exact: SM_WARPS x 2 n_lv kk words, real: SM_THREADS x n_lv kk doubles), then the staged records as in sm_pairs.
+__global__ void __launch_bounds__(SM_THREADS, 1) sm_wl_pairs(SmParams P) {
+  extern __shared__ __align__(16) unsigned char sm_smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool elab = P.ke != SM_W_NONE;
+  double* vtab = reinterpret_cast<double*>(sm_smem);
+  const int nvt = P.kv == SM_W_TABLE ? P.n_vl * P.n_vl : 0;
+  const int net = P.ke == SM_W_TABLE ? P.n_el * P.n_el : 0;
+  double* etab = vtab + nvt;
+  for (int i = threadIdx.x; i < nvt; i += SM_THREADS) vtab[i] = P.vtab[i];
+  for (int i = threadIdx.x; i < net; i += SM_THREADS) etab[i] = P.etab[i];
+  const int n_lv = P.n_lv, kk = P.kk, nb = n_lv * kk;
+  unsigned long long* bins = reinterpret_cast<unsigned long long*>(etab + net);
+  const int bin_words = P.exact ? SM_WARPS * 2 * nb : SM_THREADS * nb;
+  for (int i = threadIdx.x; i < bin_words; i += SM_THREADS) bins[i] = 0ull;
+  __syncthreads();
+  unsigned long long* wbin = bins + (size_t)warp * 2 * nb;
+  double* lbin = reinterpret_cast<double*>(bins) + threadIdx.x;
+  unsigned* stage = reinterpret_cast<unsigned*>(bins + bin_words) + (size_t)warp * P.stage_words;
+  const size_t gwarp = (size_t)blockIdx.x * SM_WARPS + warp;
+  unsigned* stk = P.stack + gwarp * 32 * (size_t)P.stack_cap + lane;
+  for (;;) {
+    long long pi = 0;
+    if (lane == 0) pi = (long long)atomicAdd(P.next, 1ull);
+    pi = __shfl_sync(0xffffffffu, pi, 0);
+    if (pi >= P.n_pairs) break;
+    int r, c, gi, gj;
+    rw_pair_of(P.pairs, P.cols, P.row_g0, P.ordered, pi, r, c, gi, gj);
+    const int x0 = P.graph_ptr[gi], y0 = P.graph_ptr[gj];
+    const int nx = P.graph_ptr[gi + 1] - x0, ny = P.graph_ptr[gj + 1] - y0;
+    const long long rx = sm_record_words(nx, elab), ry = sm_record_words(ny, elab);
+    const unsigned* ax = P.rec + P.rec_off[gi];
+    const unsigned* ay = P.rec + P.rec_off[gj];
+    if (rx + ry <= P.stage_words) {
+      for (long long i = lane; i < rx; i += 32) stage[i] = ax[i];
+      for (long long i = lane; i < ry; i += 32) stage[rx + i] = ay[i];
+      __syncwarp();
+      ax = stage; ay = stage + rx;
+    }
+    const SmGraph X = sm_graph(ax, nx, elab), Y = sm_graph(ay, ny, elab);
+    const SmWlAcc acc{P.wl_cls + (size_t)x0 * n_lv, P.wl_cls + (size_t)y0 * n_lv, n_lv, kk, P.kv == SM_W_NONE,
+                      wbin, lbin};
+    sm_lane_pair(P, X, Y, vtab, etab, stk, acc);
+    __syncwarp();
+    // level h's tv[s] sums the bins of depth >= h; K = ((K_0 + K_1) + K_2) ..., K_h the fma fold of lambdas x tv_h
+    double total = 0.0;
+    for (int h = 0; h < n_lv; ++h) {
+      double kh = 0.0;
+      for (int s = 0; s < P.n_tv; ++s) {
+        double tv = 0.0;
+        if (s < kk) {
+          if (P.exact) {
+            long long a = 0;
+            unsigned long long b = 0;
+            for (int d = h; d < n_lv; ++d) {
+              a += (long long)wbin[d * kk + s];
+              b += wbin[(n_lv + d) * kk + s];
+            }
+            if (lane == 0 && b >= (1ull << 53)) atomicOr(P.err, 1u);
+            tv = (double)a;
+          } else {
+            tv = rw_warp_sum(lbin[(size_t)(h * kk + s) * SM_THREADS]);
+          }
+        }
+        kh = __fma_rn(P.lam[s], tv, kh);
+        if (lane == 0 && P.tv_out) P.tv_out[((size_t)pi * n_lv + h) * P.n_tv + s] = tv;
+      }
+      total = h == 0 ? kh : total + kh;
+    }
+    if (lane == 0 && P.out) {
+      if (P.pairs == RW_PAIRS_DIAG) {
+        P.out[r] = total;
+      } else {
+        P.out[(size_t)r * P.ld + c] = total;
+        if (P.pairs == RW_PAIRS_TRIANGLE && c != r) P.out[(size_t)c * P.ld + r] = total;
+      }
+    }
+    __syncwarp();  // every lane has read the bins; the next pair overwrites them and the staged records
+    if (P.exact) {
+      for (int i = lane; i < 2 * nb; i += 32) wbin[i] = 0ull;
+    } else {
+      for (int i = 0; i < nb; ++i) lbin[(size_t)i * SM_THREADS] = 0.0;
+    }
+    __syncwarp();
   }
 }
 

@@ -2,7 +2,7 @@
 the kernels of the device hot path:
 
     "weisfeiler_lehman" / "WL"  (framework; base "vertex_histogram"/"subtree_wl"/"VH"/"ST-WL", "shortest_path",
-                                 "edge_histogram", "pyramid_match", "NSPD", "ODD")
+                                 "edge_histogram", "pyramid_match", "NSPD", "ODD", "SM")
     "vertex_histogram" / "subtree_wl" / "VH" / "ST-WL"
     "shortest_path" / "SP"      (+ with_labels, algorithm_type, as_attributes)
     "edge_histogram" / "EH"

@@ -456,11 +456,14 @@ class WeisfeilerLehman(Kernel):
     K = sum over levels 0..n_iter of the base kernel on the level's compressed
     labels.  The base kernels that run on the device: VertexHistogram (the
     subtree kernel, the reference default), EdgeHistogram, ShortestPath,
-    PyramidMatch, NeighborhoodSubgraphPairwiseDistance and OddSth.  Over the
-    last two every level's labels are numbered the reference's way on the host
-    (they read label numbers, not only the partition); OddSth's levels share
-    one DAG pass and one exact Gram, NSPD's levels are folded one by one into a
-    device-resident sum added in level order (DESIGN 4.21)."""
+    PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth and
+    SubgraphMatching.  Over NSPD and OddSth every level's labels are numbered
+    the reference's way on the host (they read label numbers, not only the
+    partition); OddSth's levels share one DAG pass and one exact Gram, NSPD's
+    levels are folded one by one into a device-resident sum added in level
+    order (DESIGN 4.21).  SubgraphMatching (kv `_dirac` or None) needs only the
+    device partition: one clique enumeration gives every level's counts
+    (DESIGN 4.23)."""
 
     _graph_format = "dictionary"
     _nan_to_num = True
@@ -492,15 +495,22 @@ class WeisfeilerLehman(Kernel):
                                      "parameters names and values")
                 params.pop("normalize", None)
             if base not in (VertexHistogram, EdgeHistogram, ShortestPath, PyramidMatch,
-                            NeighborhoodSubgraphPairwiseDistance, OddSth):
+                            NeighborhoodSubgraphPairwiseDistance, OddSth, SubgraphMatching):
                 raise NotImplementedError("grakel_b200 runs WeisfeilerLehman over VertexHistogram (the subtree kernel), "
                                           "EdgeHistogram, ShortestPath, PyramidMatch, "
-                                          "NeighborhoodSubgraphPairwiseDistance or OddSth; other base kernels are "
-                                          "outside the device hot path")
+                                          "NeighborhoodSubgraphPairwiseDistance, OddSth or SubgraphMatching; other "
+                                          "base kernels are outside the device hot path")
             if base is NeighborhoodSubgraphPairwiseDistance:  # the base kernel's own checks
                 NeighborhoodSubgraphPairwiseDistance(**{k: v for k, v in params.items() if k in ("r", "d")}).initialize()
             if base is OddSth:
                 OddSth(h=params.get("h")).initialize()
+            if base is SubgraphMatching:  # the base kernel's own checks (subgraph_matching.py:70-120)
+                sm = SubgraphMatching(**{k: v for k, v in params.items() if k in ("k", "kv", "ke", "lw")})
+                sm.initialize()
+                if sm.kv is not None and sm.kv is not _dirac:
+                    raise NotImplementedError("WeisfeilerLehman over SubgraphMatching runs kv=_dirac or kv=None: a "
+                                              "custom vertex kernel reads the reference's label numbers per level")
+                self._sm = sm
             if base is PyramidMatch:  # the base kernel's own checks (pyramid_match.py:62-81)
                 PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
             if base is ShortestPath:
@@ -531,6 +541,9 @@ class WeisfeilerLehman(Kernel):
         if isinstance(X, Block):  # packed input (datasets.read_tu)
             if base is EdgeHistogram:
                 raise NotImplementedError("packed blocks carry no edge-label entries; pass the list of graphs")
+            if base is SubgraphMatching:
+                raise NotImplementedError("WeisfeilerLehman over SubgraphMatching needs every graph's edge dictionary "
+                                          "and edge labels; pass the list of graphs")
             return X.require("wl")
         if base is EdgeHistogram:
             if not isinstance(X, Iterable):
@@ -688,16 +701,17 @@ class WeisfeilerLehman(Kernel):
         return super().diagonal()
 
     def _base_data(self, X, block):
-        """NeighborhoodSubgraphPairwiseDistance / OddSth base: every element's graph as that base kernel packs it, and
-        `src`, the WL vertex of every base vertex (the base kernel sees the WL labels through the element's labels
-        dictionary, whose key order is the WL block's)."""
+        """NeighborhoodSubgraphPairwiseDistance / OddSth / SubgraphMatching base: every element's graph as that base
+        kernel packs it, and `src`, the WL vertex of every base vertex (the base kernel sees the WL labels through the
+        element's labels dictionary, whose key order is the WL block's)."""
         base = self._base_graph_kernel
         if base not in _WL_GRAPH_BASES or base is PyramidMatch:
             return None
         gp = np.asarray(block.graph_ptr, dtype=np.int64)
         src, graphs, els = [], [], []
         for x in X:
-            if isinstance(x, Graph):
+            from_graph = isinstance(x, Graph)
+            if from_graph:
                 x = x.as_element()
             x = list(x)
             if len(x) == 0:
@@ -707,6 +721,14 @@ class WeisfeilerLehman(Kernel):
                 if len(x) != 3:  # the element the reference hands on is (edges, labels) + edge labels
                     raise TypeError(_NSPD_ELEMENT_MSG)
                 n, edges, _, el, order = _nspd_graph(x[0], x[1], x[2], with_order=True)
+                graphs.append((n, edges, None, el))
+            elif base is SubgraphMatching:
+                # the reference hands on (edges, labels) + extras, extras starting with the edge labels when the
+                # element has them (weisfeiler_lehman.py:157-176): without them SubgraphMatching gets two entries
+                if len(x) != 3 or (from_graph and not x[2]):
+                    raise TypeError(_SM_ELEMENT_MSG)
+                n, edges, _, el = self._sm._graph(x[0], None, x[2] if x[2] else None, need_v=False)
+                order = adjacency_and_order(x[0])[1]
                 graphs.append((n, edges, None, el))
             else:
                 if type(x[0]) is dict and x[0] and all(type(d) is list for d in x[0].values()) and not all(x[0].values()):
@@ -724,7 +746,7 @@ class WeisfeilerLehman(Kernel):
             cols.append(rows + gp[g])
         out.src = np.concatenate(cols) if cols else np.zeros(0, dtype=np.int64)
         out.wl_vertices = int(gp[-1])
-        if base is NeighborhoodSubgraphPairwiseDistance:
+        if base in (NeighborhoodSubgraphPairwiseDistance, SubgraphMatching):
             out.graphs = graphs
         else:
             b = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
@@ -830,9 +852,40 @@ class WeisfeilerLehman(Kernel):
             K, _ = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(self.normalize), xdiag=xd, ydiag=yd_sum)
             return K, xd, yd_sum
 
+    def _wl_sm_run(self, block, ids, n_fit, want_matrix=True, row_range=None, device_ptr=None):
+        """WL over SubgraphMatching (gk_sm_wl_features): the joint device partition of the fitted and new graphs gives
+        every base vertex its class per level, and one clique enumeration per pair gives K = sum over the levels of
+        SubgraphMatching on the level's labels.  With kv=_dirac the level-h product graph is the level-0 one on the
+        vertices whose classes agree up to level h; with kv=None every level is level 0 (DESIGN 4.23)."""
+        data = self.X.base if n_fit == block.n_graphs else _WlBaseData.concat(self.X.base, self._base_y)
+        sm, n_iter = self._sm, self._n_iter - 1
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            level_ids, vl = None, None
+            if sm.kv is not None:
+                eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
+                eng.wl_features(n_iter)
+                classes = [np.asarray(ids)] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, n_iter + 1)]
+                level_ids = np.stack(classes, axis=1)[data.src]
+                vl = level_ids[:, 0]
+            graphs, v0 = [], 0
+            for n, edges, _, el in data.graphs:
+                graphs.append((n, edges, None if vl is None else vl[v0:v0 + n].tolist(), el))
+                v0 += n
+            gp, rp, ci, lab, elids, _, et, flags = sm._pack(graphs)
+            eng.pack(gp, rp, ci, lab, None, None)
+            self.stats_ = eng.sm_wl_features(int(sm.k), n_iter, level_ids, sm.lambdas_, et, elids, flags)
+            K, xd, yd = eng.gram(len(graphs), n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
+                                 device_ptr=device_ptr, stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd
+
     def _run(self, block, ids, n_fit, want_matrix=True):
         """The plain subtree fit_transform (square, un-normalised) is ONE C call, gk_wl_gram: relabel, column statistics,
         head/tail decision on the device, GEMM, tail and delivery with a single host synchronisation."""
+        if self._base_graph_kernel is SubgraphMatching:
+            return self._wl_sm_run(block, ids, n_fit, want_matrix)
         if self._base_graph_kernel in (NeighborhoodSubgraphPairwiseDistance, OddSth):
             return self._base_run(block, ids, n_fit, want_matrix)
         if (want_matrix and not self.normalize and n_fit == block.n_graphs and self._base_graph_kernel is VertexHistogram
@@ -3268,9 +3321,10 @@ class SubgraphMatching(Kernel):
             raise NotImplementedError("SubgraphMatching: k < 0 has no defined result")
 
     # ---- input
-    def _graph(self, g, node_labels, edge_labels):
-        """(n, sorted (i, j) edges without self-loops, vertex labels or None, edge labels or None)."""
-        need_v, need_e = self.kv is not None, self.ke is not None
+    def _graph(self, g, node_labels, edge_labels, need_v=None):
+        """(n, sorted (i, j) edges without self-loops, vertex labels or None, edge labels or None).  `need_v=False`
+        skips the vertex labels (WeisfeilerLehman hands its own)."""
+        need_v, need_e = self.kv is not None if need_v is None else need_v, self.ke is not None
         if need_v and not node_labels:
             raise ValueError("Graph does not have any labels for vertices.")
         if need_e and not edge_labels:
@@ -4307,4 +4361,4 @@ class GraphletSampling(Kernel):
         return self._X_diag
 
 
-_WL_GRAPH_BASES = (PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth)
+_WL_GRAPH_BASES = (PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth, SubgraphMatching)

@@ -303,6 +303,20 @@ int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double*
                    const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags, gk_stats* stats);
 int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out);
 
+/* WeisfeilerLehman over SubgraphMatching (weisfeiler_lehman.py over subgraph_matching.py) in one clique enumeration.
+ * level_ids[v * (n_iter + 1) + h] is the WL class of packed vertex v at level h (any numbering per level; level 0 is
+ * the partition of the packed labels, and each level refines the one before).  The vertex kernel is GK_SM_KV_DIRAC
+ * or GK_SM_KV_NONE (level_ids may then be null: every level has every product vertex); the edge kernel, the edge
+ * labels, k and the lambdas are those of gk_sm_features, whose checks apply.  gk_gram then returns
+ * K = ((K_0 + K_1) + K_2) ... in fp64, K_h the SubgraphMatching K of the level-h classes as vertex labels, under
+ * gk_sm_features' gk_gram rules; GK_NORMALIZE divides by that sum's own self similarities.  (n_iter + 1) *
+ * min(k, largest packed graph) above 64 is GK_ERR_UNSUPPORTED.  gk_sm_wl_counts writes tv of every level of the
+ * n_fit pairs of row `row`: out[n_fit * (n_iter + 1) * (k + 1)], pair-major then level. */
+int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
+                      const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                      gk_stats* stats);
+int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out);
+
 /* OddSth (odd_sth.py), one warp per root vertex.  The packed CSR lists every vertex's out-neighbours in the reference's
  * edge-dictionary order (every packed vertex is a root), the packed labels are one id per distinct str(label), and
  * rank[V] orders the label values within each graph (equal values share a rank).  Root v's DAG is the BFS from v cut
