@@ -136,6 +136,7 @@ _SYMBOLS = {
     "gk_event_elapsed": (C.c_int, [_P, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     "gk_profiler_range": (C.c_int, [C.c_int32]),
     "gk_selftest_gram": (C.c_int, [_P, C.c_int64, C.c_int64, _P, _P, _P]),
+    "gk_selftest_live_bytes": (C.c_int, [C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "gk_tu_open": (C.c_int, [C.c_char_p, C.c_char_p, C.c_int32, C.POINTER(_P)]),
     "gk_tu_info": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "gk_tu_pack": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
@@ -241,6 +242,15 @@ def gs_draw(rs, sizes, k, n_samples):
         raise NotImplementedError(msg) if "more than 6" in msg else GrakelB200Error(msg)
     rs.set_state((name, key, p.value, has_gauss, gauss))
     return size, idx[:n.value]
+
+
+def live_bytes():
+    """Tests only: (device, pinned) bytes the library's buffers hold right now, over every engine of the process."""
+    dev, pin = C.c_int64(), C.c_int64()
+    lib = load_library()
+    if lib.gk_selftest_live_bytes(C.byref(dev), C.byref(pin)) != 0:
+        raise GrakelB200Error(lib.gk_last_error().decode())
+    return dev.value, pin.value
 
 
 class _HostBlock:

@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <condition_variable>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <atomic>
 #include <thread>
@@ -43,6 +44,7 @@
 
 namespace gk {
 thread_local std::string g_last_error;
+std::atomic<int64_t> g_live_bytes[2] = {};
 
 static inline size_t next_pow2(size_t x) {
   size_t p = 1;
@@ -80,14 +82,14 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
+  static const EncodeTiledFn fn = [] {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
+    return cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
+                   q == cudaDriverEntryPointSuccess
+               ? reinterpret_cast<EncodeTiledFn>(p)
+               : nullptr;
+  }();
   return fn;
 }
 
@@ -154,54 +156,6 @@ static float ev_ms(cudaEvent_t a, cudaEvent_t b) {
 
 using namespace gk;
 
-// extra host-side state that does not belong in the POD-ish handle header
-struct HandleExtra {
-  std::vector<int> graph_ptr;
-  std::vector<int> graph_eptr;  // first edge of each graph (row_ptr[graph_ptr[g]])
-  std::vector<long long> sp_goff;
-  // fused WL kernel: the tile partition of the packed block (device copy in wlf_buf) is kept between calls
-  bool wl_tiles_valid = false;
-  bool wl_tiles_fused = false;
-  int wl_n_tiles = 0;
-  long long wl_tiles_key = -1;  // GRAKEL_B200_WL_TILES_PER_CTA the partition was built with
-  // Gram prologue run by gk_wl_features (pro_serial): what gk_gram would otherwise read back after a synchronisation
-  ColStats pro_hist;
-  long long pro_max_count = 0, pro_max_diag = 0, pro_n_entries = 0;
-  // GEMM tile list on the device (h->tiles): rebuilt and uploaded only when its key changes
-  long long tiles_key[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
-  long long tiles_n = 0;
-  long long head_row_bytes = 0;  // panel row width (bytes) of the last pass whose threshold came from the cost model
-                                 // (not GK_DENSE_ALL / FORCE_T)
-  long long last_max_count = 0;  // largest count of the last Gram on this handle: an asynchronous pass fills a u8 panel
-                                 // unless it was 256 (a count of 256 repeats through the synchronous route once)
-  // NeighborhoodHash: per level, distinct codes, columns and entries of the unary-expanded block
-  std::vector<long long> nh_dims, nh_cols, nh_entries;
-  // NeighborhoodSubgraphPairwiseDistance: per level (delta-major), its table's byte offset in nspd_blk, slots, pairs
-  // and columns; per graph, the mask of the distances it has pairs at
-  std::vector<long long> nspd_off, nspd_cap, nspd_M, nspd_cols;
-  std::vector<unsigned long long> nspd_mask;
-  // OddSth: node slots, child slots, identities; per bit plane of C, its table's byte offset in odd_blk, slots,
-  // entries and columns
-  long long odd_S = 0, odd_T = 0, odd_F = 0, odd_maxC = 0;
-  std::vector<long long> odd_off, odd_cap, odd_M, odd_cols;
-};
-static std::vector<std::pair<gk_handle*, HandleExtra*>> g_extra;
-static HandleExtra* extra_of(gk_handle* h) {
-  for (auto& p : g_extra)
-    if (p.first == h) return p.second;
-  HandleExtra* e = new HandleExtra();
-  g_extra.emplace_back(h, e);
-  return e;
-}
-static void drop_extra(gk_handle* h) {
-  for (size_t i = 0; i < g_extra.size(); ++i)
-    if (g_extra[i].first == h) {
-      delete g_extra[i].second;
-      g_extra.erase(g_extra.begin() + i);
-      return;
-    }
-}
-
 #define LAUNCH_CHECK(h)                                 \
   do {                                                  \
     (h)->launches++;                                    \
@@ -225,7 +179,7 @@ int gk_create(int device_ordinal, gk_handle** out) {
     return fail(GK_ERR_UNSUPPORTED, std::string("grakel_b200 needs an sm_90a (H100) device, found sm_") +
                                         std::to_string(prop.major) + std::to_string(prop.minor));
   }
-  gk_handle* h = new gk_handle();
+  std::unique_ptr<gk_handle> h(new gk_handle());
   h->dev = device_ordinal;
   h->sm_count = prop.multiProcessorCount;
   GK_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -250,7 +204,7 @@ int gk_create(int device_ordinal, gk_handle** out) {
   GK_CUDA(cudaFuncSetAttribute(gram_tc_kernel<double, false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
   GK_CUDA(cudaFuncSetAttribute(wl_fused2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WLF2_SMEM));
-  *out = h;
+  *out = h.release();
   return GK_OK;
 }
 
@@ -273,7 +227,7 @@ int gk_comm_destroy(gk_handle* h) {
   cudaStreamSynchronize(h->stream);
   for (int r = 0; r < c->nranks; ++r)
     if (r != c->rank && c->peer_base[r]) { cudaIpcCloseMemHandle(c->peer_base[r]); c->peer_base[r] = nullptr; }
-  // collective: nobody frees an exported block (gk_destroy does, right after this) before every peer has unmapped it
+  // collective: nobody frees an exported block (~gk_handle does, right after this) before every peer has unmapped it
   if (c->comm && c->nranks > 1 && nccl_api()->AllReduce) {
     nccl_api()->AllReduce(c->d_token, c->d_token, 1, ncclInt32, ncclSum, c->comm, h->stream);
     cudaStreamSynchronize(h->stream);
@@ -331,52 +285,7 @@ int gk_selftest_dist_tiles(int64_t n_rows, int32_t nranks, int32_t rank, int32_t
 }
 
 int gk_destroy(gk_handle* h) {
-  if (!h) return GK_OK;
-  cudaSetDevice(h->dev);
-  cudaStreamSynchronize(h->stream);
-  gk::DevBuf* bufs[] = {&h->graph_ptr, &h->row_ptr, &h->col_idx, &h->labels0, &h->weights, &h->attrs, &h->vgraph,
-                        &h->large_list, &h->labels_all, &h->sig_nbr, &h->slot_of, &h->ht_keys, &h->ht_rep,
-                        &h->flags, &h->block_sums, &h->scalars, &h->ft_keys, &h->ft_cnt, &h->colcnt,
-                        &h->colmin, &h->colmax, &h->colslot, &h->col_flags3, &h->col_block_sums, &h->colstats, &h->tail_desc,
-                        &h->tail_ent, &h->tail_cur, &h->part_max, &h->part_new, &h->diag_u64, &h->diag_f64, &h->panel,
-                        &h->sp_dist, &h->sp_dict_keys, &h->sp_dict_ids, &h->sp_dkeys, &h->sp_graph_off, &h->fattr, &h->tiles,
-                        &h->K, &h->K_stage, &h->wlf_buf, &h->row_map, &h->diag_rows, &h->oa_keys, &h->oa_cnt, &h->oa_colcnt, &h->wl_single,
-                        &h->diag_frozen, &h->sp_lists, &h->wl_payload, &h->gram_dyn, &h->tb_cnt, &h->tb_ent, &h->tb_ovf,
-                        &h->gh_M, &h->gh_ws, &h->gh_woff, &h->gh_gdiam, &h->gh_groups, &h->gh_pairs,
-                        &h->nh_codes, &h->nh_valid, &h->nh_blk, &h->nh_lut, &h->nh_tab, &h->nh_ws, &h->nh_cur, &h->nh_C,
-                        &h->rw_val, &h->rw_trp, &h->rw_tci, &h->rw_tval, &h->rw_q, &h->rw_w, &h->rw_coef, &h->rw_ws,
-                        &h->rw_iters, &h->rw_cap,
-                        &h->pk_P, &h->pk_bins, &h->pk_priv, &h->pk_tval, &h->pk_u, &h->pk_b, &h->pk_tab, &h->pk_cnt,
-                        &h->pm_U, &h->pm_ncols, &h->pm_skip, &h->hc_S, &h->hc_z, &h->hc_skip,
-                        &h->nspd_lvl, &h->nspd_q, &h->nspd_H, &h->nspd_aux, &h->nspd_ws, &h->nspd_pairs, &h->nspd_blk,
-                        &h->nspd_tab, &h->nspd_keys, &h->nspd_C,
-                        &h->sm_rec, &h->sm_off, &h->sm_el, &h->sm_vtab, &h->sm_etab, &h->sm_lam, &h->sm_stack, &h->sm_ctl,
-                        &h->odd_aux, &h->odd_nodes, &h->odd_ch, &h->odd_tab, &h->odd_feat, &h->odd_phi, &h->odd_blk,
-                        &h->odd_ctl, &h->odd_diag,
-                        &h->ml_adj, &h->ml_adj_off, &h->ml_ball, &h->ml_U, &h->ml_U2, &h->ml_vrec, &h->ml_samp, &h->ml_rec,
-                        &h->ml_aux, &h->ml_ctl,
-                        &h->svmt_vptr, &h->svmt_adj, &h->svmt_m, &h->svmt_alpha, &h->svmt_iters, &h->svmt_cnt,
-                        &h->svmt_off, &h->svmt_idx, &h->svmt_sums, &h->svmt_phi, &h->svmt_rec, &h->svmt_ctl,
-                        &h->gs_canon, &h->gs_first, &h->gs_colid, &h->gs_blk, &h->gs_colcnt, &h->gs_diag, &h->gs_ctl,
-                        &h->gs_samp, &h->wl_sum, &h->wl_lvl, &h->core_map};
-  for (auto* b : bufs) b->release();
-  h->h_scalars.release();
-  h->h_colstats.release();
-  h->h_dyn.release();
-  h->h_tiles.release();
-  h->h_stage.release();
-  h->h_diag.release();
-  h->h_bands.release();
-  for (auto& e : h->ev) cudaEventDestroy(e);
-  for (auto& e : h->tev) cudaEventDestroy(e);
-  cudaStreamDestroy(h->stream);
-  cudaStreamDestroy(h->stream2);
-  cudaEventDestroy(h->ev_fork);
-  cudaEventDestroy(h->ev_join);
-  for (auto& e : h->ev_stage) cudaEventDestroy(e);
-  gk_comm_destroy(h);
-  drop_extra(h);
-  delete h;
+  if (h) delete h;
   return GK_OK;
 }
 
@@ -435,11 +344,10 @@ int gk_pack_csr(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const 
   h->n_rows = 0;  // a new block starts without a row map
   h->hc_W = 0;    // ... and without HadamardCode vectors
   h->ml_w = 0;    // ... and without MultiscaleLaplacian features
-  HandleExtra* ex = extra_of(h);
-  ex->wl_tiles_valid = false;
-  ex->graph_ptr.assign(graph_ptr, graph_ptr + N + 1);
-  ex->graph_eptr.resize(N + 1);
-  for (int64_t g = 0; g <= N; ++g) ex->graph_eptr[g] = V ? row_ptr[graph_ptr[g]] : 0;
+  h->wl_tiles_valid = false;
+  h->graph_ptr_host.assign(graph_ptr, graph_ptr + N + 1);
+  h->graph_eptr_host.resize(N + 1);
+  for (int64_t g = 0; g <= N; ++g) h->graph_eptr_host[g] = V ? row_ptr[graph_ptr[g]] : 0;
 
   GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
   GK_TRY(h->graph_ptr.ensure((N + 1) * 4));
@@ -599,12 +507,11 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
   int n_tiles = 0;
   long long tiles_env = 0;
   if (const char* e = getenv("GRAKEL_B200_WL_TILES_PER_CTA")) tiles_env = atoi(e);
-  if (fused && extra_of(h)->wl_tiles_valid && extra_of(h)->wl_tiles_key == tiles_env) {
+  if (fused && h->wl_tiles_valid && h->wl_tiles_key == tiles_env) {
     // same packed block as the last call: the partition is still in wlf_buf (the kernels only touch its barrier word)
-    fused = extra_of(h)->wl_tiles_fused;
-    n_tiles = extra_of(h)->wl_n_tiles;
+    fused = h->wl_tiles_fused;
+    n_tiles = h->wl_n_tiles;
   } else if (fused) {
-    HandleExtra* ex = extra_of(h);
     std::vector<int> tv, ct(G + 1, 0);
     bool ok = false;
     int64_t per0 = std::max<int64_t>(1, std::max((V + (int64_t)G * WLF_TILE_V - 1) / ((int64_t)G * WLF_TILE_V),
@@ -618,19 +525,19 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
       size_t g = 0;
       for (int t = 1; t < T; ++t) {
         const long long want = (long long)V * t / T;
-        while (g < (size_t)h->N && ex->graph_ptr[g] < want) ++g;
+        while (g < (size_t)h->N && h->graph_ptr_host[g] < want) ++g;
         tv[t] = (int)g;
       }
       tv[T] = (int)h->N;
       ok = true;
       for (int t = 0; t < T && ok; ++t) {
-        const int nv = ex->graph_ptr[tv[t + 1]] - ex->graph_ptr[tv[t]];
-        const int ne = ex->graph_eptr[tv[t + 1]] - ex->graph_eptr[tv[t]];
+        const int nv = h->graph_ptr_host[tv[t + 1]] - h->graph_ptr_host[tv[t]];
+        const int ne = h->graph_eptr_host[tv[t + 1]] - h->graph_eptr_host[tv[t]];
         if (nv > WLF_TILE_V || ne > WLF_TILE_E) ok = false;
       }
       if (ok) {
         n_tiles = T;
-        for (int t = 0; t <= T; ++t) tv[t] = ex->graph_ptr[tv[t]];  // graph index -> first vertex
+        for (int t = 0; t <= T; ++t) tv[t] = h->graph_ptr_host[tv[t]];  // graph index -> first vertex
         for (int c = 0; c <= G; ++c) ct[c] = c * per;
         long long max_cta = 0;
         for (int c = 0; c < G; ++c) max_cta = std::max<long long>(max_cta, tv[ct[c + 1]] - tv[ct[c]]);
@@ -649,7 +556,7 @@ static int wl_setup(gk_handle* h, int n_iter, WlPlan* pl) {
       memcpy(hp + n_tiles + 1, ct.data(), (size_t)(G + 1) * 4);
       GK_CUDA(cudaMemcpyAsync(h->wlf_buf.p, hp, ((size_t)n_tiles + G + 2) * 4, cudaMemcpyHostToDevice, h->stream));
     }
-    ex->wl_tiles_valid = true; ex->wl_tiles_fused = fused; ex->wl_n_tiles = n_tiles; ex->wl_tiles_key = tiles_env;
+    h->wl_tiles_valid = true; h->wl_tiles_fused = fused; h->wl_n_tiles = n_tiles; h->wl_tiles_key = tiles_env;
   }
   // feature block: the multi-kernel path fills one open-addressing sub-table per level, the fused
   // kernel appends at most V entries per level to the same arrays used as a COO list
@@ -846,9 +753,8 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
   h->features_ready = true; h->feat_serial++;
   h->feature_kind = FK_WL;
   if (pro_enqueued) {
-    HandleExtra* ex = extra_of(h);
-    ex->pro_hist = *h->h_colstats.as<ColStats>();
-    ex->pro_max_count = (long long)hs->max_count; ex->pro_max_diag = (long long)hs->max_diag; ex->pro_n_entries = (long long)hs->n_entries;
+    h->pro_hist = *h->h_colstats.as<ColStats>();
+    h->pro_max_count = (long long)hs->max_count; h->pro_max_diag = (long long)hs->max_diag; h->pro_n_entries = (long long)hs->n_entries;
     h->pro_serial = h->feat_serial;
   }
   if (stats) {
@@ -992,7 +898,6 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
   if (with_labels && n_labels_total >= (1 << 20)) return fail(GK_ERR_UNSUPPORTED, "gk_sp_features: more than 2^20 distinct labels");
   const bool use_u16 = (!h->has_weights || h->unit_weights) && h->max_graph_size < 16000;
   const size_t esz = use_u16 ? 2 : 8;
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N;
   const int64_t launches0 = h->launches;
   h->features_ready = false; h->feat_serial++;
@@ -1003,13 +908,13 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
   std::vector<int> small, big;
   std::vector<int> bfs[4];  // unit weights: bitmask BFS with W = 1, 2, 4, 8 words (n <= 64 W)
   size_t max_small_nn = 0;
-  ex->sp_goff.assign(N + 1, 0);
+  h->sp_goff.assign(N + 1, 0);
   const bool keep = flags & GK_SP_KEEP_DIST;
   long long off_big = 0, off_all = 0;
   std::vector<long long> goff_big(N, 0);
   for (int64_t g = 0; g < N; ++g) {
-    const long long n = ex->graph_ptr[g + 1] - ex->graph_ptr[g];
-    ex->sp_goff[g] = off_all;
+    const long long n = h->graph_ptr_host[g + 1] - h->graph_ptr_host[g];
+    h->sp_goff[g] = off_all;
     off_all += n * n;
     if (use_u16 && n <= 512) {
       bfs[n <= 64 ? 0 : n <= 128 ? 1 : n <= 256 ? 2 : 3].push_back((int)g);
@@ -1022,7 +927,7 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
       off_big += n * n;
     }
   }
-  ex->sp_goff[N] = off_all;
+  h->sp_goff[N] = off_all;
   const size_t smem_small = SP_LOCAL_SLOTS * 12 + max_small_nn * esz + 16;
   const size_t smem_big = SP_LOCAL_SLOTS * 12 + 16;
 
@@ -1037,7 +942,7 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
   GK_TRY(h->sp_graph_off.ensure((size_t)(N + 1) * 8 * 2));
   long long* d_goff_all = h->sp_graph_off.as<long long>();
   long long* d_goff_big = d_goff_all + (N + 1);
-  GK_CUDA(cudaMemcpyAsync(d_goff_all, ex->sp_goff.data(), (N + 1) * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(d_goff_all, h->sp_goff.data(), (N + 1) * 8, cudaMemcpyHostToDevice, h->stream));
   GK_CUDA(cudaMemcpyAsync(d_goff_big, goff_big.data(), N * 8, cudaMemcpyHostToDevice, h->stream));
   if (off_big) GK_TRY(h->sp_dist.ensure((size_t)off_big * esz));
   double* d_keep = nullptr;
@@ -1163,7 +1068,7 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
         st = h->stream2;
       }
       int nmax = 0;
-      for (int g : bfs[i]) nmax = std::max(nmax, ex->graph_ptr[g + 1] - ex->graph_ptr[g]);
+      for (int g : bfs[i]) nmax = std::max(nmax, h->graph_ptr_host[g + 1] - h->graph_ptr_host[g]);
       const bool direct = p.n_labels <= SP_DIRECT_MAX_LABELS;
       const size_t smem = (direct ? SP_LOCAL_SLOTS * 4 : SP_LOCAL_SLOTS * 12) + (size_t)nmax * W * 8 + (size_t)16 * W * 8 +
                           (size_t)nmax * 4 + 16;
@@ -1447,8 +1352,7 @@ int gk_sp_distances(gk_handle* h, int64_t g, double* out) {
     // after gk_spattr_features: the APSP matrices of every graph are still in sp_dist (u16 with the saturated
     // value 0x3FFF for "no path", or fp64 with +inf)
     if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_sp_distances: bad graph index");
-    HandleExtra* ex = extra_of(h);
-    const long long off = ex->sp_goff[g], cnt = ex->sp_goff[g + 1] - off;
+    const long long off = h->sp_goff[g], cnt = h->sp_goff[g + 1] - off;
     GK_CUDA(cudaSetDevice(h->dev));
     if (h->sp_dist_esz == 8) {
       GK_CUDA(cudaMemcpyAsync(out, h->sp_dist.as<double>() + off, cnt * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1463,8 +1367,7 @@ int gk_sp_distances(gk_handle* h, int64_t g, double* out) {
   }
   if (h->feature_kind != FK_SP || !(h->sp_flags & GK_SP_KEEP_DIST)) return fail(GK_ERR_STATE, "gk_sp_distances: run gk_sp_features with GK_SP_KEEP_DIST (or gk_spattr_features) first");
   if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_sp_distances: bad graph index");
-  HandleExtra* ex = extra_of(h);
-  const long long off = ex->sp_goff[g], cnt = ex->sp_goff[g + 1] - off;
+  const long long off = h->sp_goff[g], cnt = h->sp_goff[g + 1] - off;
   GK_CUDA(cudaSetDevice(h->dev));
   GK_CUDA(cudaMemcpyAsync(out, h->K_stage.as<double>() + off, cnt * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
@@ -1481,7 +1384,6 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
   if (dd > 1024) return fail(GK_ERR_UNSUPPORTED, "gk_spattr_features: attribute dimension above 32");
   const bool use_u16 = (!h->has_weights || h->unit_weights) && h->max_graph_size < 16000;
   const size_t esz = use_u16 ? 2 : 8;
-  HandleExtra* ex = extra_of(h);
   const int64_t launches0 = h->launches;
   h->features_ready = false; h->feat_serial++;
   if ((size_t)h->max_graph_size * h->max_graph_size * 2 + (size_t)h->max_graph_size * da * 8 + (size_t)dd * 8 > 200 * 1024)
@@ -1490,22 +1392,22 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
   // per-graph offsets of the distance matrices (all kept in global memory for phase C)
   std::vector<int> small, big;
   size_t max_small_nn = 0;
-  ex->sp_goff.assign(N + 1, 0);
+  h->sp_goff.assign(N + 1, 0);
   long long off_all = 0;
   for (int64_t g = 0; g < N; ++g) {
-    const long long n = ex->graph_ptr[g + 1] - ex->graph_ptr[g];
-    ex->sp_goff[g] = off_all;
+    const long long n = h->graph_ptr_host[g + 1] - h->graph_ptr_host[g];
+    h->sp_goff[g] = off_all;
     off_all += n * n;
     if ((size_t)(n * n) * esz <= 160 * 1024) { small.push_back((int)g); max_small_nn = std::max(max_small_nn, (size_t)(n * n)); }
     else big.push_back((int)g);
   }
-  ex->sp_goff[N] = off_all;
+  h->sp_goff[N] = off_all;
   std::vector<int> order(small);
   order.insert(order.end(), big.begin(), big.end());
   GK_TRY(h->sp_lists.ensure((size_t)N * 4 + 16));
   GK_CUDA(cudaMemcpyAsync(h->sp_lists.p, order.data(), order.size() * 4, cudaMemcpyHostToDevice, h->stream));
   GK_TRY(h->sp_graph_off.ensure((size_t)(N + 1) * 8));
-  GK_CUDA(cudaMemcpyAsync(h->sp_graph_off.p, ex->sp_goff.data(), (N + 1) * 8, cudaMemcpyHostToDevice, h->stream));
+  GK_CUDA(cudaMemcpyAsync(h->sp_graph_off.p, h->sp_goff.data(), (N + 1) * 8, cudaMemcpyHostToDevice, h->stream));
   GK_TRY(h->sp_dist.ensure((size_t)std::max<long long>(off_all, 1) * esz));
   const size_t dict_cap = 1 << 16;
   GK_TRY(h->sp_dict_keys.ensure(dict_cap * 8));
@@ -1856,14 +1758,13 @@ static int gram_spattr(gk_handle* h, const GramReq& q, gk_stats* stats) {
 // run from shared memory, the others from a global workspace.
 template <bool MAPS>
 static int gh_dag_pass(gk_handle* h, const std::vector<int>& gdiam, double* M, long long T) {
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N;
   const size_t smem_cap = 96 * 1024;
   std::vector<int> small, big;
   std::vector<long long> woff(N, 0);
   size_t smem_max = 16, ws_total = 0;
   for (int64_t g = 0; g < N; ++g) {
-    const long long n = ex->graph_ptr[g + 1] - ex->graph_ptr[g];
+    const long long n = h->graph_ptr_host[g + 1] - h->graph_ptr_host[g];
     const size_t b = gh_ws_bytes(n, MAPS ? gdiam[g] + 1 : 0, MAPS);
     if (b <= smem_cap) { small.push_back((int)g); smem_max = std::max(smem_max, b); }
     else { big.push_back((int)g); woff[g] = (long long)ws_total; ws_total += b; }
@@ -1994,10 +1895,9 @@ int gk_gh_node_maps(gk_handle* h, int64_t g, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_gh_node_maps: null argument");
   if (h->feature_kind != FK_GH || !h->features_ready) return fail(GK_ERR_STATE, "gk_gh_node_maps: run gk_gh_features first");
   if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_gh_node_maps: bad graph index");
-  HandleExtra* ex = extra_of(h);
   const int delta = h->gh_delta;
   const long long T = (long long)delta * (delta + 1) / 2;
-  const long long v0 = ex->graph_ptr[g], n = ex->graph_ptr[g + 1] - v0;
+  const long long v0 = h->graph_ptr_host[g], n = h->graph_ptr_host[g + 1] - v0;
   std::vector<double> tri((size_t)n * T);
   GK_CUDA(cudaSetDevice(h->dev));
   if (n > 0) {
@@ -2030,7 +1930,6 @@ static void gh_groups(const std::vector<int>& gp, int g0, int g1, std::vector<in
 // Gram of the node-pair kernels (gaussian / bridge): gh_nodepair_gram over graph-group pairs, self similarities from
 // gh_nodepair_diag.  fp64, host output, GK_NORMALIZE, n_fit / row ranges as in gram_spattr.
 static int gram_gh_nodepair(gk_handle* h, const GramReq& q, gk_stats* stats) {
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows;
   const bool square = q.square;
   const int a0 = q.a0, a1 = q.a1;
@@ -2040,8 +1939,8 @@ static int gram_gh_nodepair(gk_handle* h, const GramReq& q, gk_stats* stats) {
   // groups: over all graphs (square) or over Y rows and X columns; the same groups whatever the row range, so a
   // row block reproduces the full matrix's entries bit for bit
   std::vector<int> rgroups, cgroups;
-  gh_groups(ex->graph_ptr, square ? 0 : (int)n_fit, (int)N, rgroups);
-  gh_groups(ex->graph_ptr, 0, (int)n_fit, cgroups);
+  gh_groups(h->graph_ptr_host, square ? 0 : (int)n_fit, (int)N, rgroups);
+  gh_groups(h->graph_ptr_host, 0, (int)n_fit, cgroups);
   const int nrg = (int)rgroups.size() - 1, ncg = (int)cgroups.size() - 1;
   auto touches = [&](int I) { return rgroups[I] < a1 && rgroups[I + 1] > a0; };
   std::vector<int2> pairs;
@@ -2197,22 +2096,21 @@ static int level_columns(gk_handle* h, const LevelScratch& ls, int r, int64_t M,
 // Reads the levels' column statistics back (synchronises) into the handle's per-level tables.
 static int level_finish(gk_handle* h, const LevelScratch& ls, int n_blocks, const char* who, DevScalars** hs,
                         int64_t* n_cols, int64_t* n_ent) {
-  HandleExtra* ex = extra_of(h);
   GK_CUDA(cudaMemcpyAsync(h->h_colstats.p, h->nh_cur.p, ls.cur_bytes, cudaMemcpyDeviceToHost, h->stream));
   GK_TRY(read_scalars(h, hs));  // synchronises
   if ((*hs)->ft_overflow) return fail(GK_ERR_STATE, std::string(who) + ": expanded feature block overflow");
   const OaCursors* hc = h->h_colstats.as<OaCursors>();
   const unsigned long long* hdims = reinterpret_cast<const unsigned long long*>(hc + n_blocks);
-  ex->nh_dims.assign(n_blocks, 0);
-  ex->nh_cols.assign(n_blocks, 0);
-  ex->nh_entries.assign(n_blocks, 0);
+  h->nh_dims.assign(n_blocks, 0);
+  h->nh_cols.assign(n_blocks, 0);
+  h->nh_entries.assign(n_blocks, 0);
   *n_cols = *n_ent = 0;
   for (int r = 0; r < n_blocks; ++r) {
-    ex->nh_dims[r] = (long long)hdims[r];
-    ex->nh_cols[r] = (long long)hc[r].n_cols;
-    ex->nh_entries[r] = (long long)hc[r].n_entries;
-    *n_cols += ex->nh_cols[r];
-    *n_ent += ex->nh_entries[r];
+    h->nh_dims[r] = (long long)hdims[r];
+    h->nh_cols[r] = (long long)hc[r].n_cols;
+    h->nh_entries[r] = (long long)hc[r].n_entries;
+    *n_cols += h->nh_cols[r];
+    *n_ent += h->nh_entries[r];
   }
   return GK_OK;
 }
@@ -2233,7 +2131,6 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
   const unsigned long long mask = bits == 64 ? ~0ULL : (1ULL << bits) - 1ULL;
   const int64_t launches0 = h->launches;
   h->features_ready = false; h->feat_serial++;
-  HandleExtra* ex = extra_of(h);
 
   GK_TRY(init_scalars(h, 0));  // clears ft_overflow
   GK_TRY(h->nh_codes.ensure((size_t)(R + 1) * V1 * 8));
@@ -2302,7 +2199,7 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
     stats->n_levels = R;
-    for (int r = 0; r < R; ++r) stats->level_dims[r] = ex->nh_dims[r];
+    for (int r = 0; r < R; ++r) stats->level_dims[r] = h->nh_dims[r];
     stats->n_columns = n_cols;
     stats->n_entries = n_ent;
     stats->kernel_launches = h->launches - launches0;
@@ -2358,7 +2255,6 @@ struct LevelTimes {
 
 template <class Combine>
 static int gram_levels(gk_handle* h, const GramReq& q, int n_blocks, const F64Out& out, Combine combine, LevelTimes* t) {
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
   const bool square = q.square;
   const int64_t ldc = (k_cols + 7) / 8 * 8;  // 32-byte rows: TMA stores of the Gram epilogue
@@ -2377,8 +2273,8 @@ static int gram_levels(gk_handle* h, const GramReq& q, int n_blocks, const F64Ou
     for (int r = 0; r < n_blocks; ++r) {
       // the integer Gram of level block r: its rows [cb, ce) as fp32 counts into nh_C
       IntBlock fb = nh_level(h, r);
-      fb.n_columns = ex->nh_cols[r];
-      const unsigned part[2] = {ex->nh_entries[r] ? 1u : 0u, (unsigned)ex->nh_entries[r]};
+      fb.n_columns = h->nh_cols[r];
+      const unsigned part[2] = {h->nh_entries[r] ? 1u : 0u, (unsigned)h->nh_entries[r]};
       GK_CUDA(cudaMemcpyAsync(h->part_max.p, &part[0], 4, cudaMemcpyHostToDevice, h->stream));
       GK_CUDA(cudaMemcpyAsync(h->part_new.p, &part[1], 4, cudaMemcpyHostToDevice, h->stream));
       GramReq lq;
@@ -2520,7 +2416,7 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
   // every used u must lie in [0, 1 + 2^-(L-1)): a NaN or negative u has no cell, and a larger one would give a cell
   // past the clamp 2^j - 1 that runs into the next row's keys
   if (L > 0 && V) {
-    const std::vector<int>& gp = extra_of(h)->graph_ptr;
+    const std::vector<int>& gp = h->graph_ptr_host;
     const double top = ldexp(1.0, L - 1);
     for (int s = 0; s < n_sets; ++s)
       for (int64_t g = 0; g < N; ++g)
@@ -2534,7 +2430,6 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
   }
   const int64_t launches0 = h->launches;
   h->features_ready = false; h->feat_serial++;
-  HandleExtra* ex = extra_of(h);
   GK_TRY(init_scalars(h, 0));  // clears ft_overflow
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   if (wl && h->wl_sparse_ids) {  // the histogram rows are indexed by dense label ids
@@ -2575,7 +2470,7 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
     stats->n_levels = n_blocks;
-    for (int r = 0; r < std::min(n_blocks, MAX_LEVELS); ++r) stats->level_dims[r] = ex->nh_dims[r];
+    for (int r = 0; r < std::min(n_blocks, MAX_LEVELS); ++r) stats->level_dims[r] = h->nh_dims[r];
     stats->n_columns = n_col;
     stats->n_entries = n_ent;
     stats->kernel_launches = h->launches - launches0;
@@ -2803,8 +2698,7 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
     }
   }
   const int store = (flags & GK_PK_STORE_F32) ? PK_STORE_F32 : (flags & GK_PK_STORE_INT) ? PK_STORE_INT : PK_STORE_F64;
-  HandleExtra* ex = extra_of(h);
-  const int v0 = ex->graph_ptr[n_fit];  // first vertex of the transformed graphs
+  const int v0 = h->graph_ptr_host[n_fit];  // first vertex of the transformed graphs
 
   // ---- levels: private flags, hash, propagate
   std::vector<cudaEvent_t> pev(2 * (size_t)t_max, nullptr);
@@ -2958,7 +2852,6 @@ static int rw_launch(gk_handle* h, RwParams p, size_t vec_elems) {
 // GK_OUT_DEVICE output, GK_NORMALIZE, n_fit and row ranges.  Self similarities come from the same pair kernel, so a
 // square K's diagonal equals them bit for bit.  The full square case computes the upper triangle and mirrors it.
 static int gram_rw(gk_handle* h, const GramReq& q, gk_stats* stats) {
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
   const bool square = q.square;
   const int64_t launches0 = h->launches;
@@ -2970,7 +2863,7 @@ static int gram_rw(gk_handle* h, const GramReq& q, gk_stats* stats) {
   // largest vertex count among the row graphs and among the column graphs: the vectors of the largest pair
   auto max_n = [&](int64_t g0, int64_t g1) {
     int m = 0;
-    for (int64_t g = g0; g < g1; ++g) m = std::max(m, ex->graph_ptr[g + 1] - ex->graph_ptr[g]);
+    for (int64_t g = g0; g < g1; ++g) m = std::max(m, h->graph_ptr_host[g + 1] - h->graph_ptr_host[g]);
     return (size_t)m;
   };
   const size_t nmax_all = max_n(0, N);
@@ -3068,11 +2961,10 @@ int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double*
   if (kk > SM_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: subgraphs of more than 32 vertices");
   GK_CUDA(cudaSetDevice(h->dev));
   h->sm_n_lv = 0;
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N;
   const bool elab = ke != SM_W_NONE;
   std::vector<long long> off(N + 1, 0);
-  for (int64_t g = 0; g < N; ++g) off[g + 1] = off[g] + sm_record_words(ex->graph_ptr[g + 1] - ex->graph_ptr[g], elab);
+  for (int64_t g = 0; g < N; ++g) off[g + 1] = off[g] + sm_record_words(h->graph_ptr_host[g + 1] - h->graph_ptr_host[g], elab);
   GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
   GK_TRY(h->sm_off.ensure((N + 1) * 8));
   GK_TRY(h->sm_rec.ensure(std::max<long long>(off[N], 1) * 4));
@@ -3417,7 +3309,6 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
   GK_TRY(h->colstats.ensure(sizeof(ColStats)));
   GK_TRY(h->h_colstats.ensure(sizeof(ColStats)));
   GK_TRY(h->diag_f64.ensure(N * 8));
-  HandleExtra* hx = extra_of(h);
   const bool pro = square && !d_row_map && fb.prologue_on_host && D <= fb.col_cap;
   if (!pro) GK_CUDA(cudaMemsetAsync(&sc->n_entries, 0, sizeof(unsigned long long) * 3 + sizeof(long long), h->stream));
   const unsigned long long* d_diag_u64 = fb.diag;
@@ -3457,8 +3348,8 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
   DevScalars* hs = nullptr;
   int64_t max_count, max_diag, n_entries;
   if (pro) {  // gk_wl_features ran diag_finish + col_hist and brought the results back with its own synchronisation
-    hc = hx->pro_hist;
-    max_count = hx->pro_max_count; max_diag = hx->pro_max_diag; n_entries = hx->pro_n_entries;
+    hc = h->pro_hist;
+    max_count = h->pro_max_count; max_diag = h->pro_max_diag; n_entries = h->pro_n_entries;
   } else {
     GK_CUDA(cudaMemsetAsync(cs, 0, sizeof(ColStats), h->stream));
     col_hist<<<nbc, 256, 0, h->stream>>>(D, square ? 1 : 0, (int)n_fit, fb.colcnt, h->colmin.as<int>(),
@@ -3475,7 +3366,7 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
   // panel element bytes of the tensor-core GEMM: u8 when every count fits, bf16 for a count of 256
   const int elem_bytes = (u8_panel_enabled() && max_count <= 255) ? 1 : 2;
   const int bk = panel_bk(elem_bytes);
-  hx->last_max_count = max_count;
+  h->last_max_count = max_count;
   int T = 1;
   {
     // T = 2^k minimising  head_cols * flops_per_col / rate + tail_updates * t_atomic  (COST_GEMM_RATE_*, COST_T_ATOMIC)
@@ -3526,7 +3417,7 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
   if (path == 1 && Dc == 0) path = 3;
   h->Dc = Dc;
   h->Dc_pad = (Dc + bk - 1) / bk * bk;
-  if (force_T < 0 && path == 1 && square) hx->head_row_bytes = h->Dc_pad * elem_bytes;
+  if (force_T < 0 && path == 1 && square) h->head_row_bytes = h->Dc_pad * elem_bytes;
 
   // ---- transport type.  Tensor-core results are integers < 2^24 (checked above), i.e. exact in fp32: a float64
   // HOST result is produced and moved as fp32 (half the HBM writes; a quarter of the PCIe bytes for the
@@ -3634,7 +3525,7 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
       // the tile list depends on the shape of the request only: built and uploaded when that changes
       const long long tkey[8] = {dist ? 1 : 0, dist ? (long long)N : a0, dist ? comm->nranks : a1, dist ? comm->rank : b0, b1,
                                  mirror ? 1 : 0, cta2 ? BM2 : BM, 0};
-      if (memcmp(tkey, hx->tiles_key, sizeof(tkey)) != 0 || !h->tiles.p) {
+      if (memcmp(tkey, h->tiles_key, sizeof(tkey)) != 0 || !h->tiles.p) {
         std::vector<int2> tiles;
         if (dist) dist_tiles(N, comm->nranks, comm->rank, tiles);
         else build_tiles(tiles, a0, a1, b0, b1, mirror, cta2 ? BM2 : BM);
@@ -3642,10 +3533,10 @@ static int gram_int(gk_handle* h, const GramReq& q, const IntBlock& fb, gk_stats
         memcpy(h->h_tiles.p, tiles.data(), tiles.size() * sizeof(int2));
         GK_TRY(h->tiles.ensure(tiles.size() * sizeof(int2) + 16));
         GK_CUDA(cudaMemcpyAsync(h->tiles.p, h->h_tiles.p, tiles.size() * sizeof(int2), cudaMemcpyHostToDevice, h->stream));
-        memcpy(hx->tiles_key, tkey, sizeof(tkey));
-        hx->tiles_n = (long long)tiles.size();
+        memcpy(h->tiles_key, tkey, sizeof(tkey));
+        h->tiles_n = (long long)tiles.size();
       }
-      n_tiles = hx->tiles_n;
+      n_tiles = h->tiles_n;
       CUtensorMap tmA, tmB, tmC;
       PeerMaps peer_maps;
       memset(&peer_maps, 0, sizeof(peer_maps));
@@ -3824,9 +3715,8 @@ static size_t nspd_level_bytes(long long cap, long long M, long long N) {
 }
 
 static NspdLevel nspd_level(gk_handle* h, int l) {
-  HandleExtra* ex = extra_of(h);
-  char* b = h->nspd_blk.as<char>() + ex->nspd_off[l];
-  const long long cap = ex->nspd_cap[l], M = ex->nspd_M[l];
+  char* b = h->nspd_blk.as<char>() + h->nspd_off[l];
+  const long long cap = h->nspd_cap[l], M = h->nspd_M[l];
   NspdLevel L;
   L.keys = reinterpret_cast<unsigned long long*>(b);
   L.cnt = reinterpret_cast<unsigned*>(b + cap * 8);
@@ -3852,8 +3742,7 @@ static int nspd_build_params(gk_handle* h, const int64_t* sym_hash, const int32_
                              int32_t n_ranks, const int64_t* el_off, const uint8_t* el_bytes, const int32_t* el_cp,
                              int32_t n_elabels, NspdParams* p, std::vector<long long>* lvl_off_h) {
   const int64_t N = h->N, V = h->V, E = h->E;
-  HandleExtra* ex = extra_of(h);
-  const std::vector<int>& gp = ex->graph_ptr;
+  const std::vector<int>& gp = h->graph_ptr_host;
   lvl_off_h->assign(N + 1, 0);
   for (int64_t g = 0; g < N; ++g) {
     const long long n = gp[g + 1] - gp[g];
@@ -3920,13 +3809,12 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E;
   const int64_t launches0 = h->launches;
-  HandleExtra* ex = extra_of(h);
   h->features_ready = false; h->feat_serial++;
-  const std::vector<int>& gp = ex->graph_ptr;
+  const std::vector<int>& gp = h->graph_ptr_host;
   long long max_n = 1, max_e = 1;
   for (int64_t g = 0; g < N; ++g) {
     max_n = std::max<long long>(max_n, gp[g + 1] - gp[g]);
-    max_e = std::max<long long>(max_e, ex->graph_eptr[g + 1] - ex->graph_eptr[g]);
+    max_e = std::max<long long>(max_e, h->graph_eptr_host[g + 1] - h->graph_eptr_host[g]);
   }
   // refused before any table is sized: the level matrices alone take 5 n^2 bytes per graph
   const long long ball = r > 0 ? max_n + 1 : 1;
@@ -3985,8 +3873,8 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   unsigned long long tot = 0, Mmax = 1;
   for (int t = 0; t < D1; ++t) { hb[t] = tot; tot += hc[t]; Mmax = std::max(Mmax, hc[t]); }
   if (tot >= (1ULL << 31)) return fail(GK_ERR_UNSUPPORTED, "gk_nspd_features: 2^31 or more vertex pairs");
-  ex->nspd_mask.assign(hc.begin() + D1, hc.end());
-  if (delta_mask) memcpy(delta_mask, ex->nspd_mask.data(), N * 8);
+  h->nspd_mask.assign(hc.begin() + D1, hc.end());
+  if (delta_mask) memcpy(delta_mask, h->nspd_mask.data(), N * 8);
   GK_TRY(h->nspd_pairs.ensure((size_t)std::max<unsigned long long>(tot, 1) * 8));
   unsigned* A = h->nspd_pairs.as<unsigned>();
   unsigned* Bv = A + std::max<unsigned long long>(tot, 1);
@@ -3996,14 +3884,14 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   LAUNCH_CHECK(h);
   // ---- per-level tables (delta-major), numbered with the NeighborhoodHash column passes
   const int n_lev = D1 * (r + 1);
-  ex->nspd_off.assign(n_lev, 0); ex->nspd_cap.assign(n_lev, 0); ex->nspd_M.assign(n_lev, 0); ex->nspd_cols.assign(n_lev, 0);
+  h->nspd_off.assign(n_lev, 0); h->nspd_cap.assign(n_lev, 0); h->nspd_M.assign(n_lev, 0); h->nspd_cols.assign(n_lev, 0);
   size_t blk = 0;
   for (int l = 0; l < n_lev; ++l) {
     const long long M = (long long)hc[l / (r + 1)];
-    ex->nspd_M[l] = M;
-    ex->nspd_cap[l] = (long long)std::max<size_t>(next_pow2((size_t)std::max<long long>(M, 1) * 2), 1024);
-    ex->nspd_off[l] = (long long)blk;
-    blk += nspd_level_bytes(ex->nspd_cap[l], M, N);
+    h->nspd_M[l] = M;
+    h->nspd_cap[l] = (long long)std::max<size_t>(next_pow2((size_t)std::max<long long>(M, 1) * 2), 1024);
+    h->nspd_off[l] = (long long)blk;
+    blk += nspd_level_bytes(h->nspd_cap[l], M, N);
   }
   GK_TRY(h->nspd_blk.ensure(blk));
   const size_t tcap = std::max<size_t>(next_pow2((size_t)Mmax * 2), 1024);
@@ -4021,8 +3909,8 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   GK_CUDA(cudaMemsetAsync(h->nspd_blk.p, 0, blk, h->stream));
   for (int l = 0; l < n_lev; ++l) {
     const int delta = l / (r + 1), rho = l % (r + 1);
-    const long long M = ex->nspd_M[l];
-    const size_t cap = (size_t)ex->nspd_cap[l];
+    const long long M = h->nspd_M[l];
+    const size_t cap = (size_t)h->nspd_cap[l];
     NspdLevel L = nspd_level(h, l);
     GK_CUDA(cudaMemsetAsync(L.keys, 0xFF, cap * 8, h->stream));
     if (!M) continue;
@@ -4045,7 +3933,7 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   GK_CUDA(cudaMemcpyAsync(hd.data(), dims, n_lev * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
   int64_t n_cols = 0;
-  for (int l = 0; l < n_lev; ++l) { ex->nspd_cols[l] = (long long)hd[l]; n_cols += (int64_t)hd[l]; }
+  for (int l = 0; l < n_lev; ++l) { h->nspd_cols[l] = (long long)hd[l]; n_cols += (int64_t)hd[l]; }
   h->n_columns = n_cols;
   h->features_ready = true; h->feat_serial++;
   h->feature_kind = FK_NSPD;
@@ -4053,7 +3941,7 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
     stats->n_levels = n_lev;
-    for (int l = 0; l < n_lev; ++l) stats->level_dims[l] = ex->nspd_cols[l];
+    for (int l = 0; l < n_lev; ++l) stats->level_dims[l] = h->nspd_cols[l];
     stats->n_columns = n_cols;
     stats->n_entries = (int64_t)tot;
     stats->kernel_launches = h->launches - launches0;
@@ -4102,7 +3990,6 @@ int gk_selftest_nspd_set_order(int64_t n, const int64_t* h0, const int64_t* h1, 
 // number of fitted levels, or by sqrt(levels of Y x levels of X).  Rows go in chunks when one level's count matrix of
 // the whole request would exceed 8 GiB (GRAKEL_B200_NSPD_C_BUDGET=<bytes> lowers it).
 static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
   const bool square = q.square;
   const int r1 = h->nspd_r + 1;
@@ -4110,7 +3997,7 @@ static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
   auto maxd = [&](int64_t a, int64_t b) {
     int m = -1;
     for (int64_t g = a; g < b; ++g)
-      if (ex->nspd_mask[g]) m = std::max(m, 63 - __builtin_clzll(ex->nspd_mask[g]));
+      if (h->nspd_mask[g]) m = std::max(m, 63 - __builtin_clzll(h->nspd_mask[g]));
     return m;
   };
   const int mx = maxd(0, n_fit), my = square ? mx : maxd(n_fit, N);
@@ -4137,8 +4024,8 @@ static int gram_nspd(gk_handle* h, const GramReq& q, gk_stats* stats) {
         const int l = delta * r1 + rho;
         NspdLevel L = nspd_level(h, l);
         IntBlock fb;
-        fb.keys = L.keys; fb.cnt = L.cnt; fb.cap = (size_t)ex->nspd_cap[l];
-        fb.colcnt = L.colcnt; fb.col_cap = ex->nspd_M[l] + 1; fb.n_columns = ex->nspd_cols[l];
+        fb.keys = L.keys; fb.cnt = L.cnt; fb.cap = (size_t)h->nspd_cap[l];
+        fb.colcnt = L.colcnt; fb.col_cap = h->nspd_M[l] + 1; fb.n_columns = h->nspd_cols[l];
         fb.diag = L.diag; fb.part_max = L.part; fb.part_new = L.part + 1; fb.n_part = 1;
         fb.prologue_on_host = false;
         GramReq lq;
@@ -4374,9 +4261,8 @@ int gk_core_level_add(gk_handle* h, int32_t level, int64_t n_fit, int64_t n_leve
 // identity, the self similarities, and splits the counts into one NeighborhoodSubgraphPairwiseDistance-layout table per
 // bit of C.  odd_ctl: [collision | identities | entries of plane b (32) | columns of plane b (32)] u64.
 static NspdLevel odd_plane(gk_handle* h, int b) {
-  HandleExtra* ex = extra_of(h);
-  char* p = h->odd_blk.as<char>() + ex->odd_off[b];
-  const long long cap = ex->odd_cap[b], M = ex->odd_M[b];
+  char* p = h->odd_blk.as<char>() + h->odd_off[b];
+  const long long cap = h->odd_cap[b], M = h->odd_M[b];
   NspdLevel L;
   L.keys = reinterpret_cast<unsigned long long*>(p);
   L.cnt = reinterpret_cast<unsigned*>(p + cap * 8);
@@ -4397,8 +4283,7 @@ struct OddNodes {
 };
 
 static OddNodes odd_nodes(gk_handle* h) {
-  HandleExtra* ex = extra_of(h);
-  const size_t S1 = (size_t)std::max<long long>(ex->odd_S, 1);
+  const size_t S1 = (size_t)std::max<long long>(h->odd_S, 1);
   OddNodes o;
   o.key = h->odd_nodes.as<unsigned long long>();
   o.lab = reinterpret_cast<int*>(o.key + S1);
@@ -4426,15 +4311,14 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
   GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E;
   const int64_t launches0 = h->launches;
-  HandleExtra* ex = extra_of(h);
   h->features_ready = false; h->feat_serial++;
-  const std::vector<int>& gp = ex->graph_ptr;
+  const std::vector<int>& gp = h->graph_ptr_host;
   std::vector<long long> base(2 * (N + 1), 0);
   long long* nbase = base.data();
   long long* ebase = nbase + N + 1;
   int max_n = 1;
   for (int64_t g = 0; g < N; ++g) {
-    const long long n = gp[g + 1] - gp[g], m = ex->graph_eptr[g + 1] - ex->graph_eptr[g];
+    const long long n = gp[g + 1] - gp[g], m = h->graph_eptr_host[g + 1] - h->graph_eptr_host[g];
     max_n = std::max<int>(max_n, (int)n);
     nbase[g + 1] = nbase[g] + n * n;
     ebase[g + 1] = ebase[g] + n * m;
@@ -4447,7 +4331,7 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
   if (S >= (1LL << 30) || T >= (1LL << 30))
     return fail(GK_ERR_UNSUPPORTED, std::string(who) + ": 2^30 or more (root, vertex) or (root, edge) pairs" +
                                          (n_levels > 1 ? " over all WL levels" : ""));
-  ex->odd_S = S; ex->odd_T = T; ex->odd_maxC = 0;
+  h->odd_S = S; h->odd_T = T; h->odd_maxC = 0;
   const size_t S1 = (size_t)std::max<long long>(S, 1), T1 = (size_t)std::max<long long>(T, 1);
   const size_t cap = std::max<size_t>(next_pow2(S1 * 2), 1024);
   const size_t LV = (size_t)n_levels * (size_t)V;
@@ -4539,26 +4423,26 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
   GK_CUDA(cudaMemcpyAsync(hc.data(), ctl, ODD_CTL_WORDS * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
   const long long F = (long long)hc[1];
-  ex->odd_F = F;
+  h->odd_F = F;
   int B = 0;
   for (int b = 0; b < 32; ++b)
     if (hc[2 + b]) B = b + 1;
-  ex->odd_off.assign(B, 0); ex->odd_cap.assign(B, 0); ex->odd_M.assign(B, 0); ex->odd_cols.assign(B, 0);
+  h->odd_off.assign(B, 0); h->odd_cap.assign(B, 0); h->odd_M.assign(B, 0); h->odd_cols.assign(B, 0);
   size_t blk = 0;
   for (int b = 0; b < B; ++b) {
     const long long M = (long long)hc[2 + b];
-    ex->odd_M[b] = M;
-    ex->odd_cap[b] = (long long)std::max<size_t>(next_pow2((size_t)std::max<long long>(M, 1) * 2), 1024);
-    ex->odd_off[b] = (long long)blk;
-    blk += nspd_level_bytes(ex->odd_cap[b], M, N);
+    h->odd_M[b] = M;
+    h->odd_cap[b] = (long long)std::max<size_t>(next_pow2((size_t)std::max<long long>(M, 1) * 2), 1024);
+    h->odd_off[b] = (long long)blk;
+    blk += nspd_level_bytes(h->odd_cap[b], M, N);
   }
   GK_TRY(h->odd_blk.ensure(std::max<size_t>(blk, 256)));
   if (blk) GK_CUDA(cudaMemsetAsync(h->odd_blk.p, 0, blk, h->stream));
   for (int b = 0; b < B; ++b) {
     const NspdLevel L = odd_plane(h, b);
-    const size_t pcap = (size_t)ex->odd_cap[b];
+    const size_t pcap = (size_t)h->odd_cap[b];
     GK_CUDA(cudaMemsetAsync(L.keys, 0xFF, pcap * 8, h->stream));
-    if (!ex->odd_M[b]) continue;
+    if (!h->odd_M[b]) continue;
     odd_plane_cols<<<cdiv(F, 256), 256, 0, h->stream>>>((int)F, reinterpret_cast<unsigned*>(o.Cf), b, o.colb, ctl + 34 + b);
     LAUNCH_CHECK(h);
     odd_plane_fill<<<cdiv((long long)cap, 256), 256, 0, h->stream>>>(cap, phi_keys, phi_cnt, reinterpret_cast<unsigned*>(o.Cf),
@@ -4570,7 +4454,7 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
   GK_CUDA(cudaEventRecord(h->tev[3], h->stream));
   GK_CUDA(cudaMemcpyAsync(hc.data() + 34, ctl + 34, 32 * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_CUDA(cudaStreamSynchronize(h->stream));
-  for (int b = 0; b < B; ++b) ex->odd_cols[b] = (long long)hc[34 + b];
+  for (int b = 0; b < B; ++b) h->odd_cols[b] = (long long)hc[34 + b];
   h->n_columns = F;
   h->features_ready = true; h->feat_serial++;
   h->feature_kind = FK_ODD;
@@ -4578,7 +4462,7 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
     stats->n_levels = B;
-    for (int b = 0; b < B; ++b) stats->level_dims[b] = ex->odd_cols[b];
+    for (int b = 0; b < B; ++b) stats->level_dims[b] = h->odd_cols[b];
     stats->n_columns = F;
     stats->n_entries = S;
     stats->hash_retries = retries;
@@ -4634,8 +4518,7 @@ static int odd_host_signatures(gk_handle* h, std::vector<int>* label, std::vecto
                                std::vector<int>* C) {
   if (h->feature_kind != FK_ODD || !h->features_ready) return fail(GK_ERR_STATE, "gk_odd_signatures: run gk_odd_features first");
   GK_CUDA(cudaSetDevice(h->dev));
-  HandleExtra* ex = extra_of(h);
-  const long long S = ex->odd_S, T = ex->odd_T, F = ex->odd_F;
+  const long long S = h->odd_S, T = h->odd_T, F = h->odd_F;
   const OddNodes o = odd_nodes(h);
   std::vector<int> lab(S), cb(S), nc(S), fid(S), ch(T), rep_of(F);
   C->resize(F);
@@ -4701,9 +4584,8 @@ int gk_odd_signatures(gk_handle* h, int32_t* label, int64_t* child_off, int32_t*
 // ydiag.  Rows go in chunks when one plane's count matrix of the whole request would exceed 8 GiB
 // (GRAKEL_B200_ODD_C_BUDGET=<bytes> lowers it).
 static int gram_odd(gk_handle* h, const GramReq& q, gk_stats* stats) {
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, n_fit = q.n_fit, k_rows = q.k_rows, k_cols = q.k_cols;
-  const int B = (int)ex->odd_M.size();
+  const int B = (int)h->odd_M.size();
   const int64_t launches0 = h->launches;
   F64Out out;
   GK_TRY(f64_target(h, q, &out));
@@ -4722,11 +4604,11 @@ static int gram_odd(gk_handle* h, const GramReq& q, gk_stats* stats) {
     double* o = out.p + (size_t)(cb - q.row_begin) * out.ld;
     GK_CUDA(cudaMemset2DAsync(o, (size_t)out.ld * 8, 0, (size_t)k_cols * 8, (size_t)rows, h->stream));
     for (int b = 0; b < B; ++b) {
-      if (!ex->odd_M[b]) continue;
+      if (!h->odd_M[b]) continue;
       const NspdLevel L = odd_plane(h, b);
       IntBlock fb;
-      fb.keys = L.keys; fb.cnt = L.cnt; fb.cap = (size_t)ex->odd_cap[b];
-      fb.colcnt = L.colcnt; fb.col_cap = ex->odd_M[b] + 1; fb.n_columns = ex->odd_cols[b];
+      fb.keys = L.keys; fb.cnt = L.cnt; fb.cap = (size_t)h->odd_cap[b];
+      fb.colcnt = L.colcnt; fb.col_cap = h->odd_M[b] + 1; fb.n_columns = h->odd_cols[b];
       fb.diag = L.diag; fb.part_max = L.part; fb.part_new = L.part + 1; fb.n_part = 1;
       fb.prologue_on_host = false;
       GramReq lq;
@@ -4842,11 +4724,10 @@ int gk_ml_begin(gk_handle* h, int32_t L, double gamma, double heta, const double
     return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: a graph of more than 128 vertices (the neighbourhood matrix lives in "
                                     "shared memory)");
   GK_CUDA(cudaSetDevice(h->dev));
-  HandleExtra* ex = extra_of(h);
   const int64_t N = h->N, V = h->V;
   std::vector<long long> off(N + 1, 0);
   for (int64_t g = 0; g < N; ++g) {
-    const long long n = ex->graph_ptr[g + 1] - ex->graph_ptr[g];
+    const long long n = h->graph_ptr_host[g + 1] - h->graph_ptr_host[g];
     off[g + 1] = off[g] + n * n;
   }
   GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
@@ -5356,7 +5237,7 @@ int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int
   const int64_t n_new = N - g0, S = samp_off[n_new];
   if (samp_off[0] != 0 || S < 0 || (S && !samp_size)) return fail(GK_ERR_ARG, "gk_gs_features: bad sample offsets");
   // every check on the host arguments before the first launch (the drawn indexes are checked on the device)
-  const std::vector<int>& gp = extra_of(h)->graph_ptr;
+  const std::vector<int>& gp = h->graph_ptr_host;
   std::vector<long long> ioff(n_new + 1, 0);
   std::vector<long long> per_graph(n_new, 0);
   for (int64_t w = 0; w < n_new; ++w) {
@@ -5673,14 +5554,14 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   if (dev_out && (((uintptr_t)K_out) % 16 != 0 || ((ld > 0 ? ld : N) * 4) % 16 != 0)) return GK_OK;
   // panel type: u8 unless the switch is off or the last Gram on this handle saw a count of 256 (the device checks the
   // counts of THIS pass against the type and sends it to the synchronous route if one does not fit)
-  const int elem_bytes = (u8_panel_enabled() && extra_of(h)->last_max_count <= 255) ? 1 : 2;
+  const int elem_bytes = (u8_panel_enabled() && h->last_max_count <= 255) ? 1 : 2;
   const int bk = panel_bk(elem_bytes);
   // capacities left by earlier passes, reasoned in bytes (passes of either panel type share the buffer): row pitch
   // S_bytes, a whole number of 128-byte k-blocks
   int64_t S_bytes = (int64_t)(h->panel.cap / (size_t)N) / 128 * 128;
   {  // no wider than the last cost-model pass needed, plus a quarter (a dense-all pass may have left a much larger buffer,
      // and the whole pitch is zeroed)
-    const long long want = extra_of(h)->head_row_bytes;
+    const long long want = h->head_row_bytes;
     if (!(flags & GK_DENSE_ALL) && !getenv("GRAKEL_B200_FORCE_T") && want > 0)
       S_bytes = std::min<int64_t>(S_bytes, (want + want / 4 + 127) / 128 * 128 + 128);
   }
@@ -5696,7 +5577,6 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   WlPlan pl;
   GK_TRY(wl_setup(h, n_iter, &pl));
   if (!pl.fused) return GK_OK;
-  HandleExtra* hx = extra_of(h);
   const int64_t D = (int64_t)h->n_labels0 + V * (int64_t)(L - 1);
   FeatStats fst;
   GK_TRY(reset_feature_stats(h, D + 1, (int64_t)std::max(pl.nb, pl.G) * L, &fst, false));
@@ -5742,18 +5622,18 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   // tile list (same key as gk_gram's)
   {
     const long long tkey[8] = {0, 0, (long long)N, 0, (long long)N, 1, BM2, 0};
-    if (memcmp(tkey, hx->tiles_key, sizeof(tkey)) != 0 || !h->tiles.p) {
+    if (memcmp(tkey, h->tiles_key, sizeof(tkey)) != 0 || !h->tiles.p) {
       std::vector<int2> tiles;
       build_tiles(tiles, 0, (int)N, 0, (int)N, true, BM2);
       GK_TRY(h->h_tiles.ensure(tiles.size() * sizeof(int2) + 16));
       memcpy(h->h_tiles.p, tiles.data(), tiles.size() * sizeof(int2));
       GK_TRY(h->tiles.ensure(tiles.size() * sizeof(int2) + 16));
       GK_CUDA(cudaMemcpyAsync(h->tiles.p, h->h_tiles.p, tiles.size() * sizeof(int2), cudaMemcpyHostToDevice, h->stream));
-      memcpy(hx->tiles_key, tkey, sizeof(tkey));
-      hx->tiles_n = (long long)tiles.size();
+      memcpy(h->tiles_key, tkey, sizeof(tkey));
+      h->tiles_n = (long long)tiles.size();
     }
   }
-  const int64_t n_tiles = hx->tiles_n;
+  const int64_t n_tiles = h->tiles_n;
   CUtensorMap tmA, tmC;
   PeerMaps peer_maps;
   memset(&peer_maps, 0, sizeof(peer_maps));
@@ -5877,10 +5757,10 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   h->features_ready = true; h->feat_serial++;
   h->feature_kind = FK_WL;
   h->Dc = hd.Dc; h->Dc_pad = hd.Dc_pad;
-  if (force_T < 0) hx->head_row_bytes = (long long)hd.Dc_pad * elem_bytes;
-  hx->last_max_count = (long long)hd.max_count;
-  hx->pro_hist = hd.hist;
-  hx->pro_max_count = (long long)hd.max_count; hx->pro_max_diag = (long long)hd.max_diag; hx->pro_n_entries = (long long)hd.n_entries;
+  if (force_T < 0) h->head_row_bytes = (long long)hd.Dc_pad * elem_bytes;
+  h->last_max_count = (long long)hd.max_count;
+  h->pro_hist = hd.hist;
+  h->pro_max_count = (long long)hd.max_count; h->pro_max_diag = (long long)hd.max_diag; h->pro_n_entries = (long long)hd.n_entries;
   h->pro_serial = h->feat_serial;
   if (stats) {
     memset(stats, 0, sizeof(*stats));
@@ -6038,8 +5918,14 @@ int gk_selftest_gram(gk_handle* h, int64_t n, int64_t d, const uint16_t* counts,
     GK_CUDA(cudaStreamSynchronize(h->stream));
     GK_CUDA(cudaMemcpy(out_simt, dk2.p, (size_t)n * n * 8, cudaMemcpyDeviceToHost));
   }
-  dpb.release(); dpu.release(); ddg.release(); dk1.release(); dk2.release(); dtl.release();
   return rc;
+}
+
+int gk_selftest_live_bytes(int64_t* device, int64_t* pinned) {
+  if (!device || !pinned) return fail(GK_ERR_ARG, "gk_selftest_live_bytes: null argument");
+  *device = g_live_bytes[0];
+  *pinned = g_live_bytes[1];
+  return GK_OK;
 }
 
 }  // extern "C"

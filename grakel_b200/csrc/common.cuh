@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 
+#include <atomic>
 #include <cstddef>
 #include <cstdint>
 #include <cstdio>
@@ -39,54 +40,60 @@ inline int fail(int code, const std::string& msg) {
   } while (0)
 
 // ---------------------------------------------------------------- buffers
-// Grow-only device buffer: the engine is called repeatedly on same-sized
-// workloads (bench loop, fit then transform), so capacity is kept between calls.
-struct DevBuf {
+// Bytes held by every DevBuf [0] / PinBuf [1] of the process; read by gk_selftest_live_bytes only.
+extern std::atomic<int64_t> g_live_bytes[2];
+
+// Grow-only buffer that owns its allocation: device memory (DevBuf) or pinned host staging (PinBuf: D2H of small
+// scalars, H2D of CSR).  The engine is called repeatedly on same-sized workloads (bench loop, fit then transform), so
+// capacity is kept between calls; the allocation is freed with the buffer.  Moves leave the source empty; a copy
+// would free the allocation twice, so there is none.
+template <bool Pinned>
+struct Buf {
   void* p = nullptr;
   size_t cap = 0;
+  Buf() = default;
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  Buf(Buf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  Buf& operator=(Buf&& o) noexcept {
+    if (this != &o) {
+      free_block();
+      p = o.p; cap = o.cap;
+      o.p = nullptr; o.cap = 0;
+    }
+    return *this;
+  }
+  ~Buf() { free_block(); }
   int ensure(size_t bytes) {
     if (bytes <= cap) return GK_OK;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = bytes + (bytes >> 3) + 256;
-    cudaError_t e = cudaMalloc(&p, want);
+    free_block();
+    const size_t want = Pinned ? bytes + 256 : bytes + (bytes >> 3) + 256;
+    cudaError_t e = Pinned ? cudaMallocHost(&p, want) : cudaMalloc(&p, want);
     if (e != cudaSuccess) {
-      return fail(GK_ERR_CUDA, std::string("cudaMalloc(") + std::to_string(want) + "): " + cudaGetErrorString(e));
+      p = nullptr;
+      return fail(GK_ERR_CUDA, std::string(Pinned ? "cudaMallocHost(" : "cudaMalloc(") + std::to_string(want) +
+                                   "): " + cudaGetErrorString(e));
     }
     cap = want;
+    g_live_bytes[Pinned] += (int64_t)cap;
     return GK_OK;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
   }
   template <class T>
   T* as() const { return reinterpret_cast<T*>(p); }
-};
 
-struct PinBuf {  // pinned host staging (D2H of small scalars, H2D of CSR)
-  void* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t bytes) {
-    if (bytes <= cap) return GK_OK;
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
-    cudaError_t e = cudaMallocHost(&p, bytes + 256);
-    if (e != cudaSuccess) return fail(GK_ERR_CUDA, std::string("cudaMallocHost: ") + cudaGetErrorString(e));
-    cap = bytes + 256;
-    return GK_OK;
-  }
-  void release() {
-    if (p) cudaFreeHost(p);
+ private:
+  void free_block() {
+    if (p) {
+      if (Pinned) cudaFreeHost(p);
+      else cudaFree(p);
+      g_live_bytes[Pinned] -= (int64_t)cap;
+    }
     p = nullptr;
     cap = 0;
   }
-  template <class T>
-  T* as() const { return reinterpret_cast<T*>(p); }
 };
+using DevBuf = Buf<false>;
+using PinBuf = Buf<true>;
 
 constexpr unsigned long long EMPTY64 = ~0ULL;
 constexpr int MAX_LEVELS = 64;
@@ -111,6 +118,20 @@ struct DevScalars {
 };
 
 static_assert(sizeof(DevScalars) % 8 == 0, "cleared as 64-bit words");
+
+constexpr int HIST_BUCKETS = 16;        // bucket b: 2^(b-1) < m <= 2^b ; last = saturated
+
+struct ColStats {           // device-side, zeroed per gk_gram
+  unsigned long long hist_cols[HIST_BUCKETS];
+  unsigned long long hist_work[HIST_BUCKETS];
+  unsigned long long hist_entries[HIST_BUCKETS];  // sum of m over the bucket's columns
+  long long n_dense;        // D_c (head columns)
+  long long n_tail_cols;
+  long long n_tail_entries;
+  long long tail_work;      // pair updates the tail kernel performs
+  int T;                    // chosen threshold
+  int pad;
+};
 
 // What the handle's feature block holds, i.e. which gk_gram route computes K from it.
 enum FeatureKind : int {
@@ -151,6 +172,8 @@ struct gk_handle {
   int32_t attr_dim = 0;
   int32_t max_degree = 0, max_graph_size = 0;
   gk::DevBuf graph_ptr, row_ptr, col_idx, labels0, weights, attrs, vgraph;
+  std::vector<int> graph_ptr_host;
+  std::vector<int> graph_eptr_host;  // first edge of each graph (row_ptr[graph_ptr[g]])
   bool has_labels = false;  // the current block was packed with vertex labels (labels0 may hold an older block's)
   gk::DevBuf sp_lists;      // graph lists of the shortest-path launches (kept apart from large_list: gk_wl_features reads that)
   gk::DevBuf large_list;  // vertices with degree > group width
@@ -166,6 +189,11 @@ struct gk_handle {
   size_t ht_cap = 0;
   gk::DevBuf flags, block_sums;
   gk::DevBuf wlf_buf;  // fused WL kernel: [tile_vbeg (T+1) | cta_tile (G+1) | barrier]
+  // fused WL kernel: the tile partition of the packed block (device copy in wlf_buf) is kept between calls
+  bool wl_tiles_valid = false;
+  bool wl_tiles_fused = false;
+  int wl_n_tiles = 0;
+  long long wl_tiles_key = -1;  // GRAKEL_B200_WL_TILES_PER_CTA the partition was built with
   gk::DevBuf wl_payload;  // fused WL kernel: [2][ht_cap] 32-byte slot payloads (the installing vertex's signature)
   gk::DevBuf wl_single;  // fused WL kernel: one byte per vertex (frozen flag)
   gk::DevBuf diag_frozen;  // fused WL kernel: frozen vertices' share of the self similarities (u64 per graph)
@@ -182,6 +210,9 @@ struct gk_handle {
   int64_t pro_serial = -1;   // feat_serial for which gk_wl_features already ran the Gram prologue (square case):
                              // self similarities finished, column histogram on the host -- gk_gram then needs no
                              // host synchronisation before its launches
+  // the Gram prologue's results that gk_gram would otherwise read back after a synchronisation
+  gk::ColStats pro_hist;
+  long long pro_max_count = 0, pro_max_diag = 0, pro_n_entries = 0;
   gk::FeatureKind feature_kind = gk::FK_NONE;
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
@@ -208,6 +239,7 @@ struct gk_handle {
   gk::DevBuf sp_dkeys;     // real-valued weights: dictionary of distance bit patterns
   size_t sp_dict_cap = 0;
   gk::DevBuf sp_graph_off; // per-graph offset into sp_dist (for gk_sp_distances)
+  std::vector<long long> sp_goff;  // its host copy
   int sp_flags = 0;
   int sp_dist_esz = 0;     // gk_spattr_features: element size of the matrices it left in sp_dist (2 = u16, 8 = fp64)
 
@@ -229,6 +261,7 @@ struct gk_handle {
   size_t nh_level_bytes = 0;
   int64_t nh_level_cap = 0;       // entries (and columns) one level's expanded block can hold
   int nh_R = 0;
+  std::vector<long long> nh_dims, nh_cols, nh_entries;  // per level: distinct codes, columns and entries of its block
 
   // ---- PyramidMatch (FK_PM): the levels live in the NeighborhoodHash buffers above (nh_codes / nh_valid hold the
   // current level's keys, nh_blk the expanded blocks, pm_S * pm_L of them); the embeddings [S][V][d] fp64 and the
@@ -252,6 +285,10 @@ struct gk_handle {
   // column) count tables and the fp64 count matrix of one level
   gk::DevBuf nspd_lvl, nspd_q, nspd_H, nspd_aux, nspd_ws, nspd_pairs, nspd_blk, nspd_tab, nspd_keys, nspd_C;
   int nspd_r = 0, nspd_d = 0;
+  // per level (delta-major): its table's byte offset in nspd_blk, slots, pairs and columns; per graph, the mask of the
+  // distances it has pairs at
+  std::vector<long long> nspd_off, nspd_cap, nspd_M, nspd_cols;
+  std::vector<unsigned long long> nspd_mask;
 
   // ---- WL over a base kernel whose levels cannot share one feature block (gk_wl_level_sum): the running fp64 sum of
   // the levels' K and the K of the current level; shape and square-ness of the sum, levels added so far.  No re-pack or
@@ -287,6 +324,10 @@ struct gk_handle {
   // column), the (graph, identity) counts, the bit-plane tables, counters, self similarities
   gk::DevBuf odd_aux, odd_nodes, odd_ch, odd_tab, odd_feat, odd_phi, odd_blk, odd_ctl, odd_diag;
   int odd_degen = 0;  // gk_selftest_odd_collision: degenerate identity passes still to come
+  // node slots, child slots, identities; per bit plane of C, its table's byte offset in odd_blk, slots, entries and
+  // columns
+  long long odd_S = 0, odd_T = 0, odd_F = 0, odd_maxC = 0;
+  std::vector<long long> odd_off, odd_cap, odd_M, odd_cols;
 
   // ---- MultiscaleLaplacian (FK_ML): dense per-graph adjacency and its offsets, radius-l ball masks [L][V][2], the
   // features of the current level and their successor, vertex records [V][P' P' + 1], the sample records of the current
@@ -318,7 +359,13 @@ struct gk_handle {
   int pk_levels = 0, pk_K = 0;
 
   // ---- GEMM
-  gk::DevBuf tiles;  // int2 list
+  gk::DevBuf tiles;  // int2 list: rebuilt and uploaded only when its key changes
+  long long tiles_key[8] = {-1, -1, -1, -1, -1, -1, -1, -1};
+  long long tiles_n = 0;
+  long long head_row_bytes = 0;  // panel row width (bytes) of the last pass whose threshold came from the cost model
+                                 // (not GK_DENSE_ALL / FORCE_T)
+  long long last_max_count = 0;  // largest count of the last Gram on this handle: an asynchronous pass fills a u8 panel
+                                 // unless it was 256 (a count of 256 repeats through the synchronous route once)
   gk::PinBuf h_tiles;
   gk::PinBuf h_bands;  // band table of the u16 result transport (its own buffer: h_tiles may still feed an async copy)
   gk::DevBuf K;      // device-resident result of the last gk_gram
@@ -330,4 +377,20 @@ struct gk_handle {
   gk::PinBuf h_diag;   // self similarities on the host (normalisation during the widening)
   int64_t launches = 0;
   void* comm = nullptr;  // gk::Comm (comm.h) after gk_comm_init
+
+  // Runs before any member is destroyed: the communicator's collective teardown (every peer unmaps this handle's
+  // exported blocks) completes before the buffers free themselves.  The null checks keep a partly built handle from
+  // leaving an error behind for the next cudaGetLastError on this thread.
+  ~gk_handle() {
+    cudaSetDevice(dev);
+    if (stream) cudaStreamSynchronize(stream);
+    gk_comm_destroy(this);
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : tev) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ev_stage) if (e) cudaEventDestroy(e);
+    if (ev_fork) cudaEventDestroy(ev_fork);
+    if (ev_join) cudaEventDestroy(ev_join);
+    if (stream) cudaStreamDestroy(stream);
+    if (stream2) cudaStreamDestroy(stream2);
+  }
 };

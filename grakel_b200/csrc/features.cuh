@@ -22,20 +22,6 @@
 
 namespace gk {
 
-constexpr int HIST_BUCKETS = 16;        // bucket b: 2^(b-1) < m <= 2^b ; last = saturated
-
-struct ColStats {           // device-side, zeroed per gk_gram
-  unsigned long long hist_cols[HIST_BUCKETS];
-  unsigned long long hist_work[HIST_BUCKETS];
-  unsigned long long hist_entries[HIST_BUCKETS];  // sum of m over the bucket's columns
-  long long n_dense;        // D_c (head columns)
-  long long n_tail_cols;
-  long long n_tail_entries;
-  long long tail_work;      // pair updates the tail kernel performs
-  int T;                    // chosen threshold
-  int pad;
-};
-
 // Decisions of one ASYNCHRONOUS pass, taken on the device (gram_choose) so that the host never waits between the
 // feature kernels and the GEMM: the head/tail threshold and everything that follows from it.  `bad` != 0: the pass
 // cannot be finished this way (see the bits) -- the remaining kernels then do no harm and the host repeats the pass

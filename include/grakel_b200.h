@@ -633,6 +633,10 @@ int gk_profiler_range(int32_t on);
 int gk_selftest_gram(gk_handle* h, int64_t n, int64_t d, const uint16_t* counts, double* out_tc,
                      double* out_simt);
 
+/* Bytes of device memory and of pinned host memory the library's buffers hold right now, over every handle of the
+ * process (tests only: a handle's create-use-destroy cycle must return both to where they were). */
+int gk_selftest_live_bytes(int64_t* device, int64_t* pinned);
+
 /* ---- float64 result buffers on the host (the reference returns a fresh float64 ndarray, kernel.py:167-204).
  * gk_host_alloc maps `bytes` of anonymous memory with transparent huge pages requested; gk_host_free returns
  * the block to a small per-process pool (GRAKEL_B200_HOST_POOL_MB, default 2048; 0 = unmap at once), so a loop
