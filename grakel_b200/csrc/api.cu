@@ -2823,27 +2823,28 @@ int gk_pk_hashes(gk_handle* h, int32_t level, double* out, uint8_t* priv) {
 }
 
 // Launch rw_pairs over `n_pairs` pairs: the iteration vectors in shared memory when `vec_elems` doubles fit, else in
-// a global workspace slice per CTA.
+// a global workspace slice per CTA.  The workspace holds one slice per CTA of the clamped grid and at most 896 MiB of
+// slices (1 GiB with DevBuf's growth slack): fewer CTAs, down to one, when a slice is large.
 static int rw_launch(gk_handle* h, RwParams p, size_t vec_elems) {
   if (p.n_pairs <= 0) return GK_OK;
   const size_t bytes = vec_elems * 8;
-  int grid;
+  long long grid;
   size_t smem = 0;
   if (bytes <= RW_SMEM_MAX) {
     smem = bytes;
     GK_CUDA(cudaFuncSetAttribute(rw_pairs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
     int per_sm = 0;
     GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rw_pairs, RW_THREADS, smem));
-    grid = h->sm_count * std::max(per_sm, 1);
+    grid = std::min<long long>((long long)h->sm_count * std::max(per_sm, 1), p.n_pairs);
     p.ws = nullptr;
   } else {
-    grid = h->sm_count * 2;
+    grid = std::min<long long>((long long)h->sm_count * 2, p.n_pairs);
+    grid = std::min(grid, std::max<long long>(1, (long long)((size_t)(896 << 20) / bytes)));
     GK_TRY(h->rw_ws.ensure((size_t)grid * bytes));
     p.ws = h->rw_ws.as<double>();
     p.ws_stride = (long long)vec_elems;
   }
-  grid = (int)std::min<long long>(grid, p.n_pairs);
-  rw_pairs<<<grid, RW_THREADS, smem, h->stream>>>(p);
+  rw_pairs<<<(int)grid, RW_THREADS, smem, h->stream>>>(p);
   LAUNCH_CHECK(h);
   return GK_OK;
 }

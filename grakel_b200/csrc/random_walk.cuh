@@ -190,9 +190,12 @@ __device__ double rw_max_row_sum(const RwParams& P, int g, double* red, int& par
   return m;
 }
 
-// sum_k c_k 1^T M^k 1.  Finite p: c_k = coef[k], k <= p.  Taylor (fn == RW_FN_EXP): c_k = lamda^k / k!, stopped once
-// k >= 2 lamda R_i R_j (R = largest row sum; every later term is then at most half the one before, as
-// 1^T M^{k+1} 1 <= R_i R_j 1^T M^k 1 for non-negative M) and the term is below 2^-56 of the partial sum.
+// sum_k c_k 1^T M^k 1.  Finite p: c_k = coef[k], k <= p, the vector s_k = M^k 1.  Taylor (fn == RW_FN_EXP):
+// c_k = lamda^k / k! is carried in the vector, s_k = (lamda / k) M^T s_{k-1}, and the term is 1^T s_k.  M^k 1 alone
+// grows like rho(M)^k and overflows on a hub graph while lamda^k / k! underflows, long before the stopping bound
+// (0 * inf = NaN); s_k stays finite whenever the sum is.  The series stops once k >= 2 lamda R_i R_j (R = largest row
+// sum; every later term is then at most half the one before, as 1^T s_{k+1} <= lamda R_i R_j / (k + 1) 1^T s_k for
+// non-negative M) and the term is below 2^-56 of the partial sum, or once s_k underflows to 0.
 __device__ double rw_pair_series(const RwParams& P, int gi, int gj, double* buf, double* red, int& parity, int* iters) {
   const int a0 = P.graph_ptr[gi], ni = P.graph_ptr[gi + 1] - a0;
   const int b0 = P.graph_ptr[gj], nj = P.graph_ptr[gj + 1] - b0;
@@ -205,25 +208,26 @@ __device__ double rw_pair_series(const RwParams& P, int gi, int gj, double* buf,
   const bool taylor = P.fn == RW_FN_EXP;
   double kmin = 0.0;
   if (taylor) kmin = 2.0 * P.lamda * rw_max_row_sum(P, gi, red, parity) * rw_max_row_sum(P, gj, red, parity);
-  double c = taylor ? 1.0 : P.coef[0];
-  double S = c * (double)mn;
+  double S = (taylor ? 1.0 : P.coef[0]) * (double)mn;
   const int kmax = taylor ? RW_TAYLOR_CAP : P.n_coef - 1;
   int k = 1;
   for (; k <= kmax; ++k) {
     __syncthreads();
+    const double f = taylor ? P.lamda / (double)k : 1.0;
     double tot[1] = {0.0};
     for (int e = threadIdx.x; e < mn; e += RW_THREADS) {
-      const double v = rw_matvec_series(P, a0, b0, ni, e % ni, e / ni, s);
+      const double v = f * rw_matvec_series(P, a0, b0, ni, e % ni, e / ni, s);
       t[e] = v;
       tot[0] += v;
     }
     rw_block_sum<1>(tot, red, parity);
-    c = taylor ? c * P.lamda / (double)k : P.coef[k];
-    const double term = c * tot[0];
+    const double term = taylor ? tot[0] : P.coef[k] * tot[0];
     S += term;
     double* x = s; s = t; t = x;
     if (taylor && (double)k >= kmin && fabs(term) < 0x1p-56 * fabs(S)) break;
-    if (tot[0] == 0.0 && taylor) break;  // M^k 1 = 0: every later term is 0
+    // s_k = 0 (M^k 1 = 0, or the scaled terms fell below the smallest subnormal): every later term is 0, or at most
+    // that small times n_i n_j against S >= n_i n_j
+    if (tot[0] == 0.0 && taylor) break;
   }
   if (taylor && k > kmax && threadIdx.x == 0) atomicAdd(P.cap_hits, 1ull);
   *iters = k > kmax ? kmax : k;

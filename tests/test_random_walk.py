@@ -69,6 +69,28 @@ def test_series_and_spectral_oracle_match_reference():
             assert abs(s / np.sqrt(d[i] * d[j]) - K[i, j]) <= 1e-12 * mag / np.sqrt(abs(d[i] * d[j]))
 
 
+def test_taylor_series_scaled_vector_on_hub_graphs():
+    """The device's Taylor series restated: with M^k 1 and lamda^k / k! kept apart, M^k 1 overflows on a hub graph
+    while lamda^k / k! underflows, their product is NaN and the series runs to its term cap; carrying the scaled vector
+    lamda^k / k! M^k 1 sums every case to within 1e-11 of 1^T expm(lamda M) 1 (dense expm where kron(A, A) has at most
+    3 600 rows, the eigh form above that)."""
+    for name, A in O.hub_graphs().items():
+        ref = O.expm_pair(A, A, 0.1) if A.shape[0] <= 60 else O.symmetric_expm_pair(A, A, 0.1)
+        S, terms, capped = O.device_taylor(A, A, 0.1, scaled=True)
+        assert not capped and abs(S - ref) <= 1e-11 * ref, (name, S, ref, terms)
+        S0, _, capped0 = O.device_taylor(A, A, 0.1, scaled=False)
+        if name == "K21":
+            assert not capped0 and abs(S0 - ref) <= 1e-11 * ref
+        else:
+            assert capped0 and np.isnan(S0), name
+    # the oracle's own series (taylor_pair) agrees with expm on a hub pair and on a labelled pair
+    A, B = O.hub_graphs()["K21"], O.hub_graphs()["hub60"][:30, :30]
+    assert abs(O.taylor_pair(A, B, 0.1) - O.expm_pair(A, B, 0.1)) <= 1e-11 * O.expm_pair(A, B, 0.1)
+    La, Lb = [i % 3 for i in range(21)], [i % 2 for i in range(30)]
+    ref = O.expm_pair(A, B, 0.1, La, Lb)
+    assert abs(O.taylor_pair(A, B, 0.1, La, Lb) - ref) <= 1e-12 * ref
+
+
 def test_validation_order_and_errors():
     with pytest.raises(ValueError, match="method_type"):
         RandomWalk(method_type="x", kernel_type="y").initialize()
