@@ -86,6 +86,8 @@ _SYMBOLS = {
     "gk_sm_wl_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int32,
                                     C.POINTER(GkStats)]),
     "gk_sm_wl_counts": (C.c_int, [_P, C.c_int64, C.c_int64, _P]),
+    "gk_sm_hc_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, _P, C.c_int32, _P, C.c_int32,
+                                    C.POINTER(GkStats)]),
     "gk_odd_features": (C.c_int, [_P, C.c_int32, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_wl_odd_features": (C.c_int, [_P, C.c_int32, C.c_int32, _P, _P, C.c_int32, C.POINTER(GkStats)]),
     "gk_wl_level_sum": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.POINTER(GkStats)]),
@@ -478,6 +480,21 @@ class Engine:
         with self._lock:
             self._check(self.lib.gk_sm_wl_counts(self.h, int(n_fit), int(row), _ptr(out)))
         return out
+
+    def sm_hc_features(self, k, n_iter, level_ids, lambdas, etable=None, edge_label=None, flags=0):
+        """HadamardCode over SubgraphMatching (gk_sm_hc_features): level_ids [V, n_iter] the HadamardCode class of
+        every packed vertex per level (None with GK_SM_KV_NONE); the next gram() returns the level sum in one
+        enumeration."""
+        lam = np.ascontiguousarray(lambdas, dtype=np.float64).ravel()
+        et = None if etable is None else np.ascontiguousarray(etable, dtype=np.float64)
+        el = None if edge_label is None else _i32(edge_label)
+        ids = None if level_ids is None else _i32(level_ids)
+        st = GkStats()
+        with self._lock:
+            self._check(self.lib.gk_sm_hc_features(self.h, int(k), int(n_iter), _ptr(ids), _ptr(lam), _ptr(et),
+                                                   0 if et is None else et.shape[0], _ptr(el), int(flags),
+                                                   C.byref(st)))
+        return st
 
     def ml_begin(self, L, gamma, heta, phi):
         """MultiscaleLaplacian: adjacency, balls and level-0 features phi [V, dim] of the packed block (gk_ml_begin)."""

@@ -2962,6 +2962,7 @@ int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double*
   if (kk > SM_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: subgraphs of more than 32 vertices");
   GK_CUDA(cudaSetDevice(h->dev));
   h->sm_n_lv = 0;
+  h->sm_hc = false;
   const int64_t N = h->N;
   const bool elab = ke != SM_W_NONE;
   std::vector<long long> off(N + 1, 0);
@@ -3017,7 +3018,7 @@ static int sm_launch(gk_handle* h, SmParams p) {
   p.stack_cap = cap;
   const size_t tab_bytes = ((p.kv == SM_W_TABLE ? (size_t)p.n_vl * p.n_vl : 0) +
                             (p.ke == SM_W_TABLE ? (size_t)p.n_el * p.n_el : 0)) * 8;
-  // sm_wl_pairs' (depth, size) bins: per warp when exact, per lane when real
+  // sm_wl_pairs' (depth, size) and sm_mask_pairs' (level, size) bins: per warp when exact, per lane when real
   const size_t bin_bytes = p.n_lv == 0 ? 0 : (size_t)p.n_lv * p.kk * 8 * (p.exact ? 2 * SM_WARPS : SM_THREADS);
   const long long pair_words = 2 * sm_record_words(nmax, p.ke != SM_W_NONE);
   // GRAKEL_B200_SM_GLOBAL=1 reads every record from global memory (the route of pairs too large to stage)
@@ -3026,7 +3027,7 @@ static int sm_launch(gk_handle* h, SmParams p) {
       !(e_glob && atoi(e_glob) != 0) && tab_bytes + bin_bytes + SM_WARPS * pair_words * 4 <= 96 * 1024;
   p.stage_words = staged ? (int)pair_words : 0;
   const size_t smem = tab_bytes + bin_bytes + (size_t)SM_WARPS * p.stage_words * 4;
-  const void* kern = p.n_lv > 0 ? (const void*)sm_wl_pairs : (const void*)sm_pairs;
+  const void* kern = p.n_lv == 0 ? (const void*)sm_pairs : h->sm_hc ? (const void*)sm_mask_pairs : (const void*)sm_wl_pairs;
   GK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
   int per_sm = 0;
   GK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, SM_THREADS, smem));
@@ -3039,7 +3040,9 @@ static int sm_launch(gk_handle* h, SmParams p) {
   p.stack = h->sm_stack.as<unsigned>();
   GK_CUDA(cudaMemsetAsync(h->sm_ctl.p, 0, 8, h->stream));
   p.next = h->sm_ctl.as<unsigned long long>();
-  if (p.n_lv > 0)
+  if (p.n_lv > 0 && h->sm_hc)
+    sm_mask_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
+  else if (p.n_lv > 0)
     sm_wl_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
   else
     sm_pairs<<<(int)grid, SM_THREADS, smem, h->stream>>>(p);
@@ -3179,9 +3182,37 @@ int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* le
 
 int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_wl_counts: null argument");
-  if (h->feature_kind != FK_SM || !h->features_ready || h->sm_n_lv == 0)
+  if (h->feature_kind != FK_SM || !h->features_ready || h->sm_n_lv == 0 || h->sm_hc)
     return fail(GK_ERR_STATE, "gk_sm_wl_counts: call gk_sm_wl_features first");
   return sm_counts(h, n_fit, row, out, "gk_sm_wl_counts");
+}
+
+// HadamardCode over SubgraphMatching (sm_mask_pairs): gk_sm_features' records, tables and lambdas, and the
+// HadamardCode class of every packed vertex at every level 0 .. n_iter - 1; gk_gram then returns the level sum of the
+// per-level SubgraphMatching Grams from one enumeration per pair
+int gk_sm_hc_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
+                      const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                      gk_stats* stats) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sm_hc_features: no graphs packed");
+  if (n_iter < 1) return fail(GK_ERR_ARG, "gk_sm_hc_features: n_iter < 1");
+  if (!(flags & (GK_SM_KV_NONE | GK_SM_KV_DIRAC)))
+    return fail(GK_ERR_UNSUPPORTED, "gk_sm_hc_features: the vertex kernel must be GK_SM_KV_DIRAC or GK_SM_KV_NONE");
+  const bool all_levels = (flags & GK_SM_KV_NONE) != 0;
+  if (!all_levels && !level_ids) return fail(GK_ERR_ARG, "gk_sm_hc_features: no level ids");
+  const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
+  if ((int64_t)n_iter * kk > SM_HC_BINS)
+    return fail(GK_ERR_UNSUPPORTED, "gk_sm_hc_features: n_iter * min(k, largest graph) is more than 64");
+  GK_TRY(gk_sm_features(h, k, lambdas, nullptr, 0, etable, n_elabels, edge_label, flags, stats));
+  const size_t bytes = (size_t)h->V * n_iter * 4;
+  GK_TRY(h->sm_wl_cls.ensure(std::max<size_t>(bytes, 4)));
+  if (!all_levels && bytes > 0) {
+    GK_CUDA(cudaMemcpyAsync(h->sm_wl_cls.p, level_ids, bytes, cudaMemcpyHostToDevice, h->stream));
+    GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffer may be reused once we return
+  }
+  h->sm_n_lv = n_iter;
+  h->sm_hc = true;
+  return GK_OK;
 }
 
 // ---------------------------------------------------------------------------

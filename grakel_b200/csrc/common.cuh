@@ -317,6 +317,7 @@ struct gk_handle {
   int sm_max_und = 0;  // largest number of distinct out- or in-neighbours of a packed vertex
   gk::DevBuf sm_wl_cls;  // gk_sm_wl_features: sm_n_lv WL class ids per packed vertex (0 levels: plain SubgraphMatching)
   int sm_n_lv = 0;
+  bool sm_hc = false;    // gk_sm_hc_features: sm_wl_cls holds HadamardCode classes (levels need not refine)
   bool sm_exact = true;
 
   // ---- OddSth (FK_ODD): graph offsets and label ranks, node records [S] (hash | label | graph | first child | child

@@ -31,6 +31,7 @@ constexpr int SM_WARPS = SM_THREADS / 32;
 constexpr int SM_KMAX = 32;            // largest clique size enumerated
 constexpr int SM_TAB_MAX = 4096;       // entries of one weight table (64 x 64 labels)
 constexpr int SM_WL_BINS = 64;         // sm_wl_pairs: (n_iter + 1) x sizes enumerated, at most
+constexpr int SM_HC_BINS = 64;         // sm_mask_pairs: n_iter x sizes enumerated, at most
 enum { SM_W_TABLE = 0, SM_W_NONE = 1, SM_W_DIRAC = 2 };
 
 // Per-graph record (32-bit words) of n vertices, W = ceil(n / 32):
@@ -61,8 +62,8 @@ struct SmParams {
   int stage_words;            // shared-memory words per warp for the two records (0: read them from global memory)
   unsigned long long* next;   // pair counter
   unsigned* err;              // bit 1: exact sum reached 2^53, bit 2: stack overflow
-  // sm_wl_pairs only: n_lv (WL levels 0 .. n_iter) class ids per packed vertex, vertex-major; tv_out then holds
-  // n_lv x n_tv values per pair
+  // sm_wl_pairs / sm_mask_pairs only: n_lv (WL levels 0 .. n_iter, HadamardCode levels 0 .. n_iter - 1) class ids
+  // per packed vertex, vertex-major; tv_out then holds n_lv x n_tv values per pair
   const int* wl_cls; int n_lv;
 };
 
@@ -110,6 +111,7 @@ __device__ __forceinline__ double sm_ce(const SmParams& P, const SmGraph& X, con
 // One lane's per-size sums of sm_pairs: exact sums in cnt / cabs, real sums in sum
 struct SmLaneAcc {
   static constexpr bool wl = false;
+  static constexpr bool masked = false;
   long long* cnt;
   unsigned long long* cabs;
   double* sum;
@@ -133,6 +135,7 @@ struct SmLaneAcc {
 // each level's lane sum is the one the per-level enumeration forms.
 struct SmWlAcc {
   static constexpr bool wl = true;
+  static constexpr bool masked = false;
   const int *cx, *cy;         // n_lv class ids per vertex of x and of y
   int n_lv, kk;
   bool all_levels;            // kv = None: every product vertex exists at every level
@@ -158,6 +161,51 @@ struct SmWlAcc {
   }
 };
 
+// The (level, size) bins of sm_mask_pairs.  A product vertex (a, b) has the level mask M(a, b), bit h set when
+// c_h(a) == c_h(b): HadamardCode's levels do not refine each other, so the levels of a vertex need not be a prefix.
+// The union product graph has the vertices with M != 0 (kv = None: every vertex, every mask full), and a clique counts
+// at exactly the levels of the AND of its vertices' masks.  Exact sums go to the warp's bins in shared memory
+// ([level][size] signed sums, then [level][size] absolute sums, 64-bit shared atomics); real sums go to the lane's own
+// bins ([level][size], stride SM_THREADS), added at every level of the mask in the enumeration order.
+struct SmMaskAcc {
+  static constexpr bool wl = false;
+  static constexpr bool masked = true;
+  const int *cx, *cy;         // n_lv class ids per vertex of x and of y
+  int n_lv, kk;
+  bool all_levels;            // kv = None
+  unsigned long long* wbin;   // exact: this warp's bins
+  double* lbin;               // real: this lane's bins
+  __device__ __forceinline__ unsigned long long level_mask(int a, int b) const {
+    if (all_levels) return n_lv >= 64 ? ~0ull : (1ull << n_lv) - 1;
+    const int* p = cx + (size_t)a * n_lv;
+    const int* q = cy + (size_t)b * n_lv;
+    unsigned long long m = 0;
+    for (int h = 0; h < n_lv; ++h) m |= (unsigned long long)(p[h] == q[h]) << h;
+    return m;
+  }
+  __device__ __forceinline__ void add(const SmParams& P, int s, double t, unsigned long long m) const {
+    if (P.exact) {
+      const double at = fabs(t);
+      if (at >= 0x1p53) atomicOr(P.err, 1u);
+      for (; m; m &= m - 1) {
+        const int h = __ffsll((long long)m) - 1;
+        atomicAdd(&wbin[h * kk + s], (unsigned long long)(long long)t);
+        atomicAdd(&wbin[(n_lv + h) * kk + s], (unsigned long long)at);
+      }
+    } else {
+      for (; m; m &= m - 1) lbin[(size_t)((__ffsll((long long)m) - 1) * kk + s) * SM_THREADS] += t;
+    }
+  }
+};
+
+// cv of a product vertex; under sm_mask_pairs 1 on the union product graph (kv = _dirac at some level, or kv = None)
+template <class Acc>
+__device__ __forceinline__ double sm_acc_cv(const Acc& acc, const SmParams& P, const SmGraph& X, const SmGraph& Y,
+                                            const double* vtab, int a, int b) {
+  if constexpr (Acc::masked) return acc.level_mask(a, b) ? 1.0 : 0.0;
+  else return sm_cv(P, X, Y, vtab, a, b);
+}
+
 // tv of the pair (x, y) for this lane's roots, into `acc`
 template <class Acc>
 __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph& Y, const double* vtab,
@@ -170,6 +218,7 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
   long long f_start[SM_KMAX + 1];
   int f_len[SM_KMAX + 1], f_pos[SM_KMAX + 1];
   unsigned char md[Acc::wl ? SM_KMAX : 1];  // least depth of S's first i + 1 vertices (sm_wl_pairs)
+  unsigned long long mk[Acc::masked ? SM_KMAX : 1];  // AND of the level masks of S's first i + 1 vertices
   auto push = [&](long long& top, unsigned u) {
     if (top >= cap) { atomicOr(P.err, 2u); return; }
     stk[(size_t)top * 32] = u;
@@ -177,9 +226,17 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
   };
   for (int v = lane; v < nv; v += 32) {
     const int va = v / ny, vb = v - va * ny;
-    const double c0 = sm_cv(P, X, Y, vtab, va, vb);
+    double c0;
+    if constexpr (Acc::masked) {
+      mk[0] = acc.level_mask(va, vb);
+      c0 = mk[0] ? 1.0 : 0.0;
+    } else {
+      c0 = sm_cv(P, X, Y, vtab, va, vb);
+    }
     if (c0 == 0.0) continue;
-    if constexpr (Acc::wl) {
+    if constexpr (Acc::masked) {
+      acc.add(P, 0, c0, mk[0]);
+    } else if constexpr (Acc::wl) {
       md[0] = (unsigned char)acc.depth(va, vb);
       acc.add(P, 0, c0, md[0]);
     } else {
@@ -196,7 +253,7 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
           for (unsigned mb = Y.und[vb * Y.W + wb]; mb; mb &= mb - 1) {
             const int b = wb * 32 + __ffs(mb) - 1;
             const int u = a * ny + b;
-            if (u <= v || sm_cv(P, X, Y, vtab, a, b) == 0.0) continue;
+            if (u <= v || sm_acc_cv(acc, P, X, Y, vtab, a, b) == 0.0) continue;
             if (sm_ce(P, X, Y, etab, va, vb, a, b) > 0.0) push(top, (unsigned)u);
           }
         }
@@ -214,9 +271,18 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
       const int fl = f_len[depth];
       const unsigned w = stk[(size_t)(fs + f_pos[depth]++) * 32];
       const int wa = (int)(w / (unsigned)ny), wb = (int)(w - (unsigned)wa * ny);
-      double t = term[depth - 1] * sm_cv(P, X, Y, vtab, wa, wb);
+      unsigned long long mw = 0;
+      if constexpr (Acc::masked) {
+        mw = mk[depth - 1] & acc.level_mask(wa, wb);
+        if (mw == 0) continue;  // no level has S + w, nor any set of its subtree
+      }
+      double t = term[depth - 1];
+      if constexpr (!Acc::masked) t *= sm_cv(P, X, Y, vtab, wa, wb);
       for (int i = 0; i < depth; ++i) t *= fabs(sm_ce(P, X, Y, etab, wa, wb, Sa[i], Sb[i]));
-      if constexpr (Acc::wl) {
+      if constexpr (Acc::masked) {
+        acc.add(P, depth, t, mw);
+        mk[depth] = mw;
+      } else if constexpr (Acc::wl) {
         const int dw = min((int)md[depth - 1], acc.depth(wa, wb));
         acc.add(P, depth, t, dw);
         md[depth] = (unsigned char)dw;
@@ -239,7 +305,7 @@ __device__ void sm_lane_pair(const SmParams& P, const SmGraph& X, const SmGraph&
             for (unsigned mb = Y.und[wb * Y.W + kb]; mb; mb &= mb - 1) {
               const int b = kb * 32 + __ffs(mb) - 1;
               const int u = a * ny + b;
-              if (u <= v || sm_cv(P, X, Y, vtab, a, b) == 0.0) continue;
+              if (u <= v || sm_acc_cv(acc, P, X, Y, vtab, a, b) == 0.0) continue;
               if (!(sm_ce(P, X, Y, etab, wa, wb, a, b) > 0.0)) continue;
               bool ok = true;
               for (int i = 0; i < depth && ok; ++i) ok = sm_ce(P, X, Y, etab, a, b, Sa[i], Sb[i]) < 0.0;
@@ -396,6 +462,90 @@ __global__ void __launch_bounds__(SM_THREADS, 1) sm_wl_pairs(SmParams P) {
             }
             if (lane == 0 && b >= (1ull << 53)) atomicOr(P.err, 1u);
             tv = (double)a;
+          } else {
+            tv = rw_warp_sum(lbin[(size_t)(h * kk + s) * SM_THREADS]);
+          }
+        }
+        kh = __fma_rn(P.lam[s], tv, kh);
+        if (lane == 0 && P.tv_out) P.tv_out[((size_t)pi * n_lv + h) * P.n_tv + s] = tv;
+      }
+      total = h == 0 ? kh : total + kh;
+    }
+    if (lane == 0 && P.out) {
+      if (P.pairs == RW_PAIRS_DIAG) {
+        P.out[r] = total;
+      } else {
+        P.out[(size_t)r * P.ld + c] = total;
+        if (P.pairs == RW_PAIRS_TRIANGLE && c != r) P.out[(size_t)c * P.ld + r] = total;
+      }
+    }
+    __syncwarp();  // every lane has read the bins; the next pair overwrites them and the staged records
+    if (P.exact) {
+      for (int i = lane; i < 2 * nb; i += 32) wbin[i] = 0ull;
+    } else {
+      for (int i = 0; i < nb; ++i) lbin[(size_t)i * SM_THREADS] = 0.0;
+    }
+    __syncwarp();
+  }
+}
+
+// HadamardCode over SubgraphMatching in one enumeration (DESIGN 4.24).  With kv = _dirac the level-h product graph is
+// the union product graph (the vertices whose classes agree at some level) induced on the vertices whose classes
+// agree at h.  ESU's extension sets over any vertex subset are the union's restricted to it, in the same order (a
+// child's set is the rest of its parent's, filtered by ce with the new vertex, plus candidates tested against S and
+// the new vertex only), so every level's lane sums see that level's terms in its own enumeration order.  Per pair:
+// the (level, size) bins, then each level's fma lambda fold and the level sum ((K_0 + K_1) + K_2) ...  Dynamic shared
+// memory as in sm_wl_pairs.
+__global__ void __launch_bounds__(SM_THREADS, 1) sm_mask_pairs(SmParams P) {
+  extern __shared__ __align__(16) unsigned char sm_smem[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const bool elab = P.ke != SM_W_NONE;
+  double* etab = reinterpret_cast<double*>(sm_smem);
+  const int net = P.ke == SM_W_TABLE ? P.n_el * P.n_el : 0;
+  for (int i = threadIdx.x; i < net; i += SM_THREADS) etab[i] = P.etab[i];
+  const int n_lv = P.n_lv, kk = P.kk, nb = n_lv * kk;
+  unsigned long long* bins = reinterpret_cast<unsigned long long*>(etab + net);
+  const int bin_words = P.exact ? SM_WARPS * 2 * nb : SM_THREADS * nb;
+  for (int i = threadIdx.x; i < bin_words; i += SM_THREADS) bins[i] = 0ull;
+  __syncthreads();
+  unsigned long long* wbin = bins + (size_t)warp * 2 * nb;
+  double* lbin = reinterpret_cast<double*>(bins) + threadIdx.x;
+  unsigned* stage = reinterpret_cast<unsigned*>(bins + bin_words) + (size_t)warp * P.stage_words;
+  const size_t gwarp = (size_t)blockIdx.x * SM_WARPS + warp;
+  unsigned* stk = P.stack + gwarp * 32 * (size_t)P.stack_cap + lane;
+  for (;;) {
+    long long pi = 0;
+    if (lane == 0) pi = (long long)atomicAdd(P.next, 1ull);
+    pi = __shfl_sync(0xffffffffu, pi, 0);
+    if (pi >= P.n_pairs) break;
+    int r, c, gi, gj;
+    rw_pair_of(P.pairs, P.cols, P.row_g0, P.ordered, pi, r, c, gi, gj);
+    const int x0 = P.graph_ptr[gi], y0 = P.graph_ptr[gj];
+    const int nx = P.graph_ptr[gi + 1] - x0, ny = P.graph_ptr[gj + 1] - y0;
+    const long long rx = sm_record_words(nx, elab), ry = sm_record_words(ny, elab);
+    const unsigned* ax = P.rec + P.rec_off[gi];
+    const unsigned* ay = P.rec + P.rec_off[gj];
+    if (rx + ry <= P.stage_words) {
+      for (long long i = lane; i < rx; i += 32) stage[i] = ax[i];
+      for (long long i = lane; i < ry; i += 32) stage[rx + i] = ay[i];
+      __syncwarp();
+      ax = stage; ay = stage + rx;
+    }
+    const SmGraph X = sm_graph(ax, nx, elab), Y = sm_graph(ay, ny, elab);
+    const SmMaskAcc acc{P.wl_cls + (size_t)x0 * n_lv, P.wl_cls + (size_t)y0 * n_lv, n_lv, kk, P.kv == SM_W_NONE,
+                        wbin, lbin};
+    sm_lane_pair(P, X, Y, etab, etab, stk, acc);
+    __syncwarp();
+    // K = ((K_0 + K_1) + K_2) ..., K_h the fma fold of lambdas x the level's own bins
+    double total = 0.0;
+    for (int h = 0; h < n_lv; ++h) {
+      double kh = 0.0;
+      for (int s = 0; s < P.n_tv; ++s) {
+        double tv = 0.0;
+        if (s < kk) {
+          if (P.exact) {
+            if (lane == 0 && wbin[(n_lv + h) * kk + s] >= (1ull << 53)) atomicOr(P.err, 1u);
+            tv = (double)(long long)wbin[h * kk + s];
           } else {
             tv = rw_warp_sum(lbin[(size_t)(h * kk + s) * SM_THREADS]);
           }

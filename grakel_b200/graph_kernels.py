@@ -8,7 +8,8 @@ the kernels of the device hot path:
     "edge_histogram" / "EH"
     "core_framework" / "CORE"   (framework; base "shortest_path", "weisfeiler_lehman", "vertex_histogram", "NH",
                                  "ODD", "WL-OA", "SM" with ke=None)
-    "hadamard_code" / "HC"      (framework; base "vertex_histogram", "shortest_path" or "edge_histogram")
+    "hadamard_code" / "HC"      (framework; base "vertex_histogram", "shortest_path", "edge_histogram", "SM",
+                                 "pyramid_match" or "NSPD")
     "weisfeiler_lehman_optimal_assignment" / "WL-OA"
     "graph_hopper" / "GH"
     "neighborhood_hash" / "NH"

@@ -448,6 +448,7 @@ def wl_reference_dictionaries(row_ptr, col_idx, level0_ids, n_level0, classes, n
 
 # ------------------------------------------------------------------------------
 _WL_GRAPH_BASES = ()  # set after the base classes: the bases whose WL route needs the list of graphs
+_HC_GRAPH_BASES = ()  # ... and those of HadamardCode's per-level routes
 
 
 class WeisfeilerLehman(Kernel):
@@ -596,45 +597,13 @@ class WeisfeilerLehman(Kernel):
 
     def _pm_embed(self, X, block):
         """PyramidMatch base: the embeddings of every level's fresh base kernel (weisfeiler_lehman.py:260-270,
-        478-482): n_iter + 1 passes over the graphs, level-major, each one eigs / eig call per graph.  The base kernel
-        sees every graph's edge DICTIONARY: its vertices are those of the element's adjacency matrix (range(n), or the
-        sorted symbols of the edge dictionary), each with its own label.  The packed WL block lists a graph's vertices
-        in the order of its labels dictionary and also holds labelled vertices outside the edge dictionary; so every
-        embedding row is moved to its vertex's packed position, and the vertices the base kernel does not see are
-        skipped (they never change another vertex's WL label)."""
+        478-482), see pm_level_embeddings."""
         if self._base_graph_kernel is not PyramidMatch:
             return None
-        from .packing import adjacency_and_order
-        import time
-        d, L = self._params.get("d", 6), self._params.get("L", 4)
-        mats, src = [], []
-        n_pm = 0
-        for x in X:
-            if isinstance(x, Graph):
-                x = x.as_element()
-            x = list(x)
-            if len(x) == 0:
-                continue
-            A, order = adjacency_and_order(x[0])
-            loc = {k: i for i, k in enumerate(order)}
-            rows = [loc.get(k, -1) for k in x[1].keys()]  # the packed vertices, in the pack's order
-            if sum(r >= 0 for r in rows) != len(order):
-                raise NotImplementedError("WeisfeilerLehman over PyramidMatch: a vertex of a graph's edge dictionary "
-                                          "has no label")
-            src.extend(r + n_pm if r >= 0 else -1 for r in rows)
-            mats.append(A)
-            n_pm += A.shape[0]
-        src = np.asarray(src, dtype=np.int64)
-        if len(src) != block.n_vertices:
-            raise NotImplementedError("WeisfeilerLehman over PyramidMatch: the packed vertices are not the labelled ones")
-        t0 = time.perf_counter()
-        U_pm, n_cols = pm_embed_sets(mats, d, self._n_iter)
-        self.ms_host_embed_ = (time.perf_counter() - t0) * 1e3
-        pm_check_cells(U_pm, n_cols, np.array([A.shape[0] for A in mats]), L)
-        seen = src >= 0
-        U = np.zeros((self._n_iter, len(src), d))
-        U[:, seen] = U_pm[:, src[seen]]
-        return _PmData(np.diff(np.asarray(block.graph_ptr)), U, n_cols, None, skip=None if seen.all() else ~seen)
+        d = self._params.get("d", 6)
+        data, self.ms_host_embed_ = pm_level_embeddings(X, block, d, self._params.get("L", 4), self._n_iter,
+                                                        "WeisfeilerLehman")
+        return data
 
     def fit_transform(self, X, y=None):
         self._method_calling = 2
@@ -701,60 +670,11 @@ class WeisfeilerLehman(Kernel):
         return super().diagonal()
 
     def _base_data(self, X, block):
-        """NeighborhoodSubgraphPairwiseDistance / OddSth / SubgraphMatching base: every element's graph as that base
-        kernel packs it, and `src`, the WL vertex of every base vertex (the base kernel sees the WL labels through the
-        element's labels dictionary, whose key order is the WL block's)."""
+        """NeighborhoodSubgraphPairwiseDistance / OddSth / SubgraphMatching base: see base_graph_data."""
         base = self._base_graph_kernel
         if base not in _WL_GRAPH_BASES or base is PyramidMatch:
             return None
-        gp = np.asarray(block.graph_ptr, dtype=np.int64)
-        src, graphs, els = [], [], []
-        for x in X:
-            from_graph = isinstance(x, Graph)
-            if from_graph:
-                x = x.as_element()
-            x = list(x)
-            if len(x) == 0:
-                continue
-            loc = {k: i for i, k in enumerate(x[1].keys())}
-            if base is NeighborhoodSubgraphPairwiseDistance:
-                if len(x) != 3:  # the element the reference hands on is (edges, labels) + edge labels
-                    raise TypeError(_NSPD_ELEMENT_MSG)
-                n, edges, _, el, order = _nspd_graph(x[0], x[1], x[2], with_order=True)
-                graphs.append((n, edges, None, el))
-            elif base is SubgraphMatching:
-                # the reference hands on (edges, labels) + extras, extras starting with the edge labels when the
-                # element has them (weisfeiler_lehman.py:157-176): without them SubgraphMatching gets two entries
-                if len(x) != 3 or (from_graph and not x[2]):
-                    raise TypeError(_SM_ELEMENT_MSG)
-                n, edges, _, el = self._sm._graph(x[0], None, x[2] if x[2] else None, need_v=False)
-                order = adjacency_and_order(x[0])[1]
-                graphs.append((n, edges, None, el))
-            else:
-                if type(x[0]) is dict and x[0] and all(type(d) is list for d in x[0].values()) and not all(x[0].values()):
-                    raise ValueError("vertex not inside edge dictionary")
-                els.append([x[0], x[1]])
-                order = adjacency_and_order(x[0])[1]
-            src.append([loc.get(k, -1) for k in order])
-        out = _WlBaseData()
-        cols = []
-        for g, rows in enumerate(src):
-            rows = np.asarray(rows, dtype=np.int64)
-            if np.any(rows < 0):
-                raise NotImplementedError("WeisfeilerLehman over %s: a vertex of a graph's edges has no label"
-                                          % base.__name__)
-            cols.append(rows + gp[g])
-        out.src = np.concatenate(cols) if cols else np.zeros(0, dtype=np.int64)
-        out.wl_vertices = int(gp[-1])
-        if base in (NeighborhoodSubgraphPairwiseDistance, SubgraphMatching):
-            out.graphs = graphs
-        else:
-            b = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
-                     keep_edge_order=True)
-            if b.n_vertices != len(out.src):
-                raise NotImplementedError("WeisfeilerLehman over OddSth: a graph's vertices are not those of its edges")
-            out.block = b
-        return out
+        return base_graph_data(X, block, base, getattr(self, "_sm", None), "WeisfeilerLehman")
 
     def _level_labels(self, block, ids, n_fit_vertices):
         """The reference's label of every WL vertex at every level: the device partition, numbered on the host."""
@@ -806,51 +726,13 @@ class WeisfeilerLehman(Kernel):
         return K, xd, yd
 
     def _wl_nspd_run(self, data, labels, n_fit, want_matrix, row_range):
+        def levels():
+            for lab in labels:
+                uniq, inv = np.unique(np.asarray(lab, dtype=np.int64)[data.src], return_inverse=True)
+                yield inv.reshape(-1), [str(int(u)) for u in uniq]
         p = self._params
-        r, d = p.get("r", 3), p.get("d", 4)
-        graphs = data.graphs
-        if r > 0 and max(g[0] for g in graphs) >= 65535:  # the device refuses it too; do not pack it first
-            raise NotImplementedError("NeighborhoodSubgraphPairwiseDistance: r > 0 with a graph of 65535 or more "
-                                      "vertices")
-        nsp = NeighborhoodSubgraphPairwiseDistance(r=r, d=d)
-        gp, rp, ci, _, el, sh, tok0 = nsp._pack([(n, e, ["0"] * n, l) for n, e, _, l in graphs])
-        elabels = [tok0.el_bytes[tok0.el_off[i]:tok0.el_off[i + 1]].tobytes().decode("utf-8")
-                   for i in range(tok0.n_elabels)]
-        N = len(gp) - 1
-        square = n_fit == N
-        rows_total = N if square else N - n_fit
-        rb, re_ = (0, rows_total) if row_range is None else row_range
-        with _lib.engine(getattr(self, "device_", None)) as eng:
-            for lv, lab in enumerate(labels):
-                L = np.asarray(lab, dtype=np.int64)[data.src]
-                uniq, inv = np.unique(L, return_inverse=True)
-                tokens = _NspdTokens(d, [str(int(u)) for u in uniq], elabels)
-                eng.pack(gp, rp, ci, inv.reshape(-1), None, None)
-                self.stats_, mask = eng.nspd_features(r, d, sh, el, tokens)
-                if want_matrix:
-                    eng.wl_level_sum(lv, n_fit, (rb, re_))
-            # diagonal() of every fitted level: its number of (radius, distance) levels (the reference's constant)
-            def levels(m):
-                top = max((int(x).bit_length() for x in m), default=0)
-                return (r + 1) * top
-            xd_lv = np.full(n_fit, float(levels(mask[:n_fit])))
-            yd_lv = None if square else np.full(N - n_fit, float(levels(mask[n_fit:])))
-            xd_sum = xd_lv.copy()
-            yd_sum = None if yd_lv is None else yd_lv.copy()
-            for _ in range(1, self._n_iter):
-                xd_sum += xd_lv
-                if yd_sum is not None:
-                    yd_sum += yd_lv
-            if not want_matrix:
-                return None, xd_sum, yd_sum
-            if square:
-                full = rb == 0 and re_ == N
-                K, kd = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(self.normalize), want_kdiag=full)
-                return K, kd, None
-            xd = getattr(self, "_X_diag", None)
-            xd = xd_sum if xd is None else np.asarray(xd, dtype=np.float64).reshape(-1)
-            K, _ = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(self.normalize), xdiag=xd, ydiag=yd_sum)
-            return K, xd, yd_sum
+        return nspd_level_sum(self, data, levels(), self._n_iter, n_fit, want_matrix, row_range, p.get("r", 3),
+                              p.get("d", 4))
 
     def _wl_sm_run(self, block, ids, n_fit, want_matrix=True, row_range=None, device_ptr=None):
         """WL over SubgraphMatching (gk_sm_wl_features): the joint device partition of the fitted and new graphs gives
@@ -911,6 +793,148 @@ class WeisfeilerLehman(Kernel):
         out, self.wl_labels_ = wl_reference_dictionaries(np.asarray(block.row_ptr), np.asarray(block.col_idx), ids,
                                                          len(self.X.dictionary), classes)
         return out
+
+
+def nspd_level_sum(est, data, levels, n_levels, n_fit, want_matrix, row_range, r, d):
+    """NeighborhoodSubgraphPairwiseDistance under a relabelling framework (estimator `est`): `levels` yields, level
+    by level, the label id of every base vertex and the label string of every id; each level packs its labels and
+    tokens, runs gk_nspd_features, and gk_wl_level_sum adds its un-normalised K into a device-resident sum in level
+    order.  Normalised as the frameworks do: by the sum's diagonal after fit_transform, by the base diagonals (the
+    number of (radius, distance) levels, per level) after a transform.  Returns (K, xdiag, ydiag)."""
+    graphs = data.graphs
+    if r > 0 and max(g[0] for g in graphs) >= 65535:  # the device refuses it too; do not pack it first
+        raise NotImplementedError("NeighborhoodSubgraphPairwiseDistance: r > 0 with a graph of 65535 or more "
+                                  "vertices")
+    nsp = NeighborhoodSubgraphPairwiseDistance(r=r, d=d)
+    gp, rp, ci, _, el, sh, tok0 = nsp._pack([(n, e, ["0"] * n, l) for n, e, _, l in graphs])
+    elabels = [tok0.el_bytes[tok0.el_off[i]:tok0.el_off[i + 1]].tobytes().decode("utf-8")
+               for i in range(tok0.n_elabels)]
+    N = len(gp) - 1
+    square = n_fit == N
+    rows_total = N if square else N - n_fit
+    rb, re_ = (0, rows_total) if row_range is None else row_range
+    with _lib.engine(getattr(est, "device_", None)) as eng:
+        for lv, (ids, strings) in enumerate(levels):
+            tokens = _NspdTokens(d, strings, elabels)
+            eng.pack(gp, rp, ci, ids, None, None)
+            est.stats_, mask = eng.nspd_features(r, d, sh, el, tokens)
+            if want_matrix:
+                eng.wl_level_sum(lv, n_fit, (rb, re_))
+        # diagonal() of every fitted level: its number of (radius, distance) levels (the reference's constant)
+        def n_rd(m):
+            top = max((int(x).bit_length() for x in m), default=0)
+            return (r + 1) * top
+        xd_lv = np.full(n_fit, float(n_rd(mask[:n_fit])))
+        yd_lv = None if square else np.full(N - n_fit, float(n_rd(mask[n_fit:])))
+        xd_sum = xd_lv.copy()
+        yd_sum = None if yd_lv is None else yd_lv.copy()
+        for _ in range(1, n_levels):
+            xd_sum += xd_lv
+            if yd_sum is not None:
+                yd_sum += yd_lv
+        if not want_matrix:
+            return None, xd_sum, yd_sum
+        if square:
+            full = rb == 0 and re_ == N
+            K, kd = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(est.normalize), want_kdiag=full)
+            return K, kd, None
+        xd = getattr(est, "_X_diag", None)
+        xd = xd_sum if xd is None else np.asarray(xd, dtype=np.float64).reshape(-1)
+        K, _ = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(est.normalize), xdiag=xd, ydiag=yd_sum)
+        return K, xd, yd_sum
+
+
+def base_graph_data(X, block, base, sm, who):
+    """NeighborhoodSubgraphPairwiseDistance / OddSth / SubgraphMatching under a relabelling framework (`sm`: the
+    SubgraphMatching that checks the elements): every element's graph as that base kernel packs it, and `src`, the
+    packed vertex of every base vertex (the base kernel sees the level labels through the element's labels dictionary,
+    whose key order is the packed block's)."""
+    gp = np.asarray(block.graph_ptr, dtype=np.int64)
+    src, graphs, els = [], [], []
+    for x in X:
+        from_graph = isinstance(x, Graph)
+        if from_graph:
+            x = x.as_element()
+        x = list(x)
+        if len(x) == 0:
+            continue
+        loc = {k: i for i, k in enumerate(x[1].keys())}
+        if base is NeighborhoodSubgraphPairwiseDistance:
+            if len(x) != 3:  # the element the reference hands on is (edges, labels) + edge labels
+                raise TypeError(_NSPD_ELEMENT_MSG)
+            n, edges, _, el, order = _nspd_graph(x[0], x[1], x[2], with_order=True)
+            graphs.append((n, edges, None, el))
+        elif base is SubgraphMatching:
+            # the reference hands on (edges, labels) + extras, extras starting with the edge labels when the
+            # element has them (weisfeiler_lehman.py:157-176): without them SubgraphMatching gets two entries
+            if len(x) != 3 or (from_graph and not x[2]):
+                raise TypeError(_SM_ELEMENT_MSG)
+            n, edges, _, el = sm._graph(x[0], None, x[2] if x[2] else None, need_v=False)
+            order = adjacency_and_order(x[0])[1]
+            graphs.append((n, edges, None, el))
+        else:
+            if type(x[0]) is dict and x[0] and all(type(d) is list for d in x[0].values()) and not all(x[0].values()):
+                raise ValueError("vertex not inside edge dictionary")
+            els.append([x[0], x[1]])
+            order = adjacency_and_order(x[0])[1]
+        src.append([loc.get(k, -1) for k in order])
+    out = _WlBaseData()
+    cols = []
+    for g, rows in enumerate(src):
+        rows = np.asarray(rows, dtype=np.int64)
+        if np.any(rows < 0):
+            raise NotImplementedError("%s over %s: a vertex of a graph's edges has no label" % (who, base.__name__))
+        cols.append(rows + gp[g])
+    out.src = np.concatenate(cols) if cols else np.zeros(0, dtype=np.int64)
+    out.wl_vertices = int(gp[-1])
+    if base in (NeighborhoodSubgraphPairwiseDistance, SubgraphMatching):
+        out.graphs = graphs
+    else:
+        b = pack(els, "sp", need_labels=True, len_ok=lambda n: n == 2, type_error_msg=_ODD_ELEMENT_MSG,
+                 keep_edge_order=True)
+        if b.n_vertices != len(out.src):
+            raise NotImplementedError(who + " over OddSth: a graph's vertices are not those of its edges")
+        out.block = b
+    return out
+
+
+def pm_level_embeddings(X, block, d, L, n_sets, who):
+    """PyramidMatch under a relabelling framework: the embeddings of every level's fresh base kernel, n_sets passes
+    over the graphs, level-major, each one eigs / eig call per graph.  The base kernel sees every graph's adjacency:
+    its vertices are those of the element's adjacency matrix (range(n), or the sorted symbols of the edge dictionary),
+    each with its own label.  The packed block lists a graph's vertices in the order of its labels dictionary and also
+    holds labelled vertices outside the edge dictionary; so every embedding row is moved to its vertex's packed
+    position, and the vertices the base kernel does not see are skipped (they never change another vertex's label).
+    Returns (_PmData, host embedding milliseconds)."""
+    from .packing import adjacency_and_order
+    import time
+    mats, src = [], []
+    n_pm = 0
+    for x in X:
+        if isinstance(x, Graph):
+            x = x.as_element()
+        x = list(x)
+        if len(x) == 0:
+            continue
+        A, order = adjacency_and_order(x[0])
+        loc = {k: i for i, k in enumerate(order)}
+        rows = [loc.get(k, -1) for k in x[1].keys()]  # the packed vertices, in the pack's order
+        if sum(r >= 0 for r in rows) != len(order):
+            raise NotImplementedError(who + " over PyramidMatch: a vertex of a graph's edge dictionary has no label")
+        src.extend(r + n_pm if r >= 0 else -1 for r in rows)
+        mats.append(A)
+        n_pm += A.shape[0]
+    src = np.asarray(src, dtype=np.int64)
+    if len(src) != block.n_vertices:
+        raise NotImplementedError(who + " over PyramidMatch: the packed vertices are not the labelled ones")
+    t0 = time.perf_counter()
+    U_pm, n_cols = pm_embed_sets(mats, d, n_sets)
+    ms = (time.perf_counter() - t0) * 1e3
+    pm_check_cells(U_pm, n_cols, np.array([A.shape[0] for A in mats]), L)
+    seen = src >= 0
+    U = np.zeros((n_sets, len(src), d))
+    U[:, seen] = U_pm[:, src[seen]]
+    return _PmData(np.diff(np.asarray(block.graph_ptr)), U, n_cols, None, skip=None if seen.all() else ~seen), ms
 
 
 class _WlBaseData:
@@ -2768,7 +2792,12 @@ def _enum_ids(labels, enum):
 
 
 class _HcData:
-    """One parsed input of HadamardCode: the packed block, its enumeration ids, the skip flags of the levels >= 1."""
+    """One parsed input of HadamardCode: the packed block, its enumeration ids, the skip flags of the levels >= 1, and
+    for SubgraphMatching / NSPD the base kernel's graphs (`base`, _WlBaseData), for PyramidMatch its per-level
+    embeddings (`pm`, _PmData)."""
+
+    base = None
+    pm = None
 
     def __init__(self, block, ids, skip):
         self.block, self.ids, self.skip = block, ids, skip
@@ -2783,7 +2812,12 @@ class _HcData:
             fa = a.skip if a.skip is not None else np.zeros(a.block.n_vertices, dtype=bool)
             fb = b.skip if b.skip is not None else np.zeros(b.block.n_vertices, dtype=bool)
             skip = np.concatenate([fa, fb])
-        return _HcData(Block.concat(a.block, b.block), np.concatenate([a.ids, b.ids]), skip)
+        out = _HcData(Block.concat(a.block, b.block), np.concatenate([a.ids, b.ids]), skip)
+        if a.base is not None:
+            out.base = _WlBaseData.concat(a.base, b.base)
+        if a.pm is not None:
+            out.pm = _PmData.concat(a.pm, b.pm)
+        return out
 
 
 class HadamardCode(Kernel):
@@ -2794,8 +2828,15 @@ class HadamardCode(Kernel):
     the device (gk_hc_features); the host replays the reference's label enumeration, so the device vectors are the
     reference's tuples entry for entry.
 
-    Base kernels: VertexHistogram (default), ShortestPath(with_labels=True) and EdgeHistogram.  Labelled vertices that
-    are not keys of the edge dictionary count at level 0 only, as in the reference."""
+    Base kernels: VertexHistogram (default), ShortestPath(with_labels=True), EdgeHistogram, SubgraphMatching (kv
+    `_dirac` or None), PyramidMatch and NeighborhoodSubgraphPairwiseDistance.  Labelled vertices that are not keys of
+    the edge dictionary count at level 0 only, as in the reference.  SubgraphMatching counts every level's cliques in
+    one enumeration over the union of the levels' product graphs, each clique at the levels where all its vertex pairs
+    share their classes (DESIGN 4.24); PyramidMatch reads every level's device classes; NSPD hashes the reference's
+    label strings, str() of each class's tuple of numpy int64, built on the host from one device vector per class.
+    A transform whose new labels widen the Hadamard matrix shares no label with the fitted graphs: K is zero for the
+    bases that read labels, as in the reference.  A custom kv and a datasets.read_tu block raise NotImplementedError
+    for these three bases."""
 
     _graph_format = "auto"
     _nan_to_num = True
@@ -2829,9 +2870,24 @@ class HadamardCode(Kernel):
                     raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
                                      "parameters names and values")
                 params.pop("normalize", None)
-            if base not in (VertexHistogram, ShortestPath, EdgeHistogram):
-                raise NotImplementedError("grakel_b200 runs HadamardCode over VertexHistogram, ShortestPath or "
-                                          "EdgeHistogram; other base kernels are outside the device hot path")
+            if base not in (VertexHistogram, ShortestPath, EdgeHistogram, SubgraphMatching, PyramidMatch,
+                            NeighborhoodSubgraphPairwiseDistance):
+                raise NotImplementedError("grakel_b200 runs HadamardCode over VertexHistogram, ShortestPath, "
+                                          "EdgeHistogram, SubgraphMatching, PyramidMatch or "
+                                          "NeighborhoodSubgraphPairwiseDistance; other base kernels are outside the "
+                                          "device hot path")
+            self._sm = None
+            if base is SubgraphMatching:  # the base kernel's own checks (subgraph_matching.py:70-120)
+                sm = SubgraphMatching(**{k: v for k, v in params.items() if k in ("k", "kv", "ke", "lw")})
+                sm.initialize()
+                if sm.kv is not None and sm.kv is not _dirac:
+                    raise NotImplementedError("HadamardCode over SubgraphMatching runs kv=_dirac or kv=None: a custom "
+                                              "vertex kernel reads the reference's Hadamard-code tuples per level")
+                self._sm = sm
+            if base is PyramidMatch:  # pyramid_match.py:62-81
+                PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
+            if base is NeighborhoodSubgraphPairwiseDistance:
+                NeighborhoodSubgraphPairwiseDistance(**{k: v for k, v in params.items() if k in ("r", "d")}).initialize()
             if base is ShortestPath:
                 if not params.get("with_labels", True):
                     raise NotImplementedError("HadamardCode over ShortestPath(with_labels=False) ignores the Hadamard "
@@ -2865,6 +2921,9 @@ class HadamardCode(Kernel):
                     continue
                 out.append(x[:3])
             elif type(x) is Graph:
+                if self.base_graph_kernel_[0] in _HC_GRAPH_BASES:
+                    # the reference asks a Graph for its edge labels with purpose "auto" (hadamard_code.py:163)
+                    raise ValueError("unsupported label purpose")
                 el = x.as_element()
                 out.append(el if x.edge_labels else el[:2])
             else:
@@ -2880,6 +2939,10 @@ class HadamardCode(Kernel):
         if isinstance(X, Block):  # packed input (datasets.read_tu): integer labels
             if base is EdgeHistogram:
                 raise NotImplementedError("packed blocks carry no edge-label entries; pass the list of graphs")
+            if base in _HC_GRAPH_BASES:
+                raise NotImplementedError("HadamardCode over %s needs every graph's edge dictionary and edge labels "
+                                          "(its adjacency matrix for PyramidMatch); pass the list of graphs"
+                                          % base.__name__)
             block = X.require("wl", "sp")
             gp = np.asarray(block.graph_ptr)
             labels = np.asarray(block.labels)
@@ -2914,7 +2977,7 @@ class HadamardCode(Kernel):
                          fw_zero_is_absent=self.base_graph_kernel_[1].get("algorithm_type") == "floyd_warshall",
                          type_error_msg="each element of X must have at least one and at most 3 elements\n")
             return _HcData(block, _enum_ids(block.labels, enum), None), enum
-        if self.n_iter == 1:  # level 0 only: the label multisets
+        if self.n_iter == 1 and base not in _HC_GRAPH_BASES:  # level 0 only: the label multisets
             labels = [l for x in els for l in x[1].values()]
             sizes = np.concatenate([[0], np.cumsum([len(x[1]) for x in els])])
             block = Block(sizes, np.zeros(int(sizes[-1]) + 1, dtype=np.int64), np.zeros(0, dtype=np.int64), None, labels)
@@ -2932,7 +2995,14 @@ class HadamardCode(Kernel):
             skip.append(np.fromiter((k not in keys for k in x[1]), dtype=bool, count=len(x[1])))
         skip = np.concatenate(skip)
         block = pack([x[:2] for x in els], "wl", len_ok=lambda n: n >= 2)
-        return _HcData(block, _enum_ids(block.labels, enum), skip if skip.any() else None), enum
+        data = _HcData(block, _enum_ids(block.labels, enum), skip if skip.any() else None)
+        if base is PyramidMatch:
+            p = self.base_graph_kernel_[1]
+            data.pm, self.ms_host_embed_ = pm_level_embeddings(els, block, p.get("d", 6), p.get("L", 4), self.n_iter,
+                                                               "HadamardCode")
+        elif base in _HC_GRAPH_BASES:
+            data.base = base_graph_data(els, block, base, self._sm, "HadamardCode")
+        return data, enum
 
     def _eh_ids(self, data, known):
         ids, new = label_ids(data.block.labels, known, sort_new=False)
@@ -2984,11 +3054,12 @@ class HadamardCode(Kernel):
             width = hc_width(len(self._eh_labels) + len(new))
         else:
             width = hc_width(len(enum))
-        if width == self._width or self.base_graph_kernel_[0] is EdgeHistogram:
+        if width == self._width or self.base_graph_kernel_[0] is EdgeHistogram or not self._reads_labels():
             K, xdiag, ydiag = self._run(_HcData.concat(self.X, Y), n_x, width)
         else:
             # the vectors of Y are longer than every fitted vector: no label is shared (hadamard_code.py:187, 235) and
-            # every Y graph is only similar to itself, at its own width
+            # every Y graph is only similar to itself, at its own width.  (NSPD: the label strings str(tuple) of Y are
+            # longer than every fitted one, so no neighbourhood hash is shared either.)
             _, ydiag, _ = self._run(Y, n_y, width, want_matrix=False)
             try:
                 check_is_fitted(self, ["_X_diag"])
@@ -3015,10 +3086,22 @@ class HadamardCode(Kernel):
     def _dijkstra_order(self, block):
         return _path_sum_order(block, self.base_graph_kernel_[1].get("algorithm_type", "auto"))
 
-    def _run(self, data, n_fit, width, want_matrix=True):
+    def _reads_labels(self):
+        """Whether the base kernel reads the Hadamard codes: not SubgraphMatching(kv=None), not
+        PyramidMatch(with_labels=False)."""
+        base, p = self.base_graph_kernel_
+        if base is SubgraphMatching:
+            return self._sm.kv is not None
+        if base is PyramidMatch:
+            return bool(p.get("with_labels", True))
+        return True
+
+    def _run(self, data, n_fit, width, want_matrix=True, row_range=None, device_ptr=None):
         """pack -> gk_hc_features -> gk_gram.  Returns (K, xdiag, ydiag)."""
         block = data.block
         base = self.base_graph_kernel_[0]
+        if base in _HC_GRAPH_BASES:
+            return self._base_run(data, n_fit, width, want_matrix, row_range, device_ptr)
         with _lib.engine(getattr(self, "device_", None)) as eng:
             eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids,
                      block.weights if base is ShortestPath else None, None)
@@ -3028,6 +3111,73 @@ class HadamardCode(Kernel):
                 self.stats_ = eng.hc_features(self.n_iter, width, skip=data.skip)
             K, xd, yd = eng.gram(block.n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
                                  nan_to_num=True, out=None if want_matrix else False, stats=self.stats_)
+        if self.verbose:
+            print(type(self).__name__, self.stats_.as_dict())
+        return K, xd, yd
+
+    def _hc_classes(self, eng, data, width, vectors=False):
+        """The HadamardCode class of every packed vertex at every level, [V, n_iter] (gk_hc_features, gk_wl_labels:
+        exact vector classes, numbered on the device); with `vectors` also, per level, the [V, W] vectors."""
+        block = data.block
+        eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
+        eng.hc_features(self.n_iter, width, skip=data.skip)
+        cls = np.stack([eng.wl_labels(lv, block.n_vertices) for lv in range(self.n_iter)], axis=1)
+        if not vectors:
+            return cls, None
+        return cls, [eng.hc_vectors(lv, block.n_vertices, width) for lv in range(self.n_iter)]
+
+    def _base_run(self, data, n_fit, width, want_matrix, row_range, device_ptr):
+        """HadamardCode over SubgraphMatching, PyramidMatch or NSPD: K = sum over the n_iter levels of the base kernel
+        on the level's Hadamard codes, added in level order (hadamard_code.py:217-236, np.sum(axis=0)); DESIGN 4.24."""
+        base, p = self.base_graph_kernel_
+        reads = self._reads_labels()
+        if base is SubgraphMatching:  # gk_sm_hc_features' bin cap, before the relabelling runs
+            kk = max(1, min(max(int(self._sm.k), 1), max(g[0] for g in data.base.graphs)))
+            if self.n_iter * kk > 64:
+                raise NotImplementedError("HadamardCode over SubgraphMatching: n_iter * min(k, largest graph) is more "
+                                          "than 64")
+        with _lib.engine(getattr(self, "device_", None)) as eng:
+            if base is NeighborhoodSubgraphPairwiseDistance:
+                cls, vecs = self._hc_classes(eng, data, width, vectors=True)
+                src = data.base.src
+
+                def levels():
+                    # the reference hashes str(D) + "," + str(label), label the tuple of numpy int64 of the level's
+                    # vector (neighborhood_subgraph_pairwise_distance.py:443): one string per class, from one vector
+                    for lv in range(self.n_iter):
+                        uniq, first, inv = np.unique(cls[src, lv], return_index=True, return_inverse=True)
+                        rows = vecs[lv][src[first]]
+                        yield inv.reshape(-1), [str(tuple(row)) for row in rows]
+                K, xd, yd = nspd_level_sum(self, data.base, levels(), self.n_iter, n_fit, want_matrix, row_range,
+                                           p.get("r", 3), p.get("d", 4))
+                return K, xd, yd
+            if base is SubgraphMatching:
+                sm = self._sm
+                level_ids = None
+                if reads:
+                    level_ids = self._hc_classes(eng, data, width)[0][data.base.src]
+                graphs, v0 = [], 0
+                for n, edges, _, el in data.base.graphs:
+                    graphs.append((n, edges, None if level_ids is None else level_ids[v0:v0 + n, 0].tolist(), el))
+                    v0 += n
+                gp, rp, ci, lab, elids, _, et, flags = sm._pack(graphs)
+                eng.pack(gp, rp, ci, lab, None, None)
+                self.stats_ = eng.sm_hc_features(int(sm.k), self.n_iter, level_ids, sm.lambdas_, et, elids, flags)
+                n_graphs = len(graphs)
+            else:  # PyramidMatch: every level's classes label a PyramidMatch of its own
+                block = data.block
+                if reads:
+                    eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
+                    eng.hc_features(self.n_iter, width, skip=data.skip)
+                else:
+                    eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, None, None, None)
+                self.stats_ = eng.pm_features(p.get("L", 4), p.get("d", 6), data.pm.U, data.pm.n_cols,
+                                              n_iter=self.n_iter - 1,
+                                              flags=_lib.GK_PM_WL_LABELS if reads else 0, skip=data.pm.skip)
+                n_graphs = block.n_graphs
+            K, xd, yd = eng.gram(n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
+                                 nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
+                                 device_ptr=device_ptr, stats=self.stats_)
         if self.verbose:
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
@@ -4362,3 +4512,4 @@ class GraphletSampling(Kernel):
 
 
 _WL_GRAPH_BASES = (PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth, SubgraphMatching)
+_HC_GRAPH_BASES = (PyramidMatch, NeighborhoodSubgraphPairwiseDistance, SubgraphMatching)

@@ -317,6 +317,20 @@ int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* le
                       gk_stats* stats);
 int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out);
 
+/* HadamardCode over SubgraphMatching (hadamard_code.py over subgraph_matching.py) in one clique enumeration.
+ * level_ids[v * n_iter + h] is the HadamardCode class of packed vertex v at level h = 0 .. n_iter - 1 (any numbering
+ * per level: only equality within a level is read; after gk_hc_features, gk_wl_labels returns the classes of each
+ * level).  The levels need not refine each other.  The vertex kernel is GK_SM_KV_DIRAC (the level-h product graph has
+ * the vertex pairs of equal level-h classes) or GK_SM_KV_NONE (level_ids may then be null: every level is the same);
+ * the edge kernel, the edge labels, k and the lambdas are those of gk_sm_features, whose checks apply.  gk_gram then
+ * returns K = ((K_0 + K_1) + K_2) ... in fp64, K_h the SubgraphMatching K of the level-h classes as vertex labels,
+ * under gk_sm_features' gk_gram rules (GK_NORMALIZE, n_fit, row ranges, GK_OUT_DEVICE; no GK_DIST, no row map);
+ * GK_NORMALIZE divides by that sum's own self similarities.  n_iter * min(k, largest packed graph) above 64 is
+ * GK_ERR_UNSUPPORTED, before anything is launched. */
+int gk_sm_hc_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
+                      const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                      gk_stats* stats);
+
 /* OddSth (odd_sth.py), one warp per root vertex.  The packed CSR lists every vertex's out-neighbours in the reference's
  * edge-dictionary order (every packed vertex is a root), the packed labels are one id per distinct str(label), and
  * rank[V] orders the label values within each graph (equal values share a rank).  Root v's DAG is the BFS from v cut
