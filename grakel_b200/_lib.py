@@ -458,20 +458,23 @@ class Engine:
             self._check(self.lib.gk_sm_counts(self.h, int(n_fit), int(row), _ptr(out)))
         return out
 
-    def sm_wl_features(self, k, n_iter, level_ids, lambdas, etable=None, edge_label=None, flags=0):
-        """WeisfeilerLehman over SubgraphMatching (gk_sm_wl_features): level_ids [V, n_iter + 1] the WL class of every
-        packed vertex per level (None with GK_SM_KV_NONE); the next gram() returns the level sum in one enumeration."""
+    def _sm_level_features(self, fn, n_lv, k, n_iter, level_ids, lambdas, etable, edge_label, flags):
         lam = np.ascontiguousarray(lambdas, dtype=np.float64).ravel()
         et = None if etable is None else np.ascontiguousarray(etable, dtype=np.float64)
         el = None if edge_label is None else _i32(edge_label)
         ids = None if level_ids is None else _i32(level_ids)
         st = GkStats()
         with self._lock:
-            self._check(self.lib.gk_sm_wl_features(self.h, int(k), int(n_iter), _ptr(ids), _ptr(lam), _ptr(et),
-                                                   0 if et is None else et.shape[0], _ptr(el), int(flags),
-                                                   C.byref(st)))
-        self.sm_k, self.sm_n_lv = int(k), int(n_iter) + 1
+            self._check(fn(self.h, int(k), int(n_iter), _ptr(ids), _ptr(lam), _ptr(et), 0 if et is None else et.shape[0],
+                           _ptr(el), int(flags), C.byref(st)))
+        self.sm_k, self.sm_n_lv = int(k), int(n_lv)
         return st
+
+    def sm_wl_features(self, k, n_iter, level_ids, lambdas, etable=None, edge_label=None, flags=0):
+        """WeisfeilerLehman over SubgraphMatching (gk_sm_wl_features): level_ids [V, n_iter + 1] the WL class of every
+        packed vertex per level (None with GK_SM_KV_NONE); the next gram() returns the level sum in one enumeration."""
+        return self._sm_level_features(self.lib.gk_sm_wl_features, int(n_iter) + 1, k, n_iter, level_ids, lambdas,
+                                       etable, edge_label, flags)
 
     def sm_wl_counts(self, n_fit, row):
         """tv [n_fit, n_iter + 1, k + 1] of every level of the pairs of row `row` of the gram() request with this
@@ -485,16 +488,8 @@ class Engine:
         """HadamardCode over SubgraphMatching (gk_sm_hc_features): level_ids [V, n_iter] the HadamardCode class of
         every packed vertex per level (None with GK_SM_KV_NONE); the next gram() returns the level sum in one
         enumeration."""
-        lam = np.ascontiguousarray(lambdas, dtype=np.float64).ravel()
-        et = None if etable is None else np.ascontiguousarray(etable, dtype=np.float64)
-        el = None if edge_label is None else _i32(edge_label)
-        ids = None if level_ids is None else _i32(level_ids)
-        st = GkStats()
-        with self._lock:
-            self._check(self.lib.gk_sm_hc_features(self.h, int(k), int(n_iter), _ptr(ids), _ptr(lam), _ptr(et),
-                                                   0 if et is None else et.shape[0], _ptr(el), int(flags),
-                                                   C.byref(st)))
-        return st
+        return self._sm_level_features(self.lib.gk_sm_hc_features, n_iter, k, n_iter, level_ids, lambdas, etable,
+                                       edge_label, flags)
 
     def ml_begin(self, L, gamma, heta, phi):
         """MultiscaleLaplacian: adjacency, balls and level-0 features phi [V, dim] of the packed block (gk_ml_begin)."""

@@ -26,7 +26,7 @@ from sklearn.utils.validation import check_is_fitted
 
 from . import _lib
 from .kernels import (CoreLevel, Kernel, NeighborhoodHash, OddSth, ShortestPath, SubgraphMatching, VertexHistogram,
-                      WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment)
+                      WeisfeilerLehman, WeisfeilerLehmanOptimalAssignment, parse_base_kernel)
 from .packing import Block, Graph, adjacency_and_order, label_ids, pack
 
 
@@ -191,36 +191,16 @@ class CoreFramework(Kernel):
     def initialize(self):
         super().initialize()
         if not self._initialized["base_graph_kernel"]:  # core_framework.py:59-88
-            base = self.base_graph_kernel
-            if base is None:
-                base, params = ShortestPath, dict()
-            elif type(base) is type and issubclass(base, Kernel):
-                params = dict()
-            else:
-                try:
-                    base, params = base
-                except Exception:
-                    raise TypeError("Base kernel was not formulated in the correct way. Check documentation.")
-                if not (type(base) is type and issubclass(base, Kernel)):
-                    raise TypeError("The first argument must be a valid grakel.kernel.kernel Object")
-                if type(params) is not dict:
-                    raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
-                                     "parameters names and values")
-                params = dict(params)
-                params.pop("normalize", None)
-            if base not in (ShortestPath, WeisfeilerLehman, VertexHistogram) + _FOLD_BASES:
-                raise NotImplementedError("grakel_b200 runs CoreFramework over ShortestPath, WeisfeilerLehman, "
-                                          "VertexHistogram, NeighborhoodHash, OddSth, "
-                                          "WeisfeilerLehmanOptimalAssignment or SubgraphMatching; other base kernels "
-                                          "are outside the device hot path")
+            base, params = parse_base_kernel(
+                self, ShortestPath, (ShortestPath, WeisfeilerLehman, VertexHistogram) + _FOLD_BASES,
+                "grakel_b200 runs CoreFramework over ShortestPath, WeisfeilerLehman, VertexHistogram, NeighborhoodHash, "
+                "OddSth, WeisfeilerLehmanOptimalAssignment or SubgraphMatching; other base kernels are outside the "
+                "device hot path", copy=True)
             if base is SubgraphMatching and params.get("ke", SubgraphMatching().ke) is not None:
                 # a level subgraph keeps its edge labels under the original vertex ids while the adjacency view
                 # renumbers the vertices, so the reference's edge kernel reads labels of other edges or fails
                 raise NotImplementedError("CoreFramework over SubgraphMatching needs ke=None: the reference's level "
                                           "subgraphs do not carry usable edge labels")
-            params["normalize"] = False
-            params["verbose"] = self.verbose
-            params["n_jobs"] = None
             self.base_graph_kernel_ = base
             self.params_ = params
             self._base = base(**params)  # validates the parameters exactly like the reference's per-level instances

@@ -3153,22 +3153,22 @@ int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
 }
 
 
-// WeisfeilerLehman over SubgraphMatching (sm_wl_pairs): gk_sm_features' records, tables and lambdas, and the WL class
-// of every packed vertex at every level; gk_gram then returns the level sum of the per-level SubgraphMatching Grams
-int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
-                      const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
-                      gk_stats* stats) {
+// A relabelling framework over SubgraphMatching: gk_sm_features' records, tables and lambdas, and the class of every
+// packed vertex at each of n_lv levels; gk_gram then returns the level sum of the per-level SubgraphMatching Grams from
+// one enumeration per pair.  Levels that refine each other (WL) run sm_wl_pairs, others (HadamardCode) sm_mask_pairs.
+static int sm_level_features(gk_handle* h, const char* fn, int32_t k, int32_t n_iter, int n_lv, int bins,
+                             const char* cap_msg, bool refine, const int32_t* level_ids, const double* lambdas,
+                             const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                             gk_stats* stats) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sm_wl_features: no graphs packed");
-  if (n_iter < 1) return fail(GK_ERR_ARG, "gk_sm_wl_features: n_iter < 1");
+  if (h->N <= 0) return fail(GK_ERR_STATE, std::string(fn) + ": no graphs packed");
+  if (n_iter < 1) return fail(GK_ERR_ARG, std::string(fn) + ": n_iter < 1");
   if (!(flags & (GK_SM_KV_NONE | GK_SM_KV_DIRAC)))
-    return fail(GK_ERR_UNSUPPORTED, "gk_sm_wl_features: the vertex kernel must be GK_SM_KV_DIRAC or GK_SM_KV_NONE");
+    return fail(GK_ERR_UNSUPPORTED, std::string(fn) + ": the vertex kernel must be GK_SM_KV_DIRAC or GK_SM_KV_NONE");
   const bool all_levels = (flags & GK_SM_KV_NONE) != 0;
-  if (!all_levels && !level_ids) return fail(GK_ERR_ARG, "gk_sm_wl_features: no level ids");
-  const int n_lv = n_iter + 1;
+  if (!all_levels && !level_ids) return fail(GK_ERR_ARG, std::string(fn) + ": no level ids");
   const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
-  if ((int64_t)n_lv * kk > SM_WL_BINS)
-    return fail(GK_ERR_UNSUPPORTED, "gk_sm_wl_features: (n_iter + 1) * min(k, largest graph) is more than 64");
+  if ((int64_t)n_lv * kk > bins) return fail(GK_ERR_UNSUPPORTED, std::string(fn) + ": " + cap_msg);
   GK_TRY(gk_sm_features(h, k, lambdas, nullptr, 0, etable, n_elabels, edge_label, flags, stats));
   const size_t bytes = (size_t)h->V * n_lv * 4;
   GK_TRY(h->sm_wl_cls.ensure(std::max<size_t>(bytes, 4)));
@@ -3177,7 +3177,17 @@ int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* le
     GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffer may be reused once we return
   }
   h->sm_n_lv = n_lv;
+  h->sm_hc = !refine;
   return GK_OK;
+}
+
+// WeisfeilerLehman over SubgraphMatching (sm_wl_pairs): the WL class of every packed vertex at every level 0 .. n_iter
+int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
+                      const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                      gk_stats* stats) {
+  return sm_level_features(h, "gk_sm_wl_features", k, n_iter, n_iter + 1, SM_WL_BINS,
+                           "(n_iter + 1) * min(k, largest graph) is more than 64", true, level_ids, lambdas, etable,
+                           n_elabels, edge_label, flags, stats);
 }
 
 int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
@@ -3187,32 +3197,14 @@ int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
   return sm_counts(h, n_fit, row, out, "gk_sm_wl_counts");
 }
 
-// HadamardCode over SubgraphMatching (sm_mask_pairs): gk_sm_features' records, tables and lambdas, and the
-// HadamardCode class of every packed vertex at every level 0 .. n_iter - 1; gk_gram then returns the level sum of the
-// per-level SubgraphMatching Grams from one enumeration per pair
+// HadamardCode over SubgraphMatching (sm_mask_pairs): the HadamardCode class of every packed vertex at every level
+// 0 .. n_iter - 1
 int gk_sm_hc_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* level_ids, const double* lambdas,
                       const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
                       gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sm_hc_features: no graphs packed");
-  if (n_iter < 1) return fail(GK_ERR_ARG, "gk_sm_hc_features: n_iter < 1");
-  if (!(flags & (GK_SM_KV_NONE | GK_SM_KV_DIRAC)))
-    return fail(GK_ERR_UNSUPPORTED, "gk_sm_hc_features: the vertex kernel must be GK_SM_KV_DIRAC or GK_SM_KV_NONE");
-  const bool all_levels = (flags & GK_SM_KV_NONE) != 0;
-  if (!all_levels && !level_ids) return fail(GK_ERR_ARG, "gk_sm_hc_features: no level ids");
-  const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
-  if ((int64_t)n_iter * kk > SM_HC_BINS)
-    return fail(GK_ERR_UNSUPPORTED, "gk_sm_hc_features: n_iter * min(k, largest graph) is more than 64");
-  GK_TRY(gk_sm_features(h, k, lambdas, nullptr, 0, etable, n_elabels, edge_label, flags, stats));
-  const size_t bytes = (size_t)h->V * n_iter * 4;
-  GK_TRY(h->sm_wl_cls.ensure(std::max<size_t>(bytes, 4)));
-  if (!all_levels && bytes > 0) {
-    GK_CUDA(cudaMemcpyAsync(h->sm_wl_cls.p, level_ids, bytes, cudaMemcpyHostToDevice, h->stream));
-    GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffer may be reused once we return
-  }
-  h->sm_n_lv = n_iter;
-  h->sm_hc = true;
-  return GK_OK;
+  return sm_level_features(h, "gk_sm_hc_features", k, n_iter, n_iter, SM_HC_BINS,
+                           "n_iter * min(k, largest graph) is more than 64", false, level_ids, lambdas, etable,
+                           n_elabels, edge_label, flags, stats);
 }
 
 // ---------------------------------------------------------------------------

@@ -35,15 +35,36 @@ from .packing import Block, Graph, adjacency_and_order, label_ids, pack
 
 
 class Fitted:
-    """What `fit` keeps: the packed graphs, their level-0 label ids, the label dictionary."""
+    """What `fit` keeps: the packed graphs, their level-0 label ids, the label dictionary.  Under a relabelling
+    framework also `skip`, the vertices absent from the levels >= 1 (HadamardCode), and the base kernel's own data:
+    its graphs (`base`, _WlBaseData) or its per-level embeddings (`pm`, _PmData)."""
 
-    def __init__(self, block, ids, dictionary):
+    base = None
+    pm = None
+
+    def __init__(self, block, ids, dictionary=None, skip=None):
         self.block = block
         self.ids = ids
         self.dictionary = dictionary
+        self.skip = skip
 
     def __len__(self):
         return self.block.n_graphs
+
+    @staticmethod
+    def concat(a, b):
+        """The fitted input `a` followed by a transform's `b`: what one joint device run reads."""
+        skip = None
+        if a.skip is not None or b.skip is not None:
+            fa = a.skip if a.skip is not None else np.zeros(a.block.n_vertices, dtype=bool)
+            fb = b.skip if b.skip is not None else np.zeros(b.block.n_vertices, dtype=bool)
+            skip = np.concatenate([fa, fb])
+        out = Fitted(Block.concat(a.block, b.block), np.concatenate([a.ids, b.ids]), a.dictionary, skip)
+        if a.base is not None:
+            out.base = _WlBaseData.concat(a.base, b.base)
+        if a.pm is not None:
+            out.pm = _PmData.concat(a.pm, b.pm)
+        return out
 
 
 class CoreLevel:
@@ -451,6 +472,68 @@ _WL_GRAPH_BASES = ()  # set after the base classes: the bases whose WL route nee
 _HC_GRAPH_BASES = ()  # ... and those of HadamardCode's per-level routes
 
 
+def parse_base_kernel(est, default, allowed, refusal, check=None, copy=False):
+    """(base, params) of a framework estimator's `base_graph_kernel`, checked as the reference checks it
+    (weisfeiler_lehman.py:77-109, hadamard_code.py:68-97, core_framework.py:59-88): None (the framework's `default`),
+    a Kernel class or (Kernel class, params dict), `normalize` dropped from the params.  A base outside `allowed`
+    raises NotImplementedError(refusal); `check(base, params)` then runs the base kernel's own checks.  The params get
+    the reference's normalize=False, the estimator's verbose and n_jobs=None; they are the caller's dict, edited in
+    place as the reference does, unless `copy`."""
+    base = est.base_graph_kernel
+    if base is None:
+        base, params = default, dict()
+    elif type(base) is type and issubclass(base, Kernel):
+        params = dict()
+    else:
+        try:
+            base, params = base
+        except Exception:
+            raise TypeError("Base kernel was not formulated in the correct way. Check documentation.")
+        if not (type(base) is type and issubclass(base, Kernel)):
+            raise TypeError("The first argument must be a valid grakel.kernel.kernel Object")
+        if type(params) is not dict:
+            raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
+                             "parameters names and values")
+        if copy:
+            params = dict(params)
+        params.pop("normalize", None)
+    if base not in allowed:
+        raise NotImplementedError(refusal)
+    if check is not None:
+        check(base, params)
+    params["normalize"] = False
+    params["verbose"] = est.verbose
+    params["n_jobs"] = None
+    return base, params
+
+
+def level_base_check(est, who, base, params, reads, ignores, copies):
+    """The base kernel's own checks under a relabelling framework `est` (named `who`), and its refusals: a custom
+    SubgraphMatching vertex kernel (it would read the framework's `reads` per level), ShortestPath(with_labels=False)
+    (it ignores the framework's `ignores`: `copies` * ShortestPath is the same kernel).  Sets est._sm, the
+    SubgraphMatching that checks the elements, or None."""
+    est._sm = None
+    if base is NeighborhoodSubgraphPairwiseDistance:
+        NeighborhoodSubgraphPairwiseDistance(**{k: v for k, v in params.items() if k in ("r", "d")}).initialize()
+    if base is OddSth:
+        OddSth(h=params.get("h")).initialize()
+    if base is SubgraphMatching:  # subgraph_matching.py:70-120
+        sm = SubgraphMatching(**{k: v for k, v in params.items() if k in ("k", "kv", "ke", "lw")})
+        sm.initialize()
+        if sm.kv is not None and sm.kv is not _dirac:
+            raise NotImplementedError("%s over SubgraphMatching runs kv=_dirac or kv=None: a custom vertex kernel "
+                                      "reads the reference's %s per level" % (who, reads))
+        est._sm = sm
+    if base is PyramidMatch:  # pyramid_match.py:62-81
+        PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
+    if base is ShortestPath:
+        if not params.get("with_labels", True):
+            raise NotImplementedError("%s over ShortestPath(with_labels=False) ignores the %s; use %s * "
+                                      "ShortestPath(with_labels=False)" % (who, ignores, copies))
+        if params.get("algorithm_type", "auto") not in ("auto", "floyd_warshall", "dijkstra"):
+            raise ValueError('Unsupported "algorithm_type"')
+
+
 class WeisfeilerLehman(Kernel):
     """Weisfeiler-Lehman subtree kernel (weisfeiler_lehman.py:23-555).
 
@@ -479,52 +562,14 @@ class WeisfeilerLehman(Kernel):
     def initialize(self):
         super().initialize()
         if not self._initialized["base_graph_kernel"]:  # weisfeiler_lehman.py:77-109
-            base = self.base_graph_kernel
-            if base is None:
-                base, params = VertexHistogram, dict()
-            elif type(base) is type and issubclass(base, Kernel):
-                params = dict()
-            else:
-                try:
-                    base, params = base
-                except Exception:
-                    raise TypeError("Base kernel was not formulated in the correct way. Check documentation.")
-                if not (type(base) is type and issubclass(base, Kernel)):
-                    raise TypeError("The first argument must be a valid grakel.kernel.kernel Object")
-                if type(params) is not dict:
-                    raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
-                                     "parameters names and values")
-                params.pop("normalize", None)
-            if base not in (VertexHistogram, EdgeHistogram, ShortestPath, PyramidMatch,
-                            NeighborhoodSubgraphPairwiseDistance, OddSth, SubgraphMatching):
-                raise NotImplementedError("grakel_b200 runs WeisfeilerLehman over VertexHistogram (the subtree kernel), "
-                                          "EdgeHistogram, ShortestPath, PyramidMatch, "
-                                          "NeighborhoodSubgraphPairwiseDistance, OddSth or SubgraphMatching; other "
-                                          "base kernels are outside the device hot path")
-            if base is NeighborhoodSubgraphPairwiseDistance:  # the base kernel's own checks
-                NeighborhoodSubgraphPairwiseDistance(**{k: v for k, v in params.items() if k in ("r", "d")}).initialize()
-            if base is OddSth:
-                OddSth(h=params.get("h")).initialize()
-            if base is SubgraphMatching:  # the base kernel's own checks (subgraph_matching.py:70-120)
-                sm = SubgraphMatching(**{k: v for k, v in params.items() if k in ("k", "kv", "ke", "lw")})
-                sm.initialize()
-                if sm.kv is not None and sm.kv is not _dirac:
-                    raise NotImplementedError("WeisfeilerLehman over SubgraphMatching runs kv=_dirac or kv=None: a "
-                                              "custom vertex kernel reads the reference's label numbers per level")
-                self._sm = sm
-            if base is PyramidMatch:  # the base kernel's own checks (pyramid_match.py:62-81)
-                PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
-            if base is ShortestPath:
-                if not params.get("with_labels", True):
-                    raise NotImplementedError("WeisfeilerLehman over ShortestPath(with_labels=False) ignores the WL "
-                                              "labels; use (n_iter + 1) * ShortestPath(with_labels=False)")
-                if params.get("algorithm_type", "auto") not in ("auto", "floyd_warshall", "dijkstra"):
-                    raise ValueError('Unsupported "algorithm_type"')
-            params["normalize"] = False
-            params["verbose"] = self.verbose
-            params["n_jobs"] = None
-            self._base_graph_kernel = base
-            self._params = params
+            self._base_graph_kernel, self._params = parse_base_kernel(
+                self, VertexHistogram, (VertexHistogram, EdgeHistogram, ShortestPath, PyramidMatch,
+                                        NeighborhoodSubgraphPairwiseDistance, OddSth, SubgraphMatching),
+                "grakel_b200 runs WeisfeilerLehman over VertexHistogram (the subtree kernel), EdgeHistogram, "
+                "ShortestPath, PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth or SubgraphMatching; other "
+                "base kernels are outside the device hot path",
+                lambda base, params: level_base_check(self, "WeisfeilerLehman", base, params, "label numbers",
+                                                      "WL labels", "(n_iter + 1)"))
             self._initialized["base_graph_kernel"] = True
         if not self._initialized["n_iter"]:  # :111-115
             if type(self.n_iter) is not int or self.n_iter <= 0:
@@ -612,7 +657,7 @@ class WeisfeilerLehman(Kernel):
         if X is None:
             raise ValueError("transform input cannot be None")
         self.X = self.parse_input(X)
-        K, xdiag, _ = self._run(self.X.block, self.X.ids, n_fit=self._nx)
+        K, xdiag, _ = self._run(self.X, n_fit=self._nx)
         self._X_diag = xdiag
         return K
 
@@ -633,13 +678,10 @@ class WeisfeilerLehman(Kernel):
         if not isinstance(X, (Iterable, Block)):
             raise ValueError("input must be an iterable\n")
         Y = self.parse_input(X)
-        self._pm_y = Y.pm
-        self._base_y = Y.base
         if self._base_graph_kernel is OddSth and self.normalize and not getattr(self, "_fit_transformed", False):
             # the reference's diagonal() asks the fitted OddSth levels for self._phi_X, which they never set
             raise AttributeError("'OddSth' object has no attribute '_phi_X'")
-        K, xdiag, ydiag = self._run(Block.concat(self.X.block, Y.block), np.concatenate([self.X.ids, Y.ids]),
-                                    n_fit=self._nx)
+        K, xdiag, ydiag = self._run(Fitted.concat(self.X, Y), n_fit=self._nx)
         self._X_diag = xdiag
         self._Y_diag = ydiag
         self._is_transformed = True
@@ -648,26 +690,22 @@ class WeisfeilerLehman(Kernel):
     def _device_features(self, eng):
         if self._base_graph_kernel is ShortestPath:
             return eng.wl_sp_features(self._n_iter - 1, dijkstra_order=True)  # the base kernel gets edge dictionaries
-        if self._base_graph_kernel is PyramidMatch:
-            # every WL level's classes label a PyramidMatch of its own; the joint relabel of X and Y gives classes
-            # unseen at fit columns no fitted graph has (the reference's row cut)
-            p = self._params
-            pm = self.X.pm if eng.n_graphs == self._nx else _PmData.concat(self.X.pm, self._pm_y)
-            with_labels = p.get("with_labels", True)
-            eng.wl_features(self._n_iter - 1)
-            return eng.pm_features(p.get("L", 4), p.get("d", 6), pm.U, pm.n_cols, n_iter=self._n_iter - 1,
-                                   flags=_lib.GK_PM_WL_LABELS if with_labels else 0, skip=pm.skip)
         return eng.wl_features(self._n_iter - 1)
 
     def diagonal(self):
-        if self._base_graph_kernel is OddSth:
-            check_is_fitted(self, ["X"])
-            if not getattr(self, "_fit_transformed", False):
-                if not getattr(self, "_is_transformed", False):
-                    raise NotFittedError("This OddSth instance is not fitted yet. Call 'fit' with appropriate arguments "
-                                         "before using this estimator.")
-                raise AttributeError("'OddSth' object has no attribute '_phi_X'")
-        return super().diagonal()
+        check_is_fitted(self, ["X"])
+        if self._base_graph_kernel is OddSth and not getattr(self, "_fit_transformed", False):
+            if not getattr(self, "_is_transformed", False):
+                raise NotFittedError("This OddSth instance is not fitted yet. Call 'fit' with appropriate arguments "
+                                     "before using this estimator.")
+            raise AttributeError("'OddSth' object has no attribute '_phi_X'")
+        try:
+            check_is_fitted(self, ["_X_diag"])
+        except NotFittedError:
+            _, self._X_diag, _ = self._run(self.X, n_fit=self._nx, want_matrix=False)
+        if getattr(self, "_is_transformed", False):
+            return self._X_diag, self._Y_diag
+        return self._X_diag
 
     def _base_data(self, X, block):
         """NeighborhoodSubgraphPairwiseDistance / OddSth / SubgraphMatching base: see base_graph_data."""
@@ -676,30 +714,41 @@ class WeisfeilerLehman(Kernel):
             return None
         return base_graph_data(X, block, base, getattr(self, "_sm", None), "WeisfeilerLehman")
 
-    def _level_labels(self, block, ids, n_fit_vertices):
-        """The reference's label of every WL vertex at every level: the device partition, numbered on the host."""
-        with _lib.engine(getattr(self, "device_", None)) as eng:
-            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
-            eng.wl_features(self._n_iter - 1)
-            classes = [ids] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, self._n_iter)]
+    def _relabel(self, eng, block, ids):
+        """Pack the WL vertex set and relabel it on the device: every level's classes stay on `eng` (gk_wl_features)."""
+        eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
+        eng.wl_features(self._n_iter - 1)
+
+    def _level_classes(self, eng, block, ids):
+        """[V, n_iter + 1]: the WL class of every packed vertex at every level, level 0 its label id (gk_wl_labels)."""
+        self._relabel(eng, block, ids)
+        return np.stack([ids] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, self._n_iter)], axis=1)
+
+    def _base_run(self, data, n_fit, want_matrix=True, row_range=None, device_ptr=None):
+        """WL over PyramidMatch, NeighborhoodSubgraphPairwiseDistance, OddSth or SubgraphMatching: K = sum over the levels
+        of the base kernel on the level's labels (weisfeiler_lehman.py:260-270), by that base's level route.  NSPD and
+        OddSth read the reference's label numbers, so the device partition is numbered on the host first."""
+        base, p = self._base_graph_kernel, self._params
+        block, ids = data.block, data.ids
+        if base is PyramidMatch:
+            relabel = functools.partial(self._relabel, block=block, ids=ids) if p.get("with_labels", True) else None
+            return pm_level_run(self, data.pm, block, relabel, self._n_iter, p.get("L", 4), p.get("d", 6), n_fit,
+                                want_matrix, row_range, device_ptr)
+        classes = None
+        if not (base is SubgraphMatching and self._sm.kv is None):
+            with _lib.engine(getattr(self, "device_", None)) as eng:
+                classes = self._level_classes(eng, block, ids)
+        if base is SubgraphMatching:
+            return sm_level_run(self, data.base, classes, True, self._n_iter - 1, n_fit, want_matrix, row_range,
+                                device_ptr)
         t0 = time.perf_counter()
         _, labels = wl_reference_dictionaries(np.asarray(block.row_ptr), np.asarray(block.col_idx), ids,
-                                              len(self.X.dictionary), classes, n_fit_vertices=n_fit_vertices)
+                                              len(self.X.dictionary), classes.T,
+                                              n_fit_vertices=int(np.asarray(block.graph_ptr)[n_fit]))
         self.ms_host_numbering_ = (time.perf_counter() - t0) * 1e3
-        return labels
-
-    def _base_run(self, block, ids, n_fit, want_matrix=True, row_range=None):
-        """WL over NeighborhoodSubgraphPairwiseDistance or OddSth: K = sum over the levels of the base kernel on the
-        level's reference labels (weisfeiler_lehman.py:260-270)."""
-        if n_fit == block.n_graphs:
-            data = self.X.base
-        else:
-            data = _WlBaseData.concat(self.X.base, self._base_y)
-        n_fit_v = int(np.asarray(block.graph_ptr)[n_fit])
-        labels = self._level_labels(block, ids, n_fit_v)
-        if self._base_graph_kernel is OddSth:
-            return self._wl_odd_run(data, labels, n_fit, want_matrix, row_range)
-        return self._wl_nspd_run(data, labels, n_fit, want_matrix, row_range)
+        if base is OddSth:
+            return self._wl_odd_run(data.base, labels, n_fit, want_matrix, row_range)
+        return self._wl_nspd_run(data.base, labels, n_fit, want_matrix, row_range)
 
     def _wl_odd_run(self, data, labels, n_fit, want_matrix, row_range):
         b = data.block
@@ -734,42 +783,13 @@ class WeisfeilerLehman(Kernel):
         return nspd_level_sum(self, data, levels(), self._n_iter, n_fit, want_matrix, row_range, p.get("r", 3),
                               p.get("d", 4))
 
-    def _wl_sm_run(self, block, ids, n_fit, want_matrix=True, row_range=None, device_ptr=None):
-        """WL over SubgraphMatching (gk_sm_wl_features): the joint device partition of the fitted and new graphs gives
-        every base vertex its class per level, and one clique enumeration per pair gives K = sum over the levels of
-        SubgraphMatching on the level's labels.  With kv=_dirac the level-h product graph is the level-0 one on the
-        vertices whose classes agree up to level h; with kv=None every level is level 0 (DESIGN 4.23)."""
-        data = self.X.base if n_fit == block.n_graphs else _WlBaseData.concat(self.X.base, self._base_y)
-        sm, n_iter = self._sm, self._n_iter - 1
-        with _lib.engine(getattr(self, "device_", None)) as eng:
-            level_ids, vl = None, None
-            if sm.kv is not None:
-                eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
-                eng.wl_features(n_iter)
-                classes = [np.asarray(ids)] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, n_iter + 1)]
-                level_ids = np.stack(classes, axis=1)[data.src]
-                vl = level_ids[:, 0]
-            graphs, v0 = [], 0
-            for n, edges, _, el in data.graphs:
-                graphs.append((n, edges, None if vl is None else vl[v0:v0 + n].tolist(), el))
-                v0 += n
-            gp, rp, ci, lab, elids, _, et, flags = sm._pack(graphs)
-            eng.pack(gp, rp, ci, lab, None, None)
-            self.stats_ = eng.sm_wl_features(int(sm.k), n_iter, level_ids, sm.lambdas_, et, elids, flags)
-            K, xd, yd = eng.gram(len(graphs), n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
-                                 nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
-                                 device_ptr=device_ptr, stats=self.stats_)
-        if self.verbose:
-            print(type(self).__name__, self.stats_.as_dict())
-        return K, xd, yd
-
-    def _run(self, block, ids, n_fit, want_matrix=True):
-        """The plain subtree fit_transform (square, un-normalised) is ONE C call, gk_wl_gram: relabel, column statistics,
-        head/tail decision on the device, GEMM, tail and delivery with a single host synchronisation."""
-        if self._base_graph_kernel is SubgraphMatching:
-            return self._wl_sm_run(block, ids, n_fit, want_matrix)
-        if self._base_graph_kernel in (NeighborhoodSubgraphPairwiseDistance, OddSth):
-            return self._base_run(block, ids, n_fit, want_matrix)
+    def _run(self, data, n_fit, want_matrix=True):
+        """`data`: a Fitted, the fitted graphs first.  The plain subtree fit_transform (square, un-normalised) is ONE C
+        call, gk_wl_gram: relabel, column statistics, head/tail decision on the device, GEMM, tail and delivery with a
+        single host synchronisation."""
+        block, ids = data.block, data.ids
+        if self._base_graph_kernel in _WL_GRAPH_BASES:
+            return self._base_run(data, n_fit, want_matrix)
         if (want_matrix and not self.normalize and n_fit == block.n_graphs and self._base_graph_kernel is VertexHistogram
                 and type(self) is WeisfeilerLehman):
             with _lib.engine(getattr(self, "device_", None)) as eng:
@@ -787,11 +807,9 @@ class WeisfeilerLehman(Kernel):
         check_is_fitted(self, ["X", "_nx"])
         block, ids = self.X.block, self.X.ids
         with _lib.engine(getattr(self, "device_", None)) as eng:
-            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, ids, None, None)
-            eng.wl_features(self._n_iter - 1)
-            classes = [ids] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, self._n_iter)]
+            classes = self._level_classes(eng, block, ids)
         out, self.wl_labels_ = wl_reference_dictionaries(np.asarray(block.row_ptr), np.asarray(block.col_idx), ids,
-                                                         len(self.X.dictionary), classes)
+                                                         len(self.X.dictionary), classes.T)
         return out
 
 
@@ -842,6 +860,56 @@ def nspd_level_sum(est, data, levels, n_levels, n_fit, want_matrix, row_range, r
         xd = xd_sum if xd is None else np.asarray(xd, dtype=np.float64).reshape(-1)
         K, _ = eng.wl_level_sum_fetch(re_ - rb, n_fit, normalize=bool(est.normalize), xdiag=xd, ydiag=yd_sum)
         return K, xd, yd_sum
+
+
+def sm_level_features(eng, sm, data, classes, refine, n_iter):
+    """SubgraphMatching `sm` under a relabelling framework, set up on `eng` for one enumeration of every level:
+    `data` (_WlBaseData) the base graphs, `classes` [V, n_levels] the class of every packed framework vertex per level
+    (None with kv=None: every level is level 0).  Levels that refine each other (WL's) run gk_sm_wl_features, others
+    (HadamardCode's) gk_sm_hc_features; `n_iter` is the framework's own.  Returns the stats."""
+    level_ids = None if classes is None else classes[data.src]
+    graphs, v0 = [], 0
+    for n, edges, _, el in data.graphs:
+        graphs.append((n, edges, None if level_ids is None else level_ids[v0:v0 + n, 0].tolist(), el))
+        v0 += n
+    gp, rp, ci, lab, elids, _, et, flags = sm._pack(graphs)
+    eng.pack(gp, rp, ci, lab, None, None)
+    features = eng.sm_wl_features if refine else eng.sm_hc_features
+    return features(int(sm.k), n_iter, level_ids, sm.lambdas_, et, elids, flags)
+
+
+def sm_level_run(est, data, classes, refine, n_iter, n_fit, want_matrix, row_range=None, device_ptr=None):
+    """SubgraphMatching (est._sm) under a relabelling framework `est`: K = sum over the levels of SubgraphMatching on
+    the level's classes, from one clique enumeration per pair (DESIGN 4.23, 4.24); see sm_level_features.
+    Returns (K, xdiag, ydiag)."""
+    with _lib.engine(getattr(est, "device_", None)) as eng:
+        est.stats_ = sm_level_features(eng, est._sm, data, classes, refine, n_iter)
+        K, xd, yd = eng.gram(len(data.graphs), n_fit=n_fit, normalize=bool(est.normalize) and want_matrix,
+                             nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
+                             device_ptr=device_ptr, stats=est.stats_)
+    if est.verbose:
+        print(type(est).__name__, est.stats_.as_dict())
+    return K, xd, yd
+
+
+def pm_level_run(est, pm, block, relabel, n_levels, L, d, n_fit, want_matrix, row_range=None, device_ptr=None):
+    """PyramidMatch under a relabelling framework `est`: every level's classes label a PyramidMatch of its own over
+    the level's embeddings `pm` (_PmData, see pm_level_embeddings).  `relabel(eng)` packs `block` and relabels it on
+    the device, where gk_pm_features reads every level's classes; None (with_labels=False): no labels, no relabelling.
+    Returns (K, xdiag, ydiag)."""
+    with _lib.engine(getattr(est, "device_", None)) as eng:
+        if relabel is None:
+            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, None, None, None)
+        else:
+            relabel(eng)
+        est.stats_ = eng.pm_features(L, d, pm.U, pm.n_cols, n_iter=n_levels - 1,
+                                     flags=0 if relabel is None else _lib.GK_PM_WL_LABELS, skip=pm.skip)
+        K, xd, yd = eng.gram(block.n_graphs, n_fit=n_fit, normalize=bool(est.normalize) and want_matrix,
+                             nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
+                             device_ptr=device_ptr, stats=est.stats_)
+    if est.verbose:
+        print(type(est).__name__, est.stats_.as_dict())
+    return K, xd, yd
 
 
 def base_graph_data(X, block, base, sm, who):
@@ -2791,35 +2859,6 @@ def _enum_ids(labels, enum):
     return np.fromiter((enum[l] for l in labels), dtype=np.int32, count=len(labels))
 
 
-class _HcData:
-    """One parsed input of HadamardCode: the packed block, its enumeration ids, the skip flags of the levels >= 1, and
-    for SubgraphMatching / NSPD the base kernel's graphs (`base`, _WlBaseData), for PyramidMatch its per-level
-    embeddings (`pm`, _PmData)."""
-
-    base = None
-    pm = None
-
-    def __init__(self, block, ids, skip):
-        self.block, self.ids, self.skip = block, ids, skip
-
-    def __len__(self):
-        return self.block.n_graphs
-
-    @staticmethod
-    def concat(a, b):
-        skip = None
-        if a.skip is not None or b.skip is not None:
-            fa = a.skip if a.skip is not None else np.zeros(a.block.n_vertices, dtype=bool)
-            fb = b.skip if b.skip is not None else np.zeros(b.block.n_vertices, dtype=bool)
-            skip = np.concatenate([fa, fb])
-        out = _HcData(Block.concat(a.block, b.block), np.concatenate([a.ids, b.ids]), skip)
-        if a.base is not None:
-            out.base = _WlBaseData.concat(a.base, b.base)
-        if a.pm is not None:
-            out.pm = _PmData.concat(a.pm, b.pm)
-        return out
-
-
 class HadamardCode(Kernel):
     """Hadamard code kernel (hadamard_code.py:24-391): K = sum over n_iter levels of the base kernel on the vertices'
     Hadamard-code vectors.  Level 0 gives every labelled vertex row `enumeration id` of the W x W Sylvester Hadamard
@@ -2854,50 +2893,14 @@ class HadamardCode(Kernel):
             self._parallel = None
             self._initialized["n_jobs"] = True
         if not self._initialized["base_graph_kernel"]:  # hadamard_code.py:68-97
-            base = self.base_graph_kernel
-            if base is None:
-                base, params = VertexHistogram, dict()
-            elif type(base) is type and issubclass(base, Kernel):
-                params = dict()
-            else:
-                try:
-                    base, params = base
-                except Exception:
-                    raise TypeError("Base kernel was not formulated in the correct way. Check documentation.")
-                if not (type(base) is type and issubclass(base, Kernel)):
-                    raise TypeError("The first argument must be a valid grakel.kernel.kernel Object")
-                if type(params) is not dict:
-                    raise ValueError("If the second argument of base kernel exists, it must be a dictionary between "
-                                     "parameters names and values")
-                params.pop("normalize", None)
-            if base not in (VertexHistogram, ShortestPath, EdgeHistogram, SubgraphMatching, PyramidMatch,
-                            NeighborhoodSubgraphPairwiseDistance):
-                raise NotImplementedError("grakel_b200 runs HadamardCode over VertexHistogram, ShortestPath, "
-                                          "EdgeHistogram, SubgraphMatching, PyramidMatch or "
-                                          "NeighborhoodSubgraphPairwiseDistance; other base kernels are outside the "
-                                          "device hot path")
-            self._sm = None
-            if base is SubgraphMatching:  # the base kernel's own checks (subgraph_matching.py:70-120)
-                sm = SubgraphMatching(**{k: v for k, v in params.items() if k in ("k", "kv", "ke", "lw")})
-                sm.initialize()
-                if sm.kv is not None and sm.kv is not _dirac:
-                    raise NotImplementedError("HadamardCode over SubgraphMatching runs kv=_dirac or kv=None: a custom "
-                                              "vertex kernel reads the reference's Hadamard-code tuples per level")
-                self._sm = sm
-            if base is PyramidMatch:  # pyramid_match.py:62-81
-                PyramidMatch(**{k: v for k, v in params.items() if k in ("with_labels", "L", "d")}).initialize()
-            if base is NeighborhoodSubgraphPairwiseDistance:
-                NeighborhoodSubgraphPairwiseDistance(**{k: v for k, v in params.items() if k in ("r", "d")}).initialize()
-            if base is ShortestPath:
-                if not params.get("with_labels", True):
-                    raise NotImplementedError("HadamardCode over ShortestPath(with_labels=False) ignores the Hadamard "
-                                              "codes; use n_iter * ShortestPath(with_labels=False)")
-                if params.get("algorithm_type", "auto") not in ("auto", "floyd_warshall", "dijkstra"):
-                    raise ValueError('Unsupported "algorithm_type"')
-            params["normalize"] = False
-            params["verbose"] = self.verbose
-            params["n_jobs"] = None
-            self.base_graph_kernel_ = (base, params)
+            self.base_graph_kernel_ = parse_base_kernel(
+                self, VertexHistogram, (VertexHistogram, ShortestPath, EdgeHistogram, SubgraphMatching, PyramidMatch,
+                                        NeighborhoodSubgraphPairwiseDistance),
+                "grakel_b200 runs HadamardCode over VertexHistogram, ShortestPath, EdgeHistogram, SubgraphMatching, "
+                "PyramidMatch or NeighborhoodSubgraphPairwiseDistance; other base kernels are outside the device hot "
+                "path",
+                lambda base, params: level_base_check(self, "HadamardCode", base, params, "Hadamard-code tuples",
+                                                      "Hadamard codes", "n_iter"))
             self._initialized["base_graph_kernel"] = True
         if not self._initialized["n_iter"]:  # :99-102
             if type(self.n_iter) is not int or self.n_iter <= 0:
@@ -2934,7 +2937,7 @@ class HadamardCode(Kernel):
         return out
 
     def _parse(self, X, labels_enum):
-        """(_HcData, extended enumeration) of one input."""
+        """(Fitted, extended enumeration) of one input."""
         base = self.base_graph_kernel_[0]
         if isinstance(X, Block):  # packed input (datasets.read_tu): integer labels
             if base is EdgeHistogram:
@@ -2960,7 +2963,7 @@ class HadamardCode(Kernel):
             elif block.mode == "sp" and base is not ShortestPath:
                 raise ValueError("this block was packed for another kernel (vertex set 'sp', needed 'wl'): see "
                                  "grakel_b200.datasets.read_tu(kernel=...)")
-            return _HcData(block, _enum_ids(labels, enum), skip), enum
+            return Fitted(block, _enum_ids(labels, enum), skip=skip), enum
         els = self._elements(X)
         enum = hc_enumerate((x[1] for x in els), labels_enum)
         if base is EdgeHistogram:
@@ -2968,7 +2971,7 @@ class HadamardCode(Kernel):
             sizes = np.concatenate([[0], np.cumsum([len(v) for v in values])])
             block = Block(sizes, np.zeros(int(sizes[-1]) + 1, dtype=np.int64), np.zeros(0, dtype=np.int64), None,
                           [l for v in values for l in v])
-            return _HcData(block, None, None), enum
+            return Fitted(block, None), enum
         if base is ShortestPath:
             # the base kernel receives every element's own graph object (hadamard_code.py:175, 197): its vertices, and
             # Floyd-Warshall or Dijkstra path sums as the element's format implies (_path_sum_order).  Its vertices
@@ -2976,12 +2979,12 @@ class HadamardCode(Kernel):
             block = pack([x[:2] for x in els], "sp", want_weights=True,
                          fw_zero_is_absent=self.base_graph_kernel_[1].get("algorithm_type") == "floyd_warshall",
                          type_error_msg="each element of X must have at least one and at most 3 elements\n")
-            return _HcData(block, _enum_ids(block.labels, enum), None), enum
+            return Fitted(block, _enum_ids(block.labels, enum)), enum
         if self.n_iter == 1 and base not in _HC_GRAPH_BASES:  # level 0 only: the label multisets
             labels = [l for x in els for l in x[1].values()]
             sizes = np.concatenate([[0], np.cumsum([len(x[1]) for x in els])])
             block = Block(sizes, np.zeros(int(sizes[-1]) + 1, dtype=np.int64), np.zeros(0, dtype=np.int64), None, labels)
-            return _HcData(block, _enum_ids(labels, enum), None), enum
+            return Fitted(block, _enum_ids(labels, enum)), enum
         # packed vertices: the keys of every labels dictionary, in its order ('wl' packing)
         skip = []
         for x in els:
@@ -2995,7 +2998,7 @@ class HadamardCode(Kernel):
             skip.append(np.fromiter((k not in keys for k in x[1]), dtype=bool, count=len(x[1])))
         skip = np.concatenate(skip)
         block = pack([x[:2] for x in els], "wl", len_ok=lambda n: n >= 2)
-        data = _HcData(block, _enum_ids(block.labels, enum), skip if skip.any() else None)
+        data = Fitted(block, _enum_ids(block.labels, enum), skip=skip if skip.any() else None)
         if base is PyramidMatch:
             p = self.base_graph_kernel_[1]
             data.pm, self.ms_host_embed_ = pm_level_embeddings(els, block, p.get("d", 6), p.get("L", 4), self.n_iter,
@@ -3055,7 +3058,7 @@ class HadamardCode(Kernel):
         else:
             width = hc_width(len(enum))
         if width == self._width or self.base_graph_kernel_[0] is EdgeHistogram or not self._reads_labels():
-            K, xdiag, ydiag = self._run(_HcData.concat(self.X, Y), n_x, width)
+            K, xdiag, ydiag = self._run(Fitted.concat(self.X, Y), n_x, width)
         else:
             # the vectors of Y are longer than every fitted vector: no label is shared (hadamard_code.py:187, 235) and
             # every Y graph is only similar to itself, at its own width.  (NSPD: the label strings str(tuple) of Y are
@@ -3115,72 +3118,57 @@ class HadamardCode(Kernel):
             print(type(self).__name__, self.stats_.as_dict())
         return K, xd, yd
 
-    def _hc_classes(self, eng, data, width, vectors=False):
-        """The HadamardCode class of every packed vertex at every level, [V, n_iter] (gk_hc_features, gk_wl_labels:
-        exact vector classes, numbered on the device); with `vectors` also, per level, the [V, W] vectors."""
+    def _relabel(self, eng, data, width):
+        """Pack the HadamardCode vertex set and relabel it on the device: every level's classes stay on `eng`
+        (gk_hc_features)."""
         block = data.block
         eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
         eng.hc_features(self.n_iter, width, skip=data.skip)
-        cls = np.stack([eng.wl_labels(lv, block.n_vertices) for lv in range(self.n_iter)], axis=1)
+
+    def _level_classes(self, eng, data, width, vectors=False):
+        """The HadamardCode class of every packed vertex at every level, [V, n_iter] (gk_wl_labels: exact vector
+        classes, numbered on the device); with `vectors` also, per level, the [V, W] vectors."""
+        self._relabel(eng, data, width)
+        n_v = data.block.n_vertices
+        cls = np.stack([eng.wl_labels(lv, n_v) for lv in range(self.n_iter)], axis=1)
         if not vectors:
             return cls, None
-        return cls, [eng.hc_vectors(lv, block.n_vertices, width) for lv in range(self.n_iter)]
+        return cls, [eng.hc_vectors(lv, n_v, width) for lv in range(self.n_iter)]
 
     def _base_run(self, data, n_fit, width, want_matrix, row_range, device_ptr):
         """HadamardCode over SubgraphMatching, PyramidMatch or NSPD: K = sum over the n_iter levels of the base kernel
-        on the level's Hadamard codes, added in level order (hadamard_code.py:217-236, np.sum(axis=0)); DESIGN 4.24."""
+        on the level's Hadamard codes, added in level order (hadamard_code.py:217-236, np.sum(axis=0)), by that base's
+        level route; DESIGN 4.24."""
         base, p = self.base_graph_kernel_
         reads = self._reads_labels()
-        if base is SubgraphMatching:  # gk_sm_hc_features' bin cap, before the relabelling runs
+        if base is PyramidMatch:
+            relabel = functools.partial(self._relabel, data=data, width=width) if reads else None
+            return pm_level_run(self, data.pm, data.block, relabel, self.n_iter, p.get("L", 4), p.get("d", 6), n_fit,
+                                want_matrix, row_range, device_ptr)
+        if base is SubgraphMatching:
             kk = max(1, min(max(int(self._sm.k), 1), max(g[0] for g in data.base.graphs)))
-            if self.n_iter * kk > 64:
+            if self.n_iter * kk > 64:  # gk_sm_hc_features' bin cap, before the relabelling runs
                 raise NotImplementedError("HadamardCode over SubgraphMatching: n_iter * min(k, largest graph) is more "
                                           "than 64")
+            classes = None
+            if reads:
+                with _lib.engine(getattr(self, "device_", None)) as eng:
+                    classes = self._level_classes(eng, data, width)[0]
+            return sm_level_run(self, data.base, classes, False, self.n_iter, n_fit, want_matrix, row_range,
+                                device_ptr)
         with _lib.engine(getattr(self, "device_", None)) as eng:
-            if base is NeighborhoodSubgraphPairwiseDistance:
-                cls, vecs = self._hc_classes(eng, data, width, vectors=True)
-                src = data.base.src
+            cls, vecs = self._level_classes(eng, data, width, vectors=True)
+        src = data.base.src
 
-                def levels():
-                    # the reference hashes str(D) + "," + str(label), label the tuple of numpy int64 of the level's
-                    # vector (neighborhood_subgraph_pairwise_distance.py:443): one string per class, from one vector
-                    for lv in range(self.n_iter):
-                        uniq, first, inv = np.unique(cls[src, lv], return_index=True, return_inverse=True)
-                        rows = vecs[lv][src[first]]
-                        yield inv.reshape(-1), [str(tuple(row)) for row in rows]
-                K, xd, yd = nspd_level_sum(self, data.base, levels(), self.n_iter, n_fit, want_matrix, row_range,
-                                           p.get("r", 3), p.get("d", 4))
-                return K, xd, yd
-            if base is SubgraphMatching:
-                sm = self._sm
-                level_ids = None
-                if reads:
-                    level_ids = self._hc_classes(eng, data, width)[0][data.base.src]
-                graphs, v0 = [], 0
-                for n, edges, _, el in data.base.graphs:
-                    graphs.append((n, edges, None if level_ids is None else level_ids[v0:v0 + n, 0].tolist(), el))
-                    v0 += n
-                gp, rp, ci, lab, elids, _, et, flags = sm._pack(graphs)
-                eng.pack(gp, rp, ci, lab, None, None)
-                self.stats_ = eng.sm_hc_features(int(sm.k), self.n_iter, level_ids, sm.lambdas_, et, elids, flags)
-                n_graphs = len(graphs)
-            else:  # PyramidMatch: every level's classes label a PyramidMatch of its own
-                block = data.block
-                if reads:
-                    eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
-                    eng.hc_features(self.n_iter, width, skip=data.skip)
-                else:
-                    eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, None, None, None)
-                self.stats_ = eng.pm_features(p.get("L", 4), p.get("d", 6), data.pm.U, data.pm.n_cols,
-                                              n_iter=self.n_iter - 1,
-                                              flags=_lib.GK_PM_WL_LABELS if reads else 0, skip=data.pm.skip)
-                n_graphs = block.n_graphs
-            K, xd, yd = eng.gram(n_graphs, n_fit=n_fit, normalize=bool(self.normalize) and want_matrix,
-                                 nan_to_num=True, out=None if want_matrix else False, row_range=row_range,
-                                 device_ptr=device_ptr, stats=self.stats_)
-        if self.verbose:
-            print(type(self).__name__, self.stats_.as_dict())
-        return K, xd, yd
+        def levels():
+            # the reference hashes str(D) + "," + str(label), label the tuple of numpy int64 of the level's vector
+            # (neighborhood_subgraph_pairwise_distance.py:443): one string per class, from one vector
+            for lv in range(self.n_iter):
+                uniq, first, inv = np.unique(cls[src, lv], return_index=True, return_inverse=True)
+                rows = vecs[lv][src[first]]
+                yield inv.reshape(-1), [str(tuple(row)) for row in rows]
+        return nspd_level_sum(self, data.base, levels(), self.n_iter, n_fit, want_matrix, row_range, p.get("r", 3),
+                              p.get("d", 4))
 
     def hc_vectors(self, X, level):
         """[V, W] int64 Hadamard-code vectors of every packed vertex of X at `level` (zeros where a vertex is absent
@@ -3189,11 +3177,9 @@ class HadamardCode(Kernel):
         check_is_fitted(self, ["X"])
         data, enum = self._parse(X, self._labels_enum)
         width = hc_width(len(enum))
-        block = data.block
         with _lib.engine(getattr(self, "device_", None)) as eng:
-            eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, data.ids, None, None)
-            eng.hc_features(self.n_iter, width, skip=data.skip)
-            return eng.hc_vectors(level, block.n_vertices, width)
+            self._relabel(eng, data, width)
+            return eng.hc_vectors(level, data.block.n_vertices, width)
 
 
 # ------------------------------------------------------------------------------

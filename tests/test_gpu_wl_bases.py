@@ -9,7 +9,7 @@ import pytest
 import wl_bases_cases as cases
 import wl_bases_oracle as oracle
 from grakel_b200 import GraphKernel, NeighborhoodSubgraphPairwiseDistance, OddSth, WeisfeilerLehman
-from grakel_b200.packing import Block
+from grakel_b200.kernels import Fitted
 
 pytestmark = pytest.mark.gpu
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
@@ -86,14 +86,11 @@ def test_frozen_deep_levels(kind, params):
 
 
 @pytest.mark.parametrize("kind,params", [("NSPD", {"r": 1, "d": 2}), ("ODD", {"h": 2})])
-def test_transform_row_range(kind, params):
+def test_transform_row_range_from_joint_input(kind, params):
     X, Y = cases.fit_set(), cases.transform_set()
     k = wl(kind, params, 2).fit(X)
     K = k.transform(Y)
-    Yf = k.parse_input(Y)
-    k._base_y = Yf.base
-    Kr, _, _ = k._base_run(Block.concat(k.X.block, Yf.block), np.concatenate([k.X.ids, Yf.ids]), k._nx,
-                           row_range=(1, 3))
+    Kr, _, _ = k._base_run(Fitted.concat(k.X, k.parse_input(Y)), k._nx, row_range=(1, 3))
     assert np.array_equal(Kr, K[1:3])
 
 

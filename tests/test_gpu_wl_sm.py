@@ -10,6 +10,7 @@ import pytest
 import wl_sm_cases as cases
 import wl_sm_oracle as oracle
 from grakel_b200 import Graph, GraphKernel, SubgraphMatching, WeisfeilerLehman, _lib
+from grakel_b200.kernels import sm_level_features
 
 pytestmark = pytest.mark.gpu
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
@@ -84,20 +85,10 @@ def test_bench_scale_equals_the_per_level_route(k_sm):
 
 
 def wl_counts(k, n_fit, rows):
-    """gk_sm_wl_counts of `rows` for the estimator's fitted graphs (the setup of WeisfeilerLehman._wl_sm_run)."""
-    sm, n_iter, data, block = k._sm, k._n_iter - 1, k.X.base, k.X.block
+    """gk_sm_wl_counts of `rows` for the estimator's fitted graphs (the setup of the SubgraphMatching level route)."""
     with _lib.engine() as eng:
-        eng.pack(block.graph_ptr, block.row_ptr, block.col_idx, k.X.ids, None, None)
-        eng.wl_features(n_iter)
-        cls = [np.asarray(k.X.ids)] + [eng.wl_labels(lv, block.n_vertices) for lv in range(1, n_iter + 1)]
-        level_ids = np.stack(cls, axis=1)[data.src]
-        graphs, v0 = [], 0
-        for n, edges, _, el in data.graphs:
-            graphs.append((n, edges, level_ids[v0:v0 + n, 0].tolist(), el))
-            v0 += n
-        gp, rp, ci, lab, elids, _, et, flags = sm._pack(graphs)
-        eng.pack(gp, rp, ci, lab, None, None)
-        eng.sm_wl_features(int(sm.k), n_iter, level_ids, sm.lambdas_, et, elids, flags)
+        classes = k._level_classes(eng, k.X.block, k.X.ids)
+        sm_level_features(eng, k._sm, k.X.base, classes, True, k._n_iter - 1)
         return [eng.sm_wl_counts(n_fit, r) for r in rows]
 
 
@@ -129,18 +120,18 @@ def test_level_counts_equal_the_per_level_counts():
 
 
 @pytest.mark.parametrize("params", [{"k": 4}, {"k": 4, "ke": cases.ke_half}])
-def test_routes_row_ranges_and_device_output(params, monkeypatch):
+def test_level_route_row_ranges_and_device_output(params, monkeypatch):
     """Staged and global records give the same K (exact and real sums); so do row ranges and device output."""
     X = bench_workload(300)
     Xf, Y = X[:220], X[220:]
     k = wl(params, 3)
     K = k.fit_transform(Xf)
     Kt = k.transform(Y)
-    Kr, _, _ = k._wl_sm_run(k.X.block, k.X.ids, len(Xf), row_range=(7, 131))
+    Kr, _, _ = k._base_run(k.X, len(Xf), row_range=(7, 131))
     np.testing.assert_array_equal(Kr, K[7:131])
     import torch
     dev = torch.zeros((len(Xf), len(Xf)), dtype=torch.float64, device="cuda")
-    k._wl_sm_run(k.X.block, k.X.ids, len(Xf), device_ptr=dev.data_ptr())
+    k._base_run(k.X, len(Xf), device_ptr=dev.data_ptr())
     torch.cuda.synchronize()
     np.testing.assert_array_equal(dev.cpu().numpy(), K)
     monkeypatch.setenv("GRAKEL_B200_SM_GLOBAL", "1")
