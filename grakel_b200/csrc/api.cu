@@ -162,6 +162,23 @@ using namespace gk;
     GK_CUDA(cudaGetLastError());                        \
   } while (0)
 
+// The entry check of a call on the packed block.  It selects the handle's device, which some argument checks query.
+static int need_packed(gk_handle* h, const char* who) {
+  if (!h) return fail(GK_ERR_ARG, "null handle");
+  if (h->N <= 0) return fail(GK_ERR_STATE, std::string(who) + ": no graphs packed");
+  GK_CUDA(cudaSetDevice(h->dev));
+  return GK_OK;
+}
+
+// A feature pass calls features_begin after its argument checks, before it writes any handle state, and
+// features_publish as its last state change.  A refused call leaves the previous block; a failed pass leaves none.
+static void features_begin(gk_handle* h) {
+  h->feature_kind = FK_NONE;
+  h->pro_ready = false;
+}
+
+static void features_publish(gk_handle* h, FeatureKind kind) { h->feature_kind = kind; }
+
 extern "C" {
 
 int gk_version(void) { return 100; }
@@ -334,14 +351,13 @@ int gk_pack_csr(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const 
     if (n < 0 || graph_ptr[g + 1] > V) return fail(GK_ERR_ARG, "gk_pack_csr: graph_ptr not monotone");
     max_n = std::max(max_n, n);
   }
+  features_begin(h);  // a new block starts without features
   h->N = N; h->V = V; h->E = E;
   h->has_weights = weights != nullptr;
   h->has_labels = labels != nullptr;
   h->attr_dim = attrs ? attr_dim : 0;
   h->max_graph_size = max_n;
-  h->features_ready = false; h->feat_serial++;
-  h->feature_kind = FK_NONE;
-  h->n_rows = 0;  // a new block starts without a row map
+  h->n_rows = 0;  // ... without a row map
   h->hc_W = 0;    // ... and without HadamardCode vectors
   h->ml_w = 0;    // ... and without MultiscaleLaplacian features
   h->wl_tiles_valid = false;
@@ -631,15 +647,13 @@ static int wl_launch_v2(gk_handle* h, const WlPlan& pl, unsigned long long seed,
 extern "C" {
 
 int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_wl_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_wl_features"));
   if (!h->has_labels || h->V == 0) return fail(GK_ERR_ARG, "gk_wl_features: vertex labels are required");
   if (n_iter < 0 || n_iter + 1 >= MAX_LEVELS) return fail(GK_ERR_ARG, "gk_wl_features: n_iter out of range");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t V = h->V, E = h->E;
   const int L = n_iter + 1;
+  features_begin(h);
   h->n_levels = L;
-  h->features_ready = false; h->feat_serial++;
   const int64_t launches0 = h->launches;
 
   WlPlan pl;
@@ -673,7 +687,7 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
         // Gram prologue of the square (fit_transform) case, enqueued BEFORE this call's one host synchronisation:
         // self similarities + per-CTA partials (diag_finish) and the column histogram (col_hist).  gk_gram then
         // finds everything its host-side decisions need (threshold T, D_c, exactness bounds) already on the host
-        // and launches without a synchronisation of its own (pro_serial).
+        // and launches without a synchronisation of its own (pro_ready).
         const int64_t D = (int64_t)h->n_labels0 + V * (int64_t)(L - 1);
         GK_TRY(h->diag_f64.ensure(h->N * 8));
         GK_TRY(h->colstats.ensure(sizeof(ColStats)));
@@ -750,13 +764,12 @@ int gk_wl_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
   }
   DevScalars* hs = h->h_scalars.as<DevScalars>();
   h->n_columns = hs->level_base[L];
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_WL;
   if (pro_enqueued) {
     h->pro_hist = *h->h_colstats.as<ColStats>();
     h->pro_max_count = (long long)hs->max_count; h->pro_max_diag = (long long)hs->max_diag; h->pro_n_entries = (long long)hs->n_entries;
-    h->pro_serial = h->feat_serial;
+    h->pro_ready = true;
   }
+  features_publish(h, FK_WL);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = h->N; stats->n_vertices = V; stats->n_edges = E;
@@ -780,7 +793,7 @@ int gk_wl_oa_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
   gk_stats local;
   gk_stats* st = stats ? stats : &local;
   GK_TRY(gk_wl_features(h, n_iter, st));
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   const int64_t launches0 = h->launches;
   const int64_t D = std::max<int64_t>(h->n_columns, 1);
   const size_t out_cap = std::max<size_t>((size_t)h->V * (size_t)h->n_levels, 1);  // one entry per (vertex, level)
@@ -831,7 +844,7 @@ int gk_wl_oa_features(gk_handle* h, int32_t n_iter, gk_stats* stats) {
   h->ft_cap = out_cap;
   h->col_cap = (int64_t)out_cap + 1;
   h->n_columns = (int64_t)hc.n_cols;
-  h->features_ready = true; h->feat_serial++;
+  features_publish(h, FK_WL);
   st->n_columns = h->n_columns;
   st->kernel_launches += h->launches - launches0;
   st->ms_features = ev_ms(h->tev[2], h->tev[3]);
@@ -883,9 +896,7 @@ struct SpLabels {
 };
 
 static int sp_check(gk_handle* h, int32_t flags) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sp_features: no graphs packed");
-  GK_CUDA(cudaSetDevice(h->dev));
+  GK_TRY(need_packed(h, "gk_sp_features"));
   if ((flags & GK_SP_WITH_LABELS) && !h->has_labels) return fail(GK_ERR_ARG, "gk_sp_features: vertex labels are required");
   return GK_OK;
 }
@@ -900,7 +911,7 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
   const size_t esz = use_u16 ? 2 : 8;
   const int64_t N = h->N;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   h->sp_flags = flags;
 
   // plan: graphs whose distance matrix fits the shared-memory budget vs the rest
@@ -1126,8 +1137,7 @@ static int sp_features_impl(gk_handle* h, int32_t flags, const SpLabels& lab, gk
   GK_CUDA(cudaEventSynchronize(h->tev[3]));
   DevScalars* hs = h->h_scalars.as<DevScalars>();
   h->n_columns = (int64_t)dict_cap;  // column id = dictionary slot
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_SP;
+  features_publish(h, FK_SP);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = h->N; stats->n_vertices = h->V; stats->n_edges = h->E;
@@ -1151,6 +1161,7 @@ int gk_wl_sp_features(gk_handle* h, int32_t n_iter, int32_t flags, gk_stats* sta
   GK_TRY(sp_check(h, flags));
   gk_stats wst;
   GK_TRY(gk_wl_features(h, n_iter, &wst));
+  features_begin(h);
   if (h->wl_sparse_ids) {  // the base kernel's counters are indexed by dense label ids
     for (int lv = 1; lv <= n_iter; ++lv) GK_TRY(wl_densify(h, lv, h->labels_all.as<int>() + (size_t)lv * h->V));
     h->wl_sparse_ids = false;
@@ -1210,8 +1221,7 @@ static int hc_run_levels(gk_handle* h, int upto, const FeatStats* fst, bool coun
 }
 
 int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* skip, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_hc_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_hc_features"));
   if (!h->has_labels || h->V == 0) return fail(GK_ERR_ARG, "gk_hc_features: vertex labels are required");
   if (n_iter < 1 || n_iter >= MAX_LEVELS) return fail(GK_ERR_ARG, "gk_hc_features: n_iter out of range [1, 64)");
   if (width < 1 || (width & (width - 1))) return fail(GK_ERR_ARG, "gk_hc_features: width must be a power of two");
@@ -1222,7 +1232,6 @@ int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* s
   if (sp && skip)
     for (int64_t v = 0; v < V; ++v)
       if (skip[v]) return fail(GK_ERR_ARG, "gk_hc_features: the ShortestPath base needs a label for every vertex at every level");
-  GK_CUDA(cudaSetDevice(h->dev));
   const double need = 2.0 * (double)V * (double)width * 8.0;
   {
     size_t free_b = 0, total_b = 0;
@@ -1235,7 +1244,7 @@ int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* s
   const int L = n_iter;
   const int nb = cdiv(V, 256);
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   h->hc_W = 0;
   GK_TRY(h->hc_S.ensure((size_t)need));
   GK_TRY(h->hc_z.ensure((size_t)width * 8));
@@ -1303,8 +1312,7 @@ int gk_hc_features(gk_handle* h, int32_t n_iter, int32_t width, const uint8_t* s
     return GK_OK;
   }
   h->n_columns = hs.level_base[L];
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_WL;
+  features_publish(h, FK_WL);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = h->N; stats->n_vertices = V; stats->n_edges = h->E;
@@ -1375,17 +1383,15 @@ int gk_sp_distances(gk_handle* h, int64_t g, double* out) {
 }
 
 int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_spattr_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_spattr_features"));
   if (!h->attrs.p || h->attr_dim <= 0) return fail(GK_ERR_ARG, "gk_spattr_features: node attributes are required");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N;
   const int da = h->attr_dim, dd = da * da;
   if (dd > 1024) return fail(GK_ERR_UNSUPPORTED, "gk_spattr_features: attribute dimension above 32");
   const bool use_u16 = (!h->has_weights || h->unit_weights) && h->max_graph_size < 16000;
   const size_t esz = use_u16 ? 2 : 8;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   if ((size_t)h->max_graph_size * h->max_graph_size * 2 + (size_t)h->max_graph_size * da * 8 + (size_t)dd * 8 > 200 * 1024)
     return fail(GK_ERR_UNSUPPORTED, "gk_spattr_features: graph too large for the shared-memory feature kernel");
 
@@ -1507,9 +1513,8 @@ int gk_spattr_features(gk_handle* h, int32_t flags, gk_stats* stats) {
   GK_CUDA(cudaStreamSynchronize(h->stream));  // host vectors above are sources of async copies
   h->fattr_signed = *h_negative != 0;
   h->n_columns = Dfeat;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_SPATTR;
   h->sp_dist_esz = (int)esz;
+  features_publish(h, FK_SPATTR);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
@@ -1624,7 +1629,7 @@ static IntBlock block_of(gk_handle* h) {
   b.colcnt = h->colcnt.as<unsigned>(); b.col_cap = h->col_cap; b.n_columns = h->n_columns;
   b.diag = h->diag_u64.as<unsigned long long>();
   b.part_max = h->part_max.as<unsigned>(); b.part_new = h->part_new.as<unsigned>(); b.n_part = h->n_part;
-  b.prologue_on_host = h->pro_serial == h->feat_serial;
+  b.prologue_on_host = h->pro_ready;
   return b;
 }
 
@@ -1810,8 +1815,7 @@ static int gh_dag_pass(gk_handle* h, const std::vector<int>& gdiam, double* M, l
 extern "C" {
 
 int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_gh_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_gh_features"));
   if (!h->attrs.p || h->attr_dim <= 0) return fail(GK_ERR_ARG, "gk_gh_features: node attributes are required");
   if (node_kernel != GK_GH_LINEAR && node_kernel != GK_GH_GAUSSIAN && node_kernel != GK_GH_BRIDGE)
     return fail(GK_ERR_ARG, "gk_gh_features: unknown node kernel");
@@ -1819,11 +1823,10 @@ int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, 
   if (h->has_weights && !h->unit_weights)
     return fail(GK_ERR_UNSUPPORTED, "GraphHopper: edge weights other than 1 (the shortest-path DAG is defined for "
                                     "unweighted graphs only)");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V;
   const int d = h->attr_dim;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   // pass 1: eccentricities -> per-graph diameter and delta = max diameter + 1
   GK_TRY(h->gh_gdiam.ensure((size_t)(N + 1) * 4));
@@ -1876,8 +1879,7 @@ int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, 
   h->gh_node_kernel = node_kernel;
   h->gh_mu = mu;
   h->n_columns = n_columns;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_GH;
+  features_publish(h, FK_GH);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
@@ -1893,7 +1895,7 @@ int gk_gh_features(gk_handle* h, int32_t node_kernel, double mu, int32_t flags, 
 
 int gk_gh_node_maps(gk_handle* h, int64_t g, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_gh_node_maps: null argument");
-  if (h->feature_kind != FK_GH || !h->features_ready) return fail(GK_ERR_STATE, "gk_gh_node_maps: run gk_gh_features first");
+  if (h->feature_kind != FK_GH) return fail(GK_ERR_STATE, "gk_gh_node_maps: run gk_gh_features first");
   if (g < 0 || g >= h->N) return fail(GK_ERR_ARG, "gk_gh_node_maps: bad graph index");
   const int delta = h->gh_delta;
   const long long T = (long long)delta * (delta + 1) / 2;
@@ -2117,20 +2119,18 @@ static int level_finish(gk_handle* h, const LevelScratch& ls, int n_blocks, cons
 
 int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const uint64_t* code_of_label,
                    const uint8_t* label_valid, int64_t n_labels, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_nh_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_nh_features"));
   if (!h->has_labels) return fail(GK_ERR_ARG, "gk_nh_features: vertex labels are required");
   if (R < 1 || R > MAX_LEVELS) return fail(GK_ERR_ARG, "gk_nh_features: R out of range [1, 64]");
   if (nh_type != GK_NH_SIMPLE && nh_type != GK_NH_COUNT_SENSITIVE) return fail(GK_ERR_ARG, "gk_nh_features: unknown nh_type");
   if (bits < 1 || bits > 64) return fail(GK_ERR_ARG, "gk_nh_features: bits out of range [1, 64]");
   if (flags != 0) return fail(GK_ERR_ARG, "gk_nh_features: no flags are defined");
   if (!code_of_label || n_labels < h->n_labels0) return fail(GK_ERR_ARG, "gk_nh_features: a code is needed for every label id");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E;
   const int64_t V1 = std::max<int64_t>(V, 1), L1 = std::max<int64_t>(n_labels, 1);
   const unsigned long long mask = bits == 64 ? ~0ULL : (1ULL << bits) - 1ULL;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
 
   GK_TRY(init_scalars(h, 0));  // clears ft_overflow
   GK_TRY(h->nh_codes.ensure((size_t)(R + 1) * V1 * 8));
@@ -2193,8 +2193,7 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
   GK_TRY(level_finish(h, ls, R, "gk_nh_features", &hs, &n_cols, &n_ent));
   h->nh_R = R;
   h->n_columns = n_cols;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_NH;
+  features_publish(h, FK_NH);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
@@ -2213,7 +2212,7 @@ int gk_nh_features(gk_handle* h, int32_t R, int32_t nh_type, int32_t bits, const
 
 int gk_nh_labels(gk_handle* h, int32_t level, uint64_t* out, uint8_t* valid) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_nh_labels: null argument");
-  if (h->feature_kind != FK_NH || !h->features_ready || level < 0 || level >= h->nh_R)
+  if (h->feature_kind != FK_NH || level < 0 || level >= h->nh_R)
     return fail(GK_ERR_STATE, "gk_nh_labels: no such level (run gk_nh_features first)");
   GK_CUDA(cudaSetDevice(h->dev));
   const size_t V = (size_t)h->V;
@@ -2385,19 +2384,17 @@ static int pm_keys(gk_handle* h, int s, int j, unsigned long long* keys, unsigne
 
 int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const double* U, const int32_t* n_cols,
                    const uint8_t* skip, int32_t n_sets, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_pm_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_pm_features"));
   if (L < 0) return fail(GK_ERR_ARG, "gk_pm_features: L < 0");
   if (L > MAX_LEVELS) return fail(GK_ERR_UNSUPPORTED, "gk_pm_features: at most L = 64 levels are supported");
   if (d < 1 || n_sets < 1) return fail(GK_ERR_ARG, "gk_pm_features: d and n_sets must be positive");
   if (flags & ~(GK_PM_LABELS | GK_PM_WL_LABELS)) return fail(GK_ERR_ARG, "gk_pm_features: unknown flags");
   if (!n_cols || (!U && h->V)) return fail(GK_ERR_ARG, "gk_pm_features: null embeddings or column counts");
   const bool wl = flags & GK_PM_WL_LABELS;
-  if (wl && (h->feature_kind != FK_WL || !h->features_ready || h->n_levels != n_iter + 1 || n_sets != n_iter + 1))
+  if (wl && (h->feature_kind != FK_WL || h->n_levels != n_iter + 1 || n_sets != n_iter + 1))
     return fail(GK_ERR_STATE, "gk_pm_features: GK_PM_WL_LABELS needs gk_wl_features(n_iter) first and n_iter + 1 sets");
   if (!wl && n_sets != 1 && (flags & GK_PM_LABELS)) return fail(GK_ERR_ARG, "gk_pm_features: one set per label source");
   if ((flags & GK_PM_LABELS) && !wl && !h->has_labels) return fail(GK_ERR_ARG, "gk_pm_features: vertex labels are required");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, M = V * (int64_t)d;
   if (M >= (1LL << 31)) return fail(GK_ERR_UNSUPPORTED, "gk_pm_features: V * d must stay below 2^31");
   // the level Grams count in fp32: exact while every intersection (<= d * n_max) stays below 2^24
@@ -2429,7 +2426,7 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
         }
   }
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   GK_TRY(init_scalars(h, 0));  // clears ft_overflow
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   if (wl && h->wl_sparse_ids) {  // the histogram rows are indexed by dense label ids
@@ -2464,8 +2461,7 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
   GK_TRY(level_finish(h, ls, n_blocks, "gk_pm_features", &hs, &n_col, &n_ent));
   h->nh_R = n_blocks;
   h->n_columns = n_col;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_PM;
+  features_publish(h, FK_PM);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
@@ -2482,7 +2478,7 @@ int gk_pm_features(gk_handle* h, int32_t n_iter, int32_t L, int32_t d, const dou
 
 int gk_pm_cells(gk_handle* h, int32_t set, int32_t level, int64_t* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_pm_cells: null argument");
-  if (h->feature_kind != FK_PM || !h->features_ready || set < 0 || set >= h->pm_S || level < 0 || level >= h->pm_L)
+  if (h->feature_kind != FK_PM || set < 0 || set >= h->pm_S || level < 0 || level >= h->pm_L)
     return fail(GK_ERR_STATE, "gk_pm_cells: no such set / level (run gk_pm_features first)");
   GK_CUDA(cudaSetDevice(h->dev));
   const size_t M = (size_t)h->V * h->pm_d;
@@ -2564,8 +2560,7 @@ static int gram_pm(gk_handle* h, const GramReq& q, gk_stats* stats) {
 int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const double* coef, int32_t n_coef,
                    const double* values, const int32_t* t_row_ptr, const int32_t* t_col_idx, const double* t_values,
                    const double* q, const double* w, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_rw_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_rw_features"));
   if (route != GK_RW_CG && route != GK_RW_SPECTRAL && route != GK_RW_SERIES) return fail(GK_ERR_ARG, "gk_rw_features: unknown route");
   if (fn != GK_RW_FINITE && fn != GK_RW_EXP && fn != GK_RW_INV) return fail(GK_ERR_ARG, "gk_rw_features: unknown fn");
   if (flags & ~GK_RW_LABELED) return fail(GK_ERR_ARG, "gk_rw_features: unknown flags");
@@ -2577,8 +2572,10 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
   if (route == GK_RW_SERIES && fn == GK_RW_INV) return fail(GK_ERR_UNSUPPORTED, "gk_rw_features: no series for the geometric inverse");
   if (route != GK_RW_SPECTRAL && h->E > 0 && (!values || !t_row_ptr || !t_col_idx || !t_values))
     return fail(GK_ERR_ARG, "gk_rw_features: edge values and the transposed CSR are required");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t V = h->V, E = h->E;
+  if (route != GK_RW_SPECTRAL && t_row_ptr && (t_row_ptr[0] != 0 || t_row_ptr[V] != E))
+    return fail(GK_ERR_ARG, "gk_rw_features: transposed row_ptr does not match the packed block");
+  features_begin(h);
   GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
   if (route != GK_RW_SPECTRAL) {
     GK_TRY(h->rw_val.ensure(std::max<int64_t>(E, 1) * 8));
@@ -2586,7 +2583,6 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
     GK_TRY(h->rw_tci.ensure(std::max<int64_t>(E, 1) * 4));
     GK_TRY(h->rw_trp.ensure((V + 1) * 4));
     if (t_row_ptr) {
-      if (t_row_ptr[0] != 0 || t_row_ptr[V] != E) return fail(GK_ERR_ARG, "gk_rw_features: transposed row_ptr does not match the packed block");
       GK_CUDA(cudaMemcpyAsync(h->rw_trp.p, t_row_ptr, (V + 1) * 4, cudaMemcpyHostToDevice, h->stream));
     } else {
       GK_CUDA(cudaMemsetAsync(h->rw_trp.p, 0, (V + 1) * 4, h->stream));
@@ -2614,8 +2610,7 @@ int gk_rw_features(gk_handle* h, int32_t route, int32_t fn, double lamda, const 
   GK_CUDA(cudaStreamSynchronize(h->stream));  // the caller's buffers may be reused once we return
   h->rw_route = route; h->rw_fn = fn; h->rw_lamda = lamda;
   h->rw_labeled = (flags & GK_RW_LABELED) != 0;
-  h->feature_kind = FK_RW;
-  h->features_ready = true; h->feat_serial++;
+  features_publish(h, FK_RW);
   if (stats) {
     stats->n_graphs = h->N; stats->n_vertices = V; stats->n_edges = E;
     stats->ms_h2d = ev_ms(h->tev[0], h->tev[1]);
@@ -2638,8 +2633,7 @@ int gk_rw_iterations(gk_handle* h, uint8_t* out) {
 int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const double* b, int32_t dim,
                    int32_t dim_orig, int64_t n_fit, const double* t_values, const double* p0, int32_t flags,
                    gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_pk_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_pk_features"));
   if (t_max < 1 || t_max > MAX_LEVELS) return fail(GK_ERR_ARG, "gk_pk_features: t_max out of range [1, 64]");
   if (!(w != 0.0) || !std::isfinite(w)) return fail(GK_ERR_ARG, "gk_pk_features: w must be finite and non-zero");
   if (flags & ~(GK_PK_ATTR | GK_PK_SQRT | GK_PK_STORE_F32 | GK_PK_STORE_INT | GK_PK_NEW_LABELS))
@@ -2655,11 +2649,10 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
   if (attr && !p0 && h->V) return fail(GK_ERR_ARG, "gk_pk_features: attributes need p0");
   if (!attr && !h->has_labels) return fail(GK_ERR_ARG, "gk_pk_features: vertex labels are required");
   if (!attr && h->n_labels0 > dim) return fail(GK_ERR_ARG, "gk_pk_features: a label id is >= dim");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E, V1 = std::max<int64_t>(V, 1);
   const int K = attr ? dim : 1;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   h->pk_levels = 0;
 
   // the dense P the reference also holds on the host: refuse clearly when it cannot fit
@@ -2786,8 +2779,7 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
   h->n_columns = (int64_t)hc[2];
   h->pk_levels = t_max;
   h->pk_K = K;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_PK;
+  features_publish(h, FK_PK);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
@@ -2807,7 +2799,7 @@ int gk_pk_features(gk_handle* h, int32_t t_max, double w, const double* u, const
 
 int gk_pk_hashes(gk_handle* h, int32_t level, double* out, uint8_t* priv) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_pk_hashes: null argument");
-  if (h->feature_kind != FK_PK || !h->features_ready || level < 0 || level >= h->pk_levels)
+  if (h->feature_kind != FK_PK || level < 0 || level >= h->pk_levels)
     return fail(GK_ERR_STATE, "gk_pk_hashes: no such level (run gk_pk_features first)");
   GK_CUDA(cudaSetDevice(h->dev));
   const size_t V = (size_t)h->V, K = (size_t)h->pk_K;
@@ -2930,10 +2922,11 @@ static bool sm_integral(const double* t, int64_t n) {
   return true;
 }
 
-int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double* vtable, int32_t n_vlabels,
-                   const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_sm_features: no graphs packed");
+// gk_sm_features without the publication: the relabelling frameworks publish after adding their levels
+static int sm_features_impl(gk_handle* h, int32_t k, const double* lambdas, const double* vtable, int32_t n_vlabels,
+                            const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
+                            gk_stats* stats) {
+  GK_TRY(need_packed(h, "gk_sm_features"));
   if (flags & ~(GK_SM_KV_NONE | GK_SM_KV_DIRAC | GK_SM_KE_NONE | GK_SM_KE_DIRAC))
     return fail(GK_ERR_ARG, "gk_sm_features: unknown flags");
   if ((flags & GK_SM_KV_NONE) && (flags & GK_SM_KV_DIRAC)) return fail(GK_ERR_ARG, "gk_sm_features: two vertex kernels");
@@ -2960,7 +2953,7 @@ int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double*
   // cliques of the product graph have at most min(n_x, n_y) vertices
   const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
   if (kk > SM_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_sm_features: subgraphs of more than 32 vertices");
-  GK_CUDA(cudaSetDevice(h->dev));
+  features_begin(h);
   h->sm_n_lv = 0;
   h->sm_hc = false;
   const int64_t N = h->N;
@@ -2995,12 +2988,17 @@ int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double*
   h->sm_n_vl = kv == SM_W_TABLE ? n_vlabels : 0;
   h->sm_n_el = ke == SM_W_TABLE ? n_elabels : 0;
   h->sm_exact = (kv != SM_W_TABLE || sm_integral(vtable, nvt)) && (ke != SM_W_TABLE || sm_integral(etable, net));
-  h->feature_kind = FK_SM;
-  h->features_ready = true; h->feat_serial++;
   if (stats) {
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
     stats->ms_h2d = ev_ms(h->tev[0], h->tev[1]);
   }
+  return GK_OK;
+}
+
+int gk_sm_features(gk_handle* h, int32_t k, const double* lambdas, const double* vtable, int32_t n_vlabels,
+                   const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags, gk_stats* stats) {
+  GK_TRY(sm_features_impl(h, k, lambdas, vtable, n_vlabels, etable, n_elabels, edge_label, flags, stats));
+  features_publish(h, FK_SM);
   return GK_OK;
 }
 
@@ -3147,7 +3145,7 @@ static int sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out, cons
 
 int gk_sm_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_counts: null argument");
-  if (h->feature_kind != FK_SM || !h->features_ready || h->sm_n_lv != 0)
+  if (h->feature_kind != FK_SM || h->sm_n_lv != 0)
     return fail(GK_ERR_STATE, "gk_sm_counts: call gk_sm_features first");
   return sm_counts(h, n_fit, row, out, "gk_sm_counts");
 }
@@ -3160,8 +3158,7 @@ static int sm_level_features(gk_handle* h, const char* fn, int32_t k, int32_t n_
                              const char* cap_msg, bool refine, const int32_t* level_ids, const double* lambdas,
                              const double* etable, int32_t n_elabels, const int32_t* edge_label, int32_t flags,
                              gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, std::string(fn) + ": no graphs packed");
+  GK_TRY(need_packed(h, fn));
   if (n_iter < 1) return fail(GK_ERR_ARG, std::string(fn) + ": n_iter < 1");
   if (!(flags & (GK_SM_KV_NONE | GK_SM_KV_DIRAC)))
     return fail(GK_ERR_UNSUPPORTED, std::string(fn) + ": the vertex kernel must be GK_SM_KV_DIRAC or GK_SM_KV_NONE");
@@ -3169,7 +3166,7 @@ static int sm_level_features(gk_handle* h, const char* fn, int32_t k, int32_t n_
   if (!all_levels && !level_ids) return fail(GK_ERR_ARG, std::string(fn) + ": no level ids");
   const int kk = std::max(1, std::min(std::max(k, 1), h->max_graph_size));
   if ((int64_t)n_lv * kk > bins) return fail(GK_ERR_UNSUPPORTED, std::string(fn) + ": " + cap_msg);
-  GK_TRY(gk_sm_features(h, k, lambdas, nullptr, 0, etable, n_elabels, edge_label, flags, stats));
+  GK_TRY(sm_features_impl(h, k, lambdas, nullptr, 0, etable, n_elabels, edge_label, flags, stats));
   const size_t bytes = (size_t)h->V * n_lv * 4;
   GK_TRY(h->sm_wl_cls.ensure(std::max<size_t>(bytes, 4)));
   if (!all_levels && bytes > 0) {
@@ -3178,6 +3175,7 @@ static int sm_level_features(gk_handle* h, const char* fn, int32_t k, int32_t n_
   }
   h->sm_n_lv = n_lv;
   h->sm_hc = !refine;
+  features_publish(h, FK_SM);
   return GK_OK;
 }
 
@@ -3192,7 +3190,7 @@ int gk_sm_wl_features(gk_handle* h, int32_t k, int32_t n_iter, const int32_t* le
 
 int gk_sm_wl_counts(gk_handle* h, int64_t n_fit, int64_t row, double* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_sm_wl_counts: null argument");
-  if (h->feature_kind != FK_SM || !h->features_ready || h->sm_n_lv == 0 || h->sm_hc)
+  if (h->feature_kind != FK_SM || h->sm_n_lv == 0 || h->sm_hc)
     return fail(GK_ERR_STATE, "gk_sm_wl_counts: call gk_sm_wl_features first");
   return sm_counts(h, n_fit, row, out, "gk_sm_wl_counts");
 }
@@ -3820,8 +3818,7 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
                      const int32_t* tok_rank, int64_t n_labels, const int64_t* rank_off, const uint8_t* rank_bytes,
                      const int32_t* rank_cp, int32_t n_ranks, const int64_t* el_off, const uint8_t* el_bytes,
                      const int32_t* el_cp, int32_t n_elabels, uint64_t* delta_mask, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_nspd_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_nspd_features"));
   if (!h->has_labels) return fail(GK_ERR_ARG, "gk_nspd_features: vertex labels are required");
   if (r < 0 || d < 0) return fail(GK_ERR_ARG, "gk_nspd_features: r and d must be >= 0");
   if ((int64_t)(r + 1) * (d + 1) > MAX_LEVELS)
@@ -3830,10 +3827,9 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   if (!sym_hash || (!edge_label && h->E) || !tok_rank || !rank_off || !rank_cp || !el_off || (!el_cp && n_elabels))
     return fail(GK_ERR_ARG, "gk_nspd_features: null table");
   if (n_labels < h->n_labels0) return fail(GK_ERR_ARG, "gk_nspd_features: a token is needed for every label id");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   const std::vector<int>& gp = h->graph_ptr_host;
   long long max_n = 1, max_e = 1;
   for (int64_t g = 0; g < N; ++g) {
@@ -3959,8 +3955,7 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
   int64_t n_cols = 0;
   for (int l = 0; l < n_lev; ++l) { h->nspd_cols[l] = (long long)hd[l]; n_cols += (int64_t)hd[l]; }
   h->n_columns = n_cols;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_NSPD;
+  features_publish(h, FK_NSPD);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
@@ -3978,7 +3973,7 @@ int gk_nspd_features(gk_handle* h, int32_t r, int32_t d, const int64_t* sym_hash
 
 int gk_nspd_hashes(gk_handle* h, int32_t radius, uint32_t* out) {
   if (!h || !out) return fail(GK_ERR_ARG, "gk_nspd_hashes: null argument");
-  if (h->feature_kind != FK_NSPD || !h->features_ready || radius < 0 || radius > h->nspd_r)
+  if (h->feature_kind != FK_NSPD || radius < 0 || radius > h->nspd_r)
     return fail(GK_ERR_STATE, "gk_nspd_hashes: no such radius (run gk_nspd_features first)");
   GK_CUDA(cudaSetDevice(h->dev));
   if (h->V) {
@@ -4132,7 +4127,7 @@ extern "C" {
 
 int gk_wl_level_sum(gk_handle* h, int32_t level, int64_t n_fit, int64_t row_begin, int64_t row_end, gk_stats* stats) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (!h->features_ready || h->feature_kind != FK_NSPD)
+  if (h->feature_kind != FK_NSPD)
     return fail(GK_ERR_STATE, "gk_wl_level_sum: run gk_nspd_features on the level's labels first");
   if (level < 0 || (level > 0 && (level != h->wl_sum_levels || h->core_sum)))
     return fail(GK_ERR_ARG, "gk_wl_level_sum: levels must be added in order, starting at 0");
@@ -4235,7 +4230,7 @@ int gk_core_level_add(gk_handle* h, int32_t level, int64_t n_fit, int64_t n_leve
                       const int32_t* cols, double* xdiag, double* ydiag, gk_stats* stats) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
   if (!h->core_sum) return fail(GK_ERR_STATE, "gk_core_level_add: no sum begun (gk_core_sum_begin)");
-  if (!h->features_ready) return fail(GK_ERR_STATE, "gk_core_level_add: run the base kernel's feature pass first");
+  if (h->feature_kind == FK_NONE) return fail(GK_ERR_STATE, "gk_core_level_add: run the base kernel's feature pass first");
   if (level < 0 || level >= h->core_level)
     return fail(GK_ERR_ARG, "gk_core_level_add: core levels must be added in strictly descending order");
   if (!GRAM_RULES[h->feature_kind].dev_out)
@@ -4332,10 +4327,9 @@ int gk_selftest_odd_collision(gk_handle* h, int32_t attempts) {
 // identities of different levels never meet and one table of (graph, identity) counts holds the sum over the levels.
 static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const int32_t* ids, const int32_t* rank,
                              gk_stats* stats) {
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V, E = h->E;
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   const std::vector<int>& gp = h->graph_ptr_host;
   std::vector<long long> base(2 * (N + 1), 0);
   long long* nbase = base.data();
@@ -4480,8 +4474,7 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
   GK_CUDA(cudaStreamSynchronize(h->stream));
   for (int b = 0; b < B; ++b) h->odd_cols[b] = (long long)hc[34 + b];
   h->n_columns = F;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_ODD;
+  features_publish(h, FK_ODD);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = E;
@@ -4501,8 +4494,7 @@ static int odd_features_impl(gk_handle* h, int32_t depth, int n_levels, const in
 extern "C" {
 
 int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_odd_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_odd_features"));
   if (!h->has_labels) return fail(GK_ERR_ARG, "gk_odd_features: vertex labels are required");
   if (depth == 0) return fail(GK_ERR_ARG, "gk_odd_features: h must be > 0 (or < 0 for no limit)");
   if (flags != 0) return fail(GK_ERR_ARG, "gk_odd_features: no flags are defined");
@@ -4512,8 +4504,7 @@ int gk_odd_features(gk_handle* h, int32_t depth, const int32_t* rank, int32_t fl
 
 int gk_wl_odd_features(gk_handle* h, int32_t depth, int32_t n_iter, const int32_t* ids, const int32_t* rank,
                        int32_t flags, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_wl_odd_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_wl_odd_features"));
   if (depth == 0) return fail(GK_ERR_ARG, "gk_wl_odd_features: h must be > 0 (or < 0 for no limit)");
   if (n_iter < 0 || n_iter >= MAX_LEVELS) return fail(GK_ERR_ARG, "gk_wl_odd_features: n_iter out of range");
   if (flags != 0) return fail(GK_ERR_ARG, "gk_wl_odd_features: no flags are defined");
@@ -4540,7 +4531,7 @@ int gk_wl_odd_features(gk_handle* h, int32_t depth, int32_t n_iter, const int32_
 // The signature of every identity, from its representative node: label id, children's identities in order, C.
 static int odd_host_signatures(gk_handle* h, std::vector<int>* label, std::vector<int64_t>* off, std::vector<int>* child,
                                std::vector<int>* C) {
-  if (h->feature_kind != FK_ODD || !h->features_ready) return fail(GK_ERR_STATE, "gk_odd_signatures: run gk_odd_features first");
+  if (h->feature_kind != FK_ODD) return fail(GK_ERR_STATE, "gk_odd_signatures: run gk_odd_features first");
   GK_CUDA(cudaSetDevice(h->dev));
   const long long S = h->odd_S, T = h->odd_T, F = h->odd_F;
   const OddNodes o = odd_nodes(h);
@@ -4738,8 +4729,7 @@ static int ml_ready(gk_handle* h, const char* who) {
 extern "C" {
 
 int gk_ml_begin(gk_handle* h, int32_t L, double gamma, double heta, const double* phi, int32_t dim, gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_ml_begin: no graphs packed");
+  GK_TRY(need_packed(h, "gk_ml_begin"));
   if (L < 0 || L > 64) return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: L outside [0, 64]");
   if (!(gamma > 0.0) || !(heta > 0.0) || !std::isfinite(gamma) || !std::isfinite(heta))
     return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: gamma and heta must be positive and finite (the Cholesky route)");
@@ -4747,13 +4737,14 @@ int gk_ml_begin(gk_handle* h, int32_t L, double gamma, double heta, const double
   if (h->max_graph_size > ML_NMAX)
     return fail(GK_ERR_UNSUPPORTED, "gk_ml_begin: a graph of more than 128 vertices (the neighbourhood matrix lives in "
                                     "shared memory)");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t N = h->N, V = h->V;
   std::vector<long long> off(N + 1, 0);
   for (int64_t g = 0; g < N; ++g) {
     const long long n = h->graph_ptr_host[g + 1] - h->graph_ptr_host[g];
     off[g + 1] = off[g] + n * n;
   }
+  features_begin(h);
+  h->ml_w = 0;  // no session until this call completes
   GK_CUDA(cudaEventRecord(h->tev[0], h->stream));
   GK_TRY(h->ml_adj_off.ensure((N + 1) * 8));
   GK_TRY(h->ml_adj.ensure(std::max<long long>(off[N], 1) * 8));
@@ -4806,8 +4797,6 @@ int gk_ml_begin(gk_handle* h, int32_t L, double gamma, double heta, const double
   for (int l = 0; l <= L; ++l) h->ml_mcap[l] = mcap[l];
   h->ml_gamma = gamma; h->ml_heta = heta;
   h->ml_nrec = 0;
-  h->features_ready = false; h->feat_serial++;
-  h->feature_kind = FK_NONE;
   if (stats) {
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
     stats->n_levels = L;
@@ -4920,8 +4909,7 @@ int gk_ml_finish(gk_handle* h, const double* fit_rec, int64_t n_fit, double* rec
     GK_CUDA(cudaMemcpyAsync(rec_out, rec + (size_t)n_fit * stride, (size_t)N * stride * 8, cudaMemcpyDeviceToHost, h->stream));
   GK_TRY(ml_check_err(h));
   h->ml_nrec = n_fit + N;
-  h->feature_kind = FK_ML;
-  h->features_ready = true; h->feat_serial++;
+  features_publish(h, FK_ML);
   if (stats) stats->ms_features = ev_ms(h->tev[0], h->tev[1]);
   return GK_OK;
 }
@@ -5061,6 +5049,8 @@ int gk_svmt_solve(gk_handle* h, int64_t n_graphs, const int32_t* sizes, const ui
   }
   const int64_t N = n_graphs, V = vptr[N];
   GK_CUDA(cudaSetDevice(h->dev));
+  features_begin(h);
+  h->svmt_sizes.clear();  // no solve until this call completes
   GK_TRY(h->svmt_vptr.ensure((size_t)(N + 1) * 4));
   GK_TRY(h->svmt_adj.ensure((size_t)V * 16));
   GK_TRY(h->svmt_m.ensure((size_t)N * 8));
@@ -5089,7 +5079,6 @@ int gk_svmt_solve(gk_handle* h, int64_t n_graphs, const int32_t* sizes, const ui
   LAUNCH_CHECK(h);
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   h->svmt_sizes.assign(sizes, sizes + N);
-  h->features_ready = false;
   h->n_rows = 0;  // a new block starts without a row map
   if (stats) {
     memset(stats, 0, sizeof(*stats));
@@ -5158,8 +5147,7 @@ int gk_svmt_phi(gk_handle* h, int32_t lo, int32_t n_levels, const int32_t* count
     return fail(GK_ERR_RANGE, "SvmTheta: the one-class SMO did not converge within 10 000 000 iterations on a graph (libsvm "
                               "need not converge on a non-symmetric matrix)");
   h->svmt_nrec = n_fit + N;
-  h->feature_kind = FK_SVMT;
-  h->features_ready = true; h->feat_serial++;
+  features_publish(h, FK_SVMT);
   if (stats) {
     stats->n_graphs = N; stats->n_vertices = nv;
     stats->ms_h2d = ev_ms(h->tev[5], h->tev[0]) + ev_ms(h->tev[7], h->tev[3]);
@@ -5251,8 +5239,7 @@ int gk_gs_draw(uint32_t* mt_key, int32_t* mt_pos, int64_t n_graphs, const int32_
 int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int64_t* samp_off,
                    const uint8_t* samp_size, const int32_t* idx, int64_t n_idx, const int64_t* prior, int64_t n_prior,
                    gk_stats* stats) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_gs_features: no graphs packed");
+  GK_TRY(need_packed(h, "gk_gs_features"));
   if (k < 1) return fail(GK_ERR_ARG, "gk_gs_features: k must be positive");
   if (k > GS_KMAX) return fail(GK_ERR_UNSUPPORTED, "gk_gs_features: graphlets of more than 6 vertices");
   const int64_t N = h->N;
@@ -5282,9 +5269,8 @@ int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int
     if (prior[3 * i] < 0 || prior[3 * i] >= g0 || prior[3 * i + 1] < 0 || prior[3 * i + 1] >= gs_base(k + 1) ||
         prior[3 * i + 2] < 1 || prior[3 * i + 2] >= (1LL << 31) - 1)
       return fail(GK_ERR_ARG, "gk_gs_features: a bad prior count");
-  GK_CUDA(cudaSetDevice(h->dev));
   const int64_t launches0 = h->launches;
-  h->features_ready = false; h->feat_serial++;
+  features_begin(h);
   GK_TRY(init_scalars(h, 0));
   GK_CUDA(cudaEventRecord(h->tev[2], h->stream));
   // ---- class table of the code space (sizes 0 .. k), and the number of classes it has
@@ -5395,8 +5381,7 @@ int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int
       return fail(GK_ERR_RANGE, "GraphletSampling: a self similarity of 2^53 or more (K would not be exact in fp64)");
   h->gs_cols = M;
   h->n_columns = M;
-  h->feature_kind = FK_GS;
-  h->features_ready = true; h->feat_serial++;
+  features_publish(h, FK_GS);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = h->V; stats->n_edges = h->E;
@@ -5413,7 +5398,7 @@ int gk_gs_features(gk_handle* h, int32_t k, int64_t n_fit, int64_t g0, const int
 
 int gk_gs_counts(gk_handle* h, int64_t cap, int64_t* out, int64_t* n_out) {
   if (!h || !n_out || (cap > 0 && !out)) return fail(GK_ERR_ARG, "gk_gs_counts: null argument");
-  if (h->feature_kind != FK_GS || !h->features_ready) return fail(GK_ERR_STATE, "gk_gs_counts: run gk_gs_features first");
+  if (h->feature_kind != FK_GS) return fail(GK_ERR_STATE, "gk_gs_counts: run gk_gs_features first");
   GK_CUDA(cudaSetDevice(h->dev));
   const size_t tc = h->gs_cap;
   std::vector<char> b(tc * 20);
@@ -5439,7 +5424,7 @@ extern "C" {
 int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64_t row_end, void* K_out,
             int32_t out_dtype, int64_t ld, double* xdiag, double* ydiag, gk_stats* stats) {
   if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (!h->features_ready) return fail(GK_ERR_STATE, "gk_gram: no feature block (call gk_wl_features / gk_sp_features)");
+  if (h->feature_kind == FK_NONE) return fail(GK_ERR_STATE, "gk_gram: no feature block (call gk_wl_features / gk_sp_features)");
   GramReq q;
   GK_TRY(gram_request(h, h->feature_kind, n_fit, flags, row_begin, row_end, K_out, out_dtype, ld, xdiag, ydiag, &q));
   GK_CUDA(cudaSetDevice(h->dev));
@@ -5447,9 +5432,7 @@ int gk_gram(gk_handle* h, int64_t n_fit, int32_t flags, int64_t row_begin, int64
 }
 
 int gk_set_row_map(gk_handle* h, int64_t n_rows, const int32_t* row_of_graph) {
-  if (!h) return fail(GK_ERR_ARG, "null handle");
-  if (h->N <= 0) return fail(GK_ERR_STATE, "gk_set_row_map: no graphs packed");
-  GK_CUDA(cudaSetDevice(h->dev));
+  GK_TRY(need_packed(h, "gk_set_row_map"));
   if (n_rows <= 0 || !row_of_graph) {  // back to the identity
     h->n_rows = 0;
     return GK_OK;
@@ -5595,8 +5578,8 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
   const long long cap_tail_ent = (long long)(h->tail_ent.cap / sizeof(int2));
   GK_CUDA(cudaSetDevice(h->dev));
   const int L = n_iter + 1;
+  features_begin(h);
   h->n_levels = L;
-  h->features_ready = false; h->feat_serial++;
   const int64_t launches0 = h->launches;
   WlPlan pl;
   GK_TRY(wl_setup(h, n_iter, &pl));
@@ -5778,14 +5761,13 @@ static int wl_gram_async(gk_handle* h, int32_t n_iter, int32_t flags, void* K_ou
     return GK_OK;  // more block overflows than the list holds (never seen): the synchronous route recomputes everything
   // ---- state as gk_wl_features + gk_gram leave it
   h->n_columns = hd.n_columns;
-  h->features_ready = true; h->feat_serial++;
-  h->feature_kind = FK_WL;
   h->Dc = hd.Dc; h->Dc_pad = hd.Dc_pad;
   if (force_T < 0) h->head_row_bytes = (long long)hd.Dc_pad * elem_bytes;
   h->last_max_count = (long long)hd.max_count;
   h->pro_hist = hd.hist;
   h->pro_max_count = (long long)hd.max_count; h->pro_max_diag = (long long)hd.max_diag; h->pro_n_entries = (long long)hd.n_entries;
-  h->pro_serial = h->feat_serial;
+  h->pro_ready = true;
+  features_publish(h, FK_WL);
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_graphs = N; stats->n_vertices = V; stats->n_edges = h->E;
@@ -5842,14 +5824,12 @@ int gk_wl_gram(gk_handle* h, int32_t n_iter, int32_t flags, void* K_out, int32_t
 int gk_wl_fit_transform(gk_handle* h, int64_t n_graphs, const int32_t* graph_ptr, const int32_t* row_ptr,
                         const int32_t* col_idx, const int32_t* labels, int32_t n_iter, int32_t flags, void* K_out,
                         int32_t out_dtype, int64_t ld, double* diag, gk_stats* stats) {
-  gk_stats s1, s2;
-  memset(&s1, 0, sizeof(s1));
-  memset(&s2, 0, sizeof(s2));
+  gk_stats st;
+  memset(&st, 0, sizeof(st));
   GK_TRY(gk_pack_csr(h, n_graphs, graph_ptr, row_ptr, col_idx, labels, nullptr, nullptr, 0));
-  GK_TRY(gk_wl_gram(h, n_iter, flags, K_out, out_dtype, ld, diag, &s2));
-  (void)s1;
+  GK_TRY(gk_wl_gram(h, n_iter, flags, K_out, out_dtype, ld, diag, &st));
   if (stats) {
-    *stats = s2;
+    *stats = st;
     stats->ms_h2d = ev_ms(h->tev[0], h->tev[1]);
   }
   return GK_OK;

@@ -205,15 +205,15 @@ struct gk_handle {
   gk::DevBuf ft_keys, ft_cnt;
   size_t ft_cap = 0;
   int64_t n_columns = 0;
-  bool features_ready = false;
-  int64_t feat_serial = 0;   // bumped whenever the feature block changes state
-  int64_t pro_serial = -1;   // feat_serial for which gk_wl_features already ran the Gram prologue (square case):
-                             // self similarities finished, column histogram on the host -- gk_gram then needs no
-                             // host synchronisation before its launches
+  // the complete feature block the handle holds, FK_NONE for none: a feature pass clears it when it starts and sets it
+  // as its last step (features_begin / features_publish in api.cu), so a pass that fails in between leaves no block
+  gk::FeatureKind feature_kind = gk::FK_NONE;
+  bool pro_ready = false;  // the pass that published the block also ran its square Gram prologue (gk_wl_features,
+                           // the asynchronous WL pass): self similarities finished, column histogram on the host --
+                           // gk_gram then needs no host synchronisation before its launches
   // the Gram prologue's results that gk_gram would otherwise read back after a synchronisation
   gk::ColStats pro_hist;
   long long pro_max_count = 0, pro_max_diag = 0, pro_n_entries = 0;
-  gk::FeatureKind feature_kind = gk::FK_NONE;
 
   gk::DevBuf oa_keys, oa_cnt, oa_colcnt;  // WL-OA: unary-expanded block, swapped with ft_keys / ft_cnt / colcnt
   // ---- columns / panel / diag

@@ -161,7 +161,8 @@ def test_multikernel_signature_kernels(eng, monkeypatch, width, attempts):
 @pytest.mark.parametrize("route", list(ROUTES))
 def test_retry_budget(eng, monkeypatch, route, from_level):
     """Nine degenerate attempts exhaust the retries: the error names the levels, the handle holds no features (gram
-    refuses rather than returning the previous block's K), and the next call without the hook is the oracle's."""
+    refuses rather than returning the previous block's K, and the label read-back refuses rather than returning the
+    failed attempt's labels), and the next call without the hook is the oracle's."""
     from grakel_b200._lib import GrakelB200Error
     _route(monkeypatch, route)
     ref = _main()
@@ -179,6 +180,8 @@ def test_retry_budget(eng, monkeypatch, route, from_level):
         assert mask == 1
     with pytest.raises(GrakelB200Error):
         eng.gram(ref.N)
+    with pytest.raises(GrakelB200Error, match="no such level"):
+        eng.wl_labels(1, ref.V)
     st = eng.wl_features(ref.h)
     assert int(st.hash_retries) == 0
     _check_all(eng, ref, st, f"{route} after the budget", rect=False)
